@@ -1,4 +1,4 @@
-"""B200-native cascade-MVS depth engine (hot path of kwea123/CasMVSNet_pl).
+"""H100-native cascade-MVS depth engine (hot path of kwea123/CasMVSNet_pl).
 
 Public surface mirrors the reference's Python boundary (SURVEY.md §8b):
 ``casmvsnet_pl_b200.models.mvsnet.CascadeMVSNet`` and

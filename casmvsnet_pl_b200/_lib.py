@@ -1,7 +1,7 @@
 """ctypes binding of libcasmvs.so (C ABI declared in include/casmvs.h).
 
 There is deliberately no fallback: if the shared library is missing or the
-device is not a B200-class GPU the import / call fails loudly.
+device is not a H100 (sm_90a) GPU the import / call fails loudly.
 """
 import ctypes
 import os
@@ -116,7 +116,7 @@ def launch_count():
 
 
 def fallback_count():
-    """tf32-mode layers that ran on the CUDA-core kernel because no tcgen05 kernel covers
+    """tf32-mode layers that ran on the CUDA-core kernel because no wgmma kernel covers
     their shape (0 for the reference architecture)."""
     return int(load().casmvs_fallback_count())
 

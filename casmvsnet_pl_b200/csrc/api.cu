@@ -22,15 +22,11 @@ void set_error(const char* fmt, ...) {
 int conv3d_direct(const float* x, const float* wpk, const float* scale, const float* shift,
                   float slope, const float* skip, float* y, int B, int Cin, int Cout, int D,
                   int h, int w, int kind, int stride, cudaStream_t st, int round_out);
-// conv3d_tma.cu (tcgen05 + TMA producer, persistent: the default stride-1 tensor path)
+// conv3d_tma.cu (wgmma + TMA producer, persistent: the stride-1 tensor path)
 int conv3d_tma(const float* x, const float* wpk, const float* scale, const float* shift,
                float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
                int w, int kind, int stride, int precision, cudaStream_t st);
-// conv3d_tma_n8.cu (tcgen05 + TMA, stride-1 layers with Cout <= 8: kd and kw folded into N)
-int conv3d_tma_n8(const float* x, const float* wpk, const float* scale, const float* shift,
-                  float slope, const float* skip, float* y, int B, int Cin, int Cout, int D,
-                  int h, int w, int kind, int stride, int precision, cudaStream_t st);
-// conv3d_tma2.cu (tcgen05 + TMA producer, persistent: stride-2 and transposed layers)
+// conv3d_tma2.cu (wgmma + TMA producer, persistent: stride-2 and transposed layers)
 int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
                 float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
                 int w, int kind, int stride, int precision, cudaStream_t st);
@@ -69,8 +65,8 @@ extern "C" int casmvs_device_check(int device) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device);
-  if (major != 10) {
-    set_error("device_check: compute capability %d.%d; libcasmvs is built for sm_100a only "
+  if (major != 9 || minor != 0) {
+    set_error("device_check: compute capability %d.%d; libcasmvs is built for sm_90a only "
               "(no fallback path)", major, minor);
     return -3;
   }
@@ -97,11 +93,8 @@ extern "C" int casmvs_conv3d_fwd(const float* x, const float* w_packed, const fl
   cudaStream_t st = as_stream(stream);
   if (precision == CASMVS_TF32) {
     const int pf = precision | flags;
-    // tcgen05 kernels: each returns 0 (handled), <0 (failed) or 1 (shape not covered)
-    int rc = conv3d_tma_n8(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
-                           stride, pf, st);
-    if (rc <= 0) return rc;
-    rc = conv3d_tma(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
+    // tensor-core kernels: each returns 0 (handled), <0 (failed) or 1 (shape not covered)
+    int rc = conv3d_tma(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
                     stride, pf, st);
     if (rc <= 0) return rc;
     if (kind != CASMVS_CONV_PLANAR) {

@@ -1,4 +1,4 @@
-// Shared helpers for libcasmvs (sm_100a only).
+// Shared helpers for libcasmvs (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,8 +7,8 @@
 
 #include "casmvs.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libcasmvs is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libcasmvs is written for sm_90a (H100) only"
 #endif
 
 namespace casmvs {
@@ -54,7 +54,7 @@ inline int num_sms() {
   int v = n[dev].load(std::memory_order_relaxed);
   if (v == 0) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    if (v <= 0) v = 148;
+    if (v <= 0) v = 132;
     n[dev].store(v, std::memory_order_relaxed);
   }
   return v;

@@ -8,7 +8,7 @@
 //
 // This is the bit-faithful-products path (CASMVS_FP32: every layer of both networks, the
 // data gradients of the training path) and the counted fallback of the TF32 mode for a layer
-// shape no tcgen05 kernel covers (casmvs_fallback_count; none in the reference architecture).
+// shape no tensor-core kernel covers (casmvs_fallback_count; none in the reference architecture).
 //
 // Thread = TW consecutive-w output voxels x COT output channels.  The block's
 // slice of the packed weights ([27][Cin][COT]) sits in shared memory and is read

@@ -1,30 +1,27 @@
 // K2 (tensor-core variant, TMA producer) — 3x3x3 stride-1 convolution as an im2col-free
-// implicit GEMM on tcgen05 (kind::tf32, fp32 accumulators in TMEM) with the norm-act (+skip)
-// epilogue fused.  sm_100a only.
+// implicit GEMM on wgmma (tf32 operands from shared memory, fp32 accumulators in registers)
+// with the norm-act (+skip) epilogue fused.  sm_90a.
 //
-// Replaces (reference, relative to /root/reference): ConvBnReLU3D
-// (models/modules.py:21-31) and the `prob` head (models/mvsnet.py:89,103) for the
-// stride-1 layers of CostRegNet (conv0, conv2, conv4, conv6, prob).
+// Replaces (reference): ConvBnReLU3D (models/modules.py:21-31) and the `prob` head
+// (models/mvsnet.py:89,103) for the stride-1 layers of CostRegNet (conv0, conv2, conv4, conv6,
+// prob), and the 1x3x3 planar convolutions of FeatureNet.
 //
 // The GEMM: M = 128 voxels = 8(w) x 16(h) of one depth slice, K = Cin per tap, N = 3 x GW (the
-// three kd taps share one A operand: an input slice feeds up to three output slices in ONE
-// MMA).  The input brick of a depth slice (18 x 10 voxels with halo, up to 32 channels) is
-// brought in by ONE TMA tiled load (cp.async.bulk.tensor.5d over x viewed as {C, W, H, D, B};
+// three kd taps share one A operand: an input slice feeds three output slices in ONE wgmma).
+// The input brick of a depth slice (18 x 10 voxels with halo) is brought in by Cin/4 TMA tiled
+// loads (cp.async.bulk.tensor.5d over x viewed as {C, W, H, D, B}, a box of 4 channels each;
 // out-of-bounds elements are zero-filled by the TMA unit = the conv's zero padding, in all
-// three spatial dimensions) -- the first generation of this kernel issued 180-1440 16-byte
-// cp.async per slice from four producer warps and was bound by them.  The brick
-// is voxel-major [18][10][CB] with the TMA swizzle matching the row size (CB*4 = 128/64/32
-// bytes -> SWIZZLE_128B/64B/32B); the A operand of tap (kh,kw) is a SHIFTED VIEW of it:
-// descriptor start = brick + (kh*10 + kw)*rowbytes (+32 B per K=8 step), stride between
-// 8-voxel groups (SBO) = one brick row of 10 voxels.  The hardware swizzle is a function of
-// absolute shared-memory address bits, so a start address that is not atom-aligned reads
-// consistently what the TMA wrote (profiles/microbench/umma_swizzle_view.cu: exact for all
-// nine shifts and all three swizzle modes with base_offset = 0).
+// three spatial dimensions).  Each load writes one [18][10][4 channels] brick: 16 bytes per
+// voxel, so 8 consecutive voxels of a brick row are one 128-byte wgmma core matrix and the A
+// operand of tap (kh,kw) is a SHIFTED VIEW of the bricks: descriptor start = brick +
+// (kh*10 + kw)*16 B, K direction = next brick (LBO), next 8-voxel row group = next brick row
+// (SBO = 160 B).  No swizzle, so any 16-byte-aligned start address is a valid view.
 //
-// Persistent CTAs (one launch wave), 6 warps: 0-3 epilogue, 4 TMA producer (one elected
-// thread), 5 MMA issuer.  Ring full barriers are armed with expect_tx and completed by the
-// TMA unit; ring empty barriers by tcgen05.commit; per output slice tfull (MMA -> epilogue)
-// and tempty (epilogue -> MMA, accumulator read and re-zeroed) barriers.
+// Persistent CTAs, 9 warps: two consumer warpgroups (rows 0-63 and 64-127 of the tile) and a
+// TMA producer warp.  Ring full barriers are armed with expect_tx and completed by the TMA
+// unit; ring empty barriers by the 256 consumer threads once their wgmma have retired.  The
+// accumulator of one input slice covers output slices it-2, it-1, it (column groups 0, 1, 2);
+// after the slice, group 0 is complete and goes through the epilogue, and the window rolls.
 #include <cudaTypedefs.h>
 #include <stdlib.h>
 
@@ -40,9 +37,6 @@ namespace tma {
 
 using namespace tc;
 
-constexpr int kThreadsTma = 6 * 32;
-constexpr int kProdWarp = 4, kIssueWarp = 5;
-
 struct Params {
   const float* bimg;    // pre-built B operand image [chunk][kh][kw][CIN/4][3*GW][4] (tf32-rounded)
   const float* scale;   // [Cout] or null
@@ -55,49 +49,61 @@ struct Params {
   int tiles_w, tiles_h, nchunks, dchunk;
   int round_out;        // round the stored activations to tf32 (unbiased next-layer operand)
   int planar;           // 1x3x3 kernel: input slice s feeds output slice s only (kd = 1)
-  long long* dbg;       // optional timeline of CTA 0: [role][slice][4] clock64 stamps
 };
-// per-role clock64 timeline of CTA 0 (profiles/tc_timeline.py): compiled in only with
-// `make TIMELINE=1` -- each stamp costs ~6 instructions in loops whose roles are bound by
-// their own scalar instruction stream (profiles/r2_k2_n8_stalls.txt)
-#ifdef CASMVS_TIMELINE
-#define TMA_STAMP(role, idx, k)                                                                 \
-  do {                                                                                          \
-    if (p.dbg && blockIdx.x == 0 && (idx) < 64) p.dbg[((role) * 64 + (idx)) * 4 + (k)] = clock64(); \
-  } while (0)
-#else
-#define TMA_STAMP(role, idx, k) do { } while (0)
-#endif
 
 template <int CIN, int GW, int SLOTS_>
 struct Smem {
   static constexpr int SLOTS = SLOTS_;
-  static constexpr int CB = CIN > 32 ? 32 : CIN;                    // channels per brick
-  static constexpr int NB = CIN / CB;                               // bricks per slice
-  static constexpr int ROWB = CB * 4;                               // bytes per voxel = swizzle span
-  static constexpr int kBrickData = kHaloH * kHaloW * ROWB;         // bytes one TMA load writes
-  static constexpr int kBrickBytes = (kBrickData + 1023) / 1024 * 1024;
-  static constexpr int kSlotBytes = NB * kBrickBytes;
+  static constexpr int CQ = CIN / 4;                                // bricks (4 channels) per slice
+  static constexpr int kBrickData = kHaloH * kHaloW * 16;           // bytes one TMA load writes
+  static constexpr int kBrickBytes = (kBrickData + 127) / 128 * 128;
+  static constexpr int kSlotBytes = CQ * kBrickBytes;
   static constexpr int kWBytes = 9 * CIN * 3 * GW * 4;              // [kh][kw][cq][3*GW][4]
-  static constexpr int kRingOff = 0;                                // 1024-aligned (swizzle atoms)
+  static constexpr int kRingOff = 0;
   static constexpr int kWOff = SLOTS * kSlotBytes;
   static constexpr int kParamOff = kWOff + kWBytes;                 // scale/shift [2][GW]
   static constexpr int kBarOff = kParamOff + 2 * GW * 4;
-  // barriers: full[8] @0, empty[8] @64, tmem ptr @128, tfull[32] @192, tempty[32] @448
-  static constexpr int kTotal = kBarOff + 192 + 32 * 8 + 32 * 8 + 1024;   // + alignment slack
-  // UMMA layout type of the A operand: SWIZZLE_128B = 2, 64B = 4, 32B = 6
-  static constexpr uint32_t kLayout = ROWB == 128 ? 2u : ROWB == 64 ? 4u : 6u;
+  // barriers: full[8] @0, empty[8] @64, weight image @128
+  static constexpr int kTotal = kBarOff + 192 + 1024;               // + alignment slack
 };
 
-__host__ __device__ constexpr int tmem_cols_for(int n) {
-  return n <= 32 ? 32 : n <= 64 ? 64 : n <= 128 ? 128 : n <= 256 ? 256 : 512;
+// Epilogue of one output slice from the accumulator columns [OFF, OFF + GW) of this thread's
+// fragment: scale/shift, leaky ReLU, optional skip, optional tf32 rounding, channel-last store.
+template <int GW, int OFF>
+__device__ __forceinline__ void store_slice(const float* acc, const Params& p, const float* s_param,
+                                            int b, int od, int h0, int w0, int row0, int wl,
+                                            int lane, int co_base) {
+  for_each_pair<OFF, GW>(acc, wl, lane, [&](int r, int c, float a0, float a1) {
+    const int m = row0 + r;
+    const int oh = h0 + (m >> 3), ow = w0 + (m & 7);
+    if (oh >= p.H || ow >= p.W || c >= p.Cout) return;
+    const size_t o = ((((size_t)b * p.D + od) * p.H + oh) * p.W + ow) * p.cout_total + co_base + c;
+    float v0 = fmaf(a0, s_param[c], s_param[GW + c]);
+    float v1 = fmaf(a1, s_param[c + 1], s_param[GW + c + 1]);
+    v0 = v0 >= 0.f ? v0 : v0 * p.slope;
+    v1 = v1 >= 0.f ? v1 : v1 * p.slope;
+    if (c + 1 < p.Cout && (p.cout_total & 1) == 0) {
+      if (p.skip) {
+        const float2 s2 = __ldg(reinterpret_cast<const float2*>(p.skip + o));
+        v0 += s2.x; v1 += s2.y;
+      }
+      if (p.round_out) { v0 = to_tf32(v0); v1 = to_tf32(v1); }
+      *reinterpret_cast<float2*>(p.y + o) = make_float2(v0, v1);
+    } else {
+      if (p.skip) v0 += __ldg(p.skip + o);
+      p.y[o] = p.round_out ? to_tf32(v0) : v0;
+      if (c + 1 < p.Cout) {
+        if (p.skip) v1 += __ldg(p.skip + o + 1);
+        p.y[o + 1] = p.round_out ? to_tf32(v1) : v1;
+      }
+    }
+  });
 }
 
-template <int CIN, int GW, int SLOTS_>
-__global__ void __launch_bounds__(kThreadsTma, 1)
+template <int CIN, int GW, int SLOTS_, bool PLANAR>
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   using S = Smem<CIN, GW, SLOTS_>;
-  constexpr int CQ = CIN / 4;
   constexpr int SLOTS = S::SLOTS;
   extern __shared__ unsigned char smem_raw[];
   const uint32_t s_raw = smem_u32(smem_raw);
@@ -106,58 +112,34 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   const uint32_t s_ring = s_base + S::kRingOff, s_w = s_base + S::kWOff,
                  s_bar = s_base + S::kBarOff;
   float* s_param = reinterpret_cast<float*>(smem + S::kParamOff);
-  const uint32_t bar_full = s_bar, bar_empty = s_bar + 64, bar_tfull = s_bar + 192,
-                 bar_tempty = s_bar + 448, bar_w = s_bar + 136;   // bar_w: weight image landed
-  volatile uint32_t* s_tmem_ptr = reinterpret_cast<volatile uint32_t*>(smem + S::kBarOff + 128);
+  const uint32_t bar_full = s_bar, bar_empty = s_bar + 64, bar_w = s_bar + 128;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t tmem_cols = tmem_cols_for(p.dchunk * GW);
+  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int total_items = p.B * p.nchunks * p.tiles_h * p.tiles_w;
 
   // ---- one-time setup ----
-  if (threadIdx.x == 0) TMA_STAMP(3, 0, 0);
   {
     const int t = threadIdx.x;
     if (t < SLOTS) mbar_init(bar_full + 8 * t, 1);
-    else if (t < 2 * SLOTS) mbar_init(bar_empty + 8 * (t - SLOTS), 1);
-    else if (t >= 32 && t < 64) mbar_init(bar_tfull + 8 * (t - 32), 1);
-    else if (t >= 64 && t < 96) mbar_init(bar_tempty + 8 * (t - 64), 128);
-    else if (t == 96) mbar_init(bar_w, 1);
-    if (t < 97) fence_barrier_init();
+    else if (t < 2 * SLOTS) mbar_init(bar_empty + 8 * (t - SLOTS), kConsumerThreads);
+    else if (t == 2 * SLOTS) mbar_init(bar_w, 1);
+    if (t <= 2 * SLOTS) fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(smem_u32((const void*)s_tmem_ptr), tmem_cols);
   const int co_base = blockIdx.y * p.Cout;
-  for (int i = threadIdx.x; i < GW; i += kThreadsTma) {
+  for (int i = threadIdx.x; i < GW; i += kConvThreads) {
     s_param[i] = (i < p.Cout) ? (p.scale ? __ldg(p.scale + co_base + i) : 1.f) : 0.f;
     s_param[GW + i] = (i < p.Cout) ? (p.shift ? __ldg(p.shift + co_base + i) : 0.f) : 0.f;
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem_ptr;
   if (threadIdx.x == 0) load_image_bulk(s_w, p.bimg + (size_t)blockIdx.y * (S::kWBytes / 4), S::kWBytes, bar_w);
-  // One accumulator (GW columns) per output slice of a chunk, laid out linearly, so the three
-  // slices an input slice feeds are always adjacent columns.  Zeroed here, and re-zeroed by the
-  // epilogue after every read: all MMAs accumulate (the accumulate flag is per instruction, not
-  // per column, so a first-touch overwrite is not expressible for one group of three).
-  if (warp < 4) {
-    for (int c = 0; c < p.dchunk * GW; c += 16)
-      tmem_zero16(tmem_base + ((uint32_t)(warp * 32) << 16) + c);
-    tmem_wait_st();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
 
-  if (threadIdx.x == 0) TMA_STAMP(3, 0, 1);
   // nothing above depends on the previous kernel of the stream (see tma_common.cuh)
   tma::pdl_trigger();
   tma::pdl_wait();
-  bool w_ready = false;                             // MMA issuer: weight image has landed
+  bool w_ready = false;                             // consumers: weight image has landed
   uint32_t gs = 0;                                  // slices processed before this item (all roles)
-  int ep = 0;                                       // items processed by this CTA
-  for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x, ++ep) {
+  for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x) {
     int item = item0;
     const int tw = item % p.tiles_w; item /= p.tiles_w;
     const int th = item % p.tiles_h; item /= p.tiles_h;
@@ -166,150 +148,91 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
     const int w0 = tw * kTileW, h0 = th * kTileH;
     const int d0 = ck * p.dchunk, d1 = min(p.D, d0 + p.dchunk);
     const int nd = d1 - d0;
-    const int halo = p.planar ? 0 : 1;
+    const int halo = PLANAR ? 0 : 1;
     const int nslices = nd + 2 * halo;              // input slices d0-halo .. d1-1+halo
 
     if (warp == kProdWarp) {
-      // ===================== producer: one TMA load per brick =====================
+      // ===================== producer: Cin/4 TMA loads per slice =====================
       if (lane == 0) {
         for (int it = 0; it < nslices; ++it) {
           const uint32_t g = gs + it;
           const int slot = g % SLOTS;
-          TMA_STAMP(0, g, 0);
           if (g >= (uint32_t)SLOTS) mbar_wait(bar_empty + 8 * slot, ((g / SLOTS) - 1) & 1);
-          TMA_STAMP(0, g, 1);
           const uint32_t dst = s_ring + slot * S::kSlotBytes;
-          mbar_expect_tx(bar_full + 8 * slot, S::NB * S::kBrickData);
+          mbar_expect_tx(bar_full + 8 * slot, S::CQ * S::kBrickData);
 #pragma unroll
-          for (int nb = 0; nb < S::NB; ++nb)
-            tma_load_5d(dst + nb * S::kBrickBytes, &xmap, bar_full + 8 * slot, nb * S::CB,
-                        w0 - 1, h0 - 1, d0 - halo + it, b);
-          TMA_STAMP(0, g, 2);
+          for (int q = 0; q < S::CQ; ++q)
+            tma_load_5d(dst + q * S::kBrickBytes, &xmap, bar_full + 8 * slot, q * 4, w0 - 1,
+                        h0 - 1, d0 - halo + it, b);
         }
       }
       __syncwarp();
-    } else if (warp == kIssueWarp) {
-      // ===================== MMA issuer =====================
-      // Warp-uniform code with elect-predicated issue (descriptors stay in uniform registers);
-      // everything per MMA is base + compile-time offset.
-      constexpr uint32_t a_lbo = 16, a_sbo = kHaloW * S::ROWB;          // 8-voxel group stride
+    } else {
+      // ============ consumer warpgroups: wgmma into registers, then the epilogue ============
+      const int wg = warp >> 2, wl = warp & 3;
+      const int row0 = 64 * wg;                      // first GEMM row of this warpgroup
+      constexpr uint32_t a_lbo = S::kBrickBytes, a_sbo = kHaloW * 16;   // 8-voxel group stride
       constexpr uint32_t b_lbo = 3 * GW * 16, b_sbo = 128;
-      constexpr int KPB = S::CB / 8;                                      // K=8 steps per brick
-      const uint32_t elected = elect_one();
-      const uint64_t a_desc0 = make_desc(s_ring, a_lbo, a_sbo) | ((uint64_t)S::kLayout << 61);
+      const uint64_t a_desc0 = make_desc(s_ring + 8 * wg * a_sbo, a_lbo, a_sbo);
       const uint64_t b_desc0 = make_desc(s_w, b_lbo, b_sbo);
-      const uint32_t a_hi = (uint32_t)(a_desc0 >> 32), b_hi = (uint32_t)(b_desc0 >> 32);
+      float acc[3 * GW / 2];
+#pragma unroll
+      for (int i = 0; i < 3 * GW / 2; ++i) acc[i] = 0.f;
       for (int it = 0; it < nslices; ++it) {
         const uint32_t g = gs + it;
-        // input slice `it` feeds output slices j = it - kd, kd = 0,1,2, clipped to [0,nd):
-        // columns [j_lo*GW, (j_hi+1)*GW), B rows [(2-kd_hi)*GW, (3-kd_lo)*GW)
-        const int kd_lo = p.planar ? 1 : max(0, it - (nd - 1));
-        const int kd_hi = p.planar ? 1 : min(2, it);
-        const int j_lo = p.planar ? it : it - kd_hi;
-        const uint32_t idesc = make_idesc(128, (kd_hi - kd_lo + 1) * GW);
-        const uint32_t acc = tmem_base + j_lo * GW;
-        if (lane == 0) TMA_STAMP(1, g, 0);
         mbar_wait(bar_full + 8 * (g % SLOTS), (g / SLOTS) & 1);
         if (!w_ready) { mbar_wait(bar_w, 0); w_ready = true; }
-        if (lane == 0) TMA_STAMP(1, g, 1);
-        // first touch of group `it` in this item: the epilogue must have drained + re-zeroed it
-        if (ep > 0 && it < nd) mbar_wait(bar_tempty + 8 * it, (ep - 1) & 1);   // (it < nd always when planar)
-        if (lane == 0) TMA_STAMP(1, g, 2);
-        tc_fence_after();
-        const uint32_t a_lo0 = (uint32_t)a_desc0 + (((g % SLOTS) * S::kSlotBytes) >> 4);
-        const uint32_t b_lo0 = (uint32_t)b_desc0 + (((2 - kd_hi) * GW * 16) >> 4);
+        const uint64_t a_s = a_desc0 + (((g % SLOTS) * S::kSlotBytes) >> 4);
+        if constexpr (PLANAR) {
+          // kd = 1 only: B column group 1, one output slice per input slice
 #pragma unroll
-        for (int khw = 0; khw < 9; ++khw) {
-          const int kh = khw / 3, kw = khw % 3;
+          for (int i = 0; i < GW / 2; ++i) acc[i] = 0.f;
+          wgmma_fence();
 #pragma unroll
-          for (int k8 = 0; k8 < CIN / 8; ++k8) {
-            const uint32_t a_off = ((kh * kHaloW + kw) * S::ROWB + (k8 % KPB) * 32 +
-                                    (k8 / KPB) * S::kBrickBytes) >> 4;
-            const uint32_t b_off = (khw * (CIN * 3 * GW * 4) + k8 * 2 * 3 * GW * 16) >> 4;
-            umma_tf32(acc, a_lo0 + a_off, a_hi, b_lo0 + b_off, b_hi, idesc, elected);
-          }
-        }
-        if (p.planar) umma_commit(bar_tfull + 8 * it, elected);        // slice it complete
-        else if (it >= 2) umma_commit(bar_tfull + 8 * (it - 2), elected);   // slice it-2 complete
-        umma_commit(bar_empty + 8 * (g % SLOTS), elected);             // smem slot free
-        if (lane == 0) TMA_STAMP(1, g, 3);
-      }
-      // groups this (short) chunk did not use go through the same handshake (empty -> full)
-      // so that every barrier sees exactly one completion per item and no phase can alias
-      for (int j = nd; j < p.dchunk; ++j) {
-        if (ep > 0) mbar_wait(bar_tempty + 8 * j, (ep - 1) & 1);
-        if (elected) mbar_arrive(bar_tfull + 8 * j);
-        __syncwarp();
-      }
-    } else {
-      // ===================== epilogue warps 0..3 =====================
-      const int m = warp * 32 + lane;              // GEMM row = TMEM lane
-      const int oh = h0 + (m >> 3), ow = w0 + (m & 7);
-      const bool in_range = oh < p.H && ow < p.W;
-      const uint32_t lane_base = tmem_base + ((uint32_t)(warp * 32) << 16);
-      for (int j = 0; j < p.dchunk; ++j) {
-        if (threadIdx.x == 0) TMA_STAMP(2, ep * p.dchunk + j, 0);
-        mbar_wait(bar_tfull + 8 * j, ep & 1);
-        if (threadIdx.x == 0) TMA_STAMP(2, ep * p.dchunk + j, 1);
-        if (j >= nd) {                             // unused group: handshake only
-          mbar_arrive(bar_tempty + 8 * j);
-          continue;
-        }
-        tc_fence_after();
-        float acc[GW];
-        tmem_ld<GW>(lane_base + j * GW, acc);
+          for (int khw = 0; khw < 9; ++khw) {
+            const int kh = khw / 3, kw = khw % 3;
 #pragma unroll
-        for (int c = 0; c < GW; c += 16) tmem_zero16(lane_base + j * GW + c);
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(bar_tempty + 8 * j);           // group j drained and zero again
-        if (threadIdx.x == 0) TMA_STAMP(2, ep * p.dchunk + j, 2);
-        if (in_range) {
-          const size_t o =
-              ((((size_t)b * p.D + (d0 + j)) * p.H + oh) * p.W + ow) * p.cout_total + co_base;
-          if (p.Cout % 4 == 0) {
-#pragma unroll
-            for (int c = 0; c < GW; c += 4) {
-              if (c < p.Cout) {
-                float v[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  float t = fmaf(acc[c + k], s_param[c + k], s_param[GW + c + k]);
-                  v[k] = t >= 0.f ? t : t * p.slope;
-                }
-                if (p.skip) {
-                  const float4 s4 = ldg4(p.skip + o + c);
-                  v[0] += s4.x; v[1] += s4.y; v[2] += s4.z; v[3] += s4.w;
-                }
-                if (p.round_out) {
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) v[k] = to_tf32(v[k]);
-                }
-                st4(p.y + o + c, make_float4(v[0], v[1], v[2], v[3]));
-              }
+            for (int k8 = 0; k8 < CIN / 8; ++k8) {
+              const uint32_t a_off = ((kh * kHaloW + kw) * 16 + 2 * k8 * S::kBrickBytes) >> 4;
+              const uint32_t b_off = (khw * (CIN * 3 * GW * 4) + k8 * 2 * 3 * GW * 16 + GW * 16) >> 4;
+              wgmma_tf32<GW>(acc, a_s + a_off, b_desc0 + b_off);
             }
-          } else {
+          }
+        } else {
+          wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < GW; ++c) {
-              if (c < p.Cout) {
-                float t = fmaf(acc[c], s_param[c], s_param[GW + c]);
-                t = t >= 0.f ? t : t * p.slope;
-                if (p.skip) t += __ldg(p.skip + o + c);
-                p.y[o + c] = t;
-              }
+          for (int khw = 0; khw < 9; ++khw) {
+            const int kh = khw / 3, kw = khw % 3;
+#pragma unroll
+            for (int k8 = 0; k8 < CIN / 8; ++k8) {
+              const uint32_t a_off = ((kh * kHaloW + kw) * 16 + 2 * k8 * S::kBrickBytes) >> 4;
+              const uint32_t b_off = (khw * (CIN * 3 * GW * 4) + k8 * 2 * 3 * GW * 16) >> 4;
+              wgmma_tf32<3 * GW>(acc, a_s + a_off, b_desc0 + b_off);
             }
           }
         }
+        wgmma_commit();
+        wgmma_wait_all();
+        mbar_arrive(bar_empty + 8 * (g % SLOTS));   // this thread's reads of the slot are done
+        // output slice of column group 0: `it` when planar, else it - 2 (complete after its
+        // third input slice).  Group 0 is copied out before the (per-thread) stores so that no
+        // accumulator register is touched on a divergent path: that would make ptxas serialize
+        // the wgmma of the next slice.
+        float done[GW / 2];
+#pragma unroll
+        for (int i = 0; i < GW / 2; ++i) done[i] = acc[i];
+        if constexpr (!PLANAR) {
+#pragma unroll
+          for (int i = 0; i < GW; ++i) acc[i] = acc[i + GW / 2];   // groups 1, 2 -> 0, 1
+#pragma unroll
+          for (int i = 0; i < GW / 2; ++i) acc[GW + i] = 0.f;
+        }
+        const int j = PLANAR ? it : it - 2;
+        if (j >= 0 && j < nd)
+          store_slice<GW, 0>(done, p, s_param, b, d0 + j, h0, w0, row0, wl, lane, co_base);
       }
     }
     gs += nslices;
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -387,7 +310,8 @@ const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, 
   const cuuint32_t estr[5] = {1, (cuuint32_t)stride_w, 1, 1, 1};
   const CUtensorMapSwizzle sw = CB * 4 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                 : CB * 4 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                               : CU_TENSOR_MAP_SWIZZLE_32B;
+                                : CB * 4 == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                               : CU_TENSOR_MAP_SWIZZLE_NONE;
   const CUresult r = enc(&e.map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(x), gdim,
                          gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -403,30 +327,23 @@ const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, 
 }
 
 
-template <int CIN, int GW, int SLOTS>
+template <int CIN, int GW, int SLOTS, bool PLANAR>
 static int launch(const float* x, const float* wpk, Params p, cudaStream_t st) {
   using S = Smem<CIN, GW, SLOTS>;
-  auto kfn = conv3d_tma_kernel<CIN, GW, SLOTS>;
+  static_assert(S::kTotal <= 227 * 1024, "shared memory budget");
+  auto kfn = conv3d_tma_kernel<CIN, GW, SLOTS, PLANAR>;
   static std::atomic<bool> attr_set[kMaxDevices];
   if (int rc = opt_in_smem(kfn, S::kTotal, attr_set, "conv3d_tma")) return rc;
-  const CUtensorMap* map = input_map(x, p.B, p.D, p.H, p.W, CIN, S::CB, kHaloW, kHaloH);
+  const CUtensorMap* map = input_map(x, p.B, p.D, p.H, p.W, CIN, 4, kHaloW, kHaloH);
   if (!map) return -2;
-  // resident CTAs per SM by shared memory (1 KB per CTA is reserved by the system); the TMEM
-  // of all of them must fit in 512 columns: one accumulator group (GW columns) per output slice
-  static int per_sm_env = -1, dchunk_env = -1;
-  if (per_sm_env < 0) {
-    const char* e = getenv("CASMVS_TMA_PER_SM");
-    per_sm_env = e ? atoi(e) : 0;
+  static int dchunk_env = -1;
+  if (dchunk_env < 0) {
     const char* d = getenv("CASMVS_TMA_DCHUNK");
     dchunk_env = d ? atoi(d) : 0;
   }
-  int per_sm = (228 * 1024) / (S::kTotal + 1024);
-  if (per_sm > 4) per_sm = 4;
-  if (per_sm < 1) per_sm = 1;
-  if (per_sm_env > 0 && per_sm_env < per_sm) per_sm = per_sm_env;
+  const int per_sm = resident_per_sm(kfn, kConvThreads, S::kTotal);
   const int nco = p.cout_total / p.Cout;
-  int cap = pow2_floor(512 / per_sm) / GW;
-  if (cap > 32) cap = 32;
+  const int cap = 32;
   const long cols = (long)p.B * p.tiles_w * p.tiles_h;
   int dchunk = pick_dchunk(p.D, cap, cols, (long)num_sms() * per_sm / nco, 1, p.planar ? 0 : 2);
   if (dchunk_env > 0 && dchunk_env <= cap) dchunk = dchunk_env < p.D ? dchunk_env : p.D;
@@ -443,7 +360,7 @@ static int launch(const float* x, const float* wpk, Params p, cudaStream_t st) {
   int resident = num_sms() * per_sm / nco;
   if (resident < 1) resident = 1;
   const long gx = items < resident ? items : resident;
-  launch_pdl(ir.settled, kfn, dim3((unsigned)gx, (unsigned)nco), kThreadsTma, S::kTotal, st, *map, p);
+  launch_pdl(ir.settled, kfn, dim3((unsigned)gx, (unsigned)nco), kConvThreads, S::kTotal, st, *map, p);
   return after_launch("conv3d_tma");
 }
 
@@ -455,12 +372,10 @@ int conv3d_tma(const float* x, const float* wpk, const float* scale, const float
                int w, int kind, int stride, int precision_flags, cudaStream_t st) {
   const int precision = precision_flags & 0xff;
   static int enabled = -1, round_out = 1;
-  static long long* dbg = nullptr;
   if (enabled < 0) {
     const char* e = getenv("CASMVS_TMA");
     enabled = e ? atoi(e) : 1;
     if (const char* s = getenv("CASMVS_TC_ROUND")) round_out = atoi(s);
-    if (const char* s = getenv("CASMVS_TC_DBG")) dbg = (long long*)strtoull(s, nullptr, 0);
   }
   if (!enabled || precision != CASMVS_TF32) return 1;
   if ((kind != CASMVS_CONV && kind != CASMVS_CONV_PLANAR) || stride != 1) return 1;
@@ -475,12 +390,13 @@ int conv3d_tma(const float* x, const float* wpk, const float* scale, const float
   p.tiles_w = (w + tc::kTileW - 1) / tc::kTileW;
   p.tiles_h = (h + tc::kTileH - 1) / tc::kTileH;
   const int npad = p.Cout <= 16 ? 16 : 32;
-  p.dbg = dbg;
   p.planar = kind == CASMVS_CONV_PLANAR ? 1 : 0;
   // the prob head feeds the softmax: keep fp32; callers can ask for unrounded outputs
   p.round_out = (round_out && Cout > 1 && !(precision_flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
-#define TMA_CASE(CI, NP, SL) \
-  if (Cin == CI && npad == NP) return tma::launch<CI, NP, SL>(x, wpk, p, st);
+#define TMA_CASE(CI, NP, SL)                                                    \
+  if (Cin == CI && npad == NP)                                                  \
+    return p.planar ? tma::launch<CI, NP, SL, true>(x, wpk, p, st)              \
+                    : tma::launch<CI, NP, SL, false>(x, wpk, p, st);
   TMA_CASE(8, 16, 4) TMA_CASE(8, 32, 4) TMA_CASE(16, 16, 4) TMA_CASE(16, 32, 4)
   TMA_CASE(32, 16, 4) TMA_CASE(32, 32, 4) TMA_CASE(64, 16, 2)
 #undef TMA_CASE

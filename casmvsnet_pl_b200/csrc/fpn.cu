@@ -147,7 +147,7 @@ __device__ __forceinline__ float round_tf32_if(float x, int on) {
 
 // feat[n,y,x,:] = up2_bilinear(prev)[n,y,x,:] + lat_w @ c[n,y,x,:] + lat_b  (32 channels).
 // Four threads per pixel (8 channels each) x kMergeP pixels per thread.  The kernel is bound
-// by the L1/shared pipe (ncu: l1tex 89 % with one pixel per thread, profiles/r1_misc_full):
+// by the L1/shared pipe with one pixel per thread:
 // every 128-bit shared or global access costs a warp four L1 cycles, so the lateral weights
 // of a channel group are read from shared memory once per kMergeP pixels instead of once per
 // pixel.  HBM traffic: reads c + prev (a quarter of the pixels), writes 128 B per pixel.

@@ -7,7 +7,8 @@ namespace casmvs {
 
 constexpr int kCPT = 8;          // channels per thread
 
-// ---- packed fp32x2 helpers (Blackwell FFMA2 / 256-bit LDG, STG) -----------------
+// ---- fp32 pair helpers: two values in one 64-bit register (32-byte texel loads / stores);
+// the arithmetic is one IEEE fp32 operation per lane, round to nearest -----------------
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pk2(float lo, float hi) {
   u64 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi)); return r;
@@ -16,24 +17,30 @@ __device__ __forceinline__ void unpk2(u64 v, float& lo, float& hi) {
   asm("mov.b64 {%0,%1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-  u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpk2(a, a0, a1); unpk2(b, b0, b1); unpk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-  u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d;
+  float a0, a1, b0, b1;
+  unpk2(a, a0, a1); unpk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ u64 add2(u64 a, u64 b) {
-  u64 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d;
+  float a0, a1, b0, b1;
+  unpk2(a, a0, a1); unpk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 struct Tex8 { u64 v[4]; };   // 8 channels of one texel, as 4 packed pairs
-__device__ __forceinline__ Tex8 ldg256(const float* p) {   // 32-byte aligned
+__device__ __forceinline__ Tex8 ldg256(const float* p) {   // 32-byte aligned: two 16-byte loads
   Tex8 t;
-  asm volatile("ld.global.nc.v4.b64 {%0,%1,%2,%3}, [%4];"
-               : "=l"(t.v[0]), "=l"(t.v[1]), "=l"(t.v[2]), "=l"(t.v[3]) : "l"(p));
+  asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[0]), "=l"(t.v[1]) : "l"(p));
+  asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[2]), "=l"(t.v[3]) : "l"(p + 4));
   return t;
 }
 __device__ __forceinline__ void stg256(float* p, const u64 (&v)[4]) {
-  asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(v[0]), "l"(v[1]), "l"(v[2]),
-               "l"(v[3]) : "memory");
+  asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
+  asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p + 4), "l"(v[2]), "l"(v[3]) : "memory");
 }
 
 __device__ __forceinline__ float round_tf32_f(float x) {
@@ -44,13 +51,13 @@ __device__ __forceinline__ float rcp_approx(float x) {
 }
 
 
-// The kernel is instruction-issue bound (ncu: issue ~50 %, DRAM ~10 % in the first
-// version), so the sampler is written for instruction count:
+// The kernel is instruction-issue bound rather than DRAM bound, so the sampler is written for
+// instruction count:
 //  * the 2x2 window is addressed as ONE base (clamped to [0,w-2]x[0,h-2]) plus
 //    compile-time offsets {0, C, w*C, w*C + C}; the zero-padding rule of
 //    grid_sample becomes a remap of the four weights at the image border,
 //  * reciprocals are MUFU.RCP (1 ulp) instead of the IEEE sequence,
-//  * the blend runs on packed FFMA2 with 256-bit texel loads.
+//  * the blend runs on fp32 pairs loaded as two 16-byte texel loads.
 struct Window {
   Tex8 t00, t01, t10, t11;
 };

@@ -116,8 +116,8 @@ regress_kernel(const float* __restrict__ logits, const float* __restrict__ dv, i
 
 // Plane-parallel variant (the default): the generic kernel above runs ~80 instructions per
 // hypothesis in ONE thread per pixel (precise expf, IEEE division, 64-bit addressing) -- at
-// 160x128 that is 640 warps with a 3 800-instruction dependent chain each (ncu: 6.6 % of the
-// warp slots, 36 us for 7.9 MB).  Here a block owns 32 pixels and NL = 8 warps split the D
+// 160x128 that is 640 warps with a 3 800-instruction dependent chain each, far too few to hide
+// the latency.  Here a block owns 32 pixels and NL = 8 warps split the D
 // planes: max, exp, the division and the two products are evaluated plane-parallel; only the
 // ORDERED sums (sequential denominator, cascade-16 depth / index) are walked by one warp, from
 // shared memory.  Every value and every summation order is the generic kernel's, so the two
@@ -270,7 +270,7 @@ static int regress_impl(const float* logits, const float* depth_values, int dv_i
   const size_t smem = ((size_t)3 * D * 32 + kK3Lanes * 32) * sizeof(float);
   if (D == 8 && par_path) {
     // 8 hypotheses fit a thread's registers and there are plenty of pixels at the finest level:
-    // one thread per pixel (14.9 us at 640x512 against 30.2 us plane-parallel, profiles/)
+    // one thread per pixel (about twice as fast as the plane-parallel kernel at 640x512)
     dim3 grd8((hw + kK3Threads - 1) / kK3Threads, B);
     if (input_is_prob)
       regress_kernel<true, 8><<<grd8, kK3Threads, 0, st>>>(logits, depth_values, dv_is_vector, hyp, depth,

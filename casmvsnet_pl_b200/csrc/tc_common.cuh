@@ -1,20 +1,23 @@
-// PTX wrappers shared by the tcgen05 convolution kernels (sm_100a only): mbarrier,
-// cp.async, tcgen05 alloc/fence/commit/mma/ld/st, UMMA descriptors.
+// PTX wrappers shared by the tensor-core convolution kernels (sm_90a): mbarrier, wgmma
+// (kind tf32, fp32 accumulators in registers) and its shared-memory matrix descriptors.
 #pragma once
 #include "common.cuh"
 
 namespace casmvs {
 namespace tc {
 
-constexpr int kTileW = 8, kTileH = 16;           // M = 128
+constexpr int kTileW = 8, kTileH = 16;           // M = 128 output voxels per tile
 constexpr int kHaloW = kTileW + 2, kHaloH = kTileH + 2;
-constexpr int kSlots = 4;
-// warps 0-3 epilogue (TMEM lane quadrants), kProducerWarps producer warps, last warp MMA issuer
-constexpr int kProducerWarps = 4;   // 8 was slower: 416 threads x 64-80 regs leave one CTA per SM
-constexpr int kProducerThreads = kProducerWarps * 32;
-constexpr int kMmaWarp = 4 + kProducerWarps;
-constexpr int kThreads = (kMmaWarp + 1) * 32;
+// Kernel layout shared by the TMA-fed conv kernels: two consumer warpgroups (warps 0-7; each
+// owns 64 of the tile's 128 GEMM rows, issues its wgmma and runs the epilogue from its
+// registers), then one TMA producer warp.
+constexpr int kConsumerThreads = 256;
+constexpr int kProdWarp = 8;
+constexpr int kConvThreads = kConsumerThreads + 32;
 
+// A value the compiler can prove equal across the warp (role selection: the wgmma of a
+// warpgroup must not sit on a path ptxas considers divergent)
+__device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -42,145 +45,101 @@ __device__ __forceinline__ void fence_barrier_init() {
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src),
-               "r"(src_bytes)
-               : "memory");
+
+// ---- wgmma ----
+// Register accumulators must be ordered before the next wgmma that reads them.
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void cp_async_commit() {
-  asm volatile("cp.async.commit_group;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+__device__ __forceinline__ void wgmma_wait_all() {
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar, uint32_t elected) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "setp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-      ::"r"(bar), "r"(elected)
-      : "memory");
-}
-// One lane of a converged warp (the MMA warp runs warp-uniform code so that the
-// descriptors stay in uniform registers; only the issue itself is predicated).
-__device__ __forceinline__ uint32_t elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred;
-}
-// D[tmem] += A[smem desc] * B[smem desc], tf32 operands, fp32 accumulate; issued by the
-// lane whose `elected` is non-zero
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi,
-                                          uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                          uint32_t elected) {
-  // descriptors travel as (lo,hi) words: only the low word (start address) changes per tap
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 q, %6, 0;\n\t"
-      "setp.ne.b32 p, %6, 0xffffffff;\n\t"          // always true: accumulate
-      "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(elected)
-      : "memory");
-}
-// shared-memory matrix descriptor, SWIZZLE_NONE, K-major (cute::UMMA::SmemDescriptor):
-// [0,14) start>>4 | [16,30) leading byte offset>>4 | [32,46) stride byte offset>>4 |
-// [46,48) version = 1 (Blackwell) | [61,64) layout type = 0 (no swizzle)
+// Shared-memory matrix descriptor, no swizzle, K-major: [0,14) start>>4 | [16,30) leading
+// byte offset>>4 (between the two 16-byte core-matrix columns of one K=8 step) | [32,46)
+// stride byte offset>>4 (between 8-row groups) | base offset 0 | [62,64) layout 0.  A core
+// matrix is 8 rows x 16 bytes stored as 128 contiguous bytes.
 __device__ __forceinline__ uint64_t make_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
   return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | (1ull << 46);
+         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) @4,
-// a/b format TF32 (2) @7/@10, a/b major K (0), N>>3 @17, M>>4 @24
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+// D[64 x N] += A[64 x 8] * B[N x 8]^T, tf32 operands from shared memory, fp32 accumulate.
+// d: the N/2 accumulator registers of this thread.  Issued by all 128 threads of a warpgroup.
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t a, uint64_t b);
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(1));
 }
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<48>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<96>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<192>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95}, %96, %97, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(a), "l"(b), "r"(1));
+}
+
+
+// Fragment layout of an m64nN accumulator: register 4j + 2h + e of lane l in warp w of the
+// warpgroup holds row 16w + l/4 + 8h and column 8j + 2(l%4) + e.  f(row, col, v0, v1) is
+// called once per pair of adjacent columns [OFF, OFF + NCOL) of the fragment, with col
+// relative to OFF.
+template <int OFF, int NCOL, typename F>
+__device__ __forceinline__ void for_each_pair(const float* acc, int warp_in_wg, int lane, F&& f) {
+  static_assert(OFF % 8 == 0 && NCOL % 8 == 0, "column groups of 8");
+#pragma unroll
+  for (int j = 0; j < NCOL / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int i = (OFF / 2) + 4 * j + 2 * h;
+      f(16 * warp_in_wg + (lane >> 2) + 8 * h, 8 * j + 2 * (lane & 3), acc[i], acc[i + 1]);
+    }
+  }
+}
+
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
-}
-
-template <int NPAD>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, float (&v)[NPAD]) {
-  static_assert(NPAD == 16 || NPAD == 32, "NPAD");
-  uint32_t r[NPAD];
-  if constexpr (NPAD == 16) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-          "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-          "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-  } else {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-          "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-          "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-          "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-          "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-  }
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < NPAD; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// zero 16 consecutive fp32 columns of this warp's 32 TMEM lanes
-__device__ __forceinline__ void tmem_zero16(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1};" ::"r"(taddr), "r"(z)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-
-// Cooperative smem fill of the pre-built B operand image (global, 16 B aligned, bytes % 16 == 0)
-__device__ __forceinline__ void load_image_async(uint32_t dst_smem, const float* src, int bytes) {
-  for (int i = threadIdx.x * 16; i < bytes; i += blockDim.x * 16)
-    cp_async16(dst_smem + i, reinterpret_cast<const char*>(src) + i, 16u);
-  cp_async_commit();
-  cp_async_wait<0>();
-}
-// barrier init spread over the first threads of the CTA (one mbarrier each)
-__device__ __forceinline__ void init_barriers(uint32_t bar_full, uint32_t bar_empty,
-                                              uint32_t bar_tfull, int slots) {
-  const int t = threadIdx.x;
-  if (t < slots) mbar_init(bar_full + 8 * t, kProducerThreads);
-  else if (t < 2 * slots) mbar_init(bar_empty + 8 * (t - slots), 1);
-  else if (t < 2 * slots + 32) mbar_init(bar_tfull + 8 * (t - 2 * slots), 1);
-  if (t < 2 * slots + 32) fence_barrier_init();
 }
 
 // Persistent cache of built B-operand images keyed by (packed-weight pointer, kernel tag,

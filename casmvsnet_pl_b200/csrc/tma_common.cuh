@@ -1,4 +1,4 @@
-// TMA helpers shared by the TMA-fed tcgen05 convolution kernels (sm_100a only).
+// TMA helpers shared by the TMA-fed tensor-core convolution kernels (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -40,8 +40,8 @@ __device__ __forceinline__ void load_image_bulk(uint32_t dst_smem, const float* 
 
 // Programmatic dependent launch: the kernels are launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, so a CTA may start while the previous
-// kernel of the stream is still draining.  Everything before pdl_wait() -- barrier init, TMEM
-// allocation, the weight-image bulk copy, parameter loads: nothing that depends on the previous
+// kernel of the stream is still draining.  Everything before pdl_wait() -- barrier init,
+// the weight-image bulk copy, parameter loads: nothing that depends on the previous
 // kernel's output -- overlaps that tail; pdl_wait() returns once the previous grid has completed
 // and its writes are visible.  pdl_trigger() lets the next kernel of the stream do the same.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -73,7 +73,8 @@ inline cudaError_t launch_pdl(bool allow, Kernel kfn, dim3 grid, int threads, si
 }
 
 // Tiled tensor map over the activation tensor x (B,D,H,W,C) viewed as {C, W, H, D, B} with box
-// {CB, box_w, box_h, 1, 1}, swizzle = CB*4 bytes (128/64/32), out-of-bounds elements zero-filled
+// {CB, box_w, box_h, 1, 1}, swizzle = CB*4 bytes (128/64/32; none for the 16-byte boxes of the
+// conv kernels), out-of-bounds elements zero-filled
 // (= the convolution's zero padding).  stride_w = 2: the box walks every second voxel along W
 // (box_w counts traversed positions, so ceil(box_w / 2) voxels are loaded): the even / odd
 // column planes of the stride-2 convolutions.  Memoised by (pointer, shape, box); null +
@@ -97,6 +98,14 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 }
 
 inline int pow2_floor(int v) { int r = 1; while (r * 2 <= v) r *= 2; return r; }
+
+// Resident CTAs per SM of a persistent kernel (registers and shared memory), at least 1.
+template <typename K>
+inline int resident_per_sm(K kfn, int threads, int smem) {
+  int n = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kfn, threads, smem) != cudaSuccess) n = 1;
+  return n < 1 ? 1 : n;
+}
 
 // Depth-chunk length for the persistent kernels.  An item (tile column x depth chunk of dc
 // output groups) costs mul*dc + add input slices (+ `fixed` for pipeline fill / drain); CTA k

@@ -191,7 +191,7 @@ warp_cost_kernel(const float* __restrict__ feats,   // (B,V,h,w,C)
         o[k] = fma2(mn, m, mul2(Q[k], inv_v2));
       }
       if (round_tf32) {
-        // the tcgen05 conv reads fp32 bits as tf32 by truncation; rounding here keeps the
+        // the tensor-core conv reads fp32 bits as tf32 by truncation; rounding here keeps the
         // next layer's operand unbiased (round-to-nearest instead of toward zero)
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -267,11 +267,10 @@ warp_cost_kernel(const float* __restrict__ feats,   // (B,V,h,w,C)
 
 // ---------------------------------------------------------------------------------------
 // Specialised hot variant: variance cost, channels-last output, compile-time C and V-1.
-// Bound analysis (profiles/r1_k1_bound_experiment.txt): with the stores AND the tap loads
-// removed the kernel still takes 76 % of its time, i.e. it is instruction/FP32-pipe bound:
+// Bound analysis: the kernel is close to instruction / FP32-pipe bound as well as HBM bound:
 // 17 fp32 ops per output channel (2 views x (4 blend + 2 accumulate) + 4 variance + 1) plus
-// ~6 of per-pixel coordinate math amortised over 8 channels put the FP32-pipe floor (~23 us
-// at level 2) right next to the HBM floor (21 us).  More warps (CPT=4) or fewer L1 requests
+// ~6 of per-pixel coordinate math amortised over 8 channels put the FP32-pipe floor next to
+// the HBM floor.  More warps (CPT=4) or fewer L1 requests
 // (SKIP) do not help; both options are kept for experiments (CASMVS_K1_CPT / CASMVS_K1_SKIP).
 // CPT channels per thread (4 or 8): 4 halves the register footprint (more resident warps to
 // hide the L1/L2 latency that bounds this kernel) at the price of more redundant coordinate
@@ -282,8 +281,8 @@ template <int CPT>
 __device__ __forceinline__ TexN<CPT> ldg_tex(const float* p) {
   TexN<CPT> t;
   if constexpr (CPT == 8) {
-    asm volatile("ld.global.nc.v4.b64 {%0,%1,%2,%3}, [%4];"
-                 : "=l"(t.v[0]), "=l"(t.v[1]), "=l"(t.v[2]), "=l"(t.v[3]) : "l"(p));
+    asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[0]), "=l"(t.v[1]) : "l"(p));
+    asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[2]), "=l"(t.v[3]) : "l"(p + 4));
   } else {
     asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[0]), "=l"(t.v[1]) : "l"(p));
   }
@@ -292,8 +291,8 @@ __device__ __forceinline__ TexN<CPT> ldg_tex(const float* p) {
 template <int CPT>
 __device__ __forceinline__ void stg_tex(float* p, const u64 (&v)[CPT / 2]) {
   if constexpr (CPT == 8) {
-    asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(v[0]), "l"(v[1]), "l"(v[2]),
-                 "l"(v[3]) : "memory");
+    asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
+    asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p + 4), "l"(v[2]), "l"(v[3]) : "memory");
   } else {
     asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
   }
@@ -413,9 +412,8 @@ warp_var_kernel(const float* __restrict__ feats, const float* __restrict__ proj,
 template <int NSRC, int CT>
 static bool launch_var(cudaStream_t st, const float* f, const float* p, const float* dv,
                        float* cost, int B, int D, int h, int w, int dchunk, int rnd) {
-  // 8 channels per thread, no window skip, 6 resident blocks per SM (80 registers): the best of
-  // the round-1 sweep (profiles/r1_k1_ab_0*.jsonl: 4 channels per thread, window skip and the
-  // 4 / 5 / 8-block register budgets all measured slower and were removed)
+  // 8 channels per thread, no window skip, 6 resident blocks per SM (80 registers): 4 channels
+  // per thread, window skip and 4 / 5 / 8-block register budgets were slower and were removed
   const long threads = (long)h * w * (CT / 8);
   dim3 grd((unsigned)((threads + kK1Threads - 1) / kK1Threads), (unsigned)B,
            (unsigned)((D + dchunk - 1) / dchunk));
@@ -573,7 +571,7 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   const bool nhwc = cost_layout == CASMVS_NHWC;
   const long threads = (long)h * w * (C / kCPT);
   const unsigned xblocks = (unsigned)((threads + kK1Threads - 1) / kK1Threads);
-  // depth chunks: enough CTAs to fill 148 SMs several times over, but chunks long
+  // depth chunks: enough CTAs to fill every SM several times over, but chunks long
   // enough (>= 8 planes) for the texel-window cache to pay off
   static bool env_read = false;
   if (!env_read) {

@@ -6,8 +6,8 @@
 //   variance accumulation          models/mvsnet.py:137-141,147-156,166-168
 //
 // Why: the gather-from-L1 kernel (warp_cost.cu) fetches 4 taps x (V-1) views per output
-// through the L1 tag stage and leaves every L1 miss to the 300+-cycle L2 round trip
-// (profiles/r1_k1_v3.summary.txt: l1tex 66 %, long-scoreboard stalls, DRAM 17-24 %).  Here a
+// through the L1 tag stage and leaves every L1 miss to the several-hundred-cycle L2 round
+// trip, so it stalls on long-scoreboard waits well below the HBM bound.  Here a
 // CTA owns a TW x TH tile of reference pixels x a run of depth planes:
 //   1. every thread evaluates its sample position in each source view at the first and last
 //      plane of the run (positions are monotonic along the epipolar line in 1/depth), a block
@@ -24,7 +24,7 @@
 //      tile, exotic geometry) takes the robust gather path for that sample only; if the
 //      footprint of the whole run does not fit, the CTA halves the run and stages again.
 // The warped (B,V-1,C,D,h,w) volumes never exist; features are read from L2 once per
-// (tile, run), hypotheses once, the cost volume is written once with 256-bit stores.
+// (tile, run), hypotheses once, the cost volume is written once, 32 bytes per thread as two 16-byte stores.
 #include <limits.h>
 #include <stdlib.h>
 
@@ -339,10 +339,9 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
 }
 
 // ---- plane-group variant: window reuse WITHOUT persistent registers -----------------------------
-// ncu on the kernel above (profiles/r2_k1_variants.txt): the LSU data pipe sits at 62-74 % of its
-// peak (the gather kernel: 66-72 %) -- both generations are bound by the 32 B of tap traffic per
-// output float, not by latency.  Keeping the 2x2 windows of both views in registers across
-// planes (REUSE) cuts the shared-memory wavefronts by 38 % but needs 166 registers (or spills,
+// Both K1 generations are bound by the LSU data pipe (32 B of tap traffic per output float),
+// not by latency.  Keeping the 2x2 windows of both views in registers across planes (REUSE)
+// cuts the shared-memory wavefronts but needs far more registers (or spills,
 // whose local-memory traffic goes through the same LSU pipe).  Here a thread walks PG planes
 // of ONE view before turning to the next view: the window lives only inside that short walk
 // (32 registers, re-loaded only when it moves: ~0.43 texel per plane in the cascade), and what
@@ -663,9 +662,8 @@ int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* c
   if (!enabled) return 1;
   if ((reinterpret_cast<uintptr_t>(feats) & 15) != 0 || B > 65535) return 1;
   using namespace k1s;
-  // Measured (profiles/r2_k1_variants.txt): with 4 / 6 source views the staged boxes leave one
-  // CTA per SM and the gather kernels of warp_cost.cu are 1.2x / 1.9x faster (cfg4 / cfg5
-  // shapes), so those shapes are left to them unless CASMVS_K1S_MANYVIEWS=1.
+  // With 4 / 6 source views the staged boxes leave one CTA per SM, so those shapes (cfg4 / cfg5)
+  // are left to the gather kernels of warp_cost.cu unless CASMVS_K1S_MANYVIEWS=1.
   static const int many = env_int("CASMVS_K1S_MANYVIEWS", 0);
   if (V - 1 > 2 && !many) return 1;
   if (num_groups != 1) {
@@ -679,14 +677,14 @@ int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* c
 #undef K1G
     return 1;
   }
-  // Variants (CASMVS_K1S_VARIANT), measured on cfg2 -- profiles/r2_k1_variants.txt:
+  // Variants (CASMVS_K1S_VARIANT):
   //   16 (default) plane groups of 2: a view's window is re-used across the planes of a group
   //   11           plane groups of 4
   //    4           no window reuse (every plane loads its 2x2 windows)
-  // Also measured and removed again: windows of both views kept in registers across ALL planes
-  // (166 registers or spills through the same LSU pipe: 1.2-1.6x slower), coordinate math
-  // shared between the threads of a pixel by warp shuffles (1.2x slower: shuffles use the
-  // bound pipe), 16 channels per thread (1.04x slower: 163 registers, 12 warps per SM).
+  // Tried and removed: windows of both views kept in registers across ALL planes (register
+  // pressure or spills through the same LSU pipe), coordinate math shared between the threads
+  // of a pixel by warp shuffles (shuffles use the bound pipe), 16 channels per thread (register
+  // pressure).
   static const int variant = env_int("CASMVS_K1S_VARIANT", 16);
 #define K1S(VAR, NS, CC, TW_, TH_, MB) \
   if (variant == VAR && V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, st);

@@ -1,4 +1,4 @@
-// Tensor-core operand ("weight image") cache shared by the tcgen05 convolution kernels, and the
+// Tensor-core operand ("weight image") cache shared by the tensor-core convolution kernels, and the
 // image builder of the stride-1 kernel (conv3d_tma.cu).
 //
 // The kernels read their B operand from a UMMA-ready image built once per layer from the

@@ -1,4 +1,4 @@
-"""The reference's eval.py end to end on the B200 engine (SURVEY.md 8 f-3 / f-4 callers):
+"""The reference's eval.py end to end on the H100 engine (SURVEY.md 8 f-3 / f-4 callers):
 
     step 1 (eval.py:198-243)  depth + confidence for every reference view of a scan
     step 2 (eval.py:245-353)  geometric filter, refinement, fusion, PLY

@@ -1,4 +1,4 @@
-"""Operator surface of the reference's ``models/modules.py`` on the B200 engine.
+"""Operator surface of the reference's ``models/modules.py`` on the H100 engine.
 
 Same names, argument meaning and shapes as the reference (SURVEY.md §8b); the
 bodies call the hand-written CUDA kernels through the C ABI (../ops.py).

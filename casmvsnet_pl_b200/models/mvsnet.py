@@ -1,6 +1,6 @@
 """``CascadeMVSNet`` with the reference's constructor, attributes, state-dict
 keys and forward contract (reference models/mvsnet.py:107-244), running the
-three-stage hot path on the B200 kernels.
+three-stage hot path on the H100 kernels.
 
 Host side (this file) is glue: it owns the parameters, runs the 2D FeatureNet
 with PyTorch/cuDNN in channels-last (so the fused warp kernel gets HWC features
@@ -18,7 +18,7 @@ from .modules import ConvBnReLU, ConvBnReLU3D, InPlaceABN
 
 class FeatureNet(nn.Module):
     """3-level FPN (reference models/mvsnet.py:7-57).  Inference on the GPU runs entirely on this
-    library's kernels in both precision modes (tf32: tcgen05 planar / 5x5 convs; fp32: CUDA-core
+    library's kernels in both precision modes (tf32: wgmma planar / 5x5 convs; fp32: CUDA-core
     FMA kernels); PyTorch modules are only the parameter holders and the training / CPU path."""
 
     def __init__(self, norm_act=InPlaceABN):
@@ -41,10 +41,10 @@ class FeatureNet(nn.Module):
     def _up2(x):
         return F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True)
 
-    # cuDNN would run fp32 convs as TF32 on B200 by default; the reference path is fp32
+    # cuDNN would run fp32 convs as TF32 on H100 by default; the reference path is fp32
     # (opt.py:69-70), so IEEE fp32 is kept unless the model runs in its tf32 precision mode.
     allow_tf32 = False
-    # tf32 precision mode, inference: the 3x3 stride-1 and 5x5 stride-2 convs run on tcgen05 as
+    # tf32 precision mode, inference: the 3x3 stride-1 and 5x5 stride-2 convs run on wgmma as
     # planar convolutions over the (views, H, W) volume, the first block and the top-down
     # merges in this library's own kernels: no cuDNN kernel is left on this path
     tensor_path = True
@@ -370,7 +370,7 @@ class CascadeMVSNet(nn.Module):
         self.set_precision(precision)
 
     def set_precision(self, precision):
-        """'fp32' (CUDA-core FMA, bit-faithful products) or 'tf32' (tcgen05) for the convs."""
+        """'fp32' (CUDA-core FMA, bit-faithful products) or 'tf32' (wgmma) for the convs."""
         if precision not in ops.PRECISIONS:
             raise ValueError(f"precision must be one of {list(ops.PRECISIONS)}")
         self.precision = precision
@@ -478,7 +478,7 @@ class CascadeMVSNet(nn.Module):
         B, V, _, H, W = imgs.shape
         if not imgs.is_cuda:
             raise ops._lib.CasMVSError(
-                "CascadeMVSNet (B200 engine) needs CUDA inputs; there is no CPU fallback")
+                "CascadeMVSNet (H100 engine) needs CUDA inputs; there is no CPU fallback")
         differentiable = torch.is_grad_enabled() and (
             imgs.requires_grad or any(p.requires_grad for p in self.parameters()))
         # (B,1) depth parameters may arrive as CPU tensors from the reference's data loader

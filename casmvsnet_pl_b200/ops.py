@@ -54,7 +54,7 @@ def _require_cuda(*tensors):
             continue
         if not t.is_cuda:
             raise _lib.CasMVSError(
-                "casmvsnet_pl_b200 ops need CUDA tensors on a B200 (no CPU fallback); "
+                "casmvsnet_pl_b200 ops need CUDA tensors on a H100 (no CPU fallback); "
                 f"got a tensor on {t.device}")
         if t.dtype != torch.float32:
             raise _lib.CasMVSError(f"fp32 only (reference opt.py:69-70), got {t.dtype}")
@@ -75,7 +75,7 @@ def _require_cuda(*tensors):
 def _no_grad_only(*tensors):
     if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
         raise _lib.CasMVSError(
-            "the B200 engine is forward-only this round (SURVEY.md §8f-1): call it under "
+            "the H100 engine is forward-only this round (SURVEY.md §8f-1): call it under "
             "torch.no_grad() or with tensors that do not require grad")
 
 
@@ -501,7 +501,7 @@ def pack_conv2d_5x5s2_weight(weight):
 
 @_on_tensor_device
 def conv2d_5x5s2(x, w, shift, slope, round_tf32=False):
-    """5x5 stride-2 pad-2 Conv2d + shift + LeakyReLU on tcgen05 (FeatureNet conv1.0 / conv2.0
+    """5x5 stride-2 pad-2 Conv2d + shift + LeakyReLU on wgmma (FeatureNet conv1.0 / conv2.0
     with folded ABN).  x (N,Cin,H,W) channels-last, w (Cout,Cin,5,5) from
     pack_conv2d_5x5s2_weight -> (N,Cout,H/2,W/2)."""
     _require_cuda(x, w, shift)

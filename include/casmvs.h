@@ -1,5 +1,5 @@
 /*
- * casmvs.h — C ABI of libcasmvs.so, the B200 (sm_100a) cascade-MVS depth engine.
+ * casmvs.h — C ABI of libcasmvs.so, the H100 (sm_90a) cascade-MVS depth engine.
  *
  * The reference (kwea123/CasMVSNet_pl) has NO FFI layer: its boundary for the
  * hot path is the Python surface models/mvsnet.py + models/modules.py
@@ -18,8 +18,8 @@
  *    the call returns without synchronising (CUDA-graph capturable).
  *  - fp32 everywhere (the reference declares AMP unsupported, opt.py:69-70);
  *    depth_index is int64 like torch's .long().
- *  - there is no CPU fallback: casmvs_device_check() fails on anything below
- *    compute capability 10.0.
+ *  - there is no CPU fallback: casmvs_device_check() fails on anything other than
+ *    compute capability 9.0 (sm_90a).
  *
  * Memory layouts (enum casmvs_layout)
  *   CASMVS_NCHW : channels-first, the reference's public layout
@@ -41,14 +41,14 @@ extern "C" {
 
 enum casmvs_layout { CASMVS_NCHW = 0, CASMVS_NHWC = 1 };
 /* OR-ed into casmvs_warp_cost_fwd's cost_layout: store the cost volume rounded to
- * TF32 (round-to-nearest) because the consumer is the tcgen05 kind::tf32 conv, which
+ * TF32 (round-to-nearest) because the consumer is the wgmma tf32 conv, which
  * would otherwise truncate the operand (biased). */
 #define CASMVS_ROUND_TF32 256
 
 /* precision of the 3D-conv contraction (K2) */
 enum casmvs_precision {
   CASMVS_FP32 = 0,  /* CUDA-core fp32 FMA (bit-faithful products)            */
-  CASMVS_TF32 = 1   /* tcgen05 kind::tf32, fp32 accumulate in TMEM           */
+  CASMVS_TF32 = 1   /* wgmma tf32, fp32 accumulate in registers         */
 };
 
 /* OR-ed into casmvs_conv3d_fwd's precision: store the output unrounded even in the TF32
@@ -71,11 +71,11 @@ enum casmvs_conv_kind {
 /* ---- library / device ------------------------------------------------- */
 int casmvs_version(void);
 const char* casmvs_last_error(void);
-/* 0 iff `device` exists and has compute capability >= 10.0 (no fallback). */
+/* 0 iff `device` exists and has compute capability 9.0 (no fallback). */
 int casmvs_device_check(int device);
 /* number of kernels this library has launched since load (bench evidence). */
 uint64_t casmvs_launch_count(void);
-/* number of CASMVS_TF32 layers that no tcgen05 kernel covered and that therefore ran on the
+/* number of CASMVS_TF32 layers that no wgmma kernel covered and that therefore ran on the
  * CUDA-core kernel (same results up to TF32 rounding, several times slower).  0 for the
  * reference architecture at every BASELINE configuration; bench.py and the full-size tests
  * assert that. */
@@ -229,7 +229,7 @@ int casmvs_fpn_level_fwd(const float* prev, const float* c, const float* lat_w,
 /* The same level split in two for the tensor-core path: this call produces
  *   feat = upsample_x2_bilinear(prev, align_corners=True) + conv1x1(c, lat_w) + lat_b
  * (N,h,w,32), optionally TF32-rounded, and the 3x3 smooth runs as a CASMVS_CONV_PLANAR
- * casmvs_conv3d_fwd on tcgen05.  prev == NULL: feat = conv1x1(c) + lat_b (the `toplayer`,
+ * casmvs_conv3d_fwd on wgmma.  prev == NULL: feat = conv1x1(c) + lat_b (the `toplayer`,
  * mvsnet.py:27,41).  lat_w (32,CLAT[,1,1]) torch layout; CLAT % 4 == 0. */
 int casmvs_fpn_merge_fwd(const float* prev, const float* c, const float* lat_w,
                          const float* lat_b, float* feat, int N, int h, int w, int CLAT,
@@ -243,7 +243,7 @@ int casmvs_conv2d_rgb8_fwd(const float* x, const float* w, const float* bias, fl
                            float* y, int N, int H, int W, int round_tf32, void* stream);
 
 /* The 5x5 stride-2 blocks of FeatureNet (ConvBnReLU(8,16,5,2,2) / (16,32,5,2,2), mvsnet.py:16,20
- * + modules.py:8-18) with the eval-mode ABN folded, on tcgen05 (TF32 operands):
+ * + modules.py:8-18) with the eval-mode ABN folded, on wgmma (TF32 operands):
  *   y = LeakyReLU(conv5x5_s2_p2(x, w) + shift)
  * x (N,H,W,Cin) channels-last, w (Cout,Cin,5,5) torch layout already multiplied by the ABN
  * scale, y (N,(H-1)/2+1,(W-1)/2+1,Cout) channels-last, optionally stored TF32-rounded.  The

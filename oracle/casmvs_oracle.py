@@ -3,11 +3,10 @@
 A plain-PyTorch (CPU, fp32) restatement of the reference algorithm for the path
 SURVEY.md §8(a) lists, written as state-dict-driven *functions* (the reference
 is nn.Module code).  Each function cites the reference file:line it follows
-(paths relative to /root/reference).  It uses the same torch primitives in the
-same order as the reference, so on CPU it is bit-identical to the reference
-run in this container; that is pinned by ``tests/golden/*.npz`` (generated from
-the REAL reference by ``oracle/make_golden.py``) and by
-``tests/test_oracle_vs_reference.py`` when /root/reference is present.
+(paths relative to the reference repository).  It uses the same torch primitives
+in the same order as the reference, so on CPU it is bit-identical to the
+reference; that is pinned by ``tests/golden/*.npz`` (generated from the REAL
+reference by ``oracle/make_golden.py`` and ``oracle/make_golden_live.py``).
 
 Parity status: the reference ships no tests / golden vectors of its own
 ("parity unpinned" by the reference, SURVEY.md §8c); the pins above are outputs

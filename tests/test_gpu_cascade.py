@@ -224,7 +224,7 @@ def test_feature_net_channels_last_matches_oracle():
 
 
 def test_feature_net_tensor_path_matches_fp32_path():
-    """tf32 mode: 3x3 convs as planar tcgen05 convolutions + own first block / merges, against
+    """tf32 mode: 3x3 convs as planar wgmma convolutions + own first block / merges, against
     the fp32 cuDNN path of the same model (10-bit operand mantissas through 8 conv layers)."""
     model, sd = build(1, "tf32")
     x = torch.randn(3, 3, 128, 160)

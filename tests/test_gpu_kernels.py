@@ -463,7 +463,7 @@ def test_conv2d_rgb8_vs_torch_cpu(hw):
                                          (32, 16, (33, 47)), (32, 8, (64, 90))])
 def test_planar_conv_tensor_core_vs_torch_cpu(cin, cout, hw):
     """The 3x3 Conv2d layers of FeatureNet as a CONV_PLANAR (1x3x3) convolution over the
-    (views, H, W) volume on tcgen05, against torch fp32 on the CPU; and the CUDA-core kernel
+    (views, H, W) volume on wgmma, against torch fp32 on the CPU; and the CUDA-core kernel
     running the same packed weights (zero outer planes) in fp32."""
     import torch.nn.functional as F
     g = torch.Generator().manual_seed(cin + cout)
@@ -487,7 +487,7 @@ def test_planar_conv_tensor_core_vs_torch_cpu(cin, cout, hw):
 
 @pytest.mark.parametrize("cin,cout,hw", [(8, 16, (64, 96)), (16, 32, (36, 50)), (8, 16, (18, 34))])
 def test_conv2d_5x5s2_tensor_core_vs_torch_cpu(cin, cout, hw):
-    """FeatureNet's 5x5 stride-2 blocks on tcgen05 (even/odd TMA planes, 25 taps) vs torch fp32."""
+    """FeatureNet's 5x5 stride-2 blocks on wgmma (even/odd TMA planes, 25 taps) vs torch fp32."""
     import torch.nn.functional as F
     g = torch.Generator().manual_seed(cin * 7 + cout)
     x = torch.randn(3, cin, *hw, generator=g)
@@ -502,7 +502,7 @@ def test_conv2d_5x5s2_tensor_core_vs_torch_cpu(cin, cout, hw):
     assert err.max() < 1.5e-3 * want.abs().max().item()
 
 
-# ----------------------------------------------------------------------------- K2 on tcgen05
+# ----------------------------------------------------------------------------- K2 on wgmma
 @pytest.mark.parametrize("kind,cin,cout,dims", [
     ("conv1", 8, 8, (5, 20, 13)), ("conv1", 16, 8, (16, 40, 24)), ("conv1", 32, 8, (8, 32, 40)),
     ("conv1", 16, 16, (6, 32, 24)), ("conv1", 32, 32, (4, 16, 16)), ("conv1", 8, 1, (8, 32, 16)),
@@ -510,7 +510,7 @@ def test_conv2d_5x5s2_tensor_core_vs_torch_cpu(cin, cout, hw):
     ("conv2", 8, 16, (8, 32, 40)), ("conv2", 16, 32, (6, 20, 24)), ("conv2", 32, 64, (4, 16, 16)),
     ("convT", 16, 8, (5, 18, 11)), ("convT", 32, 16, (3, 16, 16)), ("convT", 64, 32, (2, 16, 24))])
 def test_tensor_core_conv_vs_cuda_core_fp32(kind, cin, cout, dims):
-    """Every CostRegNet layer type on the tcgen05 path (tf32 operands, fp32 accumulate) against
+    """Every CostRegNet layer type on the wgmma path (tf32 operands, fp32 accumulate) against
     the fp32 CUDA-core kernel on the same inputs (ragged tiles, halos, skip, ABN epilogue).
     Operands carry 10 mantissa bits => relative error ~2^-11 per product, K = 27*Cin terms."""
     g = torch.Generator().manual_seed(cin * 131 + cout)

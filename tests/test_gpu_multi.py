@@ -1,4 +1,4 @@
-"""Multi-GPU (>= 2 B200s on one box): view-sharded inference through the real engine
+"""Multi-GPU (>= 2 H100s on one box): view-sharded inference through the real engine
 with the single NCCL all_gather equals the single-GPU result bit for bit."""
 import os
 import socket

@@ -1,42 +1,31 @@
-"""Live cross-check of the oracle against the REAL reference on fresh random
-inputs (beyond the committed goldens).  Skipped where /root/reference is absent
-(e.g. the GPU box)."""
+"""Cross-check of the oracle against what the REAL reference computed on seeded random
+inputs beyond the cascade goldens (tests/golden/reference_live.npz, recorded by
+oracle/make_golden_live.py).  CPU only, bit-exact like tests/test_oracle_golden.py."""
 import pytest
 import torch
 
 from oracle import casmvs_oracle as O
-from oracle import ref_loader
-
-pytestmark = pytest.mark.skipif(not ref_loader.reference_available(),
-                                reason="/root/reference absent")
+from oracle.live_inputs import feature_input, predict_depth_inputs
 
 
 @pytest.mark.parametrize("G", [1, 4])
-def test_predict_depth_matches_reference(G):
-    from casmvsnet_pl_b200 import synth
+def test_predict_depth_matches_reference(golden, G):
     from oracle.make_golden import seeded_state_dict
+    g = golden("reference_live")
     sd = seeded_state_dict((8, 32, 48), (1, 2, 4), G, seed=5)
-    ref = ref_loader.make_reference_model((8, 32, 48), (1, 2, 4), G)
-    ref.load_state_dict(sd)
-    g = torch.Generator().manual_seed(9)
-    feats = torch.randn(2, 4, 16, 16, 24, generator=g)
-    pms = synth.projection_matrices(4, W=96, H=64, stress=True, behind_view=3)[:, 1]
-    pms = pms.unsqueeze(0).expand(2, -1, -1, -1).contiguous()
-    dv = 430.0 + 5.3 * torch.arange(16).float().reshape(1, 16, 1, 1) + torch.rand(2, 16, 16, 24, generator=g)
+    feats, pms, dv = predict_depth_inputs()
     with torch.no_grad():
-        d_ref, c_ref = ref.predict_depth(feats, pms, dv, ref.cost_reg_1)
         d_o, c_o = O.predict_depth(feats, pms, dv, sd, "cost_reg_1.", G)
-    assert torch.equal(d_ref, d_o) and torch.equal(c_ref, c_o)
+    assert torch.equal(g[f"depth_g{G}"], d_o) and torch.equal(g[f"confidence_g{G}"], c_o)
 
 
-def test_feature_pyramid_matches_reference():
+def test_feature_pyramid_matches_reference(golden):
     from oracle.make_golden import seeded_state_dict
+    g = golden("reference_live")
     sd = seeded_state_dict((8, 32, 48), (1, 2, 4), 1, seed=2)
-    ref = ref_loader.make_reference_model((8, 32, 48), (1, 2, 4), 1)
-    ref.load_state_dict(sd)
-    x = torch.randn(2, 3, 64, 96)
     with torch.no_grad():
-        a = ref.feature(x)
-        b = O.feature_pyramid(x, sd)
-    for k in a:
-        assert torch.equal(a[k], b[k])
+        b = O.feature_pyramid(feature_input(), sd)
+    keys = [k[len("feature."):] for k in g if k.startswith("feature.")]
+    assert sorted(keys) == sorted(b)
+    for k in keys:
+        assert torch.equal(g["feature." + k], b[k])
