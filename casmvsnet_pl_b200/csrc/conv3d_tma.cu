@@ -21,7 +21,9 @@
 // TMA producer warp.  Ring full barriers are armed with expect_tx and completed by the TMA
 // unit; ring empty barriers by the 256 consumer threads once their wgmma have retired.  The
 // accumulator of one input slice covers output slices it-2, it-1, it (column groups 0, 1, 2);
-// after the slice, group 0 is complete and goes through the epilogue, and the window rolls.
+// after the slice, group 0 is complete: it is copied out, the window rolls, the next slice's
+// wgmma are issued and group 0's epilogue runs while they execute.  N = 3 x GW with GW = 8 for
+// Cout <= 8 (conv0, prob, FeatureNet's last smoothing layer), else 16 or 32.
 #include <cudaTypedefs.h>
 #include <stdlib.h>
 
@@ -139,6 +141,16 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   tma::pdl_wait();
   bool w_ready = false;                             // consumers: weight image has landed
   uint32_t gs = 0;                                  // slices processed before this item (all roles)
+  // consumers: the accumulator, column groups 0, 1, 2 = output slices it-2, it-1, it (planar:
+  // one group, output slice it); and the completed output slice whose epilogue is pending
+  // (od < 0: none).  Both carry over into the CTA's next item.
+  float acc[(PLANAR ? 1 : 3) * GW / 2];
+#pragma unroll
+  for (int i = 0; i < (PLANAR ? 1 : 3) * GW / 2; ++i) acc[i] = 0.f;
+  float done[GW / 2];
+  int pend_od = -1, pend_b = 0, pend_h0 = 0, pend_w0 = 0;
+  const int wg = warp >> 2, wl = warp & 3;
+  const int row0 = 64 * wg;                         // consumers: first GEMM row of the warpgroup
   for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x) {
     int item = item0;
     const int tw = item % p.tiles_w; item /= p.tiles_w;
@@ -168,72 +180,64 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
       }
       __syncwarp();
     } else {
-      // ============ consumer warpgroups: wgmma into registers, then the epilogue ============
-      const int wg = warp >> 2, wl = warp & 3;
-      const int row0 = 64 * wg;                      // first GEMM row of this warpgroup
+      // == consumer warpgroups: wgmma into registers; the previous output slice's epilogue ==
+      // == runs while they execute                                                        ==
       constexpr uint32_t a_lbo = S::kBrickBytes, a_sbo = kHaloW * 16;   // 8-voxel group stride
       constexpr uint32_t b_lbo = 3 * GW * 16, b_sbo = 128;
       const uint64_t a_desc0 = make_desc(s_ring + 8 * wg * a_sbo, a_lbo, a_sbo);
       const uint64_t b_desc0 = make_desc(s_w, b_lbo, b_sbo);
-      float acc[3 * GW / 2];
-#pragma unroll
-      for (int i = 0; i < 3 * GW / 2; ++i) acc[i] = 0.f;
       for (int it = 0; it < nslices; ++it) {
         const uint32_t g = gs + it;
         mbar_wait(bar_full + 8 * (g % SLOTS), (g / SLOTS) & 1);
         if (!w_ready) { mbar_wait(bar_w, 0); w_ready = true; }
         const uint64_t a_s = a_desc0 + (((g % SLOTS) * S::kSlotBytes) >> 4);
-        if constexpr (PLANAR) {
-          // kd = 1 only: B column group 1, one output slice per input slice
+        wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < GW / 2; ++i) acc[i] = 0.f;
-          wgmma_fence();
+        for (int khw = 0; khw < 9; ++khw) {
+          const int kh = khw / 3, kw = khw % 3;
 #pragma unroll
-          for (int khw = 0; khw < 9; ++khw) {
-            const int kh = khw / 3, kw = khw % 3;
-#pragma unroll
-            for (int k8 = 0; k8 < CIN / 8; ++k8) {
-              const uint32_t a_off = ((kh * kHaloW + kw) * 16 + 2 * k8 * S::kBrickBytes) >> 4;
-              const uint32_t b_off = (khw * (CIN * 3 * GW * 4) + k8 * 2 * 3 * GW * 16 + GW * 16) >> 4;
-              wgmma_tf32<GW>(acc, a_s + a_off, b_desc0 + b_off);
-            }
-          }
-        } else {
-          wgmma_fence();
-#pragma unroll
-          for (int khw = 0; khw < 9; ++khw) {
-            const int kh = khw / 3, kw = khw % 3;
-#pragma unroll
-            for (int k8 = 0; k8 < CIN / 8; ++k8) {
-              const uint32_t a_off = ((kh * kHaloW + kw) * 16 + 2 * k8 * S::kBrickBytes) >> 4;
-              const uint32_t b_off = (khw * (CIN * 3 * GW * 4) + k8 * 2 * 3 * GW * 16) >> 4;
+          for (int k8 = 0; k8 < CIN / 8; ++k8) {
+            const uint32_t a_off = ((kh * kHaloW + kw) * 16 + 2 * k8 * S::kBrickBytes) >> 4;
+            const uint32_t b_off = (khw * (CIN * 3 * GW * 4) + k8 * 2 * 3 * GW * 16) >> 4;
+            if constexpr (PLANAR)   // kd = 1 only: B column group 1
+              wgmma_tf32<GW>(acc, a_s + a_off, b_desc0 + b_off + ((GW * 16) >> 4));
+            else
               wgmma_tf32<3 * GW>(acc, a_s + a_off, b_desc0 + b_off);
-            }
           }
         }
         wgmma_commit();
+        // the epilogue of the output slice completed by the previous input slice (possibly
+        // the last one of the previous item) overlaps this slice's wgmma
+        if (pend_od >= 0)
+          store_slice<GW, 0>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl, lane,
+                             co_base);
         wgmma_wait_all();
         mbar_arrive(bar_empty + 8 * (g % SLOTS));   // this thread's reads of the slot are done
         // output slice of column group 0: `it` when planar, else it - 2 (complete after its
         // third input slice).  Group 0 is copied out before the (per-thread) stores so that no
         // accumulator register is touched on a divergent path: that would make ptxas serialize
-        // the wgmma of the next slice.
-        float done[GW / 2];
+        // the wgmma of the next slice.  At an item boundary groups 0 and 1 hold the output
+        // slices -2 and -1 of the next item, which are never stored.
 #pragma unroll
         for (int i = 0; i < GW / 2; ++i) done[i] = acc[i];
-        if constexpr (!PLANAR) {
+        if constexpr (PLANAR) {
+#pragma unroll
+          for (int i = 0; i < GW / 2; ++i) acc[i] = 0.f;
+        } else {
 #pragma unroll
           for (int i = 0; i < GW; ++i) acc[i] = acc[i + GW / 2];   // groups 1, 2 -> 0, 1
 #pragma unroll
           for (int i = 0; i < GW / 2; ++i) acc[GW + i] = 0.f;
         }
         const int j = PLANAR ? it : it - 2;
-        if (j >= 0 && j < nd)
-          store_slice<GW, 0>(done, p, s_param, b, d0 + j, h0, w0, row0, wl, lane, co_base);
+        pend_od = (j >= 0 && j < nd) ? d0 + j : -1;
+        pend_b = b; pend_h0 = h0; pend_w0 = w0;
       }
     }
     gs += nslices;
   }
+  if (pend_od >= 0)                                 // consumers: the CTA's last output slice
+    store_slice<GW, 0>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl, lane, co_base);
 }
 
 // ---- host side ----
@@ -389,7 +393,7 @@ int conv3d_tma(const float* x, const float* wpk, const float* scale, const float
   p.Cout = deep ? 16 : Cout; p.cout_total = Cout;
   p.tiles_w = (w + tc::kTileW - 1) / tc::kTileW;
   p.tiles_h = (h + tc::kTileH - 1) / tc::kTileH;
-  const int npad = p.Cout <= 16 ? 16 : 32;
+  const int npad = p.Cout <= 8 ? 8 : p.Cout <= 16 ? 16 : 32;
   p.planar = kind == CASMVS_CONV_PLANAR ? 1 : 0;
   // the prob head feeds the softmax: keep fp32; callers can ask for unrounded outputs
   p.round_out = (round_out && Cout > 1 && !(precision_flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
@@ -397,8 +401,9 @@ int conv3d_tma(const float* x, const float* wpk, const float* scale, const float
   if (Cin == CI && npad == NP)                                                  \
     return p.planar ? tma::launch<CI, NP, SL, true>(x, wpk, p, st)              \
                     : tma::launch<CI, NP, SL, false>(x, wpk, p, st);
-  TMA_CASE(8, 16, 4) TMA_CASE(8, 32, 4) TMA_CASE(16, 16, 4) TMA_CASE(16, 32, 4)
-  TMA_CASE(32, 16, 4) TMA_CASE(32, 32, 4) TMA_CASE(64, 16, 2)
+  TMA_CASE(8, 8, 4) TMA_CASE(8, 32, 4) TMA_CASE(16, 8, 4) TMA_CASE(16, 16, 4)
+  TMA_CASE(16, 32, 4) TMA_CASE(32, 8, 4) TMA_CASE(32, 16, 4) TMA_CASE(32, 32, 4)
+  TMA_CASE(64, 16, 2)
 #undef TMA_CASE
   return 1;
 }
