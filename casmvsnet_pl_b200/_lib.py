@@ -5,7 +5,7 @@ device is not a H100 (sm_90a) GPU the import / call fails loudly.
 """
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_size_t, c_uint64, c_void_p, POINTER
+from ctypes import c_char_p, c_double, c_float, c_int, c_size_t, c_uint64, c_void_p, POINTER
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libcasmvs.so")
@@ -75,7 +75,17 @@ SIGNATURES = {
                                     POINTER(c_float), POINTER(c_float), c_void_p, c_int, c_int,
                                     c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),
-    "casmvs_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
+    "casmvs_pcd_cell_keys": (c_int, [c_void_p, c_int, c_double, c_double, c_double, c_double,
+                                     c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "casmvs_pcd_thin_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "casmvs_pcd_thin_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                        c_void_p, c_size_t, c_void_p]),
+    "casmvs_pcd_thin_round": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_double,
+                                      c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "casmvs_pcd_capped_nn": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                     POINTER(c_double), c_double, POINTER(c_int), POINTER(c_double),
+                                     POINTER(c_double), c_double, c_void_p, c_void_p]),
+    "casmvs_nchw_to_nhwc":(c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
 }
 

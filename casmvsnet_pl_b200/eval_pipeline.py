@@ -2,6 +2,8 @@
 
     step 1 (eval.py:198-243)  depth + confidence for every reference view of a scan
     step 2 (eval.py:245-353)  geometric filter, refinement, fusion, PLY
+    step 3 (optional)         DTU scores of the fused cloud (dtu_eval, evaluations/dtu/*.m),
+                              straight from the device tensors when --dtu_gt is given
 
 over the DTU *test* layout the reference reads (datasets/dtu.py:31-75,150-166, eval.py:76-98):
 
@@ -12,11 +14,12 @@ Everything between decoding the PNGs and writing the PLY stays on the GPU: image
 bytes and normalised by casmvs_normalize_u8_fwd, depth maps never pass through PFM files unless
 `depth_dir` is given (then the reference's depth_XXXX.pfm / proba_XXXX.pfm are written as well).
 
-    python -m casmvsnet_pl_b200.eval_pipeline --root_dir DTU --scan scan1 --ckpt ckpt.ckpt
+    python -m casmvsnet_pl_b200.eval_pipeline --root_dir DTU --scan scan1 --ckpt ckpt.ckpt [--dtu_gt GT]
 """
 from __future__ import annotations
 
 import argparse
+import json
 import os
 
 import numpy as np
@@ -73,8 +76,12 @@ class DTUTestScan:
 
 @torch.no_grad()
 def run_scan(model, scan: DTUTestScan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
-             skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None):
-    """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs."""
+             skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
+             dtu_gt=None, dtu_seed=0):
+    """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
+    With `dtu_gt` (a DTU ground-truth directory) the fused cloud is also scored by
+    dtu_eval.evaluate_scan from the device tensors, the scores are written next to the PLY as
+    <ply>_scores.json when ply_path is given, and (xyz, rgb, scores) is returned."""
     depths, probas = {}, {}
     writer = io.DepthWriter(depth_dir) if depth_dir else None
     for ref, imgs, pm in scan.views(device):
@@ -90,7 +97,14 @@ def run_scan(model, scan: DTUTestScan, depth_interval=2.65, conf=0.999, min_geo_
                                 skip, max_ref_views)
     if ply_path:
         fusion.write_ply(ply_path, xyz, rgb)
-    return xyz, rgb
+    if dtu_gt is None:
+        return xyz, rgb
+    from . import dtu_eval
+    scores = dtu_eval.evaluate_scan(xyz, dtu_eval.scan_number(scan.scan), dtu_gt, seed=dtu_seed)
+    if ply_path:
+        with open(os.path.splitext(ply_path)[0] + "_scores.json", "w") as f:
+            json.dump(scores, f, indent=1)
+    return xyz, rgb, scores
 
 
 def main():
@@ -109,6 +123,8 @@ def main():
     ap.add_argument("--skip", type=int, default=1)
     ap.add_argument("--precision", default="tf32", choices=["fp32", "tf32"])
     ap.add_argument("--out", default="results/dtu")
+    ap.add_argument("--dtu_gt", default=None, help="DTU ground-truth directory: score the fused cloud")
+    ap.add_argument("--dtu_seed", type=int, default=0)
     a = ap.parse_args()
     from . import ABN
     from .models.mvsnet import CascadeMVSNet
@@ -122,10 +138,14 @@ def main():
     model = model.eval().cuda()
     scan = DTUTestScan(a.root_dir, a.scan, tuple(a.img_wh), a.n_views)
     os.makedirs(os.path.join(a.out, "points"), exist_ok=True)
-    xyz, _ = run_scan(model, scan, a.depth_interval, a.conf, a.min_geo_consistent, a.skip,
-                      depth_dir=os.path.join(a.out, "depth"),
-                      ply_path=os.path.join(a.out, "points", f"{a.scan}.ply"))
-    print(f"{a.scan} contains {len(xyz) / 1e6:.2f} M points")
+    out = run_scan(model, scan, a.depth_interval, a.conf, a.min_geo_consistent, a.skip,
+                   depth_dir=os.path.join(a.out, "depth"),
+                   ply_path=os.path.join(a.out, "points", f"{a.scan}.ply"), dtu_gt=a.dtu_gt,
+                   dtu_seed=a.dtu_seed)
+    print(f"{a.scan} contains {len(out[0]) / 1e6:.2f} M points")
+    if a.dtu_gt is not None:
+        from .dtu_eval import _fmt
+        print(_fmt(out[2]))
 
 
 if __name__ == "__main__":

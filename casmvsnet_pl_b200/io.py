@@ -13,6 +13,8 @@ Host-side Python like the reference's (it is data plumbing, not arithmetic on th
                                uint8 HWC images are uploaded AS BYTES (4x less H2D traffic than
                                fp32) and converted + normalised + re-laid-out to planar fp32 on the
                                GPU by casmvs_normalize_u8_fwd
+  read_ply                     PLY vertices (binary little-endian or ASCII, scalar properties): reads
+                               fusion.write_ply output and the DTU ground-truth STL clouds
   DepthWriter / infer_views    reference eval.py:213-229 (the per-view inference loop): views are
                                streamed through PipelinedCascade (H2D, forward and D2H of
                                neighbouring views overlap), NaNs scrubbed, depth_XXXX.pfm and
@@ -75,6 +77,70 @@ def save_pfm(filename, image, scale=1):
         f.write(f"{image.shape[1]} {image.shape[0]}\n".encode("utf-8"))
         f.write(("%f\n" % scale).encode("utf-8"))
         np.ascontiguousarray(np.flipud(image)).tofile(f)
+
+
+# ------------------------------------------------------------------------------ PLY
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2",
+              "int16": "i2", "ushort": "u2", "uint16": "u2", "int": "i4", "int32": "i4",
+              "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4", "double": "f8",
+              "float64": "f8"}
+
+
+def read_ply(filename):
+    """-> numpy structured array of the vertex element, one field per property.
+
+    Reads `format binary_little_endian 1.0` and `format ascii 1.0` files whose vertex element is
+    the first element and has scalar properties only; elements after it (faces, ...) are ignored.
+    Anything else (big-endian, list properties on vertices, a missing vertex element) raises
+    ValueError."""
+    with open(filename, "rb") as f:
+        if f.readline().rstrip(b"\r\n") != b"ply":
+            raise ValueError(f"{filename}: not a PLY file")
+        fmt, elements = None, []
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{filename}: PLY header has no end_header")
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1] if len(tok) == 3 and tok[2] == "1.0" else None
+                if fmt not in ("binary_little_endian", "ascii"):
+                    raise ValueError(f"{filename}: unsupported PLY format {' '.join(tok[1:])}")
+            elif tok[0] == "element" and len(tok) == 3:
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property" and elements:
+                if tok[1] == "list" or len(tok) != 3 or tok[1] not in _PLY_TYPES:
+                    elements[-1][2].append(None)            # unsupported; fatal only on vertices
+                else:
+                    elements[-1][2].append((tok[2], _PLY_TYPES[tok[1]]))
+            else:
+                raise ValueError(f"{filename}: malformed PLY header line {line!r}")
+        if fmt is None:
+            raise ValueError(f"{filename}: PLY header has no format line")
+        if not elements or elements[0][0] != "vertex":
+            raise ValueError(f"{filename}: the first PLY element must be 'vertex'")
+        _, n, props = elements[0]
+        if not props or any(p is None for p in props):
+            raise ValueError(f"{filename}: vertex properties must be scalars")
+        if fmt == "binary_little_endian":
+            dtype = np.dtype([(name, "<" + t) for name, t in props])
+            data = np.frombuffer(f.read(n * dtype.itemsize), dtype=dtype)
+            if len(data) != n:
+                raise ValueError(f"{filename}: {len(data)} vertices, header says {n}")
+            return data.copy()
+        dtype = np.dtype([(name, t) for name, t in props])
+        rows = [f.readline().split() for _ in range(n)]
+    if any(len(r) != len(props) for r in rows):
+        raise ValueError(f"{filename}: ASCII vertex rows must hold {len(props)} values")
+    out = np.empty(n, dtype=dtype)
+    cols = np.array(rows, dtype=object).reshape(n, len(props))
+    for j, (name, t) in enumerate(props):
+        out[name] = cols[:, j].astype(np.float64 if t[0] == "f" else np.int64).astype(t) if n else []
+    return out
 
 
 # ------------------------------------------------------------------------------ cameras

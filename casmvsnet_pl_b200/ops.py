@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import functools
+import math
 
 import torch
 
@@ -547,3 +548,100 @@ def bias_lrelu_(x, bias, slope, round_tf32=False):
                                            x.shape[1], 1 if round_tf32 else 0, _stream()),
           "bias_lrelu")
     return x
+
+
+# ------------------------------------------------------------------ DTU point-cloud scoring
+def _require_cuda_typed(**tensors):
+    """name=(tensor, dtype): CUDA tensors of the given dtypes on one device (no CPU fallback)."""
+    first = None
+    for name, (t, dtype) in tensors.items():
+        if not (torch.is_tensor(t) and t.is_cuda):
+            raise _lib.CasMVSError(f"{name} must be a CUDA tensor (no CPU fallback)")
+        if t.dtype != dtype:
+            raise _lib.CasMVSError(f"{name} must be {dtype}, got {t.dtype}")
+        if first is not None and t.device != first.device:
+            raise _lib.CasMVSError(f"tensors on different devices: {first.device} and {t.device}")
+        if first is None:
+            first = t
+    _require_cuda(torch.empty(0, device=first.device))
+
+
+def _points(name, t):
+    if not (torch.is_tensor(t) and t.dim() == 2 and t.shape[1] == 3):
+        raise _lib.CasMVSError(f"{name} must be an (N,3) tensor")
+    if t.shape[0] >= 2 ** 31:
+        raise _lib.CasMVSError(f"{name}: at most 2^31 - 1 points")
+    return t.contiguous()
+
+
+@_on_tensor_device
+def pcd_cell_keys(points, origin, cell, dims, sub=1):
+    """int64 cell key of every point of an (N,3) float32 cloud (casmvs_pcd_cell_keys): cells of
+    edge `cell` from `origin`, grid `dims`; sub = 8 orders keys by super cells of 8^3 cells.
+    Points outside the grid get the largest int64."""
+    pts = _points("points", points)
+    _require_cuda_typed(points=(pts, torch.float32))
+    keys = torch.empty(pts.shape[0], device=pts.device, dtype=torch.int64)
+    ox, oy, oz = (float(v) for v in origin)
+    gx, gy, gz = (int(v) for v in dims)
+    check(_lib.load().casmvs_pcd_cell_keys(_ptr(pts), pts.shape[0], ox, oy, oz, float(cell),
+                                           gx, gy, gz, int(sub), _ptr(keys), _stream()),
+          "pcd_cell_keys")
+    return keys
+
+
+@_on_tensor_device
+def pcd_thin_prepare(cell_keys, cell_start, n, dims):
+    """Workspace of pcd_thin_round for a sub = 1 grid: 27-neighbour table and cell of each point."""
+    _require_cuda_typed(cell_keys=(cell_keys, torch.int64), cell_start=(cell_start, torch.int32))
+    ncells = cell_keys.shape[0]
+    if cell_start.shape[0] != ncells + 1:
+        raise _lib.CasMVSError("cell_start must hold ncells + 1 offsets")
+    lib = _lib.load()
+    nbytes = lib.casmvs_pcd_thin_workspace_bytes(int(n), ncells)
+    ws = torch.empty(max(nbytes, 1), device=cell_keys.device, dtype=torch.uint8)
+    gx, gy, gz = (int(v) for v in dims)
+    check(lib.casmvs_pcd_thin_prepare(_ptr(cell_keys.contiguous()), _ptr(cell_start.contiguous()),
+                                      int(n), ncells, gx, gy, gz, _ptr(ws), ws.numel(), _stream()),
+          "pcd_thin_prepare")
+    return ws
+
+
+@_on_tensor_device
+def pcd_thin_round(points, rank, cell_start, dst, state, undecided, workspace):
+    """One join + remove round of the parallel thinning (casmvs_pcd_thin_round); writes the number
+    of points still undecided to the device int32 `undecided` (no synchronisation)."""
+    pts = _points("points", points)
+    _require_cuda_typed(points=(pts, torch.float32), rank=(rank, torch.int32),
+                        cell_start=(cell_start, torch.int32), state=(state, torch.uint8),
+                        undecided=(undecided, torch.int32), workspace=(workspace, torch.uint8))
+    n = pts.shape[0]
+    if rank.shape != (n,) or state.shape != (n,) or not state.is_contiguous():
+        raise _lib.CasMVSError("rank and state must be contiguous (N,) tensors")
+    check(_lib.load().casmvs_pcd_thin_round(
+        _ptr(pts), _ptr(rank.contiguous()), _ptr(cell_start.contiguous()), n,
+        cell_start.shape[0] - 1, float(dst), _ptr(state), _ptr(undecided), _ptr(workspace),
+        workspace.numel(), _stream()), "pcd_thin_round")
+
+
+@_on_tensor_device
+def pcd_capped_nn(queries, targets, cell_keys, cell_start, super_begin, origin, h, super_dims,
+                  box_lo, box_hi, cap):
+    """min(nearest-target distance, cap) as float64 for queries inside [box_lo, box_hi), cap
+    outside (casmvs_pcd_capped_nn).  Targets sorted by their sub = 8 keys; see the header."""
+    q = _points("queries", queries)
+    t = _points("targets", targets)
+    _require_cuda_typed(queries=(q, torch.float32), targets=(t, torch.float32),
+                        cell_keys=(cell_keys, torch.int64), cell_start=(cell_start, torch.int32),
+                        super_begin=(super_begin, torch.int32))
+    ncells = cell_keys.shape[0]
+    if cell_start.shape[0] != ncells + 1 or super_begin.shape[0] != math.prod(int(v) for v in super_dims) + 1:
+        raise _lib.CasMVSError("cell_start / super_begin sizes do not match the grid")
+    dist = torch.empty(q.shape[0], device=q.device, dtype=torch.float64)
+    d3 = ctypes.c_double * 3
+    check(_lib.load().casmvs_pcd_capped_nn(
+        _ptr(q), q.shape[0], _ptr(t), _ptr(cell_keys.contiguous()), _ptr(cell_start.contiguous()),
+        ncells, _ptr(super_begin.contiguous()), d3(*map(float, origin)), float(h),
+        (ctypes.c_int * 3)(*map(int, super_dims)), d3(*map(float, box_lo)), d3(*map(float, box_hi)),
+        float(cap), _ptr(dist), _stream()), "pcd_capped_nn")
+    return dist

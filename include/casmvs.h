@@ -317,6 +317,44 @@ int casmvs_geo_fuse_fwd(const float* depth_ref, const float* image_ref, const fl
                         int* geo_count, unsigned char* mask_final, float* points,
                         float* reproj_dbg, unsigned char* mask_dbg, void* stream);
 
+/* ---- DTU point-cloud scoring (reference evaluations/dtu, MATLAB)--------------------------
+ * The two heavy steps of the DTU scorer on the device; the masks, statistics and the sort /
+ * run-length scan that turn cell keys into cells are torch ops (casmvsnet_pl_b200/dtu_eval.py).
+ * points / targets / queries are (N,3) float32; cell lists are the sorted unique keys, with
+ * cell_start (ncells+1) int32 offsets into the key-sorted points.
+ *
+ * casmvs_pcd_cell_keys: int64 cell key of each point for cells of edge `cell` with corner (0,0,0)
+ *   at (ox,oy,oz), grid dims g < 2^20.  sub == 1: key = (ix*gy + iy)*gz + iz.  sub == 8: super
+ *   cells of 8^3 cells first, key = ((sx*SY + sy)*SZ + sz) << 9 | lx << 6 | ly << 3 | lz with
+ *   s = i >> 3, l = i & 7, S = ceil(g/8).  Points outside the grid (or NaN) get INT64_MAX.
+ * Thinning (reducePts_haa.m): the kept set is the lexicographically-first maximal set of points
+ *   pairwise more than `dst` apart for the visiting order `rank` (a permutation of 0..n-1), i.e.
+ *   what visiting the points in rank order and keeping each point no kept point lies within dst
+ *   of gives.  |p - q| <= dst is evaluated in double as (dx*dx + dy*dy) + dz*dz <= dst*dst.
+ *   Points, rank and state are in key order of a sub == 1 grid whose cell edge is > dst.
+ *   casmvs_pcd_thin_prepare fills the workspace (a 27-neighbour table per cell and the cell of
+ *   each point); then call casmvs_pcd_thin_round, starting from state = 0 (undecided), until the
+ *   device int *undecided it writes is 0.  state ends 1 (kept) or 2 (removed).
+ * casmvs_pcd_capped_nn (MaxDistCP.m): dist[i] = min(nearest-target distance, cap) in double for a
+ *   query with box_lo <= q < box_hi on every axis, cap otherwise.  Targets are in key order of a
+ *   sub == 8 grid of edge h at origin3 that covers [box_lo - cap, box_hi + cap]; super_begin
+ *   (prod(super_dims3)+1) int32 = index of the first cell of each super cell in the cell list.
+ *   origin3, super_dims3, box_lo3, box_hi3 are HOST arrays of 3. */
+int casmvs_pcd_cell_keys(const float* points, int n, double ox, double oy, double oz, double cell,
+                         int gx, int gy, int gz, int sub, int64_t* keys, void* stream);
+size_t casmvs_pcd_thin_workspace_bytes(int n, int ncells);
+int casmvs_pcd_thin_prepare(const int64_t* cell_keys, const int* cell_start, int n, int ncells,
+                            int gx, int gy, int gz, void* workspace, size_t workspace_bytes,
+                            void* stream);
+int casmvs_pcd_thin_round(const float* points, const int* rank, const int* cell_start, int n,
+                          int ncells, double dst, unsigned char* state, int* undecided,
+                          const void* workspace, size_t workspace_bytes, void* stream);
+int casmvs_pcd_capped_nn(const float* queries, int nq, const float* targets,
+                         const int64_t* cell_keys, const int* cell_start, int ncells,
+                         const int* super_begin, const double* origin3, double h,
+                         const int* super_dims3, const double* box_lo3, const double* box_hi3,
+                         double cap, double* dist, void* stream);
+
 /* ---- layout helpers ------------------------------------------------------ */
 /* (N,C,S) -> (N,S,C) and back, S = product of spatial dims. */
 int casmvs_nchw_to_nhwc(const float* in, float* out, int N, int C, size_t S, void* stream);
