@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libcasmvs.so")
 NCHW, NHWC = 0, 1
 ROUND_TF32 = 256
 KEEP_FP32_OUT = 256      # OR-ed into conv3d precision
+BLOCKED = 512            # OR-ed into costreg precision / warp_cost_ladder round_tf32
 FP32, TF32 = 0, 1
 CONV, CONV_TRANSPOSE, CONV_PLANAR = 0, 1, 2
 PRECISIONS = {"fp32": FP32, "tf32": TF32}
@@ -45,6 +46,7 @@ SIGNATURES = {
                                           POINTER(c_int), POINTER(c_int), POINTER(c_size_t),
                                           POINTER(c_size_t), POINTER(c_size_t)]),
     "casmvs_costreg_workspace_bytes": (c_size_t, [c_int] * 5),
+    "casmvs_costreg_blocked_supported": (c_int, [c_int, c_int]),
     "casmvs_costreg_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                    c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "casmvs_regress_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,

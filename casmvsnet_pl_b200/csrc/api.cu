@@ -25,11 +25,13 @@ int conv3d_direct(const float* x, const float* wpk, const float* scale, const fl
 // conv3d_tma.cu (wgmma + TMA producer, persistent: the stride-1 tensor path)
 int conv3d_tma(const float* x, const float* wpk, const float* scale, const float* shift,
                float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-               int w, int kind, int stride, int precision, cudaStream_t st);
+               int w, int kind, int stride, int precision, int layout, cudaStream_t st);
 // conv3d_tma2.cu (wgmma + TMA producer, persistent: stride-2 and transposed layers)
 int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
                 float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-                int w, int kind, int stride, int precision, cudaStream_t st);
+                int w, int kind, int stride, int precision, int layout, cudaStream_t st);
+bool conv3d_tma_enabled();   // CASMVS_TMA
+int conv3d_tma2_modes();     // CASMVS_TMA2: bit 0 stride-2, bit 1 transposed
 
 struct LayerSpec { int cin, cout, kind, stride; };
 
@@ -73,10 +75,12 @@ extern "C" int casmvs_device_check(int device) {
   return 0;
 }
 
-extern "C" int casmvs_conv3d_fwd(const float* x, const float* w_packed, const float* scale,
-                                 const float* shift, float slope, const float* skip, float* y,
-                                 int B, int Cin, int Cout, int D, int h, int w, int kind,
-                                 int stride, int precision, void* stream) {
+// casmvs_conv3d_fwd with the kLayout* bits of common.cuh.  Only the tensor-core kernels read and
+// write the blocked layout: a blocked layer they do not cover is an error.
+static int conv_layer(const float* x, const float* w_packed, const float* scale,
+                      const float* shift, float slope, const float* skip, float* y, int B,
+                      int Cin, int Cout, int D, int h, int w, int kind, int stride, int precision,
+                      int layout, void* stream) {
   CASMVS_REQUIRE(x && w_packed && y, "conv3d: null pointer");
   CASMVS_REQUIRE(B >= 0 && Cin > 0 && Cout > 0 && D > 0 && h > 0 && w > 0, "conv3d: bad dims");
   CASMVS_REQUIRE(Cin % 4 == 0, "conv3d: Cin must be a multiple of 4 (got %d)", Cin);
@@ -95,13 +99,15 @@ extern "C" int casmvs_conv3d_fwd(const float* x, const float* w_packed, const fl
     const int pf = precision | flags;
     // tensor-core kernels: each returns 0 (handled), <0 (failed) or 1 (shape not covered)
     int rc = conv3d_tma(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
-                    stride, pf, st);
+                        stride, pf, layout, st);
     if (rc <= 0) return rc;
     if (kind != CASMVS_CONV_PLANAR) {
       rc = conv3d_tma2(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
-                       stride, precision, st);
+                       stride, precision, layout, st);
       if (rc <= 0) return rc;
     }
+    CASMVS_REQUIRE(layout == 0, "conv3d: no tensor-core kernel for the blocked layer %d -> %d "
+                   "(kind %d, stride %d)", Cin, Cout, kind, stride);
     // no tensor-core kernel covers this layer shape: it runs on the CUDA cores (same TF32-rounded
     // storage convention).  Counted, so callers can assert the fast path was taken.
     g_fallbacks.fetch_add(1, std::memory_order_relaxed);
@@ -112,6 +118,14 @@ extern "C" int casmvs_conv3d_fwd(const float* x, const float* w_packed, const fl
       (precision == CASMVS_TF32 && Cout > 1 && !(flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
   return conv3d_direct(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
                        stride, st, round_out);
+}
+
+extern "C" int casmvs_conv3d_fwd(const float* x, const float* w_packed, const float* scale,
+                                 const float* shift, float slope, const float* skip, float* y,
+                                 int B, int Cin, int Cout, int D, int h, int w, int kind,
+                                 int stride, int precision, void* stream) {
+  return conv_layer(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind, stride,
+                    precision, 0, stream);
 }
 
 // ---- CostRegNet driver ------------------------------------------------------
@@ -152,10 +166,26 @@ extern "C" size_t casmvs_costreg_workspace_bytes(int B, int Cin, int D, int h, i
          sizeof(float);
 }
 
+extern "C" int casmvs_costreg_blocked_supported(int Cin, int precision) {
+  // the blocked layout has only tensor-core kernels: every layer must be one of theirs.  conv1 ..
+  // prob have fixed shapes that they cover; conv0 is covered for Cin in {8, 16, 32}
+  return precision == CASMVS_TF32 && conv3d_tma_enabled() && (conv3d_tma2_modes() & 3) == 3 &&
+         (Cin == 8 || Cin == 16 || Cin == 32);
+}
+
 extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* logits, int B,
                                   int Cin, int D, int h, int w, int precision, void* workspace,
                                   size_t workspace_bytes, void* stream) {
   CASMVS_REQUIRE(x && params && logits, "costreg: null pointer");
+  const bool blocked_in = (precision & CASMVS_BLOCKED) != 0;
+  precision &= ~CASMVS_BLOCKED;
+  // the tensor maps need 16-byte aligned bases (the workspace offsets are multiples of 256 B)
+  const bool blocked = casmvs_costreg_blocked_supported(Cin, precision) &&
+                       ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(workspace)) &
+                        15) == 0;
+  CASMVS_REQUIRE(!blocked_in || blocked,
+                 "costreg: a blocked input needs the TF32 precision, Cin in {8,16,32}, the "
+                 "tensor-core kernels enabled and 16-byte aligned x and workspace (got Cin=%d)", Cin);
   CASMVS_REQUIRE(D % 8 == 0 && h % 8 == 0 && w % 8 == 0,
                  "costreg: D,h,w must be divisible by 8 (got %d,%d,%d)", D, h, w);
   const size_t need = casmvs_costreg_workspace_bytes(B, Cin, D, h, w);
@@ -186,22 +216,27 @@ extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* lo
   float* u9 = ws;            ws += 2 * n;
   float* u11 = ws;
   const float slope = 0.01f;  // inplace_abn LeakyReLU default
+  // blocked: the activations c0 .. u11 are stored blocked by channel quads (DESIGN.md §2), the
+  // input as the caller says, the logits (B,D,h,w).  Otherwise (FP32, or a layer some
+  // tensor-core kernel does not cover) everything is channels-last, as casmvs_conv3d_fwd is.
+  const int blk = blocked ? kLayoutXBlocked | kLayoutYBlocked : 0;
   int rc;
-#define LAYER(i, in, skip, out, d_, h_, w_, sl)                                                   \
-  rc = casmvs_conv3d_fwd(in, W[i], SC[i], SH[i], sl, skip, out, B, L[i].cin, L[i].cout, d_, h_,  \
-                         w_, L[i].kind, L[i].stride, precision, stream);                          \
+#define LAYER(i, in, skip, out, d_, h_, w_, sl, lay)                                              \
+  rc = conv_layer(in, W[i], SC[i], SH[i], sl, skip, out, B, L[i].cin, L[i].cout, d_, h_, w_,     \
+                  L[i].kind, L[i].stride, precision, lay, stream);                                \
   if (rc) return rc;
-  LAYER(0, x, nullptr, c0, D, h, w, slope)
-  LAYER(1, c0, nullptr, c1, D, h, w, slope)
-  LAYER(2, c1, nullptr, c2, D / 2, h / 2, w / 2, slope)
-  LAYER(3, c2, nullptr, c3, D / 2, h / 2, w / 2, slope)
-  LAYER(4, c3, nullptr, c4, D / 4, h / 4, w / 4, slope)
-  LAYER(5, c4, nullptr, c5, D / 4, h / 4, w / 4, slope)
-  LAYER(6, c5, nullptr, c6, D / 8, h / 8, w / 8, slope)
-  LAYER(7, c6, c4, u7, D / 8, h / 8, w / 8, slope)     // conv4 + conv7(x)   mvsnet.py:97
-  LAYER(8, u7, c2, u9, D / 4, h / 4, w / 4, slope)     // conv2 + conv9(x)   mvsnet.py:99
-  LAYER(9, u9, c0, u11, D / 2, h / 2, w / 2, slope)    // conv0 + conv11(x)  mvsnet.py:101
-  LAYER(10, u11, nullptr, logits, D, h, w, 1.0f)       // prob: bias, no norm/act  :103
+  LAYER(0, x, nullptr, c0, D, h, w, slope,
+        (blk & kLayoutYBlocked) | (blocked_in ? kLayoutXBlocked : 0))
+  LAYER(1, c0, nullptr, c1, D, h, w, slope, blk)
+  LAYER(2, c1, nullptr, c2, D / 2, h / 2, w / 2, slope, blk)
+  LAYER(3, c2, nullptr, c3, D / 2, h / 2, w / 2, slope, blk)
+  LAYER(4, c3, nullptr, c4, D / 4, h / 4, w / 4, slope, blk)
+  LAYER(5, c4, nullptr, c5, D / 4, h / 4, w / 4, slope, blk)
+  LAYER(6, c5, nullptr, c6, D / 8, h / 8, w / 8, slope, blk)
+  LAYER(7, c6, c4, u7, D / 8, h / 8, w / 8, slope, blk)     // conv4 + conv7(x)   mvsnet.py:97
+  LAYER(8, u7, c2, u9, D / 4, h / 4, w / 4, slope, blk)     // conv2 + conv9(x)   mvsnet.py:99
+  LAYER(9, u9, c0, u11, D / 2, h / 2, w / 2, slope, blk)    // conv0 + conv11(x)  mvsnet.py:101
+  LAYER(10, u11, nullptr, logits, D, h, w, 1.0f, blk & kLayoutXBlocked)   // prob: bias  :103
 #undef LAYER
   return 0;
 }

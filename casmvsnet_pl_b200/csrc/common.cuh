@@ -21,6 +21,11 @@ extern std::atomic<uint64_t> g_fallbacks;
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// Layout bits of the internal conv entry points (conv3d_tma / conv3d_tma2): the input, or the
+// output and the skip, stored blocked by channel quads (B, C/4, D, H, W, 4) instead of
+// channels-last (B, D, H, W, C).  Only the CostRegNet driver passes them; see DESIGN.md §2.
+constexpr int kLayoutXBlocked = 1, kLayoutYBlocked = 2;
+
 // call after every kernel launch: counts it and converts launch errors
 inline int after_launch(const char* what) {
   g_launches.fetch_add(1, std::memory_order_relaxed);

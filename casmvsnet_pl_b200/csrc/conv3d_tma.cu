@@ -9,7 +9,8 @@
 // The GEMM: M = 128 voxels = 8(w) x 16(h) of one depth slice, K = Cin per tap, N = 3 x GW (the
 // three kd taps share one A operand: an input slice feeds three output slices in ONE wgmma).
 // The input brick of a depth slice (18 x 10 voxels with halo) is brought in by Cin/4 TMA tiled
-// loads (cp.async.bulk.tensor.5d over x viewed as {C, W, H, D, B}, a box of 4 channels each;
+// loads (cp.async.bulk.tensor.5d over x viewed as {C, W, H, D, B}, a box of 4 channels each, or,
+// for x blocked by channel quads, as {4W, H, D, C/4, B}, a box of one quad's 160-byte rows;
 // out-of-bounds elements are zero-filled by the TMA unit = the conv's zero padding, in all
 // three spatial dimensions).  Each load writes one [18][10][4 channels] brick: 16 bytes per
 // voxel, so 8 consecutive voxels of a brick row are one 128-byte wgmma core matrix and the A
@@ -51,6 +52,8 @@ struct Params {
   int tiles_w, tiles_h, nchunks, dchunk;
   int round_out;        // round the stored activations to tf32 (unbiased next-layer operand)
   int planar;           // 1x3x3 kernel: input slice s feeds output slice s only (kd = 1)
+  int x_blocked;        // x stored blocked by channel quads (input_map); else channels-last
+  int y_blocked;        // y and skip stored blocked by channel quads; else channels-last
 };
 
 template <int CIN, int GW, int SLOTS_>
@@ -70,8 +73,9 @@ struct Smem {
 };
 
 // Epilogue of one output slice from the accumulator columns [OFF, OFF + GW) of this thread's
-// fragment: scale/shift, leaky ReLU, optional skip, optional tf32 rounding, channel-last store.
-template <int GW, int OFF>
+// fragment: scale/shift, leaky ReLU, optional skip, optional tf32 rounding, channels-last or
+// blocked store (p.y_blocked).
+template <int GW, int OFF, bool PLANAR>
 __device__ __forceinline__ void store_slice(const float* acc, const Params& p, const float* s_param,
                                             int b, int od, int h0, int w0, int row0, int wl,
                                             int lane, int co_base) {
@@ -79,7 +83,8 @@ __device__ __forceinline__ void store_slice(const float* acc, const Params& p, c
     const int m = row0 + r;
     const int oh = h0 + (m >> 3), ow = w0 + (m & 7);
     if (oh >= p.H || ow >= p.W || c >= p.Cout) return;
-    const size_t o = ((((size_t)b * p.D + od) * p.H + oh) * p.W + ow) * p.cout_total + co_base + c;
+    const size_t o =
+        vol_offset(!PLANAR && p.y_blocked, b, od, oh, ow, co_base + c, p.D, p.H, p.W, p.cout_total);
     float v0 = fmaf(a0, s_param[c], s_param[GW + c]);
     float v1 = fmaf(a1, s_param[c + 1], s_param[GW + c + 1]);
     v0 = v0 >= 0.f ? v0 : v0 * p.slope;
@@ -173,9 +178,12 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
           const uint32_t dst = s_ring + slot * S::kSlotBytes;
           mbar_expect_tx(bar_full + 8 * slot, S::CQ * S::kBrickData);
 #pragma unroll
-          for (int q = 0; q < S::CQ; ++q)
-            tma_load_5d(dst + q * S::kBrickBytes, &xmap, bar_full + 8 * slot, q * 4, w0 - 1,
-                        h0 - 1, d0 - halo + it, b);
+          for (int q = 0; q < S::CQ; ++q) {
+            const Coords5 k = brick_coords(!PLANAR && p.x_blocked, 1, S::CQ, q, w0 - 1, h0 - 1,
+                                           d0 - halo + it, b);
+            tma_load_5d(dst + q * S::kBrickBytes, &xmap, bar_full + 8 * slot, k.c[0], k.c[1],
+                        k.c[2], k.c[3], k.c[4]);
+          }
         }
       }
       __syncwarp();
@@ -209,8 +217,8 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
         // the epilogue of the output slice completed by the previous input slice (possibly
         // the last one of the previous item) overlaps this slice's wgmma
         if (pend_od >= 0)
-          store_slice<GW, 0>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl, lane,
-                             co_base);
+          store_slice<GW, 0, PLANAR>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl,
+                                     lane, co_base);
         wgmma_wait_all();
         mbar_arrive(bar_empty + 8 * (g % SLOTS));   // this thread's reads of the slot are done
         // output slice of column group 0: `it` when planar, else it - 2 (complete after its
@@ -237,7 +245,8 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
     gs += nslices;
   }
   if (pend_od >= 0)                                 // consumers: the CTA's last output slice
-    store_slice<GW, 0>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl, lane, co_base);
+    store_slice<GW, 0, PLANAR>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl, lane,
+                               co_base);
 }
 
 // ---- host side ----
@@ -283,20 +292,21 @@ int encode_tiled(CUtensorMap* out, const void* base, int rank, const uint64_t* d
 
 // Tensor maps are pure functions of (pointer, shape, box): memoised, since inference calls
 // every layer with the same workspace pointers each step.
-struct MapEntry { const void* x; int B, D, H, W, C, CB, bw, bh, sw; CUtensorMap map; };
+struct MapEntry { const void* x; int B, D, H, W, C, CB, bw, bh, sw, blk; CUtensorMap map; };
 static MapEntry g_maps[128];
 static int g_maps_n = 0, g_maps_next = 0;
 static std::mutex g_maps_mu;
 
 const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, int CB, int box_w,
-                             int box_h, int stride_w) {
+                             int box_h, int stride_w, bool blocked) {
   // the returned map is a per-thread copy: ring slots may be recycled by other threads
   static thread_local CUtensorMap t_ret;
+  const int blk = blocked ? 1 : 0;
   std::lock_guard<std::mutex> lock(g_maps_mu);
   for (int i = 0; i < g_maps_n; ++i) {
     const MapEntry& e = g_maps[i];
     if (e.x == x && e.B == B && e.D == D && e.H == H && e.W == W && e.C == C && e.CB == CB &&
-        e.bw == box_w && e.bh == box_h && e.sw == stride_w) {
+        e.bw == box_w && e.bh == box_h && e.sw == stride_w && e.blk == blk) {
       t_ret = e.map;
       return &t_ret;
     }
@@ -306,12 +316,31 @@ const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, 
   MapEntry& e = g_maps[g_maps_next];
   g_maps_next = (g_maps_next + 1) % 128;
   if (g_maps_n < 128) ++g_maps_n;
-  const cuuint64_t gdim[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D,
+  const cuuint64_t vox = (cuuint64_t)D * H * W;      // voxels per channel plane
+  // channels-last (B,D,H,W,C) as {C, W, H, D, B}, box {CB, box_w, box_h, 1, 1}
+  cuuint64_t gdim[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)B};
+  cuuint64_t gstr[4] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4,
+                        vox * C * 4};
+  cuuint32_t box[5] = {(cuuint32_t)CB, (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1};
+  cuuint32_t estr[5] = {1, (cuuint32_t)stride_w, 1, 1, 1};
+  if (blocked && stride_w == 1) {
+    // blocked (B,C/4,D,H,W,4) as {4W, H, D, C/4, B}: the quad folded into the inner dimension,
+    // box {4 box_w, box_h, 1, 1, 1}: one brick row is 16 box_w contiguous bytes
+    const cuuint64_t d2[5] = {4 * (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)C / 4,
                               (cuuint64_t)B};
-  const cuuint64_t gstr[4] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4,
-                              (cuuint64_t)D * H * W * C * 4};
-  const cuuint32_t box[5] = {(cuuint32_t)CB, (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1};
-  const cuuint32_t estr[5] = {1, (cuuint32_t)stride_w, 1, 1, 1};
+    const cuuint64_t s2[4] = {(cuuint64_t)W * 16, (cuuint64_t)H * W * 16, vox * 16, vox * C * 4};
+    const cuuint32_t b2[5] = {4 * (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1, 1};
+    for (int i = 0; i < 5; ++i) { gdim[i] = d2[i]; box[i] = b2[i]; estr[i] = 1; }
+    for (int i = 0; i < 4; ++i) gstr[i] = s2[i];
+  } else if (blocked) {
+    // blocked, W walked with element stride 2: {4, W, H, D, C/4 * B}, box {4, box_w, box_h, 1, 1}
+    const cuuint64_t d2[5] = {4, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D,
+                              (cuuint64_t)C / 4 * B};
+    const cuuint64_t s2[4] = {16, (cuuint64_t)W * 16, (cuuint64_t)H * W * 16, vox * 16};
+    for (int i = 0; i < 5; ++i) gdim[i] = d2[i];
+    for (int i = 0; i < 4; ++i) gstr[i] = s2[i];
+    box[0] = 4;
+  }
   const CUtensorMapSwizzle sw = CB * 4 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                 : CB * 4 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                                 : CB * 4 == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
@@ -325,7 +354,8 @@ const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, 
               (int)r, C, W, H, D, B);
     return nullptr;
   }
-  e.x = x; e.B = B; e.D = D; e.H = H; e.W = W; e.C = C; e.CB = CB; e.bw = box_w; e.bh = box_h; e.sw = stride_w;
+  e.x = x; e.B = B; e.D = D; e.H = H; e.W = W; e.C = C; e.CB = CB; e.bw = box_w; e.bh = box_h;
+  e.sw = stride_w; e.blk = blk;
   t_ret = e.map;
   return &t_ret;
 }
@@ -338,7 +368,7 @@ static int launch(const float* x, const float* wpk, Params p, cudaStream_t st) {
   auto kfn = conv3d_tma_kernel<CIN, GW, SLOTS, PLANAR>;
   static std::atomic<bool> attr_set[kMaxDevices];
   if (int rc = opt_in_smem(kfn, S::kTotal, attr_set, "conv3d_tma")) return rc;
-  const CUtensorMap* map = input_map(x, p.B, p.D, p.H, p.W, CIN, 4, kHaloW, kHaloH);
+  const CUtensorMap* map = input_map(x, p.B, p.D, p.H, p.W, CIN, 4, kHaloW, kHaloH, 1, p.x_blocked);
   if (!map) return -2;
   static int dchunk_env = -1;
   if (dchunk_env < 0) {
@@ -370,19 +400,27 @@ static int launch(const float* x, const float* wpk, Params p, cudaStream_t st) {
 
 }  // namespace tma
 
+// CASMVS_TMA (default 1): 0 leaves every layer to the other kernels.
+bool conv3d_tma_enabled() {
+  static const int enabled = [] {
+    const char* e = getenv("CASMVS_TMA");
+    return e ? atoi(e) : 1;
+  }();
+  return enabled != 0;
+}
+
 // Returns 0 when handled, 1 when the layer shape is left to the other kernels.
 int conv3d_tma(const float* x, const float* wpk, const float* scale, const float* shift,
                float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-               int w, int kind, int stride, int precision_flags, cudaStream_t st) {
+               int w, int kind, int stride, int precision_flags, int layout, cudaStream_t st) {
   const int precision = precision_flags & 0xff;
-  static int enabled = -1, round_out = 1;
-  if (enabled < 0) {
-    const char* e = getenv("CASMVS_TMA");
-    enabled = e ? atoi(e) : 1;
-    if (const char* s = getenv("CASMVS_TC_ROUND")) round_out = atoi(s);
-  }
-  if (!enabled || precision != CASMVS_TF32) return 1;
+  static const int round_out = [] {
+    const char* s = getenv("CASMVS_TC_ROUND");
+    return s ? atoi(s) : 1;
+  }();
+  if (!conv3d_tma_enabled() || precision != CASMVS_TF32) return 1;
   if ((kind != CASMVS_CONV && kind != CASMVS_CONV_PLANAR) || stride != 1) return 1;
+  if (kind == CASMVS_CONV_PLANAR && layout != 0) return 1;   // planar layers are channels-last only
   const bool deep = Cin == 64 && Cout == 64;          // conv6: 16-channel Cout slices
   if (!deep && (!(Cin == 8 || Cin == 16 || Cin == 32) || Cout > 32)) return 1;
   // the TMA global strides must be multiples of 16 B and the base 16 B aligned
@@ -395,6 +433,8 @@ int conv3d_tma(const float* x, const float* wpk, const float* scale, const float
   p.tiles_h = (h + tc::kTileH - 1) / tc::kTileH;
   const int npad = p.Cout <= 8 ? 8 : p.Cout <= 16 ? 16 : 32;
   p.planar = kind == CASMVS_CONV_PLANAR ? 1 : 0;
+  p.x_blocked = (layout & kLayoutXBlocked) ? 1 : 0;
+  p.y_blocked = (layout & kLayoutYBlocked) ? 1 : 0;
   // the prob head feeds the softmax: keep fp32; callers can ask for unrounded outputs
   p.round_out = (round_out && Cout > 1 && !(precision_flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
 #define TMA_CASE(CI, NP, SL)                                                    \

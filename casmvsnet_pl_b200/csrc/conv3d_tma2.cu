@@ -59,6 +59,8 @@ struct Params {
                                            // a CTA handles the COUT-channel chunk blockIdx.y
   int tiles_w, tiles_h, nchunks, dchunk;   // tiles over the M space (output for S2, input for T)
   int round_out;
+  int x_blocked;       // x stored blocked by channel quads (tma::input_map); else channels-last
+  int y_blocked;       // y and skip stored blocked by channel quads; else channels-last
 };
 
 template <int MODE, int CIN, int COUT>
@@ -158,8 +160,11 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
             const int wc = MODE == MODE_S2 ? 2 * w0 - 1 + par
                            : MODE == MODE_T ? w0 : 2 * w0 - 2 + par;
             const int hc = MODE == MODE_S2 ? 2 * h0 - 1 : MODE == MODE_T ? h0 : 2 * h0 - 2;
-            tma_load_5d(dst + pl * C::kPlaneBytes, &xmap, bar_full + 8 * slot, 4 * q, wc,
-                        hc, s_first + it, b);
+            const tma::Coords5 k = tma::brick_coords(MODE != MODE_P5 && p.x_blocked,
+                                                     MODE == MODE_T ? 1 : 2, C::CQ,
+                                                     q, wc, hc, s_first + it, b);
+            tma_load_5d(dst + pl * C::kPlaneBytes, &xmap, bar_full + 8 * slot, k.c[0], k.c[1],
+                        k.c[2], k.c[3], k.c[4]);
           }
         }
       }
@@ -215,7 +220,9 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
 
       // stores two adjacent channels (c, c+1) of output voxel (od, oh, ow)
       auto store2 = [&](int od, int oh, int ow, int c, float a0, float a1, bool has_skip) {
-        const size_t o = ((((size_t)b * p.Do + od) * p.Ho + oh) * p.Wo + ow) * p.Cout + co_base + c;
+        const size_t o =
+            tma::vol_offset(MODE != MODE_P5 && p.y_blocked, b, od, oh, ow, co_base + c, p.Do, p.Ho,
+                            p.Wo, p.Cout);
         float v0 = fmaf(a0, s_param[c], s_param[32 + c]);
         float v1 = fmaf(a1, s_param[c + 1], s_param[32 + c + 1]);
         v0 = v0 >= 0.f ? v0 : v0 * p.slope;
@@ -238,8 +245,63 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
           if (c < COUT && mh < p.Ho && mw < p.Wo) store2(od, mh, mw, c, a0, a1, false);
         });
       };
+      // T, blocked output, COUT >= 16: the output voxels 2mw and 2mw+1 of one row come from the
+      // parity classes (ph, 0) and (ph, 1), which this thread holds for the same channel pair
+      // (c, c+1) (class columns cls*COUT + c).  Lanes l and l^1 hold the pairs c and c^2 of one
+      // channel quad: they swap one class each, so that the even lane stores the whole quad of
+      // voxel 2mw and the odd lane that of 2mw+1 -- one 32-byte sector per lane pair, not two
+      // halves in different instructions.  Measured on conv9 (COUT = 16) this is 15-20 % faster
+      // than the per-pair stores; on conv11 (COUT = 8) it is 20 % slower, so COUT = 8 (conv11,
+      // conv7's 8-channel chunks) keeps the per-pair stores of store2.
+      auto store_t_blocked = [&](const float* src, int od) {
+        const bool odd = lane & 1;
+        // element (quad cq of this CTA's chunk, output voxel (od, oh, ow)) at
+        // yoff + cq * qstr + (oh * Wo + ow) * 4: 64-bit arithmetic once per slice
+        const size_t qstr = (size_t)p.Do * p.Ho * p.Wo * 4;
+        const size_t yoff = ((size_t)b * (p.Cout / 4) + co_base / 4) * qstr +
+                            (size_t)od * p.Ho * p.Wo * 4;
+#pragma unroll
+        for (int ph = 0; ph < 2; ++ph) {
+#pragma unroll
+          for (int jj = 0; jj < COUT / 8; ++jj) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int i0 = 4 * (2 * ph * (COUT / 8) + jj) + 2 * h;   // class (ph, 0)
+              const int i1 = i0 + COUT / 2;                             // class (ph, 1)
+              const int c = 8 * jj + 2 * (lane & 3);
+              float e[4] = {src[i0], src[i0 + 1], src[i1], src[i1 + 1]};
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const float v = fmaf(e[k], s_param[c + (k & 1)], s_param[32 + c + (k & 1)]);
+                e[k] = v >= 0.f ? v : v * p.slope;
+              }
+              const float s0 = __shfl_xor_sync(0xffffffffu, odd ? e[0] : e[2], 1);
+              const float s1 = __shfl_xor_sync(0xffffffffu, odd ? e[1] : e[3], 1);
+              float4 v = odd ? make_float4(s0, s1, e[2], e[3]) : make_float4(e[0], e[1], s0, s1);
+              const int m = row0 + 16 * wl + (lane >> 2) + 8 * h;
+              const int mh = h0 + (m >> 3), mw = w0 + (m & 7);
+              if (mh >= p.Hi || mw >= p.Wi) continue;
+              const size_t o = yoff + (c >> 2) * qstr +
+                               (uint32_t)(((2 * mh + ph) * p.Wo + 2 * mw + (odd ? 1 : 0)) * 4);
+              if (p.skip) {
+                const float4 s4 = __ldg(reinterpret_cast<const float4*>(p.skip + o));
+                v.x += s4.x; v.y += s4.y; v.z += s4.z; v.w += s4.w;
+              }
+              if (p.round_out) {
+                v.x = to_tf32(v.x); v.y = to_tf32(v.y); v.z = to_tf32(v.z); v.w = to_tf32(v.w);
+              }
+              *reinterpret_cast<float4*>(p.y + o) = v;
+            }
+          }
+        }
+      };
       // T: input-slice group jd: pd=0 classes from prev0, pd=1 classes from `pd1` (acc block 0)
       auto store_t = [&](const float* pd1, int jd) {
+        if (COUT >= 16 && p.y_blocked) {
+          store_t_blocked(prev0, 2 * jd);
+          store_t_blocked(pd1, 2 * jd + 1);
+          return;
+        }
         auto one = [&](int pd, int r, int col, float a0, float a1) {
           const int m = row0 + r;
           const int mh = h0 + (m >> 3), mw = w0 + (m & 7);
@@ -379,9 +441,11 @@ static int launch2(const float* x, const float* wpk, Params p, cudaStream_t st) 
   // S2: box {4, 17 traversed -> 9 loaded, 33, 1, 1} walking W with stride 2; T: {4, 9, 17}
   // P5: box {4, 19 traversed -> 10 loaded, 35, 1, 1} walking W with stride 2
   const CUtensorMap* map =
-      MODE == MODE_S2   ? tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 17, C::BR, 2)
+      MODE == MODE_S2   ? tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 17, C::BR, 2,
+                                         p.x_blocked)
       : MODE == MODE_P5 ? tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 19, C::BR, 2)
-                        : tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, C::BW, C::BR, 1);
+                        : tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, C::BW, C::BR, 1,
+                                         p.x_blocked);
   if (!map) return -2;
   const int per_sm = tma::resident_per_sm(kfn, kConvThreads, C::kTotal);
   const int Dm = MODE == MODE_T ? p.Di : p.Do;
@@ -419,20 +483,27 @@ static int launch2(const float* x, const float* wpk, Params p, cudaStream_t st) 
 
 }  // namespace tma2
 
+// CASMVS_TMA2 (default 3): bit 0 enables the stride-2 layers, bit 1 the transposed ones.
+int conv3d_tma2_modes() {
+  static const int modes = [] {
+    const char* e = getenv("CASMVS_TMA2");
+    return e ? atoi(e) : 3;
+  }();
+  return modes;
+}
+
 // Returns 0 when handled, 1 when the layer shape is left to the other kernels.
 int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
                 float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-                int w, int kind, int stride, int precision, cudaStream_t st) {
-  static int enabled = -1;
-  if (enabled < 0) {
-    const char* e = getenv("CASMVS_TMA2");
-    enabled = e ? atoi(e) : 3;                      // bit 0: stride-2, bit 1: transposed
-  }
+                int w, int kind, int stride, int precision, int layout, cudaStream_t st) {
+  const int enabled = conv3d_tma2_modes();
   if (!enabled || precision != CASMVS_TF32) return 1;
   if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) return 1;
   tma2::Params p;
   p.scale = scale; p.shift = shift; p.skip = skip; p.y = y;
   p.slope = slope; p.B = B; p.Di = D; p.Hi = h; p.Wi = w; p.Cout = Cout; p.round_out = 1;
+  p.x_blocked = (layout & kLayoutXBlocked) ? 1 : 0;
+  p.y_blocked = (layout & kLayoutYBlocked) ? 1 : 0;
   if (kind == CASMVS_CONV && stride == 2 && (enabled & 1)) {
     if (skip) return 1;
     p.Do = (D - 1) / 2 + 1; p.Ho = (h - 1) / 2 + 1; p.Wo = (w - 1) / 2 + 1;
@@ -466,6 +537,7 @@ extern "C" int casmvs_conv2d_5x5s2_fwd(const float* x, const float* w, const flo
   p.scale = nullptr; p.shift = shift; p.skip = nullptr; p.y = y; p.slope = slope;
   p.B = 1; p.Di = N; p.Hi = H; p.Wi = W; p.Do = N; p.Ho = (H - 1) / 2 + 1; p.Wo = (W - 1) / 2 + 1;
   p.Cout = Cout; p.round_out = round_tf32 ? 1 : 0;
+  p.x_blocked = p.y_blocked = 0;
   cudaStream_t st = as_stream(stream);
   if (Cin == 8 && Cout == 16) return tma2::launch2<tma2::MODE_P5, 8, 16>(x, w, p, st);
   if (Cin == 16 && Cout == 32) return tma2::launch2<tma2::MODE_P5, 16, 32>(x, w, p, st);

@@ -42,6 +42,12 @@ __device__ __forceinline__ void stg256(float* p, const u64 (&v)[4]) {
   asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
   asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p + 4), "l"(v[2]), "l"(v[3]) : "memory");
 }
+// The same 8 channels as two channel quads qstride floats apart: 4 for a channels-last volume,
+// D*h*w*4 for one blocked by channel quads (B, C/4, D, h, w, 4).
+__device__ __forceinline__ void stg256q(float* p, size_t qstride, const u64 (&v)[4]) {
+  asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
+  asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p + qstride), "l"(v[2]), "l"(v[3]) : "memory");
+}
 
 __device__ __forceinline__ float round_tf32_f(float x) {
   uint32_t r; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x)); return __uint_as_float(r);

@@ -79,8 +79,33 @@ inline cudaError_t launch_pdl(bool allow, Kernel kfn, dim3 grid, int threads, si
 // (box_w counts traversed positions, so ceil(box_w / 2) voxels are loaded): the even / odd
 // column planes of the stride-2 convolutions.  Memoised by (pointer, shape, box); null +
 // casmvs error when the driver entry point is missing or the encode fails.  (conv3d_tma.cu)
+//
+// blocked = true: x is stored blocked by channel quads, (B, C/4, D, H, W, 4) fp32 (CB must be
+// 4), so a row of box_w voxels of one quad is 16 box_w contiguous bytes.  The map writes the
+// same [box_h][box_w][4] brick to shared memory as the channels-last one; only the load
+// coordinates differ (brick_coords).
 const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, int CB, int box_w,
-                             int box_h, int stride_w = 1);
+                             int box_h, int stride_w = 1, bool blocked = false);
+
+// Load coordinates of the brick of channel quad q whose first voxel is (w, h, d) of batch item
+// b, for the map input_map built (cq = C/4).  Blocked, stride 1: {4w, h, d, q, b}; blocked,
+// stride 2: {0, w, h, d, b cq + q}; channels-last: {4q, w, h, d, b}.
+struct Coords5 { int c[5]; };
+__host__ __device__ __forceinline__ Coords5 brick_coords(bool blocked, int stride_w, int cq, int q,
+                                                         int w, int h, int d, int b) {
+  if (!blocked) return {{4 * q, w, h, d, b}};
+  if (stride_w == 1) return {{4 * w, h, d, q, b}};
+  return {{0, w, h, d, b * cq + q}};
+}
+
+// Element offset of channel c of voxel (b, d, h, w) in a (B, D, H, W, C) volume stored
+// channels-last or blocked by channel quads (C % 4 == 0 when blocked).  Channels c and c + 1
+// with c even are adjacent in both layouts.
+__host__ __device__ __forceinline__ size_t vol_offset(bool blocked, int b, int d, int h, int w,
+                                                      int c, int D, int H, int W, int C) {
+  if (!blocked) return ((((size_t)b * D + d) * H + h) * W + w) * C + c;
+  return (((((size_t)b * (C >> 2) + (c >> 2)) * D + d) * H + h) * W + w) * 4 + (c & 3);
+}
 
 // Generic fp32 tiled map (rank <= 5, unit element strides, zero fill out of bounds); dims /
 // box innermost first, strides_bytes for dims 1..rank-1.  0 on success.  (conv3d_tma.cu)

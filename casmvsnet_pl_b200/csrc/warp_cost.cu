@@ -496,7 +496,8 @@ int g_k1_dchunk = 0;  // CASMVS_K1_DCHUNK overrides the depth-chunk heuristic
 
 // warp_cost_smem.cu
 int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
-                  int V, int C, int D, int h, int w, int num_groups, int rnd, cudaStream_t st);
+                  int V, int C, int D, int h, int w, int num_groups, int rnd, int blocked,
+                  cudaStream_t st);
 
 template <int NSRC, int CT>
 static void launch_k1(bool gwc, bool nhwc, dim3 grd, cudaStream_t st, const float* f,
@@ -588,7 +589,7 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   if (nhwc) {
     // TMA-staged generation (warp_cost_smem.cu): 0 = handled, 1 = shape left to the gather kernels
     const Hyp hyp{depth_values, nullptr, nullptr, nullptr, 0.f, 0.f};
-    const int rc = warp_var_smem(f, proj, hyp, cost, B, V, C, D, h, w, num_groups, rnd, st);
+    const int rc = warp_var_smem(f, proj, hyp, cost, B, V, C, D, h, w, num_groups, rnd, 0, st);
     if (rc <= 0) return rc;
   }
   if (!gwc && nhwc && (V == 3 || V == 2) && (C == 8 || C == 16 || C == 32)) {
@@ -661,9 +662,11 @@ extern "C" int casmvs_warp_cost_ladder_fwd(const float* feats, const float* proj
                  "warp_cost_ladder: bad dims (h,w >= 2)");
   CASMVS_REQUIRE((size_t)h * w * C < (1u << 31), "warp_cost_ladder: view too large");
   if (B == 0) return 0;
+  const int blocked = (round_tf32 & CASMVS_BLOCKED) ? 1 : 0;
+  const int rnd = (round_tf32 & ~CASMVS_BLOCKED) ? 1 : 0;
   const Hyp hyp{nullptr, first_map, first_b, step_b, first, step};
-  const int rc = warp_var_smem(feats, proj, hyp, cost, B, V, C, D, h, w, num_groups,
-                               round_tf32 ? 1 : 0, as_stream(stream));
+  const int rc = warp_var_smem(feats, proj, hyp, cost, B, V, C, D, h, w, num_groups, rnd, blocked,
+                               as_stream(stream));
   if (rc == 1) {
     set_error("warp_cost_ladder: shape not covered by the staged kernel (V-1 in {1,2}, C in "
               "{8,16,32}, groups 1 or 8, channels-last features): materialise the hypotheses and "

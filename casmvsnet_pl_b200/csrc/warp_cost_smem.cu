@@ -89,7 +89,11 @@ __device__ __forceinline__ TexP<CP> ldg_texp(const float* p) {
 
 // NSRC source views, C channels, TW x TH pixel tile.  Every plane loads its 2x2 windows (the
 // plane-group kernel below re-uses them); variance or 8-group correlation epilogue.
-template <int NSRC, int C, int TW, int TH, int MINB, bool GWC = false, int CP = 8>
+// BLOCKED: the cost volume is stored blocked by channel quads (B, COUT/4, D, h, w, 4) instead of
+// channels-last.  A template parameter: as a run-time value it cost the channels-last kernels
+// about 5 % of their rate.
+template <int NSRC, int C, int TW, int TH, int MINB, bool GWC = false, int CP = 8,
+          bool BLOCKED = false>
 __global__ void __launch_bounds__(TW* TH*(C / CP), MINB)
 warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __restrict__ feats,
                      const float* __restrict__ proj, const Hyp hyp,
@@ -142,7 +146,13 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
   const int d_begin = blockIdx.z * dchunk;
   const int d_end = min(D, d_begin + dchunk);
   const HypPix hp(hyp, b, D, (size_t)hw, pix);
-  float* optr = cost + ((size_t)(b * D + d_begin) * hw + pix) * COUT + (GWC ? sub * NG : c0);
+  // output: channels-last, or blocked by channel quads (B, COUT/4, D, h, w, 4)
+  const int co = GWC ? sub * NG : c0;
+  const size_t pstr = BLOCKED ? (size_t)hw * 4 : (size_t)hw * COUT;      // next plane
+  const size_t qstr = BLOCKED ? (size_t)D * hw * 4 : 4;                 // next channel quad
+  float* optr = cost + (BLOCKED ? (((size_t)b * (COUT / 4) + co / 4) * D + d_begin) * hw * 4 +
+                                      (size_t)pix * 4 + (co & 3)
+                                : ((size_t)(b * D + d_begin) * hw + pix) * COUT + co);
   const int row_b = BW * TEXB;
 
   uint32_t phase = 0;
@@ -300,14 +310,14 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
         if (active) {
           if constexpr (NG == 8) {
             u64 ov[4] = {pk2(o[0], o[1]), pk2(o[2], o[3]), pk2(o[4], o[5]), pk2(o[6], o[7])};
-            stg256(optr, ov);
+            stg256q(optr, qstr, ov);
           } else if constexpr (NG == 4) {
             st4(optr, make_float4(o[0], o[1], o[2], o[3]));
           } else {
             *reinterpret_cast<float2*>(optr) = make_float2(o[0], o[1]);
           }
         }
-        optr += (size_t)hw * COUT;
+        optr += pstr;
         continue;
       }
       // var = Q/V - (S/V)^2   (mvsnet.py:166-168)
@@ -329,10 +339,10 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
 #pragma unroll
         for (int hh = 0; hh < CP / 8; ++hh) {
           const u64 oo[4] = {o[4 * hh], o[4 * hh + 1], o[4 * hh + 2], o[4 * hh + 3]};
-          stg256(optr + 8 * hh, oo);
+          stg256q(optr + 2 * hh * qstr, qstr, oo);
         }
       }
-      optr += (size_t)hw * C;
+      optr += pstr;
     }
     d0 += n;
   }
@@ -348,7 +358,7 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
 // persists between the views is one blended value per (plane, channel) -- 8 registers per plane.
 // 2 source views, variance cost.  out = (ref^2 + r1^2 + r2^2)/3 - ((ref + r1 + r2)/3)^2, summed
 // in the order of the kernel above (bit-identical).
-template <int C, int TW, int TH, int PG, int MINB>
+template <int C, int TW, int TH, int PG, int MINB, bool BLOCKED>
 __global__ void __launch_bounds__(TW* TH*(C / kCPT), MINB)
 warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* __restrict__ feats,
                         const float* __restrict__ proj, const Hyp hyp, float* __restrict__ cost,
@@ -394,7 +404,12 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
   const int d_begin = blockIdx.z * dchunk;
   const int d_end = min(D, d_begin + dchunk);
   const HypPix hp(hyp, b, D, (size_t)hw, pix);
-  float* optr = cost + ((size_t)(b * D + d_begin) * hw + pix) * C + c0;
+  // output: channels-last, or blocked by channel quads (B, C/4, D, h, w, 4)
+  const size_t pstr = BLOCKED ? (size_t)hw * 4 : (size_t)hw * C;        // next plane
+  const size_t qstr = BLOCKED ? (size_t)D * hw * 4 : 4;                 // next channel quad
+  float* optr = cost + (BLOCKED ? (((size_t)b * (C / 4) + c0 / 4) * D + d_begin) * hw * 4 +
+                                      (size_t)pix * 4
+                                : ((size_t)(b * D + d_begin) * hw + pix) * C + c0);
   const int row_b = BW * TEXB;
   // a row pitch that is a multiple of 1024 B leaves the swizzle bits of an address unchanged:
   // the second window row is then the first one + row_b (launch_pg picks BW accordingly)
@@ -549,13 +564,13 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
                 o[k] = pk2(round_tf32_f(lo), round_tf32_f(hi));
               }
             }
-            if (active) stg256(optr + (size_t)p * hw * C, o);
+            if (active) stg256q(optr + p * pstr, qstr, o);
           }
         }
       }
-      optr += (size_t)PG * hw * C;
+      optr += PG * pstr;
     }
-    optr -= (size_t)(((n + PG - 1) / PG) * PG - n) * hw * C;      // a short last group advanced too far
+    optr -= (((n + PG - 1) / PG) * PG - n) * pstr;      // a short last group advanced too far
     d0 += n;
   }
 }
@@ -595,7 +610,7 @@ static int env_int(const char* name, int dflt) {
 
 template <int NSRC, int C, int TW, int TH, int MINB, bool GWC = false, int CP = 8>
 static int launch(const float* feats, const float* proj, const Hyp& dv, float* cost, int B, int D,
-                  int h, int w, int rnd, cudaStream_t st) {
+                  int h, int w, int rnd, int blocked, cudaStream_t st) {
   constexpr int NT = TW * TH * (C / CP);
   // box = tile + margins: sweep of the depth run + scale/rotation of the view + the 2x2 window
   static const int mx = env_int("CASMVS_K1_MARGIN_X", NSRC <= 2 ? 16 : 8);
@@ -604,9 +619,10 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   const int BW = TW + mx, BH = TH + my;
   const int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
   const size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
-  auto kfn = warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, CP>;
-  static std::atomic<bool> attr_set[kMaxDevices];
-  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set, "warp_cost")) return rc;
+  auto kfn = blocked ? warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, CP, true>
+                     : warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, CP, false>;
+  static std::atomic<bool> attr_set[2][kMaxDevices];
+  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[blocked ? 1 : 0], "warp_cost")) return rc;
   if (smem > 200 * 1024) return 1;
   CUtensorMap map;
   if (!feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return -2;
@@ -625,7 +641,7 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
 
 template <int C, int TW, int TH, int PG, int MINB>
 static int launch_pg(const float* feats, const float* proj, const Hyp& dv, float* cost, int B, int D,
-                     int h, int w, int rnd, cudaStream_t st) {
+                     int h, int w, int rnd, int blocked, cudaStream_t st) {
   constexpr int NSRC = 2, NT = TW * TH * (C / kCPT);
   static const int mx = env_int("CASMVS_K1_MARGIN_X", 16);
   static const int my = env_int("CASMVS_K1_MARGIN_Y", 4);
@@ -635,9 +651,10 @@ static int launch_pg(const float* feats, const float* proj, const Hyp& dv, float
   const int BW = (TW + mx + wq - 1) / wq * wq, BH = TH + my;
   const int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
   const size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
-  auto kfn = warp_var_smem_pg_kernel<C, TW, TH, PG, MINB>;
-  static std::atomic<bool> attr_set[kMaxDevices];
-  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set, "warp_cost")) return rc;
+  auto kfn = blocked ? warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, true>
+                     : warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, false>;
+  static std::atomic<bool> attr_set[2][kMaxDevices];
+  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[blocked ? 1 : 0], "warp_cost")) return rc;
   if (smem > 200 * 1024) return 1;
   CUtensorMap map;
   if (!feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return -2;
@@ -654,10 +671,12 @@ static int launch_pg(const float* feats, const float* proj, const Hyp& dv, float
 
 }  // namespace k1s
 
-// Variance cost volume, channels-last features and output.  Returns 0 when handled, 1 when the
-// shape is left to the gather kernels of warp_cost.cu, <0 on error.
+// Variance cost volume, channels-last features, channels-last or (blocked != 0) blocked output.
+// Returns 0 when handled, 1 when the shape is left to the gather kernels of warp_cost.cu, <0 on
+// error.
 int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
-                  int V, int C, int D, int h, int w, int num_groups, int rnd, cudaStream_t st) {
+                  int V, int C, int D, int h, int w, int num_groups, int rnd, int blocked,
+                  cudaStream_t st) {
   static const int enabled = k1s::env_int("CASMVS_K1_SMEM", 1);
   if (!enabled) return 1;
   if ((reinterpret_cast<uintptr_t>(feats) & 15) != 0 || B > 65535) return 1;
@@ -670,7 +689,7 @@ int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* c
     // group-wise correlation: the reference's default G = 8
     if (num_groups != 8) return 1;
 #define K1G(NS, CC, TW_, TH_, MB) \
-  if (V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB, true>(feats, proj, dv, cost, B, D, h, w, rnd, st);
+  if (V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB, true>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
     K1G(1, 8, 32, 4, 5) K1G(1, 16, 32, 2, 5) K1G(1, 32, 16, 2, 5)
     K1G(2, 8, 32, 4, 5) K1G(2, 16, 32, 2, 5) K1G(2, 32, 16, 2, 5)
     K1G(4, 8, 32, 4, 4) K1G(4, 16, 32, 4, 2) K1G(4, 32, 16, 4, 2)
@@ -687,9 +706,9 @@ int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* c
   // pressure).
   static const int variant = env_int("CASMVS_K1S_VARIANT", 16);
 #define K1S(VAR, NS, CC, TW_, TH_, MB) \
-  if (variant == VAR && V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, st);
+  if (variant == VAR && V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
 #define K1P(VAR, CC, TW_, TH_, PG_, MB) \
-  if (variant == VAR && V - 1 == 2 && C == CC) return launch_pg<CC, TW_, TH_, PG_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, st);
+  if (variant == VAR && V - 1 == 2 && C == CC) return launch_pg<CC, TW_, TH_, PG_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
   K1P(16, 8, 32, 4, 2, 4) K1P(16, 16, 32, 2, 2, 4) K1P(16, 32, 16, 2, 2, 4)
   K1P(11, 8, 32, 4, 4, 4) K1P(11, 16, 32, 2, 4, 4) K1P(11, 32, 16, 2, 4, 4)
   K1S(4, 2, 8, 32, 4, 5) K1S(4, 2, 16, 32, 2, 5) K1S(4, 2, 32, 16, 2, 5)

@@ -328,19 +328,35 @@ class CostRegNet(nn.Module):
         x = conv0 + up(self.conv11, x)
         return AG.conv3d(x, self.prob.weight, ops.CONV, 1, prec) + self.prob.bias.view(1, -1, 1, 1, 1)
 
-    def forward(self, x):
-        if torch.is_grad_enabled() and (x.requires_grad or
-                                        any(p.requires_grad for p in self.parameters())):
-            return self._forward_autograd(x)
+    def _check_inference(self):
         for bn in self._norm_modules():
             if bn.training:
                 raise ops._lib.CasMVSError("CostRegNet inference path needs .eval() (training "
                                            "runs through the autograd path: enable grad)")
             if abs(activation_slope(bn) - 0.01) > 1e-12:
                 raise ops._lib.CasMVSError("casmvs_costreg_fwd assumes LeakyReLU(0.01) norm_act")
+
+    def forward(self, x):
+        if torch.is_grad_enabled() and (x.requires_grad or
+                                        any(p.requires_grad for p in self.parameters())):
+            return self._forward_autograd(x)
+        self._check_inference()
         logits = ops.costreg(x, self.packed_params(), self.in_channels,
                              ops.PRECISIONS[self.precision])
         return logits.unsqueeze(1)                                   # (B,1,D,h,w)
+
+    def blocked_supported(self):
+        """forward_blocked applies: tf32, and the tensor-core kernels cover every layer."""
+        return self.precision == "tf32" and ops.costreg_blocked_supported(self.in_channels)
+
+    def forward_blocked(self, x):
+        """Inference in the tf32 precision from the (B,Cin/4,D,h,w,4) cost volume of
+        ops.warp_cost_ladder(blocked=True) -> logits (B,D,h,w)."""
+        self._check_inference()
+        if not self.blocked_supported():
+            raise ops._lib.CasMVSError("CostRegNet.forward_blocked needs the tf32 precision and "
+                                       "tensor-core kernels for every layer (in_channels 8, 16, 32)")
+        return ops.costreg(x, self.packed_params(), self.in_channels, ops.TF32, blocked=True)
 
 
 class CascadeMVSNet(nn.Module):
@@ -457,9 +473,12 @@ class CascadeMVSNet(nn.Module):
                 ops.is_channels_last_feats(feats_l):
             first = init_depth_min if depth_prev is None else ops.depth_first(depth_prev, D, depth_interval_l)
             lad = ops.Ladder(first, depth_interval_l, D, B, h, w, feats_l.device)
+            # the cost volume goes to CostRegNet blocked by channel quads where its tensor-core
+            # path takes that layout (DESIGN.md §2)
+            blocked = cost_reg.blocked_supported()
             cost = ops.warp_cost_ladder(feats_l, proj_mats_l, lad, self.G,
-                                        round_tf32=(cost_reg.precision == "tf32"))
-            logits = cost_reg(cost).squeeze(1)
+                                        round_tf32=(cost_reg.precision == "tf32"), blocked=blocked)
+            logits = cost_reg.forward_blocked(cost) if blocked else cost_reg(cost).squeeze(1)
             del cost
             depth, confidence, self._last_index = ops.regress_ladder(logits, lad,
                                                                      want_index=self.return_index)

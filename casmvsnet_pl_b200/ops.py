@@ -13,7 +13,7 @@ import math
 import torch
 
 from . import _lib
-from ._lib import (CONV, CONV_PLANAR, CONV_TRANSPOSE, FP32, KEEP_FP32_OUT, NCHW, NHWC, PRECISIONS, TF32,  # noqa: F401
+from ._lib import (BLOCKED, CONV, CONV_PLANAR, CONV_TRANSPOSE, FP32, KEEP_FP32_OUT, NCHW, NHWC, PRECISIONS, TF32,  # noqa: F401
                    check)
 
 _checked_devices = set()
@@ -228,14 +228,30 @@ def costreg_layer_info(cin, layer):
                 w_off=wo.value, scale_off=so.value, shift_off=ho.value)
 
 
+def costreg_blocked_supported(cin, precision=TF32):
+    """True when costreg runs blocked activations for this Cin and precision, and so accepts
+    costreg(blocked=True) (the tensor-core kernels cover every layer)."""
+    return bool(_lib.load().casmvs_costreg_blocked_supported(cin, precision))
+
+
 @_on_tensor_device
-def costreg(x, params, cin, precision=FP32):
-    """Whole CostRegNet.  x logical (B,Cin,D,h,w) -> logits (B,D,h,w)."""
+def costreg(x, params, cin, precision=FP32, blocked=False):
+    """Whole CostRegNet.  x logical (B,Cin,D,h,w) -> logits (B,D,h,w).  blocked=True (TF32
+    only, where costreg_blocked_supported): x is a contiguous (B,Cin/4,D,h,w,4) tensor, e.g. from
+    warp_cost_ladder(blocked=True)."""
     _require_cuda(x, params)
     _no_grad_only(x)
-    xs = volume_storage(x)
-    B, D, h, w, c = xs.shape
-    assert c == cin
+    if blocked:
+        if x.dim() != 6 or x.shape[-1] != 4 or x.shape[1] * 4 != cin or not x.is_contiguous():
+            raise ValueError(f"costreg: blocked input must be a contiguous (B,{cin // 4},D,h,w,4) "
+                             f"tensor, got {tuple(x.shape)}")
+        xs = x
+        B, _, D, h, w, _ = xs.shape
+        precision |= BLOCKED
+    else:
+        xs = volume_storage(x)
+        B, D, h, w, c = xs.shape
+        assert c == cin
     lib = _lib.load()
     ws_bytes = lib.casmvs_costreg_workspace_bytes(B, cin, D, h, w)
     ws = torch.empty(ws_bytes // 4, device=x.device, dtype=torch.float32)
@@ -360,20 +376,24 @@ def ladder_supported(V, C, num_groups):
 
 
 @_on_tensor_device
-def warp_cost_ladder(feats, proj_mats, ladder, num_groups=1, round_tf32=False):
-    """warp_cost with the hypotheses given as a Ladder; feats must be channels-last."""
+def warp_cost_ladder(feats, proj_mats, ladder, num_groups=1, round_tf32=False, blocked=False):
+    """warp_cost with the hypotheses given as a Ladder; feats must be channels-last.  Returns the
+    logical (B,Cout,D,h,w) channels-last volume, or with blocked=True the (B,Cout/4,D,h,w,4)
+    tensor that costreg(blocked=True) takes."""
     _require_cuda(feats, proj_mats)
     _no_grad_only(feats)
     B, V, C, h, w = feats.shape
     assert is_channels_last_feats(feats) and (ladder.B, ladder.h, ladder.w) == (B, h, w)
     cout = C if num_groups == 1 else num_groups
-    out = torch.empty(B, ladder.D, h, w, cout, device=feats.device, dtype=torch.float32)
+    shape = (B, cout // 4, ladder.D, h, w, 4) if blocked else (B, ladder.D, h, w, cout)
+    out = torch.empty(shape, device=feats.device, dtype=torch.float32)
     fm, fb, f, sb, s = ladder._args()
     check(_lib.load().casmvs_warp_cost_ladder_fwd(_ptr(feats), _ptr(proj_mats.contiguous()), _ptr(fm),
                                                   _ptr(fb), f, _ptr(sb), s, _ptr(out),
-                                                  1 if round_tf32 else 0, B, V, C, ladder.D, h, w,
-                                                  num_groups, _stream()), "warp_cost_ladder")
-    return as_volume_view(out)
+                                                  (1 if round_tf32 else 0) | (BLOCKED if blocked else 0),
+                                                  B, V, C, ladder.D, h, w, num_groups, _stream()),
+          "warp_cost_ladder")
+    return out if blocked else as_volume_view(out)
 
 
 @_on_tensor_device

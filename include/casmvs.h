@@ -57,6 +57,13 @@ enum casmvs_precision {
  * keep the fp32 accumulator). */
 #define CASMVS_KEEP_FP32_OUT 256
 
+/* Blocked volume layout (B, C/4, D, h, w, 4): channel quads outermost, so one quad of a row of
+ * voxels is contiguous.  The CostRegNet driver stores its TF32-mode activations this way.
+ * OR-ed into casmvs_costreg_fwd's precision: x is blocked instead of channels-last (where
+ * casmvs_costreg_blocked_supported).
+ * OR-ed into casmvs_warp_cost_ladder_fwd's round_tf32: write the cost volume blocked. */
+#define CASMVS_BLOCKED 512
+
 enum casmvs_conv_kind {
   CASMVS_CONV = 0,           /* Conv3d(k=3, pad=1, stride 1|2)   modules.py:26      */
   CASMVS_CONV_TRANSPOSE = 1, /* ConvTranspose3d(k=3,s=2,p=1,op=1) mvsnet.py:75,80,85 */
@@ -150,7 +157,11 @@ int casmvs_conv3d_fwd(const float* x, const float* w_packed, const float* scale,
 
 /* Whole CostRegNet (models/mvsnet.py:91-104) in one call.  `params` is a
  * device array produced by casmvs_costreg_pack (see casmvs_costreg_param_floats).
- * x (B,D,h,w,Cin) -> logits (B,D,h,w) ; D,h,w divisible by 8.                */
+ * x (B,D,h,w,Cin) -> logits (B,D,h,w) ; D,h,w divisible by 8.
+ * precision | CASMVS_BLOCKED: x is (B,Cin/4,D,h,w,4) instead, e.g. the cost volume of
+ * casmvs_warp_cost_ladder_fwd with CASMVS_BLOCKED; only where
+ * casmvs_costreg_blocked_supported(Cin, precision), an error otherwise.  There the activations
+ * in the workspace are blocked as well; the workspace size does not depend on it.          */
 size_t casmvs_costreg_param_floats(int Cin);
 /* Layout of the params blob: layers 0..10 = conv0..conv6, conv7, conv9, conv11,
  * prob; each is packed weights [27][cin][cout], scale[cout], shift[cout]
@@ -159,6 +170,11 @@ size_t casmvs_costreg_param_floats(int Cin);
 int casmvs_costreg_layer_info(int Cin, int layer, int* cin, int* cout, int* kind, int* stride,
                               size_t* w_off, size_t* scale_off, size_t* shift_off);
 size_t casmvs_costreg_workspace_bytes(int B, int Cin, int D, int h, int w);
+/* 1 when casmvs_costreg_fwd stores its activations blocked for this Cin and precision and so
+ * accepts a CASMVS_BLOCKED input (TF32, Cin in {8,16,32}, tensor-core kernels not switched off
+ * by CASMVS_TMA / CASMVS_TMA2; x and workspace must then be 16-byte aligned), else 0.  The
+ * other cases run channels-last, layers no tensor-core kernel covers on the CUDA cores. */
+int casmvs_costreg_blocked_supported(int Cin, int precision);
 int casmvs_costreg_fwd(const float* x, const float* params, float* logits,
                        int B, int Cin, int D, int h, int w, int precision,
                        void* workspace, size_t workspace_bytes, void* stream);
@@ -202,7 +218,9 @@ int casmvs_uniform_hypotheses_fwd(float depth_min, float step, const float* dept
  * scalar `first`; step: `step_b` (B) else the scalar `step`.
  * casmvs_depth_first_fwd writes only the first rung (B,h,w) of casmvs_depth_hypotheses_fwd.
  * casmvs_warp_cost_ladder_fwd: channels-last features and cost volume; shapes of the staged
- * kernel only (V-1 in {1,2}, C in {8,16,32}, num_groups 1 or 8), error otherwise. */
+ * kernel only (V-1 in {1,2}, C in {8,16,32}, num_groups 1 or 8), error otherwise.
+ * round_tf32: nonzero = store the cost TF32-rounded; | CASMVS_BLOCKED = store it blocked,
+ * (B,Cout/4,D,h,w,4), for casmvs_costreg_fwd with CASMVS_BLOCKED. */
 int casmvs_depth_first_fwd(const float* cur, int upsample, float half_range, float step,
                            const float* step_dev, float* out, int B, int D, int h, int w,
                            void* stream);
