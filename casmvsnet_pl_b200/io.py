@@ -226,6 +226,145 @@ def normalize_images(images_u8, device=None, out=None):
     return out
 
 
+_PIL_PRECISION_BITS = 22        # Pillow Resample.c PRECISION_BITS (8-bit images)
+_CV_COEF_SCALE = 2048           # OpenCV INTER_RESIZE_COEF_SCALE (1 << 11)
+
+
+def pil_bilinear_coeffs(in_size, out_size):
+    """Pillow's BILINEAR coefficients along one axis of `in_size` -> `out_size` pixels:
+    bounds (out,2) int32 = (first tap, taps), coef (out,ksize) int32.  In double: support =
+    max(scale, 1), triangle filter, normalised by the sequential sum; then rounded half away from
+    zero to 22 fractional bits (Resample.c precompute_coeffs / normalize_coeffs_8bpc)."""
+    scale = in_size / out_size
+    filterscale = max(scale, 1.0)
+    support = 1.0 * filterscale
+    ss = 1.0 / filterscale
+    ksize = int(np.ceil(support)) * 2 + 1
+    bounds = np.zeros((out_size, 2), np.int32)
+    coef = np.zeros((out_size, ksize), np.int32)
+    for xx in range(out_size):
+        center = (xx + 0.5) * scale
+        xmin = max(int(center - support + 0.5), 0)
+        n = min(int(center + support + 0.5), in_size) - xmin
+        w = [max(0.0, 1.0 - abs((x + xmin - center + 0.5) * ss)) for x in range(n)]
+        total = 0.0
+        for v in w:
+            total += v
+        for x, v in enumerate(w):
+            v = v / total if total != 0.0 else v
+            coef[xx, x] = int(0.5 + v * (1 << _PIL_PRECISION_BITS)) if v >= 0 else \
+                int(-0.5 + v * (1 << _PIL_PRECISION_BITS))
+        bounds[xx] = (xmin, n)
+    return bounds, coef
+
+
+def cv2_linear_table(in_size, out_size, clamp):
+    """OpenCV INTER_LINEAR taps along one axis -> (out,4) int32 (i0, i1, w0, w1).  Source
+    position fx = (float)((d + 0.5) * (1 / (out/in)) - 0.5), split into floor and fraction in
+    float32, weights saturate_cast<short>((1 - f, f) * 2048) (round half even).  Along x
+    (`clamp`) positions left of 0 or at/right of the last pixel take that pixel alone; along y
+    the weights are kept and only the row indices are clipped (resize.cpp)."""
+    scale = 1.0 / (out_size / in_size)
+    f = ((np.arange(out_size, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
+    s = np.floor(f).astype(np.int64)
+    f = (f - s.astype(np.float32)).astype(np.float32)
+    if clamp:
+        lo, hi = s < 0, s >= in_size - 1
+        f[lo | hi] = 0
+        s[lo], s[hi] = 0, in_size - 1
+    w1 = np.rint(f * np.float32(_CV_COEF_SCALE)).astype(np.int64)
+    w0 = np.rint((np.float32(1) - f) * np.float32(_CV_COEF_SCALE)).astype(np.int64)
+    return np.stack([np.clip(s, 0, in_size - 1), np.clip(s + 1, 0, in_size - 1), w0, w1],
+                    1).astype(np.int32)
+
+
+_TABLES = {}
+
+
+def _device_tables(kind, hw, ohw, device):
+    key = (kind, hw, ohw, str(device))
+    if key not in _TABLES:
+        (H, W), (OH, OW) = hw, ohw
+        if kind == "pil":
+            xb, xc = pil_bilinear_coeffs(W, OW)
+            yb, yc = pil_bilinear_coeffs(H, OH)
+            t = [torch.from_numpy(a).to(device) for a in (xb, xc, yb, yc)]
+        else:
+            t = [torch.from_numpy(cv2_linear_table(W, OW, True)).to(device),
+                 torch.from_numpy(cv2_linear_table(H, OH, False)).to(device)]
+        _TABLES[key] = t
+    return _TABLES[key]
+
+
+def _check_u8_images(images, what):
+    from . import _lib
+    if not torch.is_tensor(images) or not images.is_cuda or images.dtype != torch.uint8 \
+            or images.dim() != 4 or images.shape[-1] != 3:
+        raise _lib.CasMVSError(f"{what} expects a uint8 (N,H,W,3) CUDA tensor")
+    return images.contiguous()
+
+
+def resize_u8_pil(images, wh, out=None):
+    """Pillow Image.resize(wh, Image.BILINEAR) of uint8 (N,H,W,3) CUDA images ->
+    (N,h,w,3) uint8, byte-identical (casmvs_resize_u8_pil_fwd)."""
+    import ctypes
+
+    from . import _lib
+    t = _check_u8_images(images, "resize_u8_pil")
+    N, H, W, _ = t.shape
+    OW, OH = int(wh[0]), int(wh[1])
+    if OW <= 0 or OH <= 0:
+        raise _lib.CasMVSError(f"resize_u8_pil: bad size {tuple(wh)}")
+    if out is None:
+        out = torch.empty(N, OH, OW, 3, device=t.device, dtype=torch.uint8)
+    xb, xc, yb, yc = _device_tables("pil", (H, W), (OH, OW), t.device)
+    tmp = torch.empty(N, H, OW, 3, device=t.device, dtype=torch.uint8) \
+        if OW != W and OH != H else None
+    p = lambda x: ctypes.c_void_p(x.data_ptr() if x is not None else 0)   # noqa: E731
+    with torch.cuda.device(t.device):
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        _lib.check(_lib.load().casmvs_resize_u8_pil_fwd(
+            p(t), p(out), p(tmp), N, H, W, OH, OW, p(xb), p(xc), xc.shape[1], p(yb), p(yc),
+            yc.shape[1], st), "resize_u8_pil")
+    return out
+
+
+def resize_u8_linear(images, wh, out=None):
+    """cv2.resize(img, wh, interpolation=cv2.INTER_LINEAR) of uint8 (N,H,W,3) CUDA images ->
+    (N,h,w,3) uint8, byte-identical (casmvs_resize_u8_linear_fwd)."""
+    import ctypes
+
+    from . import _lib
+    t = _check_u8_images(images, "resize_u8_linear")
+    N, H, W, _ = t.shape
+    OW, OH = int(wh[0]), int(wh[1])
+    if OW <= 0 or OH <= 0:
+        raise _lib.CasMVSError(f"resize_u8_linear: bad size {tuple(wh)}")
+    if out is None:
+        out = torch.empty(N, OH, OW, 3, device=t.device, dtype=torch.uint8)
+    xt, yt = _device_tables("cv2", (H, W), (OH, OW), t.device)
+    with torch.cuda.device(t.device):
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        _lib.check(_lib.load().casmvs_resize_u8_linear_fwd(
+            ctypes.c_void_p(t.data_ptr()), ctypes.c_void_p(out.data_ptr()), N, H, W, OH, OW,
+            ctypes.c_void_p(xt.data_ptr()), ctypes.c_void_p(yt.data_ptr()), st),
+            "resize_u8_linear")
+    return out
+
+
+def save_visual(depth_dir, scan, vid, depth, proba, conf):
+    """eval.py:230-239: JET-coloured depth (min over positive depths .. max, to uint8) and the
+    confidence mask proba > conf as JPEGs next to the PFMs."""
+    import cv2
+    d = os.path.join(depth_dir, scan)
+    os.makedirs(d, exist_ok=True)
+    mi = np.min(depth[depth > 0])
+    ma = np.max(depth)
+    depth = (255 * ((depth - mi) / (ma - mi + 1e-8))).astype(np.uint8)
+    cv2.imwrite(os.path.join(d, f"depth_visual_{vid:04d}.jpg"), cv2.applyColorMap(depth, cv2.COLORMAP_JET))
+    cv2.imwrite(os.path.join(d, f"proba_visual_{vid:04d}.jpg"), (255 * (proba > conf)).astype(np.uint8))
+
+
 # ------------------------------------------------------------------------------ eval loop
 def scrub(x):
     """np.nan_to_num of eval.py:225-227 (NaN -> 0; +-inf -> largest finite)."""

@@ -313,6 +313,25 @@ int casmvs_regress_bwd(const float* logits, const float* depth_values, int dv_is
 int casmvs_normalize_u8_fwd(const uint8_t* images, float* out, int N, int H, int W,
                             const float* mean3, const float* std3, void* stream);
 
+/* Resamplers of the scan readers, byte-identical to the host libraries the reference uses:
+ * images (N,H,W,3) uint8 -> out (N,OH,OW,3) uint8.  The weight tables are DEVICE int32 arrays
+ * the caller computes once per (H,W) -> (OH,OW) pair (casmvsnet_pl_b200/io.py).
+ * casmvs_resize_u8_pil_fwd: Pillow Image.resize(size, BILINEAR) (datasets/tanks.py:134-135,
+ *   blendedmvs.py:161-163, dtu.py:159-162).  Horizontal pass (skipped when OW == W) then vertical
+ *   pass (skipped when OH == H), each out = clip8(((1 << 21) + sum_k in[lo + k] * coef[k]) >> 22);
+ *   xbounds (OW,2) / ybounds (OH,2) = (lo, taps), xcoef (OW,xks) / ycoef (OH,yks) = Pillow's
+ *   22-bit coefficients.  Tables of a skipped pass may be NULL; tmp (N,H,OW,3) holds the
+ *   intermediate and is needed only when both passes run.  Same size: a device copy.
+ * casmvs_resize_u8_linear_fwd: cv2.resize(..., INTER_LINEAR) of 8-bit images (eval.py:266-268),
+ *   per channel, so BGR and RGB input give the same bytes.  xtab (OW,4) / ytab (OH,4) =
+ *   (i0, i1, w0, w1) with 11-bit weights, 16-byte aligned; h = in[i0]*w0 + in[i1]*w1 along x,
+ *   out = (((w0*(h0>>4))>>16) + ((w1*(h1>>4))>>16) + 2) >> 2 along y. */
+int casmvs_resize_u8_pil_fwd(const uint8_t* images, uint8_t* out, uint8_t* tmp, int N, int H,
+                             int W, int OH, int OW, const int* xbounds, const int* xcoef, int xks,
+                             const int* ybounds, const int* ycoef, int yks, void* stream);
+int casmvs_resize_u8_linear_fwd(const uint8_t* images, uint8_t* out, int N, int H, int W, int OH,
+                                int OW, const int* xtab, const int* ytab, void* stream);
+
 /* ---- geometric-consistency filter + refinement + back-projection (SURVEY.md 8 f-3) ------
  * One reference view of eval.py:262-318 on the device; replaces xy_ref2src / xy_src2ref /
  * check_geo_consistency (eval.py:113-182, numba + cv2.remap on the CPU).  For every reference
