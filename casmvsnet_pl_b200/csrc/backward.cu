@@ -21,7 +21,7 @@ namespace casmvs {
 
 struct TapPos { unsigned off; float w00, w01, w10, w11; };
 
-// same arithmetic as sample_view (k1_common.cuh): clamped 2x2 window + remapped weights
+// same arithmetic as gather_sample (k1_common.cuh): clamped 2x2 window + remapped weights
 __device__ __forceinline__ TapPos tap_pos(float qx, float qy, float qz, int h, int w, int C) {
   const float rz = rcp_approx(qz);
   const float u = qx * rz, v = qy * rz;

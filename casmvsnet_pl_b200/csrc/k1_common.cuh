@@ -1,5 +1,5 @@
-// Device helpers shared by the K1 kernels (warp_cost.cu: gather-from-L1 generation and the
-// generic / group-wise-correlation variants; warp_cost_smem.cu: TMA-staged generation).
+// Device helpers shared by the K1 kernels (warp_cost.cu: the gather kernel;
+// warp_cost_smem.cu: the TMA-staged kernels).
 #pragma once
 #include "common.cuh"
 
@@ -68,15 +68,31 @@ struct Window {
   Tex8 t00, t01, t10, t11;
 };
 
-// Branch-free: a sample that contributes nothing (behind the camera / fully outside
+// Bilinear blend of 8 channels, tap order nw, ne, sw, se like ATen grid_sampler_2d.  out(k, r)
+// takes channel pair k as soon as it is blended: the gather kernel accumulates it right there,
+// which keeps its register allocation (blending all four pairs first made it spill more).
+template <class Out>
+__device__ __forceinline__ void blend(const Window& win, float w00, float w01, float w10, float w11,
+                                      Out&& out) {
+  const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10), p11 = pk2(w11, w11);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    u64 a = mul2(win.t00.v[k], p00);
+    a = fma2(win.t01.v[k], p01, a);
+    a = fma2(win.t10.v[k], p10, a);
+    out(k, fma2(win.t11.v[k], p11, a));
+  }
+}
+
+// One sample of 8 channels gathered from the channels-last view at vbase (channel c0 already
+// added).  Branch-free: a sample that contributes nothing (behind the camera / fully outside
 // the source image) gets four zero weights and a clamped, always-valid address, so
 // the loop body is straight-line code and ptxas can keep the loads of all views in
 // flight at once.  CT = compile-time channel count (0: use C).
-template <int CT>
-__device__ __forceinline__ void sample_view(const float* __restrict__ vbase, float qx, float qy,
-                                            float qz, int h, int w, int C, int row_floats,
-                                            Window& win, float& w00, float& w01, float& w10,
-                                            float& w11) {
+template <int CT, class Out>
+__device__ __forceinline__ void gather_sample(const float* __restrict__ vbase, float qx, float qy,
+                                              float qz, int h, int w, int C, int row_floats,
+                                              Out&& out) {
   const float rz = rcp_approx(qz);
   const float u = qx * rz, v = qy * rz;
   const float x0f = floorf(u), y0f = floorf(v);
@@ -95,14 +111,37 @@ __device__ __forceinline__ void sample_view(const float* __restrict__ vbase, flo
   if (y0 > h - 2) { wyb = wya; wya = 0.f; }
   if (!valid) { wxa = 0.f; wxb = 0.f; }
   const int xs = min(max(x0, 0), w - 2), ys = min(max(y0, 0), h - 2);
-  w00 = wxa * wya; w01 = wxb * wya; w10 = wxa * wyb; w11 = wxb * wyb;
+  const float w00 = wxa * wya, w01 = wxb * wya, w10 = wxa * wyb, w11 = wxb * wyb;
   const int cc = CT > 0 ? CT : C;
   const unsigned off = (unsigned)(ys * row_floats + xs * cc);
   const float* p = vbase + off;
+  Window win;
   win.t00 = ldg256(p);
   win.t01 = ldg256(p + cc);
   win.t10 = ldg256(p + row_floats);
   win.t11 = ldg256(p + row_floats + cc);
+  blend(win, w00, w01, w10, w11, out);
+}
+
+// Variance cost of 8 channels from the sums S and Q of the V views: Q/V - (S/V)^2
+// (mvsnet.py:166-168), inv_v2 = (1/V, 1/V), ninv_v2 = -inv_v2.  round_tf32: the tensor-core conv
+// reads fp32 bits as tf32 by truncation; rounding here keeps the next layer's operand unbiased
+// (round-to-nearest instead of toward zero).
+__device__ __forceinline__ void variance(const u64 (&S)[4], const u64 (&Q)[4], u64 inv_v2,
+                                         u64 ninv_v2, int round_tf32, u64 (&o)[4]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const u64 m = mul2(S[k], inv_v2), mn = mul2(S[k], ninv_v2);
+    o[k] = fma2(mn, m, mul2(Q[k], inv_v2));
+  }
+  if (round_tf32) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      float lo, hi;
+      unpk2(o[k], lo, hi);
+      o[k] = pk2(round_tf32_f(lo), round_tf32_f(hi));
+    }
+  }
 }
 
 

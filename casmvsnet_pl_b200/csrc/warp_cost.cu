@@ -13,8 +13,6 @@
 // HBM model (DESIGN.md): read V*C*h*w feature floats once (they live in L2 for
 // the whole launch), read D*h*w hypotheses once, write Cout*D*h*w cost floats
 // once.  The kernel is write-bound.
-#include <stdlib.h>
-
 #include "k1_common.cuh"
 
 namespace casmvs {
@@ -163,43 +161,17 @@ warp_cost_kernel(const float* __restrict__ feats,   // (B,V,h,w,C)
           qy = fmaf(P[7], inv_d, fmaf(P[4], xf, fmaf(P[5], yf, P[6])));
           qz = fmaf(P[11], inv_d, fmaf(P[8], xf, fmaf(P[9], yf, P[10])));
         }
-        float w00, w01, w10, w11;
-        Window win;
-        sample_view<CT>(fb + (size_t)(vv + 1) * view_stride, qx, qy, qz, h, w, C, row_floats,
-                        win, w00, w01, w10, w11);
-        const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10),
-                  p11 = pk2(w11, w11);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          // tap order nw, ne, sw, se like ATen grid_sampler_2d
-          u64 r = mul2(win.t00.v[k], p00);
-          r = fma2(win.t01.v[k], p01, r);
-          r = fma2(win.t10.v[k], p10, r);
-          r = fma2(win.t11.v[k], p11, r);
-          S[k] = add2(S[k], r);
-          if (!GWC) Q[k] = fma2(r, r, Q[k]);
-        }
+        gather_sample<CT>(fb + (size_t)(vv + 1) * view_stride, qx, qy, qz, h, w, C, row_floats,
+                          [&](int k, u64 r) {
+                            S[k] = add2(S[k], r);
+                            if (!GWC) Q[k] = fma2(r, r, Q[k]);
+                          });
       }
     }
 
     if (!GWC) {
-      // var = Q/V - (S/V)^2   (mvsnet.py:166-168)
       u64 o[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const u64 m = mul2(S[k], inv_v2), mn = mul2(S[k], ninv_v2);
-        o[k] = fma2(mn, m, mul2(Q[k], inv_v2));
-      }
-      if (round_tf32) {
-        // the tensor-core conv reads fp32 bits as tf32 by truncation; rounding here keeps the
-        // next layer's operand unbiased (round-to-nearest instead of toward zero)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float lo, hi;
-          unpk2(o[k], lo, hi);
-          o[k] = pk2(round_tf32_f(lo), round_tf32_f(hi));
-        }
-      }
+      variance(S, Q, inv_v2, ninv_v2, round_tf32, o);
       if (active) {
         if (OUT_NHWC) {
           stg256(cost + ((size_t)(b * D + d) * hw + pix) * C + c0, o);
@@ -263,162 +235,6 @@ warp_cost_kernel(const float* __restrict__ feats,   // (B,V,h,w,C)
       }
     }
   }
-}
-
-// ---------------------------------------------------------------------------------------
-// Specialised hot variant: variance cost, channels-last output, compile-time C and V-1.
-// Bound analysis: the kernel is close to instruction / FP32-pipe bound as well as HBM bound:
-// 17 fp32 ops per output channel (2 views x (4 blend + 2 accumulate) + 4 variance + 1) plus
-// ~6 of per-pixel coordinate math amortised over 8 channels put the FP32-pipe floor next to
-// the HBM floor.  More warps (CPT=4) or fewer L1 requests
-// (SKIP) do not help; both options are kept for experiments (CASMVS_K1_CPT / CASMVS_K1_SKIP).
-// CPT channels per thread (4 or 8): 4 halves the register footprint (more resident warps to
-// hide the L1/L2 latency that bounds this kernel) at the price of more redundant coordinate
-// arithmetic.  SKIP: a view whose 2x2 window did not move since the previous plane keeps its
-// texels in registers (they are live anyway) and issues no loads.
-template <int CPT> struct TexN { u64 v[CPT / 2]; };
-template <int CPT>
-__device__ __forceinline__ TexN<CPT> ldg_tex(const float* p) {
-  TexN<CPT> t;
-  if constexpr (CPT == 8) {
-    asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[0]), "=l"(t.v[1]) : "l"(p));
-    asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[2]), "=l"(t.v[3]) : "l"(p + 4));
-  } else {
-    asm volatile("ld.global.nc.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[0]), "=l"(t.v[1]) : "l"(p));
-  }
-  return t;
-}
-template <int CPT>
-__device__ __forceinline__ void stg_tex(float* p, const u64 (&v)[CPT / 2]) {
-  if constexpr (CPT == 8) {
-    asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
-    asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p + 4), "l"(v[2]), "l"(v[3]) : "memory");
-  } else {
-    asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(v[0]), "l"(v[1]) : "memory");
-  }
-}
-
-template <int NSRC, int CT, int CPT, bool SKIP, int MINB>
-__global__ void __launch_bounds__(kK1Threads, MINB)
-warp_var_kernel(const float* __restrict__ feats, const float* __restrict__ proj,
-                const float* __restrict__ dv, float* __restrict__ cost, int D, int h, int w,
-                int dchunk, int round_tf32) {
-  __shared__ float s_proj[NSRC * 12];
-  constexpr int V = NSRC + 1, C = CT, NP = CPT / 2;
-  const int b = blockIdx.y;
-  for (int i = threadIdx.x; i < NSRC * 12; i += blockDim.x)
-    s_proj[i] = proj[(size_t)b * NSRC * 12 + i];
-  __syncthreads();
-  constexpr int tpp = C / CPT;
-  const int gtid = blockIdx.x * blockDim.x + threadIdx.x;
-  const int pix = gtid / tpp;
-  const int c0 = (gtid - pix * tpp) * CPT;
-  const int hw = h * w;
-  const bool active = pix < hw;
-  const int pixc = active ? pix : hw - 1;
-  const int y = pixc / w, x = pixc - y * w;
-  const float xf = (float)x, yf = (float)y;
-  const int row_floats = w * C;
-  const size_t view_stride = (size_t)hw * C;
-  const float* fb = feats + (size_t)b * V * view_stride + c0;
-
-  const TexN<CPT> ref = ldg_tex<CPT>(fb + (size_t)pixc * C);
-  float ax[NSRC], ay[NSRC], az[NSRC], tx[NSRC], ty[NSRC], tz[NSRC];
-  int cx[NSRC], cy[NSRC];
-  TexN<CPT> t00[NSRC], t01[NSRC], t10[NSRC], t11[NSRC];
-#pragma unroll
-  for (int v = 0; v < NSRC; ++v) {
-    const float* P = s_proj + v * 12;
-    ax[v] = fmaf(P[0], xf, fmaf(P[1], yf, P[2]));
-    ay[v] = fmaf(P[4], xf, fmaf(P[5], yf, P[6]));
-    az[v] = fmaf(P[8], xf, fmaf(P[9], yf, P[10]));
-    tx[v] = P[3]; ty[v] = P[7]; tz[v] = P[11];
-    cx[v] = -1; cy[v] = -1;                      // no window cached (clamped corners are >= 0)
-  }
-  const float inv_v = 1.f / (float)V;
-  const u64 inv_v2 = pk2(inv_v, inv_v), ninv_v2 = pk2(-inv_v, -inv_v);
-  const int d_begin = blockIdx.z * dchunk;
-  const int d_end = min(D, d_begin + dchunk);
-  const float* dptr = dv + (size_t)b * D * hw + pixc + (size_t)d_begin * hw;
-  float depth_next = d_begin < d_end ? __ldg(dptr) : 1.f;
-  float* optr = cost + ((size_t)(b * D + d_begin) * hw + pixc) * C + c0;
-
-  for (int d = d_begin; d < d_end; ++d) {
-    const float depth = depth_next;
-    dptr += hw;
-    if (d + 1 < d_end) depth_next = __ldg(dptr);
-    const float inv_d = rcp_approx(depth);
-    u64 S[NP], Q[NP];
-#pragma unroll
-    for (int k = 0; k < NP; ++k) { S[k] = ref.v[k]; Q[k] = mul2(ref.v[k], ref.v[k]); }
-#pragma unroll
-    for (int v = 0; v < NSRC; ++v) {
-      const float qx = fmaf(tx[v], inv_d, ax[v]);
-      const float qy = fmaf(ty[v], inv_d, ay[v]);
-      const float qz = fmaf(tz[v], inv_d, az[v]);
-      const float rz = rcp_approx(qz);
-      const float u = qx * rz, vv = qy * rz;
-      const float x0f = floorf(u), y0f = floorf(vv);
-      const int x0 = __float2int_rd(u), y0 = __float2int_rd(vv);
-      const bool valid = (qz > 1e-7f) && (unsigned)(x0 + 1) <= (unsigned)w &&
-                         (unsigned)(y0 + 1) <= (unsigned)h;
-      const float fx = u - x0f, fy = vv - y0f;
-      float wxa = 1.f - fx, wxb = fx, wya = 1.f - fy, wyb = fy;
-      if (x0 < 0) { wxa = wxb; wxb = 0.f; }
-      if (x0 > w - 2) { wxb = wxa; wxa = 0.f; }
-      if (y0 < 0) { wya = wyb; wyb = 0.f; }
-      if (y0 > h - 2) { wyb = wya; wya = 0.f; }
-      if (!valid) { wxa = 0.f; wxb = 0.f; }
-      const int xs = min(max(x0, 0), w - 2), ys = min(max(y0, 0), h - 2);
-      if (!SKIP || xs != cx[v] || ys != cy[v]) {
-        const float* p = fb + (size_t)(v + 1) * view_stride + (unsigned)(ys * row_floats + xs * C);
-        t00[v] = ldg_tex<CPT>(p);
-        t01[v] = ldg_tex<CPT>(p + C);
-        t10[v] = ldg_tex<CPT>(p + row_floats);
-        t11[v] = ldg_tex<CPT>(p + row_floats + C);
-        cx[v] = xs; cy[v] = ys;
-      }
-      const float w00 = wxa * wya, w01 = wxb * wya, w10 = wxa * wyb, w11 = wxb * wyb;
-      const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10), p11 = pk2(w11, w11);
-#pragma unroll
-      for (int k = 0; k < NP; ++k) {
-        u64 r = mul2(t00[v].v[k], p00);
-        r = fma2(t01[v].v[k], p01, r);
-        r = fma2(t10[v].v[k], p10, r);
-        r = fma2(t11[v].v[k], p11, r);
-        S[k] = add2(S[k], r);
-        Q[k] = fma2(r, r, Q[k]);
-      }
-    }
-    u64 o[NP];
-#pragma unroll
-    for (int k = 0; k < NP; ++k) {
-      const u64 m = mul2(S[k], inv_v2), mn = mul2(S[k], ninv_v2);
-      o[k] = fma2(mn, m, mul2(Q[k], inv_v2));
-    }
-    if (round_tf32) {
-#pragma unroll
-      for (int k = 0; k < NP; ++k) {
-        float lo, hi;
-        unpk2(o[k], lo, hi);
-        o[k] = pk2(round_tf32_f(lo), round_tf32_f(hi));
-      }
-    }
-    if (active) stg_tex<CPT>(optr, o);
-    optr += (size_t)hw * C;
-  }
-}
-
-template <int NSRC, int CT>
-static bool launch_var(cudaStream_t st, const float* f, const float* p, const float* dv,
-                       float* cost, int B, int D, int h, int w, int dchunk, int rnd) {
-  // 8 channels per thread, no window skip, 6 resident blocks per SM (80 registers): 4 channels
-  // per thread, window skip and 4 / 5 / 8-block register budgets were slower and were removed
-  const long threads = (long)h * w * (CT / 8);
-  dim3 grd((unsigned)((threads + kK1Threads - 1) / kK1Threads), (unsigned)B,
-           (unsigned)((D + dchunk - 1) / dchunk));
-  warp_var_kernel<NSRC, CT, 8, false, 6><<<grd, kK1Threads, 0, st>>>(f, p, dv, cost, D, h, w, dchunk, rnd);
-  return true;
 }
 
 // Stand-alone homo_warp: one thread = one pixel x 8 channels, all planes.
@@ -491,8 +307,6 @@ static int launch_transpose(const float* in, float* out, int N, size_t R, size_t
   transpose_rs_kernel<<<grd, blk, 0, st>>>(in, out, R, S, (unsigned)tiles_s);
   return after_launch(what);
 }
-
-int g_k1_dchunk = 0;  // CASMVS_K1_DCHUNK overrides the depth-chunk heuristic
 
 // warp_cost_smem.cu
 int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
@@ -572,40 +386,18 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   const bool nhwc = cost_layout == CASMVS_NHWC;
   const long threads = (long)h * w * (C / kCPT);
   const unsigned xblocks = (unsigned)((threads + kK1Threads - 1) / kK1Threads);
-  // depth chunks: enough CTAs to fill every SM several times over, but chunks long
-  // enough (>= 8 planes) for the texel-window cache to pay off
-  static bool env_read = false;
-  if (!env_read) {
-    env_read = true;
-    if (const char* e = getenv("CASMVS_K1_DCHUNK")) g_k1_dchunk = atoi(e);
-  }
-  int dchunk = D;
-  if (g_k1_dchunk > 0) dchunk = g_k1_dchunk;
-  else {
-    const long want_ctas = (long)num_sms() * 16;
-    while (dchunk > 8 && (long)xblocks * B * ((D + dchunk - 1) / dchunk) < want_ctas)
-      dchunk = (dchunk + 1) / 2;
-  }
   if (nhwc) {
-    // TMA-staged generation (warp_cost_smem.cu): 0 = handled, 1 = shape left to the gather kernels
+    // TMA-staged generation (warp_cost_smem.cu): 0 = handled, 1 = shape left to the gather kernel
     const Hyp hyp{depth_values, nullptr, nullptr, nullptr, 0.f, 0.f};
     const int rc = warp_var_smem(f, proj, hyp, cost, B, V, C, D, h, w, num_groups, rnd, 0, st);
     if (rc <= 0) return rc;
   }
-  if (!gwc && nhwc && (V == 3 || V == 2) && (C == 8 || C == 16 || C == 32)) {
-    // specialised variance kernel (the round-1 hot case; now behind the staged kernels)
-    bool ok = false;
-    if (V == 3) {
-      if (C == 8) ok = launch_var<2, 8>(st, f, proj, depth_values, cost, B, D, h, w, dchunk, rnd);
-      else if (C == 16) ok = launch_var<2, 16>(st, f, proj, depth_values, cost, B, D, h, w, dchunk, rnd);
-      else ok = launch_var<2, 32>(st, f, proj, depth_values, cost, B, D, h, w, dchunk, rnd);
-    } else {
-      if (C == 8) ok = launch_var<1, 8>(st, f, proj, depth_values, cost, B, D, h, w, dchunk, rnd);
-      else if (C == 16) ok = launch_var<1, 16>(st, f, proj, depth_values, cost, B, D, h, w, dchunk, rnd);
-      else ok = launch_var<1, 32>(st, f, proj, depth_values, cost, B, D, h, w, dchunk, rnd);
-    }
-    if (ok) return after_launch("warp_cost");
-  }
+  // depth chunks: enough CTAs to fill every SM several times over, but chunks long
+  // enough (>= 8 planes) for the texel-window cache to pay off
+  int dchunk = D;
+  const long want_ctas = (long)num_sms() * 16;
+  while (dchunk > 8 && (long)xblocks * B * ((D + dchunk - 1) / dchunk) < want_ctas)
+    dchunk = (dchunk + 1) / 2;
   dim3 grd(xblocks, (unsigned)B, (unsigned)((D + dchunk - 1) / dchunk));
   switch (V - 1) {
     case 1: launch_k1_c<1>(gwc, nhwc, grd, st, f, proj, depth_values, cost, V, C, D, h, w, num_groups, dchunk, rnd); break;

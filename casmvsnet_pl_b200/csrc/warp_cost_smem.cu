@@ -41,7 +41,8 @@ using tc::mbar_init;
 using tc::mbar_wait;
 using tc::smem_u32;
 
-constexpr int kMaxSrcSmem = 6;
+constexpr int kMaxSrcSmem = 2;
+constexpr int kMarginX = 16, kMarginY = 4;    // box = tile + margins (see launch)
 constexpr float kMagic = 12582912.f;          // 1.5 * 2^23: u + kMagic (round down) = floor(u) + kMagic
 constexpr int kMagicBits = 0x4B400000;
 
@@ -60,31 +61,129 @@ __device__ __forceinline__ void lds_tex(uint32_t addr, Tex8& t) {   // 2 x 16 B,
 struct Small {            // lives behind the boxes in dynamic shared memory
   float proj[kMaxSrcSmem * 12];
   int mm[kMaxSrcSmem * 4];      // minx, miny, maxx, maxy per view (block reduction)
-  int box[kMaxSrcSmem * 2];     // box origin per view
   unsigned long long bar;
 };
 
-// CP channels per thread (8 or 16).  16 halves the per-output share of everything that is per
-// (pixel, plane, view) -- homography, reciprocal, floor, window address, swizzle, predicates:
-// ~60 % of the instruction stream at CP = 8 -- at the price of a 64-register window.
-template <int CP> struct TexP { u64 v[CP / 2]; };
-template <int CP>
-__device__ __forceinline__ void lds_texp(uint32_t addr, TexP<CP>& t) {   // CP*4 bytes, 16 B chunks
+// What a thread of either kernel knows after the per-CTA set-up.
+template <int NSRC>
+struct Tile {
+  uint32_t base;            // 1024 B-aligned start of the boxes (shared-window address)
+  uint32_t bar;             // the CTA's mbarrier
+  Small* sm;
+  int sub, c0, pix;         // channel group of this thread, its first channel, its pixel
+  bool active;              // the pixel is inside the image
+  float ax[NSRC], ay[NSRC], az[NSRC], tx[NSRC], ty[NSRC], tz[NSRC];   // R*(x,y,1) and T per view
+};
+
+// Tile coordinates, projection rows of the NSRC source views into Small, mbarrier init, and
+// the per-view terms of the homography at this thread's pixel.
+template <int NSRC, int TW, int TH, int TPP>
+__device__ __forceinline__ Tile<NSRC> setup_tile(uint8_t* smem_raw, const float* __restrict__ proj,
+                                                 int h, int w, int box_stride, int tiles_x) {
+  Tile<NSRC> t;
+  t.base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  t.sm = reinterpret_cast<Small*>(smem_raw + (t.base - smem_u32(smem_raw)) + NSRC * box_stride);
+  t.bar = smem_u32(&t.sm->bar);
+  const int tid = threadIdx.x;
+  const int b = blockIdx.y;
+  const int tile_y = blockIdx.x / tiles_x, tile_x = blockIdx.x - tile_y * tiles_x;
+  const int lp = tid / TPP;
+  t.sub = tid - lp * TPP;
+  t.c0 = t.sub * kCPT;   // before the barrier: computed after it, ptxas spends 3-6 more registers
+  const int py = lp / TW, px = lp - py * TW;
+  const int xr = tile_x * TW + px, yr = tile_y * TH + py;
+  t.active = xr < w && yr < h;
+  const int x = min(xr, w - 1), y = min(yr, h - 1);
+  t.pix = y * w + x;
+
+  for (int i = tid; i < NSRC * 12; i += TW * TH * TPP) t.sm->proj[i] = proj[(size_t)b * NSRC * 12 + i];
+  if (tid == 0) {
+    mbar_init(t.bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const float xf = (float)x, yf = (float)y;
 #pragma unroll
-  for (int k = 0; k < CP / 4; ++k)
-    asm volatile("ld.shared.v2.b64 {%0,%1}, [%2];" : "=l"(t.v[2 * k]), "=l"(t.v[2 * k + 1])
-                 : "r"(addr ^ (16u * k)));
-}
-template <int CP>
-__device__ __forceinline__ TexP<CP> ldg_texp(const float* p) {
-  TexP<CP> t;
-#pragma unroll
-  for (int k = 0; k < CP / 8; ++k) {
-    const Tex8 a = ldg256(p + 8 * k);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) t.v[4 * k + j] = a.v[j];
+  for (int v = 0; v < NSRC; ++v) {
+    const float* P = t.sm->proj + v * 12;
+    t.ax[v] = fmaf(P[0], xf, fmaf(P[1], yf, P[2]));     // R*(x,y,1)   (modules.py:72)
+    t.ay[v] = fmaf(P[4], xf, fmaf(P[5], yf, P[6]));
+    t.az[v] = fmaf(P[8], xf, fmaf(P[9], yf, P[10]));
+    t.tx[v] = P[3]; t.ty[v] = P[7]; t.tz[v] = P[11];
   }
   return t;
+}
+
+// Footprint of planes [d0, d0 + n) in every view, n = d_end - d0 halved until every view's
+// footprint fits its BW x BH box (or n == 1); then one elected thread stages the boxes, one TMA
+// per view with zero fill outside the image, completing on the CTA's mbarrier.  Returns n;
+// kx / ky: the box origins plus kMagicBits, for the floor-by-add of the sampling loops.
+template <int NSRC, int TEXB>
+__device__ __forceinline__ int stage_boxes(const Tile<NSRC>& t, const CUtensorMap& fmap,
+                                           const HypPix& hp, int d0, int d_end, int h, int w,
+                                           int BW, int BH, int box_stride, int (&kx)[NSRC],
+                                           int (&ky)[NSRC]) {
+  const int tid = threadIdx.x;
+  Small* sm = t.sm;
+  int n = d_end - d0;
+  int bx[NSRC], by[NSRC];
+  for (;;) {
+    // (also: every thread is done with the previous run's boxes and min/max words)
+    __syncthreads();
+    if (tid < NSRC * 4) sm->mm[tid] = (tid & 2) ? INT_MIN : INT_MAX;
+    __syncthreads();
+    const float ia = rcp_approx(hp.at(d0));
+    const float ib = rcp_approx(hp.at(d0 + n - 1));
+#pragma unroll
+    for (int v = 0; v < NSRC; ++v) {
+      int mnx = INT_MAX, mny = INT_MAX, mxx = INT_MIN, mxy = INT_MIN;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float id = e ? ib : ia;
+        const float qz = fmaf(t.tz[v], id, t.az[v]);
+        const float rz = rcp_approx(qz);
+        const float u = fmaf(t.tx[v], id, t.ax[v]) * rz, vv = fmaf(t.ty[v], id, t.ay[v]) * rz;
+        // samples that cannot touch the image (or are not finite) do not shape the box
+        if (t.active && qz > 1e-7f && u > -2.f && u < (float)(w + 1) && vv > -2.f &&
+            vv < (float)(h + 1)) {
+          const int xi = __float2int_rd(u), yi = __float2int_rd(vv);
+          mnx = min(mnx, xi); mxx = max(mxx, xi);
+          mny = min(mny, yi); mxy = max(mxy, yi);
+        }
+      }
+      mnx = __reduce_min_sync(0xffffffffu, mnx); mny = __reduce_min_sync(0xffffffffu, mny);
+      mxx = __reduce_max_sync(0xffffffffu, mxx); mxy = __reduce_max_sync(0xffffffffu, mxy);
+      if ((tid & 31) == 0) {
+        atomicMin(&sm->mm[v * 4 + 0], mnx); atomicMin(&sm->mm[v * 4 + 1], mny);
+        atomicMax(&sm->mm[v * 4 + 2], mxx); atomicMax(&sm->mm[v * 4 + 3], mxy);
+      }
+    }
+    __syncthreads();
+    bool fits = true;
+#pragma unroll
+    for (int v = 0; v < NSRC; ++v) {
+      const int mnx = sm->mm[v * 4 + 0], mny = sm->mm[v * 4 + 1];
+      const int mxx = sm->mm[v * 4 + 2], mxy = sm->mm[v * 4 + 3];
+      if (mnx > mxx) { bx[v] = 0; by[v] = 0; continue; }      // nothing lands in the image
+      const int sx = mxx + 2 - mnx, sy = mxy + 2 - mny;       // texel columns / rows needed
+      if (sx > BW || sy > BH) fits = false;
+      bx[v] = mnx - max(0, (BW - sx) >> 1);
+      by[v] = mny - max(0, (BH - sy) >> 1);
+    }
+    if (fits || n == 1) break;
+    n = (n + 1) >> 1;
+  }
+  if (tid == 0) {
+    const int b = blockIdx.y;
+    tma::mbar_expect_tx(t.bar, (uint32_t)(NSRC * BW * BH * TEXB));
+#pragma unroll
+    for (int v = 0; v < NSRC; ++v)
+      tma::tma_load_4d(t.base + v * box_stride, &fmap, t.bar, 0, bx[v], by[v], b * (NSRC + 1) + v + 1);
+  }
+#pragma unroll
+  for (int v = 0; v < NSRC; ++v) { kx[v] = kMagicBits + bx[v]; ky[v] = kMagicBits + by[v]; }
+  return n;
 }
 
 // NSRC source views, C channels, TW x TH pixel tile.  Every plane loads its 2x2 windows (the
@@ -92,54 +191,25 @@ __device__ __forceinline__ TexP<CP> ldg_texp(const float* p) {
 // BLOCKED: the cost volume is stored blocked by channel quads (B, COUT/4, D, h, w, 4) instead of
 // channels-last.  A template parameter: as a run-time value it cost the channels-last kernels
 // about 5 % of their rate.
-template <int NSRC, int C, int TW, int TH, int MINB, bool GWC = false, int CP = 8,
-          bool BLOCKED = false>
-__global__ void __launch_bounds__(TW* TH*(C / CP), MINB)
+template <int NSRC, int C, int TW, int TH, int MINB, bool GWC, bool BLOCKED>
+__global__ void __launch_bounds__(TW* TH*(C / kCPT), MINB)
 warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __restrict__ feats,
                      const float* __restrict__ proj, const Hyp hyp,
                      float* __restrict__ cost, int D, int h, int w, int dchunk, int BW, int BH,
                      int box_stride, int tiles_x, int round_tf32) {
   // GWC (group-wise correlation, mvsnet.py:143-144,158-162,170-172) is built for 8 groups:
   // C/8 in {1,2,4} channels per group, every thread owns 8/(C/8) whole groups
-  constexpr int V = NSRC + 1, TPP = C / CP, TEXB = C * 4, NT = TW * TH * TPP, NP = CP / 2;
-  static_assert(!GWC || CP == 8, "group-wise correlation is built for 8 channels per thread");
+  constexpr int V = NSRC + 1, TPP = C / kCPT, TEXB = C * 4;
   constexpr int CPG = C / 8, NG = kCPT / CPG, COUT = GWC ? 8 : C;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  Small* sm = reinterpret_cast<Small*>(smem_raw + (base - smem_u32(smem_raw)) + NSRC * box_stride);
-  const uint32_t bar = smem_u32(&sm->bar);
-
-  const int tid = threadIdx.x;
+  const Tile<NSRC> t = setup_tile<NSRC, TW, TH, TPP>(smem_raw, proj, h, w, box_stride, tiles_x);
   const int b = blockIdx.y;
-  const int tile_y = blockIdx.x / tiles_x, tile_x = blockIdx.x - tile_y * tiles_x;
-  const int lp = tid / TPP, sub = tid - lp * TPP;
-  const int py = lp / TW, px = lp - py * TW;
-  const int xr = tile_x * TW + px, yr = tile_y * TH + py;
-  const bool active = xr < w && yr < h;
-  const int x = min(xr, w - 1), y = min(yr, h - 1);
-  const int c0 = sub * CP;
-  const int hw = h * w, pix = y * w + x;
+  const int c0 = t.c0;
+  const int hw = h * w, pix = t.pix;
 
-  for (int i = tid; i < NSRC * 12; i += NT) sm->proj[i] = proj[(size_t)b * NSRC * 12 + i];
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  const float xf = (float)x, yf = (float)y;
-  float ax[NSRC], ay[NSRC], az[NSRC], tx[NSRC], ty[NSRC], tz[NSRC];
-#pragma unroll
-  for (int v = 0; v < NSRC; ++v) {
-    const float* P = sm->proj + v * 12;
-    ax[v] = fmaf(P[0], xf, fmaf(P[1], yf, P[2]));     // R*(x,y,1)   (modules.py:72)
-    ay[v] = fmaf(P[4], xf, fmaf(P[5], yf, P[6]));
-    az[v] = fmaf(P[8], xf, fmaf(P[9], yf, P[10]));
-    tx[v] = P[3]; ty[v] = P[7]; tz[v] = P[11];
-  }
   const size_t view_stride = (size_t)hw * C;
   const float* fb = feats + (size_t)b * V * view_stride + c0;
-  const TexP<CP> ref = ldg_texp<CP>(fb + (size_t)pix * C);
+  const Tex8 ref = ldg256(fb + (size_t)pix * C);
   const float inv_v = 1.f / (float)V;
   const u64 inv_v2 = pk2(inv_v, inv_v), ninv_v2 = pk2(-inv_v, -inv_v);
 
@@ -147,7 +217,7 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
   const int d_end = min(D, d_begin + dchunk);
   const HypPix hp(hyp, b, D, (size_t)hw, pix);
   // output: channels-last, or blocked by channel quads (B, COUT/4, D, h, w, 4)
-  const int co = GWC ? sub * NG : c0;
+  const int co = GWC ? t.sub * NG : c0;
   const size_t pstr = BLOCKED ? (size_t)hw * 4 : (size_t)hw * COUT;      // next plane
   const size_t qstr = BLOCKED ? (size_t)D * hw * 4 : 4;                 // next channel quad
   float* optr = cost + (BLOCKED ? (((size_t)b * (COUT / 4) + co / 4) * D + d_begin) * hw * 4 +
@@ -158,86 +228,27 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
   uint32_t phase = 0;
 
   for (int d0 = d_begin; d0 < d_end;) {
-    // ---- 1. footprint of planes [d0, d0 + n) in every view; halve n until it fits the box
-    int n = d_end - d0;
-    int bx[NSRC], by[NSRC];
-    for (;;) {
-      // (also: every thread is done with the previous run's boxes and min/max words)
-      __syncthreads();
-      if (tid < NSRC * 4) sm->mm[tid] = (tid & 2) ? INT_MIN : INT_MAX;
-      __syncthreads();
-      const float ia = rcp_approx(hp.at(d0));
-      const float ib = rcp_approx(hp.at(d0 + n - 1));
-#pragma unroll
-      for (int v = 0; v < NSRC; ++v) {
-        int mnx = INT_MAX, mny = INT_MAX, mxx = INT_MIN, mxy = INT_MIN;
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float id = e ? ib : ia;
-          const float qz = fmaf(tz[v], id, az[v]);
-          const float rz = rcp_approx(qz);
-          const float u = fmaf(tx[v], id, ax[v]) * rz, vv = fmaf(ty[v], id, ay[v]) * rz;
-          // samples that cannot touch the image (or are not finite) do not shape the box
-          if (active && qz > 1e-7f && u > -2.f && u < (float)(w + 1) && vv > -2.f &&
-              vv < (float)(h + 1)) {
-            const int xi = __float2int_rd(u), yi = __float2int_rd(vv);
-            mnx = min(mnx, xi); mxx = max(mxx, xi);
-            mny = min(mny, yi); mxy = max(mxy, yi);
-          }
-        }
-        mnx = __reduce_min_sync(0xffffffffu, mnx); mny = __reduce_min_sync(0xffffffffu, mny);
-        mxx = __reduce_max_sync(0xffffffffu, mxx); mxy = __reduce_max_sync(0xffffffffu, mxy);
-        if ((tid & 31) == 0) {
-          atomicMin(&sm->mm[v * 4 + 0], mnx); atomicMin(&sm->mm[v * 4 + 1], mny);
-          atomicMax(&sm->mm[v * 4 + 2], mxx); atomicMax(&sm->mm[v * 4 + 3], mxy);
-        }
-      }
-      __syncthreads();
-      bool fits = true;
-#pragma unroll
-      for (int v = 0; v < NSRC; ++v) {
-        const int mnx = sm->mm[v * 4 + 0], mny = sm->mm[v * 4 + 1];
-        const int mxx = sm->mm[v * 4 + 2], mxy = sm->mm[v * 4 + 3];
-        if (mnx > mxx) { bx[v] = 0; by[v] = 0; continue; }      // nothing lands in the image
-        const int sx = mxx + 2 - mnx, sy = mxy + 2 - mny;       // texel columns / rows needed
-        if (sx > BW || sy > BH) fits = false;
-        bx[v] = mnx - max(0, (BW - sx) >> 1);
-        by[v] = mny - max(0, (BH - sy) >> 1);
-      }
-      if (fits || n == 1) break;
-      n = (n + 1) >> 1;
-    }
-    // ---- 2. stage the boxes: one TMA per view, zero fill outside the image
-    if (tid == 0) {
-      tma::mbar_expect_tx(bar, (uint32_t)(NSRC * BW * BH * TEXB));
-#pragma unroll
-      for (int v = 0; v < NSRC; ++v)
-        tma::tma_load_4d(base + v * box_stride, &fmap, bar, 0, bx[v], by[v], b * V + v + 1);
-    }
     int kx[NSRC], ky[NSRC];
-#pragma unroll
-    for (int v = 0; v < NSRC; ++v) {
-      kx[v] = kMagicBits + bx[v]; ky[v] = kMagicBits + by[v];
-    }
+    const int n = stage_boxes<NSRC, TEXB>(t, fmap, hp, d0, d_end, h, w, BW, BH, box_stride, kx, ky);
     float depth_next = hp.at(d0);
-    mbar_wait(bar, phase);
+    mbar_wait(t.bar, phase);
     phase ^= 1;
 
-    // ---- 3. the planes of this run
+    // the planes of this run
     for (int d = d0; d < d0 + n; ++d) {
       const float inv_d = rcp_approx(depth_next);
       if (d + 1 < d0 + n) depth_next = hp.at(d + 1);
-      u64 S[NP], Q[NP];
+      u64 S[4], Q[4];
 #pragma unroll
-      for (int k = 0; k < NP; ++k) {
+      for (int k = 0; k < 4; ++k) {
         S[k] = GWC ? 0ull : ref.v[k];            // gwc: the reference is NOT in the sum (:144)
         Q[k] = mul2(ref.v[k], ref.v[k]);
       }
 #pragma unroll
       for (int v = 0; v < NSRC; ++v) {
-        const float qx = fmaf(tx[v], inv_d, ax[v]);
-        const float qy = fmaf(ty[v], inv_d, ay[v]);
-        const float qz = fmaf(tz[v], inv_d, az[v]);
+        const float qx = fmaf(t.tx[v], inv_d, t.ax[v]);
+        const float qy = fmaf(t.ty[v], inv_d, t.ay[v]);
+        const float qz = fmaf(t.tz[v], inv_d, t.az[v]);
         const float rz = rcp_approx(qz);
         const float u = qx * rz, vv = qy * rz;
         // floor via round-down add: exact for |u| < 2^22, anything else fails the range test
@@ -245,52 +256,28 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
         const int xi = __float_as_int(fu) - kx[v], yi = __float_as_int(fv) - ky[v];
         const bool inbox = (unsigned)xi < (unsigned)(BW - 1) && (unsigned)yi < (unsigned)(BH - 1) &&
                            qz > 1e-7f;
-        u64 r[NP];
+        u64 r[4];
+        const auto put_r = [&r](int k, u64 x) { r[k] = x; };
         if (__builtin_expect(inbox, 1)) {
           const float fx = u - (fu - kMagic), fy = vv - (fv - kMagic);
           const float wxa = 1.f - fx, wya = 1.f - fy;
           const int l00 = v * box_stride + yi * row_b + xi * TEXB + c0 * 4;
-          TexP<CP> t00, t01, t10, t11;
-          lds_texp<CP>(base + swz<TEXB>(l00), t00);
-          lds_texp<CP>(base + swz<TEXB>(l00 + TEXB), t01);
-          lds_texp<CP>(base + swz<TEXB>(l00 + row_b), t10);
-          lds_texp<CP>(base + swz<TEXB>(l00 + row_b + TEXB), t11);
-          const float w00 = wxa * wya, w01 = fx * wya, w10 = wxa * fy, w11 = fx * fy;
-          const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10),
-                    p11 = pk2(w11, w11);
-#pragma unroll
-          for (int k = 0; k < NP; ++k) {
-            // tap order nw, ne, sw, se like ATen grid_sampler_2d
-            u64 a = mul2(t00.v[k], p00);
-            a = fma2(t01.v[k], p01, a);
-            a = fma2(t10.v[k], p10, a);
-            r[k] = fma2(t11.v[k], p11, a);
-          }
+          Window win;
+          lds_tex(t.base + swz<TEXB>(l00), win.t00);
+          lds_tex(t.base + swz<TEXB>(l00 + TEXB), win.t01);
+          lds_tex(t.base + swz<TEXB>(l00 + row_b), win.t10);
+          lds_tex(t.base + swz<TEXB>(l00 + row_b + TEXB), win.t11);
+          blend(win, wxa * wya, fx * wya, wxa * fy, fx * fy, put_r);
         } else if (qz <= 1e-7f || u <= -1.f || u >= (float)w || vv <= -1.f || vv >= (float)h) {
           // behind the camera (modules.py:76-79) or entirely outside the source image: the
           // sample is exactly zero, S and Q are unchanged
           continue;
         } else {
           // robust gather path for a window outside the staged box (NaN propagates like ATen)
-#pragma unroll
-          for (int hh = 0; hh < CP / 8; ++hh) {
-            Window win;
-            float w00, w01, w10, w11;
-            sample_view<C>(fb + (size_t)(v + 1) * view_stride + 8 * hh, qx, qy, qz, h, w, C, w * C,
-                           win, w00, w01, w10, w11);
-            const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10),
-                      p11 = pk2(w11, w11);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              u64 a = mul2(win.t00.v[k], p00);
-              a = fma2(win.t01.v[k], p01, a);
-              a = fma2(win.t10.v[k], p10, a);
-              r[4 * hh + k] = fma2(win.t11.v[k], p11, a);
-            }
-          }
+          gather_sample<C>(fb + (size_t)(v + 1) * view_stride, qx, qy, qz, h, w, C, w * C, put_r);
         }
 #pragma unroll
-        for (int k = 0; k < NP; ++k) {
+        for (int k = 0; k < 4; ++k) {
           S[k] = add2(S[k], r[k]);
           if (!GWC) Q[k] = fma2(r[k], r[k], Q[k]);
         }
@@ -299,7 +286,7 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
         // cost[g] = mean_{c in g}(S_c * ref_c) / (V-1)     (mvsnet.py:170-172)
         float pr[kCPT], o[NG];
 #pragma unroll
-        for (int k = 0; k < NP; ++k) unpk2(mul2(S[k], ref.v[k]), pr[2 * k], pr[2 * k + 1]);
+        for (int k = 0; k < 4; ++k) unpk2(mul2(S[k], ref.v[k]), pr[2 * k], pr[2 * k + 1]);
 #pragma unroll
         for (int k = 0; k < NG; ++k) {
           float acc = CPG == 1 ? pr[k] : CPG == 2 ? pr[2 * k] + pr[2 * k + 1]
@@ -307,7 +294,7 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
           float val = __fdiv_rn(acc * (1.f / (float)CPG), (float)NSRC);
           o[k] = round_tf32 ? round_tf32_f(val) : val;
         }
-        if (active) {
+        if (t.active) {
           if constexpr (NG == 8) {
             u64 ov[4] = {pk2(o[0], o[1]), pk2(o[2], o[3]), pk2(o[4], o[5]), pk2(o[6], o[7])};
             stg256q(optr, qstr, ov);
@@ -317,30 +304,10 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
             *reinterpret_cast<float2*>(optr) = make_float2(o[0], o[1]);
           }
         }
-        optr += pstr;
-        continue;
-      }
-      // var = Q/V - (S/V)^2   (mvsnet.py:166-168)
-      u64 o[NP];
-#pragma unroll
-      for (int k = 0; k < NP; ++k) {
-        const u64 m = mul2(S[k], inv_v2), mn = mul2(S[k], ninv_v2);
-        o[k] = fma2(mn, m, mul2(Q[k], inv_v2));
-      }
-      if (round_tf32) {
-#pragma unroll
-        for (int k = 0; k < NP; ++k) {
-          float lo, hi;
-          unpk2(o[k], lo, hi);
-          o[k] = pk2(round_tf32_f(lo), round_tf32_f(hi));
-        }
-      }
-      if (active) {
-#pragma unroll
-        for (int hh = 0; hh < CP / 8; ++hh) {
-          const u64 oo[4] = {o[4 * hh], o[4 * hh + 1], o[4 * hh + 2], o[4 * hh + 3]};
-          stg256q(optr + 2 * hh * qstr, qstr, oo);
-        }
+      } else {
+        u64 o[4];
+        variance(S, Q, inv_v2, ninv_v2, round_tf32, o);
+        if (t.active) stg256q(optr, qstr, o);
       }
       optr += pstr;
     }
@@ -350,7 +317,7 @@ warp_var_smem_kernel(const __grid_constant__ CUtensorMap fmap, const float* __re
 
 // ---- plane-group variant: window reuse WITHOUT persistent registers -----------------------------
 // Both K1 generations are bound by the LSU data pipe (32 B of tap traffic per output float),
-// not by latency.  Keeping the 2x2 windows of both views in registers across planes (REUSE)
+// not by latency.  Keeping the 2x2 windows of both views in registers across planes
 // cuts the shared-memory wavefronts but needs far more registers (or spills,
 // whose local-memory traffic goes through the same LSU pipe).  Here a thread walks PG planes
 // of ONE view before turning to the next view: the window lives only inside that short walk
@@ -364,38 +331,12 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
                         const float* __restrict__ proj, const Hyp hyp, float* __restrict__ cost,
                         int D, int h, int w, int dchunk, int BW, int BH, int box_stride, int tiles_x,
                         int round_tf32) {
-  constexpr int NSRC = 2, V = 3, TPP = C / kCPT, TEXB = C * 4, NT = TW * TH * TPP;
+  constexpr int NSRC = 2, V = 3, TPP = C / kCPT, TEXB = C * 4;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  Small* sm = reinterpret_cast<Small*>(smem_raw + (base - smem_u32(smem_raw)) + NSRC * box_stride);
-  const uint32_t bar = smem_u32(&sm->bar);
-  const int tid = threadIdx.x;
+  const Tile<NSRC> t = setup_tile<NSRC, TW, TH, TPP>(smem_raw, proj, h, w, box_stride, tiles_x);
   const int b = blockIdx.y;
-  const int tile_y = blockIdx.x / tiles_x, tile_x = blockIdx.x - tile_y * tiles_x;
-  const int lp = tid / TPP, sub = tid - lp * TPP;
-  const int py = lp / TW, px = lp - py * TW;
-  const int xr = tile_x * TW + px, yr = tile_y * TH + py;
-  const bool active = xr < w && yr < h;
-  const int x = min(xr, w - 1), y = min(yr, h - 1);
-  const int c0 = sub * kCPT;
-  const int hw = h * w, pix = y * w + x;
-
-  for (int i = tid; i < NSRC * 12; i += NT) sm->proj[i] = proj[(size_t)b * NSRC * 12 + i];
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  const float xf = (float)x, yf = (float)y;
-  float ax[NSRC], ay[NSRC], az[NSRC], tx[NSRC], ty[NSRC], tz[NSRC];
-#pragma unroll
-  for (int v = 0; v < NSRC; ++v) {
-    const float* P = sm->proj + v * 12;
-    ax[v] = fmaf(P[0], xf, fmaf(P[1], yf, P[2]));
-    ay[v] = fmaf(P[4], xf, fmaf(P[5], yf, P[6]));
-    az[v] = fmaf(P[8], xf, fmaf(P[9], yf, P[10]));
-    tx[v] = P[3]; ty[v] = P[7]; tz[v] = P[11];
-  }
+  const int c0 = t.c0;
+  const int hw = h * w, pix = t.pix;
   const size_t view_stride = (size_t)hw * C;
   const float* fb = feats + (size_t)b * V * view_stride + c0;
   const Tex8 ref = ldg256(fb + (size_t)pix * C);
@@ -412,7 +353,7 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
                                 : ((size_t)(b * D + d_begin) * hw + pix) * C + c0);
   const int row_b = BW * TEXB;
   // a row pitch that is a multiple of 1024 B leaves the swizzle bits of an address unchanged:
-  // the second window row is then the first one + row_b (launch_pg picks BW accordingly)
+  // the second window row is then the first one + row_b (launch picks BW accordingly)
   const bool rowal = (row_b & 1023) == 0;
   u64 refsq[4];
 #pragma unroll
@@ -420,66 +361,13 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
   uint32_t phase = 0;
 
   for (int d0 = d_begin; d0 < d_end;) {
-    int n = d_end - d0;
-    int bx[NSRC], by[NSRC];
-    for (;;) {
-      __syncthreads();
-      if (tid < NSRC * 4) sm->mm[tid] = (tid & 2) ? INT_MIN : INT_MAX;
-      __syncthreads();
-      const float ia = rcp_approx(hp.at(d0));
-      const float ib = rcp_approx(hp.at(d0 + n - 1));
-#pragma unroll
-      for (int v = 0; v < NSRC; ++v) {
-        int mnx = INT_MAX, mny = INT_MAX, mxx = INT_MIN, mxy = INT_MIN;
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float id = e ? ib : ia;
-          const float qz = fmaf(tz[v], id, az[v]);
-          const float rz = rcp_approx(qz);
-          const float u = fmaf(tx[v], id, ax[v]) * rz, vv = fmaf(ty[v], id, ay[v]) * rz;
-          if (active && qz > 1e-7f && u > -2.f && u < (float)(w + 1) && vv > -2.f &&
-              vv < (float)(h + 1)) {
-            const int xi = __float2int_rd(u), yi = __float2int_rd(vv);
-            mnx = min(mnx, xi); mxx = max(mxx, xi);
-            mny = min(mny, yi); mxy = max(mxy, yi);
-          }
-        }
-        mnx = __reduce_min_sync(0xffffffffu, mnx); mny = __reduce_min_sync(0xffffffffu, mny);
-        mxx = __reduce_max_sync(0xffffffffu, mxx); mxy = __reduce_max_sync(0xffffffffu, mxy);
-        if ((tid & 31) == 0) {
-          atomicMin(&sm->mm[v * 4 + 0], mnx); atomicMin(&sm->mm[v * 4 + 1], mny);
-          atomicMax(&sm->mm[v * 4 + 2], mxx); atomicMax(&sm->mm[v * 4 + 3], mxy);
-        }
-      }
-      __syncthreads();
-      bool fits = true;
-#pragma unroll
-      for (int v = 0; v < NSRC; ++v) {
-        const int mnx = sm->mm[v * 4 + 0], mny = sm->mm[v * 4 + 1];
-        const int mxx = sm->mm[v * 4 + 2], mxy = sm->mm[v * 4 + 3];
-        if (mnx > mxx) { bx[v] = 0; by[v] = 0; continue; }
-        const int sx = mxx + 2 - mnx, sy = mxy + 2 - mny;
-        if (sx > BW || sy > BH) fits = false;
-        bx[v] = mnx - max(0, (BW - sx) >> 1);
-        by[v] = mny - max(0, (BH - sy) >> 1);
-      }
-      if (fits || n == 1) break;
-      n = (n + 1) >> 1;
-    }
-    if (tid == 0) {
-      tma::mbar_expect_tx(bar, (uint32_t)(NSRC * BW * BH * TEXB));
-#pragma unroll
-      for (int v = 0; v < NSRC; ++v)
-        tma::tma_load_4d(base + v * box_stride, &fmap, bar, 0, bx[v], by[v], b * V + v + 1);
-    }
     int kx[NSRC], ky[NSRC];
-#pragma unroll
-    for (int v = 0; v < NSRC; ++v) { kx[v] = kMagicBits + bx[v]; ky[v] = kMagicBits + by[v]; }
+    const int n = stage_boxes<NSRC, TEXB>(t, fmap, hp, d0, d_end, h, w, BW, BH, box_stride, kx, ky);
     // hypotheses of the next plane group are fetched while the current one is processed
     float dnext[PG];
 #pragma unroll
     for (int p = 0; p < PG; ++p) dnext[p] = hp.at(min(d0 + p, d0 + n - 1));
-    mbar_wait(bar, phase);
+    mbar_wait(t.bar, phase);
     phase ^= 1;
 
     for (int d = d0; d < d0 + n; d += PG) {
@@ -492,13 +380,13 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
       u64 r1[PG][4];
 #pragma unroll
       for (int v = 0; v < NSRC; ++v) {
-        Tex8 t00, t01, t10, t11;
-        int cur = -1;                                   // window held in t00..t11
+        Window win;
+        int cur = -1;                                   // window held in win
 #pragma unroll
         for (int p = 0; p < PG; ++p) {
-          const float qx = fmaf(tx[v], inv_d[p], ax[v]);
-          const float qy = fmaf(ty[v], inv_d[p], ay[v]);
-          const float qz = fmaf(tz[v], inv_d[p], az[v]);
+          const float qx = fmaf(t.tx[v], inv_d[p], t.ax[v]);
+          const float qy = fmaf(t.ty[v], inv_d[p], t.ay[v]);
+          const float qz = fmaf(t.tz[v], inv_d[p], t.az[v]);
           const float rz = rcp_approx(qz);
           const float u = qx * rz, vv = qy * rz;
           const float fu = fadd_rd(u, kMagic), fv = fadd_rd(vv, kMagic);
@@ -506,65 +394,36 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
           const bool inbox = (unsigned)xi < (unsigned)(BW - 1) && (unsigned)yi < (unsigned)(BH - 1) &&
                              qz > 1e-7f;
           u64 r[4] = {0ull, 0ull, 0ull, 0ull};          // packed +0.f: a sample that is exactly zero
+          const auto put_r = [&r](int k, u64 x) { r[k] = x; };
           if (__builtin_expect(inbox, 1)) {
             const float fx = u - (fu - kMagic), fy = vv - (fv - kMagic);
             const float wxa = 1.f - fx, wya = 1.f - fy;
             const int l00 = v * box_stride + yi * row_b + xi * TEXB + c0 * 4;
             if (l00 != cur) {
-              const uint32_t a0 = base + swz<TEXB>(l00), a1 = base + swz<TEXB>(l00 + TEXB);
-              lds_tex(a0, t00);
-              lds_tex(a1, t01);
-              lds_tex(rowal ? a0 + row_b : base + swz<TEXB>(l00 + row_b), t10);
-              lds_tex(rowal ? a1 + row_b : base + swz<TEXB>(l00 + row_b + TEXB), t11);
+              const uint32_t a0 = t.base + swz<TEXB>(l00), a1 = t.base + swz<TEXB>(l00 + TEXB);
+              lds_tex(a0, win.t00);
+              lds_tex(a1, win.t01);
+              lds_tex(rowal ? a0 + row_b : t.base + swz<TEXB>(l00 + row_b), win.t10);
+              lds_tex(rowal ? a1 + row_b : t.base + swz<TEXB>(l00 + row_b + TEXB), win.t11);
               cur = l00;
             }
-            const float w00 = wxa * wya, w01 = fx * wya, w10 = wxa * fy, w11 = fx * fy;
-            const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10),
-                      p11 = pk2(w11, w11);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              u64 a = mul2(t00.v[k], p00);
-              a = fma2(t01.v[k], p01, a);
-              a = fma2(t10.v[k], p10, a);
-              r[k] = fma2(t11.v[k], p11, a);
-            }
+            blend(win, wxa * wya, fx * wya, wxa * fy, fx * fy, put_r);
           } else if (!(qz <= 1e-7f || u <= -1.f || u >= (float)w || vv <= -1.f || vv >= (float)h)) {
-            Window win;
-            float w00, w01, w10, w11;
-            sample_view<C>(fb + (size_t)(v + 1) * view_stride, qx, qy, qz, h, w, C, w * C, win, w00,
-                           w01, w10, w11);
-            const u64 p00 = pk2(w00, w00), p01 = pk2(w01, w01), p10 = pk2(w10, w10),
-                      p11 = pk2(w11, w11);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              u64 a = mul2(win.t00.v[k], p00);
-              a = fma2(win.t01.v[k], p01, a);
-              a = fma2(win.t10.v[k], p10, a);
-              r[k] = fma2(win.t11.v[k], p11, a);
-            }
+            gather_sample<C>(fb + (size_t)(v + 1) * view_stride, qx, qy, qz, h, w, C, w * C, put_r);
           }
           if (v == 0) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) r1[p][k] = r[k];
           } else if (d + p < d0 + n) {
-            // S = (ref + r1) + r2, Q = fma(r2, r2, fma(r1, r1, ref^2)); var = Q/V - (S/V)^2
-            u64 o[4];
+            // S = (ref + r1) + r2, Q = fma(r2, r2, fma(r1, r1, ref^2))
+            u64 S[4], Q[4], o[4];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-              const u64 S = add2(add2(ref.v[k], r1[p][k]), r[k]);
-              const u64 Q = fma2(r[k], r[k], fma2(r1[p][k], r1[p][k], refsq[k]));
-              const u64 m = mul2(S, inv_v2), mn = mul2(S, ninv_v2);
-              o[k] = fma2(mn, m, mul2(Q, inv_v2));
+              S[k] = add2(add2(ref.v[k], r1[p][k]), r[k]);
+              Q[k] = fma2(r[k], r[k], fma2(r1[p][k], r1[p][k], refsq[k]));
             }
-            if (round_tf32) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                float lo, hi;
-                unpk2(o[k], lo, hi);
-                o[k] = pk2(round_tf32_f(lo), round_tf32_f(hi));
-              }
-            }
-            if (active) stg256q(optr + p * pstr, qstr, o);
+            variance(S, Q, inv_v2, ninv_v2, round_tf32, o);
+            if (t.active) stg256q(optr + p * pstr, qstr, o);
           }
         }
       }
@@ -603,24 +462,25 @@ static bool feature_map(CUtensorMap* out, const float* feats, int BV, int h, int
   return true;
 }
 
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-
-template <int NSRC, int C, int TW, int TH, int MINB, bool GWC = false, int CP = 8>
+// One launcher for both kernels: NSRC source views, TW x TH pixel tiles.  PG > 0 launches the
+// plane-group kernel, whose box row is rounded up to a multiple of 1024 B (see rowal).
+template <int NSRC, int C, int TW, int TH, int MINB, bool GWC, int PG>
 static int launch(const float* feats, const float* proj, const Hyp& dv, float* cost, int B, int D,
                   int h, int w, int rnd, int blocked, cudaStream_t st) {
-  constexpr int NT = TW * TH * (C / CP);
+  constexpr int NT = TW * TH * (C / kCPT);
   // box = tile + margins: sweep of the depth run + scale/rotation of the view + the 2x2 window
-  static const int mx = env_int("CASMVS_K1_MARGIN_X", NSRC <= 2 ? 16 : 8);
-  static const int my = env_int("CASMVS_K1_MARGIN_Y", NSRC <= 2 ? 4 : 3);
-  static const int dc_env = env_int("CASMVS_K1S_DCHUNK", 0);
-  const int BW = TW + mx, BH = TH + my;
+  constexpr int wq = PG > 0 ? 1024 / (C * 4) : 1;
+  constexpr int BW = (TW + kMarginX + wq - 1) / wq * wq, BH = TH + kMarginY;
   const int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
   const size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
-  auto kfn = blocked ? warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, CP, true>
-                     : warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, CP, false>;
+  auto kfn = [blocked] {
+    if constexpr (PG > 0)
+      return blocked ? warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, true>
+                     : warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, false>;
+    else
+      return blocked ? warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, true>
+                     : warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, false>;
+  }();
   static std::atomic<bool> attr_set[2][kMaxDevices];
   if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[blocked ? 1 : 0], "warp_cost")) return rc;
   if (smem > 200 * 1024) return 1;
@@ -629,94 +489,50 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   // depth runs: long enough to amortise the staging (a box is re-used by every plane of the
   // run), short enough to keep the sweep inside the margin and >= ~4 CTAs per SM in flight
   const int tiles_x = (w + TW - 1) / TW, tiles_y = (h + TH - 1) / TH;
-  int dchunk = dc_env > 0 ? dc_env : (D <= 16 ? D : 16);
-  while (dc_env <= 0 && dchunk > 4 &&
-         (long)tiles_x * tiles_y * B * ((D + dchunk - 1) / dchunk) < (long)num_sms() * 8)
+  int dchunk = D <= 16 ? D : 16;
+  while (dchunk > 4 && (long)tiles_x * tiles_y * B * ((D + dchunk - 1) / dchunk) < (long)num_sms() * 8)
     dchunk = (dchunk + 1) / 2;
   dim3 grd((unsigned)(tiles_x * tiles_y), (unsigned)B, (unsigned)((D + dchunk - 1) / dchunk));
   kfn<<<grd, NT, smem, st>>>(map, feats, proj, dv, cost, D, h, w, dchunk, BW, BH, box_stride,
                              tiles_x, rnd);
-  return after_launch("warp_cost(smem)");
-}
-
-template <int C, int TW, int TH, int PG, int MINB>
-static int launch_pg(const float* feats, const float* proj, const Hyp& dv, float* cost, int B, int D,
-                     int h, int w, int rnd, int blocked, cudaStream_t st) {
-  constexpr int NSRC = 2, NT = TW * TH * (C / kCPT);
-  static const int mx = env_int("CASMVS_K1_MARGIN_X", 16);
-  static const int my = env_int("CASMVS_K1_MARGIN_Y", 4);
-  static const int dc_env = env_int("CASMVS_K1S_DCHUNK", 0);
-  // box width rounded up so that the row pitch BW * C * 4 is a multiple of 1024 B (see rowal)
-  const int wq = 1024 / (C * 4);
-  const int BW = (TW + mx + wq - 1) / wq * wq, BH = TH + my;
-  const int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
-  const size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
-  auto kfn = blocked ? warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, true>
-                     : warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, false>;
-  static std::atomic<bool> attr_set[2][kMaxDevices];
-  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[blocked ? 1 : 0], "warp_cost")) return rc;
-  if (smem > 200 * 1024) return 1;
-  CUtensorMap map;
-  if (!feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return -2;
-  const int tiles_x = (w + TW - 1) / TW, tiles_y = (h + TH - 1) / TH;
-  int dchunk = dc_env > 0 ? dc_env : (D <= 16 ? D : 16);
-  while (dc_env <= 0 && dchunk > 4 &&
-         (long)tiles_x * tiles_y * B * ((D + dchunk - 1) / dchunk) < (long)num_sms() * 8)
-    dchunk = (dchunk + 1) / 2;
-  dim3 grd((unsigned)(tiles_x * tiles_y), (unsigned)B, (unsigned)((D + dchunk - 1) / dchunk));
-  kfn<<<grd, NT, smem, st>>>(map, feats, proj, dv, cost, D, h, w, dchunk, BW, BH, box_stride,
-                             tiles_x, rnd);
-  return after_launch("warp_cost(smem,pg)");
+  return after_launch(PG > 0 ? "warp_cost(smem,pg)" : "warp_cost(smem)");
 }
 
 }  // namespace k1s
 
-// Variance cost volume, channels-last features, channels-last or (blocked != 0) blocked output.
-// Returns 0 when handled, 1 when the shape is left to the gather kernels of warp_cost.cu, <0 on
-// error.
+// Variance or 8-group correlation cost volume, channels-last features, channels-last or
+// (blocked != 0) blocked output.  Returns 0 when handled, 1 when the shape is left to the gather
+// kernel of warp_cost.cu, <0 on error.
 int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
                   int V, int C, int D, int h, int w, int num_groups, int rnd, int blocked,
                   cudaStream_t st) {
-  static const int enabled = k1s::env_int("CASMVS_K1_SMEM", 1);
+  // CASMVS_K1_SMEM=0 leaves every shape to the gather kernel (the reference of the staged kernels)
+  static const bool enabled = [] {
+    const char* e = getenv("CASMVS_K1_SMEM");
+    return !e || atoi(e) != 0;
+  }();
   if (!enabled) return 1;
   if ((reinterpret_cast<uintptr_t>(feats) & 15) != 0 || B > 65535) return 1;
   using namespace k1s;
-  // With 4 / 6 source views the staged boxes leave one CTA per SM, so those shapes (cfg4 / cfg5)
-  // are left to the gather kernels of warp_cost.cu unless CASMVS_K1S_MANYVIEWS=1.
-  static const int many = env_int("CASMVS_K1S_MANYVIEWS", 0);
-  if (V - 1 > 2 && !many) return 1;
+  // V-1 > 2: the staged boxes leave one CTA per SM, the gather kernel is faster (cfg4 / cfg5)
+  if (V - 1 > 2) return 1;
+#define K1S(NS, CC, TW_, TH_, MB, GWC_, PG_) \
+  if (V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB, GWC_, PG_>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
   if (num_groups != 1) {
     // group-wise correlation: the reference's default G = 8
     if (num_groups != 8) return 1;
-#define K1G(NS, CC, TW_, TH_, MB) \
-  if (V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB, true>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
-    K1G(1, 8, 32, 4, 5) K1G(1, 16, 32, 2, 5) K1G(1, 32, 16, 2, 5)
-    K1G(2, 8, 32, 4, 5) K1G(2, 16, 32, 2, 5) K1G(2, 32, 16, 2, 5)
-    K1G(4, 8, 32, 4, 4) K1G(4, 16, 32, 4, 2) K1G(4, 32, 16, 4, 2)
-#undef K1G
+    K1S(1, 8, 32, 4, 5, true, 0) K1S(1, 16, 32, 2, 5, true, 0) K1S(1, 32, 16, 2, 5, true, 0)
+    K1S(2, 8, 32, 4, 5, true, 0) K1S(2, 16, 32, 2, 5, true, 0) K1S(2, 32, 16, 2, 5, true, 0)
     return 1;
   }
-  // Variants (CASMVS_K1S_VARIANT):
-  //   16 (default) plane groups of 2: a view's window is re-used across the planes of a group
-  //   11           plane groups of 4
-  //    4           no window reuse (every plane loads its 2x2 windows)
-  // Tried and removed: windows of both views kept in registers across ALL planes (register
-  // pressure or spills through the same LSU pipe), coordinate math shared between the threads
-  // of a pixel by warp shuffles (shuffles use the bound pipe), 16 channels per thread (register
-  // pressure).
-  static const int variant = env_int("CASMVS_K1S_VARIANT", 16);
-#define K1S(VAR, NS, CC, TW_, TH_, MB) \
-  if (variant == VAR && V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
-#define K1P(VAR, CC, TW_, TH_, PG_, MB) \
-  if (variant == VAR && V - 1 == 2 && C == CC) return launch_pg<CC, TW_, TH_, PG_, MB>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
-  K1P(16, 8, 32, 4, 2, 4) K1P(16, 16, 32, 2, 2, 4) K1P(16, 32, 16, 2, 2, 4)
-  K1P(11, 8, 32, 4, 4, 4) K1P(11, 16, 32, 2, 4, 4) K1P(11, 32, 16, 2, 4, 4)
-  K1S(4, 2, 8, 32, 4, 5) K1S(4, 2, 16, 32, 2, 5) K1S(4, 2, 32, 16, 2, 5)
-#undef K1P
-  if (V - 1 == 2) return 1;
-  K1S(variant, 1, 8, 32, 4, 5) K1S(variant, 1, 16, 32, 2, 5) K1S(variant, 1, 32, 16, 2, 5)
-  K1S(variant, 4, 8, 32, 4, 4) K1S(variant, 4, 16, 32, 4, 2) K1S(variant, 4, 32, 16, 4, 2)
-  K1S(variant, 6, 8, 32, 4, 4) K1S(variant, 6, 16, 32, 4, 2) K1S(variant, 6, 32, 16, 4, 2)
+  // Variance, V-1 = 2: plane groups of 2, a view's window is re-used across the planes of a
+  // group.  Tried and removed: plane groups of 4 (spill at 128 registers), no window reuse (every
+  // plane loads its 2x2 windows; slower), windows of both views kept in registers across ALL
+  // planes (register pressure or spills through the same LSU pipe), coordinate math shared
+  // between the threads of a pixel by warp shuffles (shuffles use the bound pipe), 16 channels
+  // per thread (register pressure).
+  K1S(2, 8, 32, 4, 4, false, 2) K1S(2, 16, 32, 2, 4, false, 2) K1S(2, 32, 16, 2, 4, false, 2)
+  K1S(1, 8, 32, 4, 5, false, 0) K1S(1, 16, 32, 2, 5, false, 0) K1S(1, 32, 16, 2, 5, false, 0)
 #undef K1S
   return 1;
 }

@@ -370,7 +370,7 @@ def ladder_supported(V, C, num_groups):
     """Shapes the staged K1 kernel (the only one that takes a ladder) runs by default: with more
     than two source views the gather kernels are faster and take the materialised tensor."""
     import os
-    if os.environ.get("CASMVS_K1_SMEM", "1") == "0":       # experiment switch: gather kernels only
+    if os.environ.get("CASMVS_K1_SMEM", "1") == "0":       # every shape on the gather kernel
         return False
     return (V - 1) in (1, 2) and C in (8, 16, 32) and num_groups in (1, 8)
 
