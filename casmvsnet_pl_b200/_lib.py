@@ -77,7 +77,12 @@ SIGNATURES = {
     "casmvs_warp_cost_bwd": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
     "casmvs_conv3d_wgrad": (c_int, [c_void_p] * 3 + [c_int] * 10 + [c_void_p]),
     "casmvs_regress_bwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
-    "casmvs_geo_fuse_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+    "casmvs_sl1_loss_workspace_bytes": (c_size_t, []),
+    "casmvs_sl1_loss_fwd": (c_int, [POINTER(c_void_p)] * 3 + [POINTER(c_int), c_int, c_int]
+                            + [c_void_p] * 4 + [c_size_t, c_void_p]),
+    "casmvs_sl1_loss_bwd": (c_int, [POINTER(c_void_p)] * 3 + [POINTER(c_int), c_int, c_int]
+                            + [c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
+    "casmvs_geo_fuse_fwd":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     POINTER(c_float), POINTER(c_float), c_void_p, c_int, c_int,
                                     c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -341,6 +341,16 @@ def open_scans(a):
         yield BlendedMVSTestScan(a.root_dir, s, tuple(a.img_wh), a.n_views, a.depth_interval)
 
 
+def load_checkpoint(model, path):
+    """Weights of a Lightning checkpoint ('model.'-prefixed keys under 'state_dict', as the
+    reference's train.py and casmvsnet_pl_b200.train write) or of a plain state dict."""
+    sd = torch.load(path, map_location="cpu")
+    sd = sd.get("state_dict", sd)
+    sd = {k[len("model."):] if k.startswith("model.") else k: v for k, v in sd.items()}   # utils:57-59
+    model.load_state_dict(sd)
+    return model
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--root_dir", required=True)
@@ -379,10 +389,7 @@ def main(argv=None):
     model = CascadeMVSNet(n_depths=a.n_depths, interval_ratios=a.interval_ratios,
                           num_groups=a.num_groups, norm_act=ABN, precision=a.precision)
     if a.ckpt:
-        sd = torch.load(a.ckpt, map_location="cpu")
-        sd = sd.get("state_dict", sd)
-        sd = {k[len("model."):] if k.startswith("model.") else k: v for k, v in sd.items()}   # utils:57-59
-        model.load_state_dict(sd)
+        load_checkpoint(model, a.ckpt)
     model = model.eval().cuda()
     os.makedirs(os.path.join(out_dir, "points"), exist_ok=True)
     for scan in open_scans(a):

@@ -1,5 +1,6 @@
 """Seeded synthetic scans in the Tanks and Temples and BlendedMVS test layouts, for the scan
-readers of eval_pipeline (the real data sets are large and licensed separately).
+readers of eval_pipeline, and in the DTU training layout (make_dtu_train), for train_data and
+the trainer (the real data sets are large and licensed separately).
 
   tanks       <root>/<split>/<scan>/pair.txt, cams/{vid:08d}_cam.txt, images/{vid:08d}.jpg
   blendedmvs  <root>/dataset_low_res/<scan>/cams/pair.txt, cams/{vid:08d}_cam.txt,
@@ -108,6 +109,63 @@ def make_blendedmvs(root, scan="5a3ca9cb270f0e3f14d0eddb", n_views=8, image_wh=(
         with open(os.path.join(root, names[split]), "a") as f:
             f.write(scan + "\n")
     return base
+
+
+def make_dtu_train(root, scan="scan1", refs=(0, 1, 2), n_src=5, depth=650.0, seed=0):
+    """A scan in the DTU training layout datasets/dtu.py reads with img_wh=None:
+
+        <root>/Cameras/pair.txt                    the viewpoints `refs`, n_src sources each
+        <root>/Cameras/train/{vid:08d}_cam.txt     all 49 views (the reader loads every one)
+        <root>/Rectified/<scan>_train/rect_{vid+1:03d}_{light}_r5000.png   640x512, lights 0-6
+        <root>/Depths/<scan>/depth_map_{vid:04d}.pfm, depth_visual_{vid:04d}.png   1600x1200
+        <root>/lists/{train,val}.txt               the scan lists (one scan per line)
+
+    Cam files hold the intrinsics of the 160x128 coarsest level, depth_min 425 and interval
+    2.65 as DTU's do.  Each light scales and shifts the view's texture differently.  Depth maps
+    (about `depth` mm) and masks exist for the reference views only; masks have holes and grey
+    levels other than 255.  Returns the root."""
+    import cv2
+    from PIL import Image
+    rng = np.random.default_rng(seed)
+    K = np.array([[1.1 * 160, 0, 80.0], [0, 1.1 * 160, 64.0], [0, 0, 1.0]])
+    os.makedirs(os.path.join(root, "Cameras", "train"), exist_ok=True)
+    for vid in range(49):
+        t = np.deg2rad(1.5 * (vid - 3))
+        E = np.eye(4)
+        E[:3, :3] = [[np.cos(t), 0, np.sin(t)], [0, 1, 0], [-np.sin(t), 0, np.cos(t)]]
+        E[:3, 3] = [-depth * np.sin(t), 0, depth * (1 - np.cos(t))]
+        with open(os.path.join(root, "Cameras", "train", f"{vid:08d}_cam.txt"), "w") as f:
+            f.write(_cam_text(K, E, 425.0, 2.65))
+    pairs = {r: sorted((v for v in range(49) if v != r), key=lambda v: (abs(v - r), v))[:n_src]
+             for r in refs}
+    lines = [str(len(refs))]
+    for r in refs:
+        lines += [str(r), f"{n_src} " + " ".join(f"{v} {100.0 - abs(v - r):.1f}" for v in pairs[r])]
+    with open(os.path.join(root, "Cameras", "pair.txt"), "w") as f:
+        f.write("\n".join(lines) + "\n")
+    img_dir = os.path.join(root, "Rectified", f"{scan}_train")
+    os.makedirs(img_dir, exist_ok=True)
+    for vid in sorted(set(refs) | {v for s in pairs.values() for v in s}):
+        base = _image(rng, 640, 512).astype(np.float32)
+        for light in range(7):
+            img = np.clip(base * (0.55 + 0.08 * light) + 6 * light - 10, 0, 255).astype(np.uint8)
+            Image.fromarray(img).save(os.path.join(img_dir, f"rect_{vid + 1:03d}_{light}_r5000.png"))
+    ddir = os.path.join(root, "Depths", scan)
+    os.makedirs(ddir, exist_ok=True)
+    yy, xx = np.mgrid[:1200, :1600]
+    for vid in refs:
+        dep = depth * (1 + 0.15 * np.sin(xx / 1600 * 4 + vid) * np.cos(yy / 1200 * 3)) \
+            + rng.normal(0, 0.5, (1200, 1600))
+        valid = (np.sin(xx / 97.0 + vid) + np.cos(yy / 61.0) > -1.2) & (rng.random((1200, 1600)) > 0.05)
+        dep = np.where(valid, dep, 0).astype(np.float32)
+        io.save_pfm(os.path.join(ddir, f"depth_map_{vid:04d}.pfm"), dep)
+        vis = np.where(valid, rng.integers(1, 256, (1200, 1600)), 0).astype(np.uint8)
+        cv2.imwrite(os.path.join(ddir, f"depth_visual_{vid:04d}.png"), vis)
+    os.makedirs(os.path.join(root, "lists"), exist_ok=True)
+    for split in ("train", "val"):
+        with open(os.path.join(root, "lists", f"{split}.txt"), "w") as f:
+            f.write(scan + "\n")
+    return root
 
 
 def main(argv=None):

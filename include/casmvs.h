@@ -305,6 +305,28 @@ int casmvs_regress_bwd(const float* logits, const float* depth_values, int dv_is
                        const float* grad_depth, float* grad_logits, int B, int D, int h, int w,
                        void* stream);
 
+/* ---- training loss and depth metrics (reference losses.py, metrics.py) ----------------------
+ * Per level l < levels (<= 4): pred[l], gt[l] (B,h_l,w_l) float32, mask[l] (B,h_l,w_l) uint8
+ * (bool; nonzero = valid); hw is a HOST array (levels,2) of (h_l, w_l); pred / gt / mask /
+ * grad_pred are HOST arrays of device pointers.
+ * casmvs_sl1_loss_fwd: loss (device float[1]) = sum_l 2^(1-l) * mean over the mask of
+ *   smoothL1(pred_l - gt_l) (beta 1); an empty mask gives NaN.  metrics (device float[5]) =
+ *   level 0's sum |e|, #(|e| < 1), #(|e| < 2), #(|e| < 4), n_0; counts (device int64[levels]) =
+ *   n_l.  Any output may be NULL.  Sums are fp64 in a fixed order (bit-identical run to run),
+ *   stored as fp32.  workspace: casmvs_sl1_loss_workspace_bytes() bytes of device memory.
+ * casmvs_sl1_loss_bwd: grad_pred[l] (device, all pixels written) = the gradient of that loss
+ *   given d(loss) = *grad_loss (device float) and the forward's counts, in ATen's operation
+ *   order (bit-identical to autograd of the reference's loss); 0 outside the mask. */
+size_t casmvs_sl1_loss_workspace_bytes(void);
+int casmvs_sl1_loss_fwd(const float* const* pred, const float* const* gt,
+                        const uint8_t* const* mask, const int* hw, int B, int levels, float* loss,
+                        float* metrics, long long* counts, void* workspace, size_t workspace_bytes,
+                        void* stream);
+int casmvs_sl1_loss_bwd(const float* const* pred, const float* const* gt,
+                        const uint8_t* const* mask, const int* hw, int B, int levels,
+                        const long long* counts, const float* grad_loss, float* const* grad_pred,
+                        void* stream);
+
 /* ---- input pipeline (SURVEY.md 8 f-4) -------------------------------------
  * T.ToTensor() + T.Normalize(mean, std) of the reference's data sets (datasets/dtu.py:130-137)
  * for images uploaded as bytes: images (N,H,W,3) uint8 RGB -> out (N,3,H,W) float32,
