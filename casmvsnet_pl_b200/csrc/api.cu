@@ -29,7 +29,7 @@ int conv3d_tma(const float* x, const float* wpk, const float* scale, const float
 // conv3d_tma2.cu (wgmma + TMA producer, persistent: stride-2 and transposed layers)
 int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
                 float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-                int w, int kind, int stride, int precision, int layout, cudaStream_t st);
+                int w, int kind, int stride, int precision_flags, int layout, cudaStream_t st);
 bool conv3d_tma_enabled();   // CASMVS_TMA
 int conv3d_tma2_modes();     // CASMVS_TMA2: bit 0 stride-2, bit 1 transposed
 
@@ -103,7 +103,7 @@ static int conv_layer(const float* x, const float* w_packed, const float* scale,
     if (rc <= 0) return rc;
     if (kind != CASMVS_CONV_PLANAR) {
       rc = conv3d_tma2(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
-                       stride, precision, layout, st);
+                       stride, pf, layout, st);
       if (rc <= 0) return rc;
     }
     CASMVS_REQUIRE(layout == 0, "conv3d: no tensor-core kernel for the blocked layer %d -> %d "

@@ -203,6 +203,15 @@ conv3d_wgrad_kernel(const float* __restrict__ X, const float* __restrict__ Gy,
     }
     __syncthreads();
     if (ta * 4 < Ca && tb * 4 < Cb) {
+      // each tile of kWgNV voxels is summed on its own, then added to the running sum: a CTA
+      // sums ~10^5 voxels per tap at training sizes, and one sequential fp32 sum over all of
+      // them loses ~sqrt(n) ulps of sum |x| |gy| when the terms share a sign (kernel input and
+      // gradient both non-negative), ~sqrt(n / kWgNV) this way
+      float part[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) part[i][j] = 0.f;
 #pragma unroll 4
       for (int vv = 0; vv < kWgNV; ++vv) {
         float a[4], g[4];
@@ -211,8 +220,12 @@ conv3d_wgrad_kernel(const float* __restrict__ X, const float* __restrict__ Gy,
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], g[j], acc[i][j]);
+          for (int j = 0; j < 4; ++j) part[i][j] = fmaf(a[i], g[j], part[i][j]);
       }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] += part[i][j];
     }
   }
 #pragma unroll

@@ -495,13 +495,15 @@ int conv3d_tma2_modes() {
 // Returns 0 when handled, 1 when the layer shape is left to the other kernels.
 int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
                 float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-                int w, int kind, int stride, int precision, int layout, cudaStream_t st) {
+                int w, int kind, int stride, int precision_flags, int layout, cudaStream_t st) {
   const int enabled = conv3d_tma2_modes();
-  if (!enabled || precision != CASMVS_TF32) return 1;
+  if (!enabled || (precision_flags & 0xff) != CASMVS_TF32) return 1;
   if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) return 1;
   tma2::Params p;
   p.scale = scale; p.shift = shift; p.skip = skip; p.y = y;
-  p.slope = slope; p.B = B; p.Di = D; p.Hi = h; p.Wi = w; p.Cout = Cout; p.round_out = 1;
+  p.slope = slope; p.B = B; p.Di = D; p.Hi = h; p.Wi = w; p.Cout = Cout;
+  // stored TF32-rounded for the next tensor-core layer unless the caller keeps the fp32 output
+  p.round_out = (precision_flags & CASMVS_KEEP_FP32_OUT) ? 0 : 1;
   p.x_blocked = (layout & kLayoutXBlocked) ? 1 : 0;
   p.y_blocked = (layout & kLayoutYBlocked) ? 1 : 0;
   if (kind == CASMVS_CONV && stride == 2 && (enabled & 1)) {
