@@ -57,6 +57,7 @@ SIGNATURES = {
                                               c_int, c_int, c_int, c_int, c_void_p]),
     "casmvs_depth_first_fwd": (c_int, [c_void_p, c_int, c_float, c_float, c_void_p, c_void_p,
                                        c_int, c_int, c_int, c_int, c_void_p]),
+    "casmvs_warp_cost_ladder_supported": (c_int, [c_int, c_int, c_int]),
     "casmvs_warp_cost_ladder_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p,
                                             c_float, c_void_p] + [c_int] * 8 + [c_void_p]),
     "casmvs_regress_ladder_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_float,

@@ -22,27 +22,28 @@ void set_error(const char* fmt, ...) {
 int conv3d_direct(const float* x, const float* wpk, const float* scale, const float* shift,
                   float slope, const float* skip, float* y, int B, int Cin, int Cout, int D,
                   int h, int w, int kind, int stride, cudaStream_t st, int round_out);
-// conv3d_tma.cu (wgmma + TMA producer, persistent: the stride-1 tensor path)
-int conv3d_tma(const float* x, const float* wpk, const float* scale, const float* shift,
-               float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-               int w, int kind, int stride, int precision, int layout, cudaStream_t st);
-// conv3d_tma2.cu (wgmma + TMA producer, persistent: stride-2 and transposed layers)
-int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
-                float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-                int w, int kind, int stride, int precision_flags, int layout, cudaStream_t st);
-bool conv3d_tma_enabled();   // CASMVS_TMA
-int conv3d_tma2_modes();     // CASMVS_TMA2: bit 0 stride-2, bit 1 transposed
+// The tensor-core kernels' coverage tables: the launcher of a layer shape, or null.
+// conv3d_tma.cu (wgmma + TMA producer, persistent): stride-1 and planar layers
+ConvLauncher conv3d_tma_find(int Cin, int Cout, int kind, int stride);
+// conv3d_tma2.cu (wgmma + TMA producer, persistent): stride-2 and transposed layers
+ConvLauncher conv3d_tma2_find(int Cin, int Cout, int kind, int stride, bool skip);
 
-struct LayerSpec { int cin, cout, kind, stride; };
+static ConvLauncher tensor_core_launcher(int Cin, int Cout, int kind, int stride, bool skip) {
+  if (ConvLauncher run = conv3d_tma_find(Cin, Cout, kind, stride)) return run;
+  return conv3d_tma2_find(Cin, Cout, kind, stride, skip);
+}
 
-// conv0..conv6, conv7, conv9, conv11, prob   (models/mvsnet.py:63-89)
+struct LayerSpec { int cin, cout, kind, stride; bool skip; };
+
+// conv0..conv6, conv7, conv9, conv11, prob   (models/mvsnet.py:63-89); conv7 .. conv11 add a skip
 static void costreg_layers(int Cin, LayerSpec (&L)[11]) {
   const LayerSpec t[11] = {
-      {Cin, 8, CASMVS_CONV, 1},  {8, 16, CASMVS_CONV, 2},  {16, 16, CASMVS_CONV, 1},
-      {16, 32, CASMVS_CONV, 2},  {32, 32, CASMVS_CONV, 1}, {32, 64, CASMVS_CONV, 2},
-      {64, 64, CASMVS_CONV, 1},  {64, 32, CASMVS_CONV_TRANSPOSE, 2},
-      {32, 16, CASMVS_CONV_TRANSPOSE, 2}, {16, 8, CASMVS_CONV_TRANSPOSE, 2},
-      {8, 1, CASMVS_CONV, 1}};
+      {Cin, 8, CASMVS_CONV, 1, false},  {8, 16, CASMVS_CONV, 2, false},
+      {16, 16, CASMVS_CONV, 1, false},  {16, 32, CASMVS_CONV, 2, false},
+      {32, 32, CASMVS_CONV, 1, false},  {32, 64, CASMVS_CONV, 2, false},
+      {64, 64, CASMVS_CONV, 1, false},  {64, 32, CASMVS_CONV_TRANSPOSE, 2, true},
+      {32, 16, CASMVS_CONV_TRANSPOSE, 2, true}, {16, 8, CASMVS_CONV_TRANSPOSE, 2, true},
+      {8, 1, CASMVS_CONV, 1, false}};
   memcpy(L, t, sizeof(t));
 }
 
@@ -95,16 +96,15 @@ static int conv_layer(const float* x, const float* w_packed, const float* scale,
                      (flags & ~CASMVS_KEEP_FP32_OUT) == 0, "conv3d: bad precision %d", precision);
   if (B == 0) return 0;
   cudaStream_t st = as_stream(stream);
+  // in the tf32 mode every stored activation is tf32-rounded (unbiased operand for the
+  // tensor-core layers); the prob head (Cout == 1) feeds the softmax and stays fp32
+  const int round_out =
+      (precision == CASMVS_TF32 && Cout > 1 && !(flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
   if (precision == CASMVS_TF32) {
-    const int pf = precision | flags;
-    // tensor-core kernels: each returns 0 (handled), <0 (failed) or 1 (shape not covered)
-    int rc = conv3d_tma(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
-                        stride, pf, layout, st);
-    if (rc <= 0) return rc;
-    if (kind != CASMVS_CONV_PLANAR) {
-      rc = conv3d_tma2(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
-                       stride, pf, layout, st);
-      if (rc <= 0) return rc;
+    if (ConvLauncher run = tensor_core_launcher(Cin, Cout, kind, stride, skip != nullptr)) {
+      const ConvArgs a{x, w_packed, scale, shift, skip, y, slope, B, Cin, Cout, D, h, w, layout,
+                       round_out};
+      return run(a, st);
     }
     CASMVS_REQUIRE(layout == 0, "conv3d: no tensor-core kernel for the blocked layer %d -> %d "
                    "(kind %d, stride %d)", Cin, Cout, kind, stride);
@@ -112,18 +112,19 @@ static int conv_layer(const float* x, const float* w_packed, const float* scale,
     // storage convention).  Counted, so callers can assert the fast path was taken.
     g_fallbacks.fetch_add(1, std::memory_order_relaxed);
   }
-  // in the tf32 modes every stored activation is tf32-rounded (unbiased operand for
-  // the tensor-core layers); the prob head (Cout == 1) feeds the softmax and stays fp32
-  const int round_out =
-      (precision == CASMVS_TF32 && Cout > 1 && !(flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
   return conv3d_direct(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind,
                        stride, st, round_out);
 }
 
+// Every kernel reads x in 16-byte vectors; y and skip are read and written in 16-byte vectors
+// unless Cout == 1.
 extern "C" int casmvs_conv3d_fwd(const float* x, const float* w_packed, const float* scale,
                                  const float* shift, float slope, const float* skip, float* y,
                                  int B, int Cin, int Cout, int D, int h, int w, int kind,
                                  int stride, int precision, void* stream) {
+  CASMVS_REQUIRE_ALIGNED("conv3d", x, 16);
+  CASMVS_REQUIRE_ALIGNED("conv3d", y, Cout > 1 ? 16 : 4);
+  CASMVS_REQUIRE_ALIGNED("conv3d", skip, Cout > 1 ? 16 : 4);
   return conv_layer(x, w_packed, scale, shift, slope, skip, y, B, Cin, Cout, D, h, w, kind, stride,
                     precision, 0, stream);
 }
@@ -167,25 +168,30 @@ extern "C" size_t casmvs_costreg_workspace_bytes(int B, int Cin, int D, int h, i
 }
 
 extern "C" int casmvs_costreg_blocked_supported(int Cin, int precision) {
-  // the blocked layout has only tensor-core kernels: every layer must be one of theirs.  conv1 ..
-  // prob have fixed shapes that they cover; conv0 is covered for Cin in {8, 16, 32}
-  return precision == CASMVS_TF32 && conv3d_tma_enabled() && (conv3d_tma2_modes() & 3) == 3 &&
-         (Cin == 8 || Cin == 16 || Cin == 32);
+  // the blocked layout has only tensor-core kernels: every layer must be one of theirs
+  if (precision != CASMVS_TF32) return 0;
+  LayerSpec L[11];
+  costreg_layers(Cin, L);
+  for (const LayerSpec& l : L)
+    if (!tensor_core_launcher(l.cin, l.cout, l.kind, l.stride, l.skip)) return 0;
+  return 1;
 }
 
+// x and the activations in the workspace are read in 16-byte vectors (the workspace offsets are
+// multiples of 256 B); the prob head writes the logits one float at a time.
 extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* logits, int B,
                                   int Cin, int D, int h, int w, int precision, void* workspace,
                                   size_t workspace_bytes, void* stream) {
+  CASMVS_REQUIRE_ALIGNED("costreg", x, 16);
+  CASMVS_REQUIRE_ALIGNED("costreg", workspace, 16);
+  CASMVS_REQUIRE_ALIGNED("costreg", logits, 4);
   CASMVS_REQUIRE(x && params && logits, "costreg: null pointer");
   const bool blocked_in = (precision & CASMVS_BLOCKED) != 0;
   precision &= ~CASMVS_BLOCKED;
-  // the tensor maps need 16-byte aligned bases (the workspace offsets are multiples of 256 B)
-  const bool blocked = casmvs_costreg_blocked_supported(Cin, precision) &&
-                       ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(workspace)) &
-                        15) == 0;
+  const bool blocked = casmvs_costreg_blocked_supported(Cin, precision);
   CASMVS_REQUIRE(!blocked_in || blocked,
-                 "costreg: a blocked input needs the TF32 precision, Cin in {8,16,32}, the "
-                 "tensor-core kernels enabled and 16-byte aligned x and workspace (got Cin=%d)", Cin);
+                 "costreg: a blocked input needs the TF32 precision and a Cin whose conv0 a "
+                 "tensor-core kernel covers (8, 16 or 32; got Cin=%d)", Cin);
   CASMVS_REQUIRE(D % 8 == 0 && h % 8 == 0 && w % 8 == 0,
                  "costreg: D,h,w must be divisible by 8 (got %d,%d,%d)", D, h, w);
   const size_t need = casmvs_costreg_workspace_bytes(B, Cin, D, h, w);

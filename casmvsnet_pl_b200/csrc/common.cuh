@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <atomic>
 
 #include "casmvs.h"
@@ -21,10 +22,20 @@ extern std::atomic<uint64_t> g_fallbacks;
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
-// Layout bits of the internal conv entry points (conv3d_tma / conv3d_tma2): the input, or the
+// Layout bits of the tensor-core conv launchers (ConvArgs::layout): the input, or the
 // output and the skip, stored blocked by channel quads (B, C/4, D, H, W, 4) instead of
 // channels-last (B, D, H, W, C).  Only the CostRegNet driver passes them; see DESIGN.md §2.
 constexpr int kLayoutXBlocked = 1, kLayoutYBlocked = 2;
+
+// A convolution layer (input dims) for a tensor-core launcher, which returns 0 or <0 (error).
+// The coverage tables of conv3d_tma.cu and conv3d_tma2.cu map layer shapes to launchers.
+struct ConvArgs {
+  const float *x, *wpk, *scale, *shift, *skip;
+  float* y;
+  float slope;
+  int B, Cin, Cout, D, h, w, layout, round_out;
+};
+using ConvLauncher = int (*)(const ConvArgs& a, cudaStream_t st);
 
 // call after every kernel launch: counts it and converts launch errors
 inline int after_launch(const char* what) {
@@ -44,6 +55,28 @@ inline int after_launch(const char* what) {
       return -1;                         \
     }                                    \
   } while (0)
+
+// Entry-point check of a device pointer that the kernels behind it access in `bytes`-wide
+// vectors (null passes: the null checks come after).
+#define CASMVS_REQUIRE_ALIGNED(what, ptr, bytes)                                              \
+  CASMVS_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & ((bytes) - 1)) == 0,                     \
+                 "%s: %s must be %d-byte aligned (got %p)", what, #ptr, (int)(bytes),         \
+                 (const void*)(ptr))
+
+// The environment switches of DESIGN.md §5, read once per process: the function-local static
+// is initialised on first use, thread-safely.
+struct Switches { bool k1_smem, k3_reg, pdl; int tma_dchunk; };
+inline const Switches& switches() {
+  static const Switches s = [] {
+    auto get = [](const char* name, int unset) {
+      const char* e = getenv(name);
+      return e ? atoi(e) : unset;
+    };
+    return Switches{get("CASMVS_K1_SMEM", 1) != 0, get("CASMVS_K3_REG", 1) != 0,
+                    get("CASMVS_PDL", 1) != 0, get("CASMVS_TMA_DCHUNK", 0)};
+  }();
+  return s;
+}
 
 // Host-side state is kept per device ordinal: cudaFuncSetAttribute and the SM count are
 // per-device properties, and a process may drive several GPUs (model.to("cuda:1")).

@@ -26,7 +26,6 @@
 // wgmma are issued and group 0's epilogue runs while they execute.  N = 3 x GW with GW = 8 for
 // Cout <= 8 (conv0, prob, FeatureNet's last smoothing layer), else 16 or 32.
 #include <cudaTypedefs.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -361,32 +360,39 @@ const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, 
 }
 
 
+// One CTA computes GW output columns (Cout <= GW, or a GW-channel slice of a wider Cout).
 template <int CIN, int GW, int SLOTS, bool PLANAR>
-static int launch(const float* x, const float* wpk, Params p, cudaStream_t st) {
+static int launch(const ConvArgs& a, cudaStream_t st) {
   using S = Smem<CIN, GW, SLOTS>;
   static_assert(S::kTotal <= 227 * 1024, "shared memory budget");
   auto kfn = conv3d_tma_kernel<CIN, GW, SLOTS, PLANAR>;
   static std::atomic<bool> attr_set[kMaxDevices];
   if (int rc = opt_in_smem(kfn, S::kTotal, attr_set, "conv3d_tma")) return rc;
-  const CUtensorMap* map = input_map(x, p.B, p.D, p.H, p.W, CIN, 4, kHaloW, kHaloH, 1, p.x_blocked);
+  Params p;
+  p.scale = a.scale; p.shift = a.shift; p.skip = a.skip; p.y = a.y;
+  p.slope = a.slope; p.B = a.B; p.D = a.D; p.H = a.h; p.W = a.w;
+  p.Cout = a.Cout < GW ? a.Cout : GW; p.cout_total = a.Cout;
+  p.tiles_w = (a.w + tc::kTileW - 1) / tc::kTileW;
+  p.tiles_h = (a.h + tc::kTileH - 1) / tc::kTileH;
+  p.planar = PLANAR ? 1 : 0;
+  p.x_blocked = (a.layout & kLayoutXBlocked) ? 1 : 0;
+  p.y_blocked = (a.layout & kLayoutYBlocked) ? 1 : 0;
+  p.round_out = a.round_out;
+  const CUtensorMap* map = input_map(a.x, p.B, p.D, p.H, p.W, CIN, 4, kHaloW, kHaloH, 1, p.x_blocked);
   if (!map) return -2;
-  static int dchunk_env = -1;
-  if (dchunk_env < 0) {
-    const char* d = getenv("CASMVS_TMA_DCHUNK");
-    dchunk_env = d ? atoi(d) : 0;
-  }
   const int per_sm = resident_per_sm(kfn, kConvThreads, S::kTotal);
   const int nco = p.cout_total / p.Cout;
   const int cap = 32;
   const long cols = (long)p.B * p.tiles_w * p.tiles_h;
   int dchunk = pick_dchunk(p.D, cap, cols, (long)num_sms() * per_sm / nco, 1, p.planar ? 0 : 2);
+  const int dchunk_env = switches().tma_dchunk;
   if (dchunk_env > 0 && dchunk_env <= cap) dchunk = dchunk_env < p.D ? dchunk_env : p.D;
   p.dchunk = dchunk;
   p.nchunks = (p.D + dchunk - 1) / dchunk;
-  const ImageRef ir = image_cache_get(wpk, 1000 + CIN * 100 + GW, (size_t)S::kWBytes * nco, st);
+  const ImageRef ir = image_cache_get(a.wpk, 1000 + CIN * 100 + GW, (size_t)S::kWBytes * nco, st);
   if (!ir.img) return -2;
   if (!ir.hit) {
-    if (int rc = build_stride1_image(wpk, ir.img, CIN, GW, p.Cout, p.cout_total, st)) return rc;
+    if (int rc = build_stride1_image(a.wpk, ir.img, CIN, GW, p.Cout, p.cout_total, st)) return rc;
     image_cache_built(ir.img, st);
   }
   p.bimg = ir.img;
@@ -398,54 +404,29 @@ static int launch(const float* x, const float* wpk, Params p, cudaStream_t st) {
   return after_launch("conv3d_tma");
 }
 
+// Coverage: the stride-1 and planar layer shapes this kernel is instantiated for.  Cout in
+// [cout_lo, cout_hi] runs on GW output columns; conv6 (64 -> 64) as four 16-column slices.
+struct Shape {
+  int cin, cout_lo, cout_hi;
+  ConvLauncher conv, planar;
+};
+#define S1(CI, LO, HI, GW, SL) {CI, LO, HI, launch<CI, GW, SL, false>, launch<CI, GW, SL, true>}
+static const Shape kShapes[] = {
+    S1(8, 1, 8, 8, 4),    S1(8, 17, 32, 32, 4),
+    S1(16, 1, 8, 8, 4),   S1(16, 9, 16, 16, 4),  S1(16, 17, 32, 32, 4),
+    S1(32, 1, 8, 8, 4),   S1(32, 9, 16, 16, 4),  S1(32, 17, 32, 32, 4),
+    S1(64, 64, 64, 16, 2),
+};
+#undef S1
+
 }  // namespace tma
 
-// CASMVS_TMA (default 1): 0 leaves every layer to the other kernels.
-bool conv3d_tma_enabled() {
-  static const int enabled = [] {
-    const char* e = getenv("CASMVS_TMA");
-    return e ? atoi(e) : 1;
-  }();
-  return enabled != 0;
-}
-
-// Returns 0 when handled, 1 when the layer shape is left to the other kernels.
-int conv3d_tma(const float* x, const float* wpk, const float* scale, const float* shift,
-               float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-               int w, int kind, int stride, int precision_flags, int layout, cudaStream_t st) {
-  const int precision = precision_flags & 0xff;
-  static const int round_out = [] {
-    const char* s = getenv("CASMVS_TC_ROUND");
-    return s ? atoi(s) : 1;
-  }();
-  if (!conv3d_tma_enabled() || precision != CASMVS_TF32) return 1;
-  if ((kind != CASMVS_CONV && kind != CASMVS_CONV_PLANAR) || stride != 1) return 1;
-  if (kind == CASMVS_CONV_PLANAR && layout != 0) return 1;   // planar layers are channels-last only
-  const bool deep = Cin == 64 && Cout == 64;          // conv6: 16-channel Cout slices
-  if (!deep && (!(Cin == 8 || Cin == 16 || Cin == 32) || Cout > 32)) return 1;
-  // the TMA global strides must be multiples of 16 B and the base 16 B aligned
-  if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) return 1;
-  tma::Params p;
-  p.scale = scale; p.shift = shift; p.skip = skip; p.y = y;
-  p.slope = slope; p.B = B; p.D = D; p.H = h; p.W = w;
-  p.Cout = deep ? 16 : Cout; p.cout_total = Cout;
-  p.tiles_w = (w + tc::kTileW - 1) / tc::kTileW;
-  p.tiles_h = (h + tc::kTileH - 1) / tc::kTileH;
-  const int npad = p.Cout <= 8 ? 8 : p.Cout <= 16 ? 16 : 32;
-  p.planar = kind == CASMVS_CONV_PLANAR ? 1 : 0;
-  p.x_blocked = (layout & kLayoutXBlocked) ? 1 : 0;
-  p.y_blocked = (layout & kLayoutYBlocked) ? 1 : 0;
-  // the prob head feeds the softmax: keep fp32; callers can ask for unrounded outputs
-  p.round_out = (round_out && Cout > 1 && !(precision_flags & CASMVS_KEEP_FP32_OUT)) ? 1 : 0;
-#define TMA_CASE(CI, NP, SL)                                                    \
-  if (Cin == CI && npad == NP)                                                  \
-    return p.planar ? tma::launch<CI, NP, SL, true>(x, wpk, p, st)              \
-                    : tma::launch<CI, NP, SL, false>(x, wpk, p, st);
-  TMA_CASE(8, 8, 4) TMA_CASE(8, 32, 4) TMA_CASE(16, 8, 4) TMA_CASE(16, 16, 4)
-  TMA_CASE(16, 32, 4) TMA_CASE(32, 8, 4) TMA_CASE(32, 16, 4) TMA_CASE(32, 32, 4)
-  TMA_CASE(64, 16, 2)
-#undef TMA_CASE
-  return 1;
+ConvLauncher conv3d_tma_find(int Cin, int Cout, int kind, int stride) {
+  if ((kind != CASMVS_CONV && kind != CASMVS_CONV_PLANAR) || stride != 1) return nullptr;
+  for (const tma::Shape& s : tma::kShapes)
+    if (s.cin == Cin && s.cout_lo <= Cout && Cout <= s.cout_hi)
+      return kind == CASMVS_CONV_PLANAR ? s.planar : s.conv;
+  return nullptr;
 }
 
 }  // namespace casmvs

@@ -33,8 +33,6 @@
 //   ConvBnReLU(k=5, stride=2, pad=2)               models/modules.py:8-18, mvsnet.py:16,20
 //   ConvBnReLU3D(stride=2)                         models/modules.py:21-31, mvsnet.py:65,68,71
 //   ConvTranspose3d(k3,s2,p1,op1) + norm_act + skip models/mvsnet.py:74-87,99-101
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "tma_common.cuh"
@@ -431,20 +429,31 @@ __global__ void build_image_p5_kernel(const float* __restrict__ wt, float* __res
   }
 }
 
+// MODE_S2 / MODE_P5: output = (in - 1) / 2 + 1 along H and W (and D for MODE_S2); MODE_T:
+// output = 2x input.  A CTA computes a COUT-channel slice of a.Cout.
 template <int MODE, int CIN, int COUT>
-static int launch2(const float* x, const float* wpk, Params p, cudaStream_t st) {
+static int launch2(const ConvArgs& a, cudaStream_t st) {
   using C = Cfg<MODE, CIN, COUT>;
   static_assert(C::kTotal <= 227 * 1024, "shared memory budget");
   auto kfn = conv3d_tma2_kernel<MODE, CIN, COUT>;
   static std::atomic<bool> attr_set[kMaxDevices];
   if (int rc = opt_in_smem(kfn, C::kTotal, attr_set, "conv3d_tma2")) return rc;
+  Params p;
+  p.scale = a.scale; p.shift = a.shift; p.skip = a.skip; p.y = a.y;
+  p.slope = a.slope; p.B = a.B; p.Di = a.D; p.Hi = a.h; p.Wi = a.w; p.Cout = a.Cout;
+  p.Do = MODE == MODE_T ? 2 * a.D : MODE == MODE_S2 ? (a.D - 1) / 2 + 1 : a.D;
+  p.Ho = MODE == MODE_T ? 2 * a.h : (a.h - 1) / 2 + 1;
+  p.Wo = MODE == MODE_T ? 2 * a.w : (a.w - 1) / 2 + 1;
+  p.round_out = a.round_out;
+  p.x_blocked = (a.layout & kLayoutXBlocked) ? 1 : 0;
+  p.y_blocked = (a.layout & kLayoutYBlocked) ? 1 : 0;
   // S2: box {4, 17 traversed -> 9 loaded, 33, 1, 1} walking W with stride 2; T: {4, 9, 17}
   // P5: box {4, 19 traversed -> 10 loaded, 35, 1, 1} walking W with stride 2
   const CUtensorMap* map =
-      MODE == MODE_S2   ? tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 17, C::BR, 2,
+      MODE == MODE_S2   ? tma::input_map(a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 17, C::BR, 2,
                                          p.x_blocked)
-      : MODE == MODE_P5 ? tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 19, C::BR, 2)
-                        : tma::input_map(x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, C::BW, C::BR, 1,
+      : MODE == MODE_P5 ? tma::input_map(a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 19, C::BR, 2)
+                        : tma::input_map(a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, C::BW, C::BR, 1,
                                          p.x_blocked);
   if (!map) return -2;
   const int per_sm = tma::resident_per_sm(kfn, kConvThreads, C::kTotal);
@@ -461,15 +470,15 @@ static int launch2(const float* x, const float* wpk, Params p, cudaStream_t st) 
   p.dchunk = dchunk;
   p.nchunks = (Dm + dchunk - 1) / dchunk;
   const long items = cols * p.nchunks;
-  const ImageRef ir = image_cache_get(wpk, 2000 + MODE * 10000 + CIN * 100 + COUT,
+  const ImageRef ir = image_cache_get(a.wpk, 2000 + MODE * 10000 + CIN * 100 + COUT,
                                       (size_t)C::kWBytes * nco, st);
   float* img = ir.img;
   if (!img) return -2;
   if (!ir.hit) {
     if constexpr (MODE == MODE_P5)
-      build_image_p5_kernel<CIN, COUT><<<32, 256, 0, st>>>(wpk, img);
+      build_image_p5_kernel<CIN, COUT><<<32, 256, 0, st>>>(a.wpk, img);
     else
-      build_image_tma2_kernel<MODE, CIN, COUT><<<64, 256, 0, st>>>(wpk, img, p.Cout);
+      build_image_tma2_kernel<MODE, CIN, COUT><<<64, 256, 0, st>>>(a.wpk, img, p.Cout);
     if (int rc = after_launch("conv3d_tma2/build_image")) return rc;
     image_cache_built(img, st);
   }
@@ -481,47 +490,29 @@ static int launch2(const float* x, const float* wpk, Params p, cudaStream_t st) 
   return after_launch("conv3d_tma2");
 }
 
+// Coverage: the CostRegNet layer shapes this kernel is instantiated for (stride 2).  The
+// stride-2 epilogue has no skip input.
+struct Shape {
+  int kind, cin, cout;
+  bool skip;
+  ConvLauncher run;
+};
+static const Shape kShapes[] = {
+    {CASMVS_CONV, 8, 16, false, launch2<MODE_S2, 8, 16>},
+    {CASMVS_CONV, 16, 32, false, launch2<MODE_S2, 16, 32>},
+    {CASMVS_CONV, 32, 64, false, launch2<MODE_S2, 32, 16>},
+    {CASMVS_CONV_TRANSPOSE, 16, 8, true, launch2<MODE_T, 16, 8>},
+    {CASMVS_CONV_TRANSPOSE, 32, 16, true, launch2<MODE_T, 32, 16>},
+    {CASMVS_CONV_TRANSPOSE, 64, 32, true, launch2<MODE_T, 64, 8>},
+};
+
 }  // namespace tma2
 
-// CASMVS_TMA2 (default 3): bit 0 enables the stride-2 layers, bit 1 the transposed ones.
-int conv3d_tma2_modes() {
-  static const int modes = [] {
-    const char* e = getenv("CASMVS_TMA2");
-    return e ? atoi(e) : 3;
-  }();
-  return modes;
-}
-
-// Returns 0 when handled, 1 when the layer shape is left to the other kernels.
-int conv3d_tma2(const float* x, const float* wpk, const float* scale, const float* shift,
-                float slope, const float* skip, float* y, int B, int Cin, int Cout, int D, int h,
-                int w, int kind, int stride, int precision_flags, int layout, cudaStream_t st) {
-  const int enabled = conv3d_tma2_modes();
-  if (!enabled || (precision_flags & 0xff) != CASMVS_TF32) return 1;
-  if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) return 1;
-  tma2::Params p;
-  p.scale = scale; p.shift = shift; p.skip = skip; p.y = y;
-  p.slope = slope; p.B = B; p.Di = D; p.Hi = h; p.Wi = w; p.Cout = Cout;
-  // stored TF32-rounded for the next tensor-core layer unless the caller keeps the fp32 output
-  p.round_out = (precision_flags & CASMVS_KEEP_FP32_OUT) ? 0 : 1;
-  p.x_blocked = (layout & kLayoutXBlocked) ? 1 : 0;
-  p.y_blocked = (layout & kLayoutYBlocked) ? 1 : 0;
-  if (kind == CASMVS_CONV && stride == 2 && (enabled & 1)) {
-    if (skip) return 1;
-    p.Do = (D - 1) / 2 + 1; p.Ho = (h - 1) / 2 + 1; p.Wo = (w - 1) / 2 + 1;
-    if (Cin == 8 && Cout == 16) return tma2::launch2<tma2::MODE_S2, 8, 16>(x, wpk, p, st);
-    if (Cin == 16 && Cout == 32) return tma2::launch2<tma2::MODE_S2, 16, 32>(x, wpk, p, st);
-    if (Cin == 32 && Cout == 64) return tma2::launch2<tma2::MODE_S2, 32, 16>(x, wpk, p, st);
-    return 1;
-  }
-  if (kind == CASMVS_CONV_TRANSPOSE && (enabled & 2)) {
-    p.Do = 2 * D; p.Ho = 2 * h; p.Wo = 2 * w;
-    if (Cin == 16 && Cout == 8) return tma2::launch2<tma2::MODE_T, 16, 8>(x, wpk, p, st);
-    if (Cin == 32 && Cout == 16) return tma2::launch2<tma2::MODE_T, 32, 16>(x, wpk, p, st);
-    if (Cin == 64 && Cout == 32) return tma2::launch2<tma2::MODE_T, 64, 8>(x, wpk, p, st);
-    return 1;
-  }
-  return 1;
+ConvLauncher conv3d_tma2_find(int Cin, int Cout, int kind, int stride, bool skip) {
+  if (stride != 2) return nullptr;
+  for (const tma2::Shape& s : tma2::kShapes)
+    if (s.kind == kind && s.cin == Cin && s.cout == Cout && (s.skip || !skip)) return s.run;
+  return nullptr;
 }
 
 }  // namespace casmvs
@@ -531,18 +522,15 @@ using namespace casmvs;
 extern "C" int casmvs_conv2d_5x5s2_fwd(const float* x, const float* w, const float* shift,
                                        float slope, float* y, int N, int Cin, int Cout, int H,
                                        int W, int round_tf32, void* stream) {
+  CASMVS_REQUIRE_ALIGNED("conv2d_5x5s2", x, 16);
   CASMVS_REQUIRE(x && w && y, "conv2d_5x5s2: null pointer");
   CASMVS_REQUIRE(N >= 0 && H >= 2 && W >= 2, "conv2d_5x5s2: bad dims");
-  CASMVS_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "conv2d_5x5s2: x must be 16 B aligned");
   if (N == 0) return 0;
-  tma2::Params p;
-  p.scale = nullptr; p.shift = shift; p.skip = nullptr; p.y = y; p.slope = slope;
-  p.B = 1; p.Di = N; p.Hi = H; p.Wi = W; p.Do = N; p.Ho = (H - 1) / 2 + 1; p.Wo = (W - 1) / 2 + 1;
-  p.Cout = Cout; p.round_out = round_tf32 ? 1 : 0;
-  p.x_blocked = p.y_blocked = 0;
+  const ConvArgs a{x, w, nullptr, shift, nullptr, y, slope, 1, Cin, Cout, N, H, W, 0,
+                   round_tf32 ? 1 : 0};
   cudaStream_t st = as_stream(stream);
-  if (Cin == 8 && Cout == 16) return tma2::launch2<tma2::MODE_P5, 8, 16>(x, w, p, st);
-  if (Cin == 16 && Cout == 32) return tma2::launch2<tma2::MODE_P5, 16, 32>(x, w, p, st);
+  if (Cin == 8 && Cout == 16) return tma2::launch2<tma2::MODE_P5, 8, 16>(a, st);
+  if (Cin == 16 && Cout == 32) return tma2::launch2<tma2::MODE_P5, 16, 32>(a, st);
   set_error("conv2d_5x5s2: only the FeatureNet shapes 8->16 and 16->32 are built (got %d->%d)",
             Cin, Cout);
   return -1;

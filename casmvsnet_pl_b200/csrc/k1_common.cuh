@@ -170,4 +170,11 @@ struct HypPix {
   }
 };
 
+// The TMA-staged cost-volume kernels (warp_cost_smem.cu): channels-last features, channels-last
+// or (blocked != 0) blocked output.  warp_cost_staged returns the launcher of a shape from their
+// coverage table, or null (the shape runs on the gather kernel, or not at all from a ladder).
+using StagedK1 = int (*)(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
+                         int D, int h, int w, int rnd, int blocked, cudaStream_t st);
+StagedK1 warp_cost_staged(int V, int C, int num_groups);
+
 }  // namespace casmvs

@@ -7,8 +7,6 @@
 //   get_depth_values                models/modules.py:34-49
 //   x2 bilinear upsample            models/mvsnet.py:231-234
 //   initial uniform planes          models/mvsnet.py:213-229
-#include <stdlib.h>
-
 #include "k1_common.cuh"
 
 namespace casmvs {
@@ -262,11 +260,7 @@ static int regress_impl(const float* logits, const float* depth_values, int dv_i
   if (B == 0) return 0;
   const int hw = h * w;
   cudaStream_t st = as_stream(stream);
-  static int par_path = -1;
-  if (par_path < 0) {
-    const char* e = getenv("CASMVS_K3_REG");      // 0: the one-thread-per-pixel generic kernel
-    par_path = e ? atoi(e) : 1;
-  }
+  const bool par_path = switches().k3_reg;
   const size_t smem = ((size_t)3 * D * 32 + kK3Lanes * 32) * sizeof(float);
   if (D == 8 && par_path) {
     // 8 hypotheses fit a thread's registers and there are plenty of pixels at the finest level:

@@ -1,7 +1,6 @@
 // TMA helpers shared by the TMA-fed tensor-core convolution kernels (sm_90a).
 #pragma once
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "tc_common.cuh"
 
@@ -54,11 +53,6 @@ __device__ __forceinline__ void pdl_trigger() {
 template <typename Kernel, typename... Args>
 inline cudaError_t launch_pdl(bool allow, Kernel kfn, dim3 grid, int threads, size_t smem,
                               cudaStream_t st, Args... args) {
-  static int pdl = -1;
-  if (pdl < 0) {
-    const char* e = getenv("CASMVS_PDL");
-    pdl = e ? atoi(e) : 1;
-  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = dim3((unsigned)threads);
@@ -68,7 +62,7 @@ inline cudaError_t launch_pdl(bool allow, Kernel kfn, dim3 grid, int threads, si
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = (pdl && allow) ? 1 : 0;
+  cfg.numAttrs = (switches().pdl && allow) ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kfn, args...);
 }
 
@@ -133,19 +127,12 @@ inline int resident_per_sm(K kfn, int threads, int smem) {
 }
 
 // Depth-chunk length for the persistent kernels.  An item (tile column x depth chunk of dc
-// output groups) costs mul*dc + add input slices (+ `fixed` for pipeline fill / drain); CTA k
-// runs items k, k + resident, ...: the kernel lasts as long as the busiest CTA, i.e.
-// ceil(items / resident) items.  Long chunks amortise the depth halo, short ones fill the
-// machine and balance the last round; pick the cheapest (ties -> longer chunks).
-inline int pick_dchunk(int D, int cap, long cols, long resident, int mul, int add, int fixed = -1) {
-  if (fixed < 0) {                      // CASMVS_DCHUNK_FIXED: per-item overhead in slice units
-    static int env_fixed = -1;
-    if (env_fixed < 0) {
-      const char* e = getenv("CASMVS_DCHUNK_FIXED");
-      env_fixed = e ? atoi(e) : 0;   // measured on cfg2: 0 -> 1.0876, 1 -> 1.0888, 2 -> 1.0938 ms/step
-    }
-    fixed = env_fixed;
-  }
+// output groups) costs mul*dc + add input slices; CTA k runs items k, k + resident, ...: the
+// kernel lasts as long as the busiest CTA, i.e. ceil(items / resident) items.  Long chunks
+// amortise the depth halo, short ones fill the machine and balance the last round; pick the
+// cheapest (ties -> longer chunks).  Charging a further 1 or 2 slices per item for pipeline fill
+// was measured slower on cfg2 (1.0876 -> 1.0888 / 1.0938 ms per step).
+inline int pick_dchunk(int D, int cap, long cols, long resident, int mul, int add) {
   if (cap > D) cap = D;
   if (cap < 1) cap = 1;
   if (resident < 1) resident = 1;
@@ -154,7 +141,7 @@ inline int pick_dchunk(int D, int cap, long cols, long resident, int mul, int ad
   for (int dc = cap; dc >= 1; --dc) {
     const long items = cols * ((D + dc - 1) / dc);
     const long rounds = (items + resident - 1) / resident;
-    const long cost = rounds * (mul * dc + add + fixed);
+    const long cost = rounds * (mul * dc + add);
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = dc; }
   }
   return best;

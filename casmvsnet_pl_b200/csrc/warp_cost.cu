@@ -308,11 +308,6 @@ static int launch_transpose(const float* in, float* out, int N, size_t R, size_t
   return after_launch(what);
 }
 
-// warp_cost_smem.cu
-int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
-                  int V, int C, int D, int h, int w, int num_groups, int rnd, int blocked,
-                  cudaStream_t st);
-
 template <int NSRC, int CT>
 static void launch_k1(bool gwc, bool nhwc, dim3 grd, cudaStream_t st, const float* f,
                       const float* p, const float* dv, float* cost, int V, int C, int D, int h,
@@ -348,10 +343,16 @@ extern "C" size_t casmvs_warp_cost_workspace_bytes(int feat_layout, int B, int V
   return (size_t)B * V * C * h * w * sizeof(float);
 }
 
+// Every K1 kernel reads the channels-last features (feats, or the workspace NCHW features are
+// re-laid-out into) in 16-byte vectors, and writes a channels-last cost volume in vectors of up
+// to 16 bytes.
 extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const float* proj,
                                     const float* depth_values, float* cost, int cost_layout,
                                     int B, int V, int C, int D, int h, int w, int num_groups,
                                     void* workspace, size_t workspace_bytes, void* stream) {
+  if (feat_layout == CASMVS_NHWC) CASMVS_REQUIRE_ALIGNED("warp_cost", feats, 16);
+  else CASMVS_REQUIRE_ALIGNED("warp_cost", workspace, 16);
+  if ((cost_layout & ~CASMVS_ROUND_TF32) == CASMVS_NHWC) CASMVS_REQUIRE_ALIGNED("warp_cost", cost, 16);
   CASMVS_REQUIRE(feats && proj && depth_values && cost, "warp_cost: null pointer");
   CASMVS_REQUIRE(B >= 0 && V >= 2 && C > 0 && D > 0 && h >= 2 && w >= 2, "warp_cost: bad dims (h,w >= 2)");
   CASMVS_REQUIRE(V - 1 <= kMaxSrc, "warp_cost: at most %d source views", kMaxSrc);
@@ -386,11 +387,9 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   const bool nhwc = cost_layout == CASMVS_NHWC;
   const long threads = (long)h * w * (C / kCPT);
   const unsigned xblocks = (unsigned)((threads + kK1Threads - 1) / kK1Threads);
-  if (nhwc) {
-    // TMA-staged generation (warp_cost_smem.cu): 0 = handled, 1 = shape left to the gather kernel
+  if (StagedK1 run = nhwc ? warp_cost_staged(V, C, num_groups) : nullptr) {
     const Hyp hyp{depth_values, nullptr, nullptr, nullptr, 0.f, 0.f};
-    const int rc = warp_var_smem(f, proj, hyp, cost, B, V, C, D, h, w, num_groups, rnd, 0, st);
-    if (rc <= 0) return rc;
+    return run(f, proj, hyp, cost, B, D, h, w, rnd, 0, st);
   }
   // depth chunks: enough CTAs to fill every SM several times over, but chunks long
   // enough (>= 8 planes) for the texel-window cache to pay off
@@ -409,9 +408,12 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   return after_launch("warp_cost");
 }
 
+// 16-byte vectors: the features, and a channels-last output.
 extern "C" int casmvs_homo_warp_fwd(const float* src_feat, int feat_layout, const float* proj,
                                     const float* depth_values, float* warped, int out_layout,
                                     int B, int C, int D, int h, int w, void* stream) {
+  CASMVS_REQUIRE_ALIGNED("homo_warp", src_feat, 16);
+  if (out_layout == CASMVS_NHWC) CASMVS_REQUIRE_ALIGNED("homo_warp", warped, 16);
   CASMVS_REQUIRE(src_feat && proj && depth_values && warped, "homo_warp: null pointer");
   CASMVS_REQUIRE(feat_layout == CASMVS_NHWC,
                  "homo_warp: features must be channels-last (use casmvs_nchw_to_nhwc)");
@@ -442,28 +444,31 @@ extern "C" int casmvs_nhwc_to_nchw(const float* in, float* out, int N, int C, si
   return launch_transpose(in, out, N, S, (size_t)C, as_stream(stream), "nhwc_to_nchw");
 }
 
+extern "C" int casmvs_warp_cost_ladder_supported(int V, int C, int num_groups) {
+  return warp_cost_staged(V, C, num_groups) != nullptr;
+}
+
 // Cascade-internal variant of casmvs_warp_cost_fwd: the hypotheses are the ladder
-// first + step*d (see Hyp in k1_common.cuh) instead of a (B,D,h,w) tensor.
+// first + step*d (see Hyp in k1_common.cuh) instead of a (B,D,h,w) tensor.  The staged kernels
+// read the features and write the cost volume (either layout) in 16-byte vectors.
 extern "C" int casmvs_warp_cost_ladder_fwd(const float* feats, const float* proj,
                                            const float* first_map, const float* first_b,
                                            float first, const float* step_b, float step, float* cost,
                                            int round_tf32, int B, int V, int C, int D, int h, int w,
                                            int num_groups, void* stream) {
+  CASMVS_REQUIRE_ALIGNED("warp_cost_ladder", feats, 16);
+  CASMVS_REQUIRE_ALIGNED("warp_cost_ladder", cost, 16);
   CASMVS_REQUIRE(feats && proj && cost, "warp_cost_ladder: null pointer");
   CASMVS_REQUIRE(B >= 0 && B <= 65535 && V >= 2 && C > 0 && D > 0 && h >= 2 && w >= 2,
                  "warp_cost_ladder: bad dims (h,w >= 2)");
   CASMVS_REQUIRE((size_t)h * w * C < (1u << 31), "warp_cost_ladder: view too large");
   if (B == 0) return 0;
+  const StagedK1 run = warp_cost_staged(V, C, num_groups);
+  CASMVS_REQUIRE(run, "warp_cost_ladder: shape not covered by the staged kernel "
+                 "(casmvs_warp_cost_ladder_supported): materialise the hypotheses and call "
+                 "casmvs_warp_cost_fwd (got V=%d C=%d G=%d)", V, C, num_groups);
   const int blocked = (round_tf32 & CASMVS_BLOCKED) ? 1 : 0;
   const int rnd = (round_tf32 & ~CASMVS_BLOCKED) ? 1 : 0;
   const Hyp hyp{nullptr, first_map, first_b, step_b, first, step};
-  const int rc = warp_var_smem(feats, proj, hyp, cost, B, V, C, D, h, w, num_groups, rnd, blocked,
-                               as_stream(stream));
-  if (rc == 1) {
-    set_error("warp_cost_ladder: shape not covered by the staged kernel (V-1 in {1,2}, C in "
-              "{8,16,32}, groups 1 or 8, channels-last features): materialise the hypotheses and "
-              "call casmvs_warp_cost_fwd (got V=%d C=%d G=%d)", V, C, num_groups);
-    return -1;
-  }
-  return rc;
+  return run(feats, proj, hyp, cost, B, D, h, w, rnd, blocked, as_stream(stream));
 }

@@ -26,7 +26,6 @@
 // The warped (B,V-1,C,D,h,w) volumes never exist; features are read from L2 once per
 // (tile, run), hypotheses once, the cost volume is written once, 32 bytes per thread as two 16-byte stores.
 #include <limits.h>
-#include <stdlib.h>
 
 #include <mutex>
 
@@ -471,8 +470,9 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   // box = tile + margins: sweep of the depth run + scale/rotation of the view + the 2x2 window
   constexpr int wq = PG > 0 ? 1024 / (C * 4) : 1;
   constexpr int BW = (TW + kMarginX + wq - 1) / wq * wq, BH = TH + kMarginY;
-  const int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
-  const size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
+  constexpr int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
+  constexpr size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
+  static_assert(smem <= 200 * 1024, "shared memory budget");
   auto kfn = [blocked] {
     if constexpr (PG > 0)
       return blocked ? warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, true>
@@ -483,7 +483,6 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   }();
   static std::atomic<bool> attr_set[2][kMaxDevices];
   if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[blocked ? 1 : 0], "warp_cost")) return rc;
-  if (smem > 200 * 1024) return 1;
   CUtensorMap map;
   if (!feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return -2;
   // depth runs: long enough to amortise the staging (a box is re-used by every plane of the
@@ -498,43 +497,39 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   return after_launch(PG > 0 ? "warp_cost(smem,pg)" : "warp_cost(smem)");
 }
 
+// Coverage: the shapes the staged kernels are instantiated for (V-1 source views, C channels,
+// variance or 8-group correlation).  V-1 > 2 stays on the gather kernel: the staged boxes would
+// leave one CTA per SM, and the gather kernel is faster there (cfg4 / cfg5).
+// Variance, V-1 = 2: plane groups of 2, a view's window is re-used across the planes of a
+// group.  Tried and removed: plane groups of 4 (spill at 128 registers), no window reuse (every
+// plane loads its 2x2 windows; slower), windows of both views kept in registers across ALL
+// planes (register pressure or spills through the same LSU pipe), coordinate math shared
+// between the threads of a pixel by warp shuffles (shuffles use the bound pipe), 16 channels
+// per thread (register pressure).
+struct Shape {
+  int nsrc, c, groups;
+  StagedK1 run;
+};
+static const Shape kShapes[] = {
+    {2, 8, 1, launch<2, 8, 32, 4, 4, false, 2>},  {2, 16, 1, launch<2, 16, 32, 2, 4, false, 2>},
+    {2, 32, 1, launch<2, 32, 16, 2, 4, false, 2>},
+    {1, 8, 1, launch<1, 8, 32, 4, 5, false, 0>},  {1, 16, 1, launch<1, 16, 32, 2, 5, false, 0>},
+    {1, 32, 1, launch<1, 32, 16, 2, 5, false, 0>},
+    // group-wise correlation: the reference's default G = 8
+    {1, 8, 8, launch<1, 8, 32, 4, 5, true, 0>},   {1, 16, 8, launch<1, 16, 32, 2, 5, true, 0>},
+    {1, 32, 8, launch<1, 32, 16, 2, 5, true, 0>},
+    {2, 8, 8, launch<2, 8, 32, 4, 5, true, 0>},   {2, 16, 8, launch<2, 16, 32, 2, 5, true, 0>},
+    {2, 32, 8, launch<2, 32, 16, 2, 5, true, 0>},
+};
+
 }  // namespace k1s
 
-// Variance or 8-group correlation cost volume, channels-last features, channels-last or
-// (blocked != 0) blocked output.  Returns 0 when handled, 1 when the shape is left to the gather
-// kernel of warp_cost.cu, <0 on error.
-int warp_var_smem(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
-                  int V, int C, int D, int h, int w, int num_groups, int rnd, int blocked,
-                  cudaStream_t st) {
-  // CASMVS_K1_SMEM=0 leaves every shape to the gather kernel (the reference of the staged kernels)
-  static const bool enabled = [] {
-    const char* e = getenv("CASMVS_K1_SMEM");
-    return !e || atoi(e) != 0;
-  }();
-  if (!enabled) return 1;
-  if ((reinterpret_cast<uintptr_t>(feats) & 15) != 0 || B > 65535) return 1;
-  using namespace k1s;
-  // V-1 > 2: the staged boxes leave one CTA per SM, the gather kernel is faster (cfg4 / cfg5)
-  if (V - 1 > 2) return 1;
-#define K1S(NS, CC, TW_, TH_, MB, GWC_, PG_) \
-  if (V - 1 == NS && C == CC) return launch<NS, CC, TW_, TH_, MB, GWC_, PG_>(feats, proj, dv, cost, B, D, h, w, rnd, blocked, st);
-  if (num_groups != 1) {
-    // group-wise correlation: the reference's default G = 8
-    if (num_groups != 8) return 1;
-    K1S(1, 8, 32, 4, 5, true, 0) K1S(1, 16, 32, 2, 5, true, 0) K1S(1, 32, 16, 2, 5, true, 0)
-    K1S(2, 8, 32, 4, 5, true, 0) K1S(2, 16, 32, 2, 5, true, 0) K1S(2, 32, 16, 2, 5, true, 0)
-    return 1;
-  }
-  // Variance, V-1 = 2: plane groups of 2, a view's window is re-used across the planes of a
-  // group.  Tried and removed: plane groups of 4 (spill at 128 registers), no window reuse (every
-  // plane loads its 2x2 windows; slower), windows of both views kept in registers across ALL
-  // planes (register pressure or spills through the same LSU pipe), coordinate math shared
-  // between the threads of a pixel by warp shuffles (shuffles use the bound pipe), 16 channels
-  // per thread (register pressure).
-  K1S(2, 8, 32, 4, 4, false, 2) K1S(2, 16, 32, 2, 4, false, 2) K1S(2, 32, 16, 2, 4, false, 2)
-  K1S(1, 8, 32, 4, 5, false, 0) K1S(1, 16, 32, 2, 5, false, 0) K1S(1, 32, 16, 2, 5, false, 0)
-#undef K1S
-  return 1;
+// CASMVS_K1_SMEM=0 leaves every shape to the gather kernel (the reference of the staged kernels).
+StagedK1 warp_cost_staged(int V, int C, int num_groups) {
+  if (!switches().k1_smem) return nullptr;
+  for (const k1s::Shape& s : k1s::kShapes)
+    if (s.nsrc == V - 1 && s.c == C && s.groups == num_groups) return s.run;
+  return nullptr;
 }
 
 }  // namespace casmvs

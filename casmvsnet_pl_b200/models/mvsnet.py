@@ -369,17 +369,16 @@ class CascadeMVSNet(nn.Module):
         self.G = num_groups
         self.feature = FeatureNet(norm_act)
         # run the top-down half of the pyramid on a side stream, concurrently with the coarsest
-        # cascade stage (tf32 inference path; CASMVS_OVERLAP=0 turns it off)
-        import os
-        self.overlap_pyramid = os.environ.get("CASMVS_OVERLAP", "1") != "0"
+        # cascade stage (tf32 inference path)
+        self.overlap_pyramid = True
         # diagnostics: also return the int64 depth_index_l maps (mvsnet.py:185-190) that the
         # confidence gather uses; the reference keeps them internal
         self.return_index = False
         self._last_index = None
         # cascade-internal fusion: K4 writes only the first rung of each stage's hypothesis ladder
         # and K1 / K3 generate first + step*d themselves (bit-identical results; the (B,D,h,w)
-        # hypothesis tensor is neither written nor read).  CASMVS_LADDER=0 turns it off.
-        self.fuse_hypotheses = os.environ.get("CASMVS_LADDER", "1") != "0"
+        # hypothesis tensor is neither written nor read)
+        self.fuse_hypotheses = True
         for l in range(self.levels):
             cin = self.G if self.G > 1 else 8 * 2 ** l
             setattr(self, f"cost_reg_{l}", CostRegNet(cin, norm_act))

@@ -100,6 +100,7 @@ uint64_t casmvs_fallback_count(void);
  *                num_groups >1: G channels  (B,G,D,h,w)|(B,D,h,w,G)
  * Workspace: casmvs_warp_cost_workspace_bytes() (only needed when feats are
  * NCHW: they are re-laid-out once to NHWC).  C % 8 == 0, C % G == 0.
+ * 16-byte aligned: NHWC feats, the workspace (NCHW feats), an NHWC cost.
  */
 size_t casmvs_warp_cost_workspace_bytes(int feat_layout, int B, int V, int C, int h, int w);
 int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const float* proj,
@@ -109,7 +110,8 @@ int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const float* proj,
 
 /* Stand-alone homo_warp (models/modules.py:52-92): materialises the warped
  * volume for API completeness.  src_feat (B,C,h,w)|(B,h,w,C), proj (B,3,4),
- * depth_values (B,D,h,w) -> warped (B,C,D,h,w)|(B,D,h,w,C).               */
+ * depth_values (B,D,h,w) -> warped (B,C,D,h,w)|(B,D,h,w,C).  src_feat and an
+ * NHWC warped 16-byte aligned.                                             */
 int casmvs_homo_warp_fwd(const float* src_feat, int feat_layout, const float* proj,
                          const float* depth_values, float* warped, int out_layout,
                          int B, int C, int D, int h, int w, void* stream);
@@ -125,6 +127,9 @@ int casmvs_homo_warp_fwd(const float* src_feat, int feat_layout, const float* pr
  * For kind == CASMVS_CONV: stride in {1,2}, out dims = (in-1)/stride+1.
  * For kind == CASMVS_CONV_TRANSPOSE: out dims = 2*in.
  * For kind == CASMVS_CONV_PLANAR: stride 1, out dims = in dims.
+ * x 16-byte aligned; y and skip too when Cout > 1.
+ * In the TF32 mode a layer shape that no tensor-core kernel covers runs on the CUDA cores
+ * (casmvs_fallback_count).
  */
 size_t casmvs_packed_conv3d_weight_floats(int Cin, int Cout);
 /* w_torch: Conv3d layout (Cout,Cin,3,3,3), ConvTranspose3d layout (Cin,Cout,3,3,3) or, for
@@ -171,9 +176,10 @@ int casmvs_costreg_layer_info(int Cin, int layer, int* cin, int* cout, int* kind
                               size_t* w_off, size_t* scale_off, size_t* shift_off);
 size_t casmvs_costreg_workspace_bytes(int B, int Cin, int D, int h, int w);
 /* 1 when casmvs_costreg_fwd stores its activations blocked for this Cin and precision and so
- * accepts a CASMVS_BLOCKED input (TF32, Cin in {8,16,32}, tensor-core kernels not switched off
- * by CASMVS_TMA / CASMVS_TMA2; x and workspace must then be 16-byte aligned), else 0.  The
- * other cases run channels-last, layers no tensor-core kernel covers on the CUDA cores. */
+ * accepts a CASMVS_BLOCKED input: TF32, and a tensor-core kernel covers every one of the 11
+ * layers (conv1 .. prob always are; conv0 for Cin in {8,16,32}), else 0.  The other cases run
+ * channels-last, layers no tensor-core kernel covers on the CUDA cores.
+ * casmvs_costreg_fwd needs x and workspace 16-byte aligned. */
 int casmvs_costreg_blocked_supported(int Cin, int precision);
 int casmvs_costreg_fwd(const float* x, const float* params, float* logits,
                        int B, int Cin, int D, int h, int w, int precision,
@@ -217,13 +223,17 @@ int casmvs_uniform_hypotheses_fwd(float depth_min, float step, const float* dept
  * results).  first: `first_map` (B,h,w) per pixel, else `first_b` (B) per batch item, else the
  * scalar `first`; step: `step_b` (B) else the scalar `step`.
  * casmvs_depth_first_fwd writes only the first rung (B,h,w) of casmvs_depth_hypotheses_fwd.
- * casmvs_warp_cost_ladder_fwd: channels-last features and cost volume; shapes of the staged
- * kernel only (V-1 in {1,2}, C in {8,16,32}, num_groups 1 or 8), error otherwise.
+ * casmvs_warp_cost_ladder_fwd: channels-last features and cost volume, both 16-byte aligned;
+ * shapes of the staged kernel only (casmvs_warp_cost_ladder_supported), error otherwise.
  * round_tf32: nonzero = store the cost TF32-rounded; | CASMVS_BLOCKED = store it blocked,
- * (B,Cout/4,D,h,w,4), for casmvs_costreg_fwd with CASMVS_BLOCKED. */
+ * (B,Cout/4,D,h,w,4), for casmvs_costreg_fwd with CASMVS_BLOCKED.
+ * casmvs_warp_cost_ladder_supported: 1 when the staged kernel covers the shape (V-1 in {1,2},
+ * C in {8,16,32}, num_groups 1 or 8) and CASMVS_K1_SMEM=0 does not send every shape to the
+ * gather kernel, else 0. */
 int casmvs_depth_first_fwd(const float* cur, int upsample, float half_range, float step,
                            const float* step_dev, float* out, int B, int D, int h, int w,
                            void* stream);
+int casmvs_warp_cost_ladder_supported(int V, int C, int num_groups);
 int casmvs_warp_cost_ladder_fwd(const float* feats, const float* proj, const float* first_map,
                                 const float* first_b, float first, const float* step_b, float step,
                                 float* cost, int round_tf32, int B, int V, int C, int D, int h, int w,

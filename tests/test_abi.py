@@ -68,6 +68,79 @@ def test_errors_are_reported_not_thrown():
         _lib.check(rc, "costreg")
 
 
+def test_costreg_blocked_coverage_is_pinned():
+    """Every CostRegNet layer has a tensor-core kernel exactly for TF32 and Cin in {8, 16, 32}
+    (conv1 .. prob always, conv0 for those input widths)."""
+    from casmvsnet_pl_b200 import _lib
+    lib = _lib.load()
+    for cin in range(4, 65, 4):
+        for prec in (_lib.FP32, _lib.TF32):
+            want = int(prec == _lib.TF32 and cin in (8, 16, 32))
+            assert lib.casmvs_costreg_blocked_supported(cin, prec) == want, (cin, prec)
+
+
+def test_ladder_coverage_is_pinned():
+    """The staged K1 kernel, the only one that takes a hypothesis ladder, covers one or two
+    source views, C in {8, 16, 32}, variance or 8-group correlation."""
+    from casmvsnet_pl_b200 import ops
+    for V in range(2, 9):
+        for C in range(4, 65, 4):
+            for G in (1, 2, 4, 8):
+                want = V - 1 in (1, 2) and C in (8, 16, 32) and G in (1, 8)
+                assert ops.ladder_supported(V, C, G) is want, (V, C, G)
+
+
+def test_misaligned_pointers_are_rejected():
+    """Entry points whose kernels use 16-byte vectors reject a misaligned pointer before any
+    device work, naming it (the message tells a rejection apart from "no device")."""
+    from casmvsnet_pl_b200 import _lib
+    lib = _lib.load()
+    ok, bad = ctypes.c_void_p(0x10000), ctypes.c_void_p(0x10004)
+    odd = ctypes.c_void_p(0x10002)
+
+    def rejected(rc, what):
+        msg = lib.casmvs_last_error()
+        assert rc < 0 and what in msg and b"aligned" in msg, (rc, msg)
+
+    NHWC, NCHW, CONV, TF32 = _lib.NHWC, _lib.NCHW, _lib.CONV, _lib.TF32
+    # casmvs_conv3d_fwd: x always, y and skip when Cout > 1
+    rejected(lib.casmvs_conv3d_fwd(bad, ok, ok, ok, 0.01, None, ok, 1, 8, 8, 8, 16, 16, CONV, 1,
+                                   TF32, None), b"x must be 16-byte")
+    rejected(lib.casmvs_conv3d_fwd(ok, ok, ok, ok, 0.01, None, bad, 1, 8, 8, 8, 16, 16, CONV, 1,
+                                   TF32, None), b"y must be 16-byte")
+    rejected(lib.casmvs_conv3d_fwd(ok, ok, ok, ok, 0.01, bad, ok, 1, 8, 8, 8, 16, 16, CONV, 1,
+                                   TF32, None), b"skip must be 16-byte")
+    rc = lib.casmvs_conv3d_fwd(ok, ok, ok, ok, 1.0, bad, bad, 1, 8, 1, 8, 16, 16, 7, 1, TF32, None)
+    assert rc < 0 and b"bad kind" in lib.casmvs_last_error()        # Cout == 1: float stores
+    # casmvs_costreg_fwd: x, workspace, logits
+    rejected(lib.casmvs_costreg_fwd(bad, ok, ok, 1, 8, 16, 16, 16, TF32, ok, 1 << 30, None),
+             b"x must be 16-byte")
+    rejected(lib.casmvs_costreg_fwd(ok, ok, ok, 1, 8, 16, 16, 16, TF32, bad, 1 << 30, None),
+             b"workspace must be 16-byte")
+    rejected(lib.casmvs_costreg_fwd(ok, ok, odd, 1, 8, 16, 16, 16, TF32, ok, 1 << 30, None),
+             b"logits must be 4-byte")
+    # casmvs_warp_cost_fwd: NHWC features, the workspace of NCHW ones, an NHWC cost volume
+    rejected(lib.casmvs_warp_cost_fwd(bad, NHWC, ok, ok, ok, NHWC, 1, 3, 8, 8, 16, 16, 1, None, 0,
+                                      None), b"feats must be 16-byte")
+    rejected(lib.casmvs_warp_cost_fwd(ok, NCHW, ok, ok, ok, NHWC, 1, 3, 8, 8, 16, 16, 1, bad,
+                                      1 << 30, None), b"workspace must be 16-byte")
+    rejected(lib.casmvs_warp_cost_fwd(ok, NHWC, ok, ok, bad, NHWC | _lib.ROUND_TF32, 1, 3, 8, 8,
+                                      16, 16, 1, None, 0, None), b"cost must be 16-byte")
+    # casmvs_warp_cost_ladder_fwd: features and cost volume
+    rejected(lib.casmvs_warp_cost_ladder_fwd(bad, ok, None, None, 500.0, None, 2.5, ok, 1, 1, 3,
+                                             8, 8, 16, 16, 1, None), b"feats must be 16-byte")
+    rejected(lib.casmvs_warp_cost_ladder_fwd(ok, ok, None, None, 500.0, None, 2.5, bad,
+                                             1 | _lib.BLOCKED, 1, 3, 8, 8, 16, 16, 1, None),
+             b"cost must be 16-byte")
+    # casmvs_homo_warp_fwd: features, an NHWC output
+    rejected(lib.casmvs_homo_warp_fwd(bad, NHWC, ok, ok, ok, NCHW, 1, 8, 8, 16, 16, None),
+             b"src_feat must be 16-byte")
+    rejected(lib.casmvs_homo_warp_fwd(ok, NHWC, ok, ok, bad, NHWC, 1, 8, 8, 16, 16, None),
+             b"warped must be 16-byte")
+    rejected(lib.casmvs_conv2d_5x5s2_fwd(bad, ok, ok, 0.01, ok, 1, 8, 16, 32, 32, 1, None),
+             b"x must be 16-byte")
+
+
 def _header_constants():
     src = open(os.path.join(ROOT, "include", "casmvs.h")).read()
     consts = {k: int(v) for k, v in re.findall(r"#define\s+(CASMVS_[A-Z0-9_]+)\s+(\d+)", src)}

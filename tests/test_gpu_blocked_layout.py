@@ -103,30 +103,6 @@ def test_costreg_uncovered_conv0_stays_channels_last(cin):
     assert torch.equal(got, want)
 
 
-def test_costreg_with_tensor_core_kernels_switched_off(tmp_path):
-    """CASMVS_TMA2=0 (child process): the stride-2 and transposed layers run on the CUDA cores,
-    so the driver keeps the activations channels-last instead of failing."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = (
-        "import sys, torch\n"
-        "sys.path.insert(0, %r)\n"
-        "from casmvsnet_pl_b200 import ABN, _lib, ops\n"
-        "from casmvsnet_pl_b200.models.mvsnet import CostRegNet\n"
-        "net = CostRegNet(8, ABN).eval().cuda().requires_grad_(False)\n"
-        "net.precision = 'tf32'\n"
-        "assert not net.blocked_supported()\n"
-        "with torch.no_grad():\n"
-        "    y = net(ops.as_volume_view(torch.randn(1, 16, 40, 56, 8, device='cuda')))\n"
-        "torch.cuda.synchronize()\n"
-        "assert y.shape == (1, 1, 16, 40, 56) and bool(torch.isfinite(y).all())\n"
-        "assert _lib.fallback_count() == 6, _lib.fallback_count()\n" % root)
-    env = dict(os.environ, CASMVS_TMA2="0")
-    subprocess.run([sys.executable, "-c", code], check=True, env=env, timeout=300)
-
-
 def test_costreg_blocked_input_is_validated():
     net = _net(8)
     with pytest.raises(ValueError):
