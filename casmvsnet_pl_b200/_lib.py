@@ -71,6 +71,8 @@ SIGNATURES = {
     "casmvs_bias_lrelu_nhwc": (c_int, [c_void_p, c_void_p, c_float, c_size_t, c_int, c_void_p]),
     "casmvs_normalize_u8_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float),
                                         POINTER(c_float), c_void_p]),
+    "casmvs_jitter_normalize_u8_fwd": (c_int, [c_void_p] * 4 + [c_int] * 3 + [POINTER(c_float),
+                                                                            POINTER(c_float), c_void_p]),
     "casmvs_resize_u8_pil_fwd": (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p, c_void_p, c_int,
                                                                           c_void_p, c_void_p, c_int,
                                                                           c_void_p]),

@@ -228,6 +228,40 @@ class TanksTestScan(_CachedScan):
         return float(np.float32(self.depth_min[ref])), float(np.float32(self.depth_interval))
 
 
+def read_blendedmvs_cams(root_dir, scan, img_wh, n_views, levels):
+    """build_metas + build_proj_mats of datasets/blendedmvs.py:32-104 for one scan ->
+    (full_wh, metas [(ref, srcs)], proj_mats {vid}, depth_min {vid}, scale_factor).  The native
+    size is 768x576 when root_dir ends in dataset_low_res, else 2048x1536 (:61-65); reference
+    views with fewer valid sources than n_views are left out of metas (:51-54), but every view
+    of pair.txt gets its projections; depth_min and the extrinsic translation are scaled by
+    100 / depth_min of the first cam read (:98-103)."""
+    d = os.path.join(root_dir, scan)
+    low = root_dir.endswith("dataset_low_res") or root_dir.endswith("dataset_low_res/")
+    full_wh = (768, 576) if low else (2048, 1536)
+    metas, refs = [], []
+    with open(os.path.join(d, "cams", "pair.txt")) as f:
+        for _ in range(int(f.readline())):
+            ref = int(f.readline().rstrip())
+            refs.append(ref)
+            line = f.readline().rstrip().split()
+            if int(line[0]) >= n_views:
+                metas.append((ref, [int(x) for x in line[1::2]]))
+    scale = []
+    proj_mats, depth_min = _read_proj_mats(lambda v: os.path.join(d, "cams", f"{v:08d}_cam.txt"),
+                                           refs, img_wh, full_wh, levels, scale)
+    return full_wh, metas, proj_mats, depth_min, (scale[0] if scale else None)
+
+
+def read_blendedmvs_depth(scan_dir, vid, scale_factor, img_wh):
+    """A view's rendered depth, scaled by the scan's factor and cv2 INTER_NEAREST-resized to
+    img_wh (datasets/blendedmvs.py:106-111) -> (h,w) float32."""
+    import cv2
+    depth = np.array(io.read_pfm(os.path.join(scan_dir, "rendered_depth_maps", f"{vid:08d}.pfm"))[0],
+                     dtype=np.float32)
+    depth *= scale_factor
+    return cv2.resize(depth, tuple(img_wh), interpolation=cv2.INTER_NEAREST)
+
+
 class BlendedMVSTestScan(_CachedScan):
     """One BlendedMVS scan in the layout datasets/blendedmvs.py reads (test mode, img_wh given):
 
@@ -249,21 +283,8 @@ class BlendedMVSTestScan(_CachedScan):
         self.root_dir, self.scan = root_dir, scan
         self.img_wh, self.n_views, self.host_images = tuple(img_wh), n_views, host_images
         self.dir = os.path.join(root_dir, scan)
-        low = root_dir.endswith("dataset_low_res") or root_dir.endswith("dataset_low_res/")
-        self.full_wh = (768, 576) if low else (2048, 1536)
-        self.metas, refs = [], []
-        with open(os.path.join(self.dir, "cams", "pair.txt")) as f:
-            for _ in range(int(f.readline())):
-                ref = int(f.readline().rstrip())
-                refs.append(ref)
-                line = f.readline().rstrip().split()
-                if int(line[0]) >= n_views:
-                    self.metas.append((ref, [int(x) for x in line[1::2]]))
-        scale = []
-        self.proj_mats, self.depth_min = _read_proj_mats(
-            lambda v: os.path.join(self.dir, "cams", f"{v:08d}_cam.txt"), refs, self.img_wh,
-            self.full_wh, levels, scale)
-        self.scale_factor = scale[0] if scale else None
+        self.full_wh, self.metas, self.proj_mats, self.depth_min, self.scale_factor = \
+            read_blendedmvs_cams(root_dir, scan, self.img_wh, n_views, levels)
         self.depth_interval = {}
         for ref, _ in self.metas:
             self.depth_interval[ref] = self._depth_interval(ref, n_depths_arg)
@@ -274,11 +295,7 @@ class BlendedMVSTestScan(_CachedScan):
             return [line.rstrip() for line in f.readlines()]
 
     def _depth_interval(self, ref, n_depths_arg):
-        import cv2
-        depth = np.array(io.read_pfm(os.path.join(self.dir, "rendered_depth_maps", f"{ref:08d}.pfm"))[0],
-                         dtype=np.float32)
-        depth *= self.scale_factor
-        depth_max = cv2.resize(depth, self.img_wh, interpolation=cv2.INTER_NEAREST).max()
+        depth_max = read_blendedmvs_depth(self.dir, ref, self.scale_factor, self.img_wh).max()
         return float(np.float32((depth_max - self.depth_min[ref]) / n_depths_arg))
 
     def image_path(self, vid):

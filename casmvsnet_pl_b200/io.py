@@ -13,6 +13,9 @@ Host-side Python like the reference's (it is data plumbing, not arithmetic on th
                                uint8 HWC images are uploaded AS BYTES (4x less H2D traffic than
                                fp32) and converted + normalised + re-laid-out to planar fp32 on the
                                GPU by casmvs_normalize_u8_fwd
+  jitter_normalize_images      the same after reference datasets/blendedmvs.py:130-137's training
+                               ColorJitter(brightness=0.25, contrast=0.5), byte-exact to Pillow
+                               (casmvs_jitter_normalize_u8_fwd)
   read_ply                     PLY vertices (binary little-endian or ASCII, scalar properties): reads
                                fusion.write_ply output and the DTU ground-truth STL clouds
   DepthWriter / infer_views    reference eval.py:213-229 (the per-view inference loop): views are
@@ -223,6 +226,43 @@ def normalize_images(images_u8, device=None, out=None):
         _lib.check(_lib.load().casmvs_normalize_u8_fwd(
             ctypes.c_void_p(t.data_ptr()), ctypes.c_void_p(out.data_ptr()), N, H, W, mean, std, st),
             "normalize_u8")
+    return out
+
+
+def jitter_normalize_images(images_u8, jitter, device=None, out=None):
+    """T.ColorJitter(brightness, contrast) on each PIL image, then ToTensor + Normalize, on the
+    GPU and bit-identical to torchvision + Pillow (the training transform of
+    datasets/blendedmvs.py:130-137): uint8 (N,H,W,3) RGB images and jitter (N,3) float32 rows
+    (brightness_first, brightness factor, contrast factor) -> float32 (N,3,H,W).  Host inputs
+    are uploaded to `device`; the factors stay on the device, so the call makes no host
+    synchronisation (casmvs_jitter_normalize_u8_fwd)."""
+    import ctypes
+
+    from . import _lib
+    t = images_u8 if torch.is_tensor(images_u8) else torch.from_numpy(np.ascontiguousarray(images_u8))
+    j = jitter if torch.is_tensor(jitter) else torch.as_tensor(np.asarray(jitter, np.float32))
+    if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
+        raise _lib.CasMVSError("jitter_normalize_images expects uint8 (N,H,W,3)")
+    if j.dtype != torch.float32 or tuple(j.shape) != (t.shape[0], 3):
+        raise _lib.CasMVSError(f"jitter_normalize_images expects float32 jitter ({t.shape[0]},3)")
+    if not t.is_cuda:
+        if device is None:
+            raise _lib.CasMVSError("jitter_normalize_images: give a CUDA device for host input (no CPU path)")
+        t = t.to(device, non_blocking=True)
+    t = t.contiguous()
+    j = j.to(t.device, non_blocking=True).contiguous()
+    N, H, W, _ = t.shape
+    if out is None:
+        out = torch.empty(N, 3, H, W, device=t.device, dtype=torch.float32)
+    lsum = torch.empty(N, device=t.device, dtype=torch.int64)
+    mean = (ctypes.c_float * 3)(*IMAGENET_MEAN)
+    std = (ctypes.c_float * 3)(*IMAGENET_STD)
+    with torch.cuda.device(t.device):
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        _lib.check(_lib.load().casmvs_jitter_normalize_u8_fwd(
+            ctypes.c_void_p(t.data_ptr()), ctypes.c_void_p(j.data_ptr()),
+            ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(lsum.data_ptr()), N, H, W, mean, std,
+            st), "jitter_normalize_u8")
     return out
 
 

@@ -1,6 +1,7 @@
 """Seeded synthetic scans in the Tanks and Temples and BlendedMVS test layouts, for the scan
-readers of eval_pipeline, and in the DTU training layout (make_dtu_train), for train_data and
-the trainer (the real data sets are large and licensed separately).
+readers of eval_pipeline, and in the DTU and BlendedMVS training layouts (make_dtu_train,
+make_blendedmvs_train), for train_data and the trainer (the real data sets are large and
+licensed separately).
 
   tanks       <root>/<split>/<scan>/pair.txt, cams/{vid:08d}_cam.txt, images/{vid:08d}.jpg
   blendedmvs  <root>/dataset_low_res/<scan>/cams/pair.txt, cams/{vid:08d}_cam.txt,
@@ -109,6 +110,20 @@ def make_blendedmvs(root, scan="5a3ca9cb270f0e3f14d0eddb", n_views=8, image_wh=(
         with open(os.path.join(root, names[split]), "a") as f:
             f.write(scan + "\n")
     return base
+
+
+BLENDEDMVS_TRAIN_SCANS = ("5a0000000000000000000a01", "5a0000000000000000000b02")
+
+
+def make_blendedmvs_train(root, n_views=(8, 6), image_wh=(96, 72), seed=0, n_few=4):
+    """Two BlendedMVS-layout scans for the training reader: BLENDEDMVS_TRAIN_SCANS[0] with
+    n_views[0] views in training_list.txt and [1] with n_views[1] views in
+    validation_list.txt, both in all_list.txt.  The scans differ in scene depth (30 and 45) and
+    texture; every n_few-th view has too few sources and is skipped by readers with n_views > 2,
+    and the top tenth of every depth map is 0 (sky).  Returns the dataset_low_res directory."""
+    train, val = BLENDEDMVS_TRAIN_SCANS
+    make_blendedmvs(root, train, n_views[0], tuple(image_wh), 30.0, seed, n_few, ("train", "all"))
+    return make_blendedmvs(root, val, n_views[1], tuple(image_wh), 45.0, seed + 10, n_few, ("val", "all"))
 
 
 def make_dtu_train(root, scan="scan1", refs=(0, 1, 2), n_src=5, depth=650.0, seed=0):

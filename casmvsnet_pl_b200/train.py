@@ -1,8 +1,18 @@
-"""Train CascadeMVSNet on DTU with the engine: the reference's train.py without
+"""Train CascadeMVSNet on DTU or BlendedMVS with the engine: the reference's train.py without
 pytorch-lightning, test_tube or inplace_abn.
 
     python -m casmvsnet_pl_b200.train --root_dir DTU/mvs_training/dtu \
         --train_list lists/dtu/train.txt --val_list lists/dtu/val.txt --exp_name exp
+    python -m casmvsnet_pl_b200.train --dataset_name blendedmvs \
+        --root_dir BlendedMVS/dataset_low_res --depth_interval 192.0 --exp_name exp
+
+DTU reads its scans from --train_list / --val_list (one scan per line).  BlendedMVS reads them
+from the data set's own training_list.txt / validation_list.txt next to root_dir, so the two
+list flags are refused for it; it trains at 768x576 with the reference's colour jitter on the
+training split and validates on the validation split.  For BlendedMVS, --depth_interval is
+what the reference passes to its reader as `n_depths`: each sample's depth interval is (max
+depth - depth_min) / --depth_interval, so the reference README's 192.0 spreads the coarsest
+stage's 48 x 4 intervals over the reference view's depth range.
 
 Flags keep the names and defaults of the reference's opt.py, plus --precision (fp32 as the
 reference, or tf32), the two scan lists and --log_every.  The loop is what Lightning 0.7.5 ran
@@ -19,7 +29,7 @@ for the reference's MVSSystem:
     best by val/acc_2mm.
 
 Not supported (the command exits with a message): radam and ranger, --use_amp, more than one
-GPU, and the BlendedMVS training set.
+GPU.
 """
 from __future__ import annotations
 
@@ -84,9 +94,12 @@ def check_supported(a):
         raise SystemExit("--use_amp is not supported: train in fp32 or --precision tf32")
     if a.num_gpus != 1:
         raise SystemExit("--num_gpus must be 1: multi-GPU training is not supported")
-    if a.dataset_name != "dtu":
-        raise SystemExit("only --dataset_name dtu can be trained")
-    if not a.train_list or not a.val_list:
+    if a.dataset_name == "blendedmvs":
+        for flag in ("train_list", "val_list"):
+            if getattr(a, flag):
+                raise SystemExit(f"--{flag} is not used with --dataset_name blendedmvs: its scans "
+                                 "come from training_list.txt / validation_list.txt next to root_dir")
+    elif not a.train_list or not a.val_list:
         raise SystemExit("--train_list and --val_list are required")
 
 
@@ -271,16 +284,23 @@ class Trainer:
         return keep.kept
 
 
+def build_datasets(a):
+    """(train, val) readers of --dataset_name."""
+    if a.dataset_name == "blendedmvs":
+        return tuple(train_data.BlendedMVSTrainDataset(a.root_dir, split, a.n_views, a.levels,
+                                                       a.depth_interval) for split in ("train", "val"))
+    return tuple(train_data.DTUTrainDataset(a.root_dir, train_data.read_scan_list(lst), a.n_views,
+                                            a.levels, a.depth_interval)
+                 for lst in (a.train_list, a.val_list))
+
+
 def main(argv=None):
     a = build_parser().parse_args(argv)
     check_supported(a)
     if not torch.cuda.is_available():
         raise SystemExit("training needs a CUDA GPU")
     device = "cuda:0"
-    train_set = train_data.DTUTrainDataset(a.root_dir, train_data.read_scan_list(a.train_list),
-                                           a.n_views, a.levels, a.depth_interval)
-    val_set = train_data.DTUTrainDataset(a.root_dir, train_data.read_scan_list(a.val_list),
-                                         a.n_views, a.levels, a.depth_interval)
+    train_set, val_set = build_datasets(a)
     model = build_model(a, device)
     print("number of parameters : %.2f M" % (sum(p.numel() for p in model.parameters()
                                                   if p.requires_grad) / 1e6))
@@ -292,6 +312,7 @@ def main(argv=None):
                        os.path.join("ckpts", a.exp_name))
     print(f"trained {trainer.global_step} steps in {time.time() - t0:.1f} s; "
           f"kept {sorted(kept)}")
+    return trainer
 
 
 if __name__ == "__main__":

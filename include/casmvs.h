@@ -344,6 +344,15 @@ int casmvs_sl1_loss_bwd(const float* const* pred, const float* const* gt,
  * torchvision).  mean3 / std3 are HOST arrays of 3 floats.  H*W % 4 == 0 when N > 1. */
 int casmvs_normalize_u8_fwd(const uint8_t* images, float* out, int N, int H, int W,
                             const float* mean3, const float* std3, void* stream);
+/* The same conversion after T.ColorJitter(brightness, contrast) on the PIL image (the training
+ * transform of datasets/blendedmvs.py:130-137), bit-identical to torchvision + Pillow.
+ * jitter: DEVICE (N,3) float32 per image = (brightness_first != 0, b, c): brightness is
+ * Image.blend(black, img, b), contrast Image.blend(gray(m), img, c) with m = int(mean L + 0.5)
+ * of the image as it stands when contrast is applied.  lsum: DEVICE scratch of N int64 (8-byte
+ * aligned), zeroed here.  No host synchronisation: graph-capturable.  H*W % 4 == 0 when N > 1. */
+int casmvs_jitter_normalize_u8_fwd(const uint8_t* images, const float* jitter, float* out,
+                                   long long* lsum, int N, int H, int W, const float* mean3,
+                                   const float* std3, void* stream);
 
 /* Resamplers of the scan readers, byte-identical to the host libraries the reference uses:
  * images (N,H,W,3) uint8 -> out (N,OH,OW,3) uint8.  The weight tables are DEVICE int32 arrays
