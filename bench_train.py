@@ -5,6 +5,7 @@ temporary directory.
     python bench_train.py [--steps 50] [--warmup 5] [--out result.json]
     python bench_train.py --profile [--out profile.json]      # one step under torch.profiler
     python bench_train.py --dataset blendedmvs [--steps 50] [--warmup 5]
+    python bench_train.py --deterministic [--dataset blendedmvs] [--steps 50] [--warmup 5]
 
 Default run, one JSON object: the card's name and power limit; the host data time per sample
 (decode + slice in the main process); for fp32 and tf32 at B = 1 and 2 the step time (forward,
@@ -17,6 +18,9 @@ dataset_low_res scans with native-size JPEGs (synth_scenes.make_blendedmvs_train
 split (colour-jittered batches); the host data time is the decode-only worker's, and the
 object adds the time of the same jitter done with Pillow on the host (ImageEnhance, what
 torchvision's ColorJitter calls) and of the fused device kernel (CUDA events).
+--deterministic: the same steps under torch.use_deterministic_algorithms(True), as
+train.py --deterministic runs them (deterministic backward kernels, no cuDNN autotuning); the
+object says so in "deterministic".
 """
 from __future__ import annotations
 
@@ -188,15 +192,20 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--out", default=None)
+    ap.add_argument("--deterministic", action="store_true",
+                    help="time the steps with deterministic algorithms on (train.py --deterministic)")
     a = ap.parse_args()
+    if a.deterministic:
+        train.set_deterministic()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train.py measures on a CUDA GPU")
     if a.dataset == "blendedmvs" and a.profile:
         raise SystemExit("--profile measures the DTU shape only")
-    res = {"card": card(), "shape": "640x512, V=3, D=48/32/8"}
+    res = {"card": card(), "shape": "640x512, V=3, D=48/32/8", "deterministic": a.deterministic}
     with tempfile.TemporaryDirectory() as tmp:
         if a.dataset == "blendedmvs":
             res = bench_blendedmvs(a, tmp)
+            res["deterministic"] = a.deterministic
         else:
             root = make_dtu_train(os.path.join(tmp, "dtu"), seed=0)
             ds = train_data.DTUTrainDataset(root, ["scan1"])

@@ -80,6 +80,11 @@ SIGNATURES = {
     "casmvs_warp_cost_bwd": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
     "casmvs_conv3d_wgrad": (c_int, [c_void_p] * 3 + [c_int] * 10 + [c_void_p]),
     "casmvs_regress_bwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
+    "casmvs_warp_cost_bwd_det_workspace_bytes": (c_size_t, [c_int] * 6),
+    "casmvs_warp_cost_bwd_det": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
+    "casmvs_conv3d_wgrad_det_workspace_bytes": (c_size_t, [c_int] * 6),
+    "casmvs_conv3d_wgrad_det": (c_int, [c_void_p] * 3 + [c_int] * 10 + [c_void_p, c_size_t, c_void_p]),
+    "casmvs_upsample2x_bilinear_bwd": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "casmvs_sl1_loss_workspace_bytes": (c_size_t, []),
     "casmvs_sl1_loss_fwd": (c_int, [POINTER(c_void_p)] * 3 + [POINTER(c_int), c_int, c_int]
                             + [c_void_p] * 4 + [c_size_t, c_void_p]),

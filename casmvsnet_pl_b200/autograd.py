@@ -9,15 +9,32 @@ training step (train.py:99-127: forward, SL1 loss on depth_l, backward) needs.
                norm-act that follows it in training mode is batch-statistics ABN
                (casmvsnet_pl_b200.norm_act: F.batch_norm + leaky_relu, torch autograd).
   RegressFn    K3: d(depth)/d(logits); confidence is computed under no_grad (mvsnet.py:179).
+  Upsample2xFn FeatureNet's bilinear x2 upsample (align_corners=True): ATen's forward, backward
+               by casmvs_upsample2x_bilinear_bwd.
+
+With torch.use_deterministic_algorithms(True) the backward ops run the deterministic entries
+(casmvs_warp_cost_bwd_det, casmvs_conv3d_wgrad_det, casmvs_upsample2x_bilinear_bwd): a training
+step is then the same bits for the same inputs.  `deterministic()` below is the one place that
+decides; without it every op runs exactly as before.
 """
 from __future__ import annotations
 
 import ctypes
 
 import torch
+import torch.nn.functional as F
 
 from . import _lib, ops
-from .ops import CONV, CONV_TRANSPOSE, FP32, NHWC, _ptr, _stream, check
+from .ops import CONV, CONV_TRANSPOSE, FP32, NCHW, NHWC, _ptr, _stream, check
+
+
+def deterministic():
+    """torch's switch: the deterministic backward kernels run when it is on."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def _workspace(nbytes, device):
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
 
 
 def _dense_ndhwc(x):
@@ -42,10 +59,18 @@ class WarpCostFn(torch.autograd.Function):
         B, V, h, w, C = f_cl.shape
         D = dv.shape[1]
         g = _dense_ndhwc(gcost)
-        gf = torch.zeros_like(f_cl)
+        lib = _lib.load()
         with torch.cuda.device(f_cl.device):
-            check(_lib.load().casmvs_warp_cost_bwd(_ptr(f_cl), _ptr(proj), _ptr(dv), _ptr(g), _ptr(gf),
-                                                   B, V, C, D, h, w, ctx.G, _stream()), "warp_cost_bwd")
+            if deterministic():
+                gf = torch.empty_like(f_cl)
+                ws = _workspace(lib.casmvs_warp_cost_bwd_det_workspace_bytes(B, V, C, D, h, w), f_cl.device)
+                check(lib.casmvs_warp_cost_bwd_det(_ptr(f_cl), _ptr(proj), _ptr(dv), _ptr(g), _ptr(gf),
+                                                   B, V, C, D, h, w, ctx.G, _ptr(ws), ws.numel(),
+                                                   _stream()), "warp_cost_bwd_det")
+            else:
+                gf = torch.zeros_like(f_cl)
+                check(lib.casmvs_warp_cost_bwd(_ptr(f_cl), _ptr(proj), _ptr(dv), _ptr(g), _ptr(gf),
+                                               B, V, C, D, h, w, ctx.G, _stream()), "warp_cost_bwd")
         return gf.permute(0, 1, 4, 2, 3), None, None, None
 
 
@@ -97,20 +122,30 @@ class Conv3dFn(torch.autograd.Function):
                 # adjoint of the transposed conv: Conv3d(k3,s2,p1), weight read as (out=Cin, in=Cout)
                 gx = _raw_conv(gy_l, w, CONV, 2, precision)
         if ctx.needs_input_grad[1]:
-            lib = _lib.load()
             with torch.cuda.device(x.device):
                 if kind == CONV:
-                    dw = torch.zeros(27, cin, cout, device=x.device, dtype=torch.float32)
-                    check(lib.casmvs_conv3d_wgrad(_ptr(xs), _ptr(gyd), _ptr(dw), B, cin, cout, Di, hi,
-                                                  wi, Do, ho, wo, stride, _stream()), "conv3d_wgrad")
+                    dw = _wgrad(xs, gyd, B, cin, cout, (Di, hi, wi), (Do, ho, wo), stride)
                     gw = dw.view(3, 3, 3, cin, cout).permute(4, 3, 0, 1, 2).contiguous()
                 else:
                     # y[2i-1+k] += x[i] w[k]: the output gradient plays the strided input
-                    dw = torch.zeros(27, cout, cin, device=x.device, dtype=torch.float32)
-                    check(lib.casmvs_conv3d_wgrad(_ptr(gyd), _ptr(xs), _ptr(dw), B, cout, cin, Do, ho,
-                                                  wo, Di, hi, wi, 2, _stream()), "conv3d_wgrad")
+                    dw = _wgrad(gyd, xs, B, cout, cin, (Do, ho, wo), (Di, hi, wi), 2)
                     gw = dw.view(3, 3, 3, cout, cin).permute(4, 3, 0, 1, 2).contiguous()
         return gx, gw, None, None, None
+
+
+def _wgrad(x, gy, B, ca, cb, xdims, ydims, stride):
+    """(27, ca, cb) weight gradient of casmvs_conv3d_wgrad, or of its deterministic variant."""
+    lib = _lib.load()
+    if deterministic():
+        dw = torch.empty(27, ca, cb, device=x.device, dtype=torch.float32)
+        ws = _workspace(lib.casmvs_conv3d_wgrad_det_workspace_bytes(B, ca, cb, *ydims), x.device)
+        check(lib.casmvs_conv3d_wgrad_det(_ptr(x), _ptr(gy), _ptr(dw), B, ca, cb, *xdims, *ydims, stride,
+                                          _ptr(ws), ws.numel(), _stream()), "conv3d_wgrad_det")
+    else:
+        dw = torch.zeros(27, ca, cb, device=x.device, dtype=torch.float32)
+        check(lib.casmvs_conv3d_wgrad(_ptr(x), _ptr(gy), _ptr(dw), B, ca, cb, *xdims, *ydims, stride,
+                                      _stream()), "conv3d_wgrad")
+    return dw
 
 
 class RegressFn(torch.autograd.Function):
@@ -133,6 +168,37 @@ class RegressFn(torch.autograd.Function):
                                                  _ptr(gdepth.contiguous()), _ptr(out), B, D, h, w,
                                                  _stream()), "regress_bwd")
         return out, None
+
+
+class Upsample2xFn(torch.autograd.Function):
+    """F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True) of a CUDA fp32
+    (N,C,h,w) tensor, NCHW or channels-last: ATen's forward, the gather backward."""
+
+    @staticmethod
+    def forward(ctx, x):
+        return F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True)
+
+    @staticmethod
+    def backward(ctx, gy):
+        N, C, H, W = gy.shape
+        nhwc = gy.is_contiguous(memory_format=torch.channels_last) and not gy.is_contiguous()
+        g = gy if nhwc else gy.contiguous()
+        gx = torch.empty(N, C, H // 2, W // 2, device=gy.device, dtype=torch.float32,
+                         memory_format=torch.channels_last if nhwc else torch.contiguous_format)
+        with torch.cuda.device(gy.device):
+            check(_lib.load().casmvs_upsample2x_bilinear_bwd(_ptr(g), _ptr(gx), N, C, H // 2, W // 2,
+                                                             NHWC if nhwc else NCHW, _stream()),
+                  "upsample2x_bilinear_bwd")
+        return gx
+
+
+def upsample2x(x):
+    """FeatureNet's x2 bilinear upsample (align_corners=True).  torch's own backward scatters
+    with atomics, and raises under torch.use_deterministic_algorithms(True): a CUDA fp32 input
+    then takes Upsample2xFn's gather backward instead."""
+    if deterministic() and x.is_cuda and x.dtype == torch.float32 and torch.is_grad_enabled():
+        return Upsample2xFn.apply(x)
+    return F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True)
 
 
 def conv3d(x, weight, kind=CONV, stride=1, precision=FP32):

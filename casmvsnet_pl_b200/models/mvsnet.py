@@ -39,7 +39,8 @@ class FeatureNet(nn.Module):
 
     @staticmethod
     def _up2(x):
-        return F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True)
+        from .. import autograd as AG
+        return AG.upsample2x(x)
 
     # cuDNN would run fp32 convs as TF32 on H100 by default; the reference path is fp32
     # (opt.py:69-70), so IEEE fp32 is kept unless the model runs in its tf32 precision mode.
@@ -58,10 +59,15 @@ class FeatureNet(nn.Module):
         stream wait for the event before touching that level (CascadeMVSNet.forward does, so the
         coarsest cascade stage -- many small, latency-bound kernels -- runs concurrently with the
         bandwidth-heavy top-down half of the pyramid)."""
+        if self.training or torch.is_grad_enabled():
+            # with deterministic algorithms on, autotuning could still pick a different (each
+            # deterministic) algorithm in another process: the heuristics' choice is fixed
+            det = torch.are_deterministic_algorithms_enabled()
+            with torch.backends.cudnn.flags(enabled=True, benchmark=self.benchmark and not det,
+                                            allow_tf32=self.allow_tf32):
+                return self._forward_modules(x)
         with torch.backends.cudnn.flags(enabled=True, benchmark=self.benchmark,
                                         allow_tf32=self.allow_tf32):
-            if self.training or torch.is_grad_enabled():
-                return self._forward_modules(x)
             if self.allow_tf32 and self.tensor_path and x.is_cuda:
                 return self._forward_tensor(x, overlap)
             return self._forward_folded(x)

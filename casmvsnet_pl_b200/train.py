@@ -28,6 +28,13 @@ for the reference's MVSSystem:
   * checkpoints in Lightning's layout, ckpts/<exp_name>/_ckpt_epoch_{e}.ckpt, keeping the 5
     best by val/acc_2mm.
 
+Reproducible runs: --deterministic turns on torch.use_deterministic_algorithms (Lightning's
+Trainer(deterministic=True)); the backward then runs the library's deterministic kernels and
+cuDNN's heuristically chosen deterministic algorithms.  --seed N seeds the model's
+initialisation, the training loader's shuffle and its workers' colour-jitter draws.  With both,
+a run's metrics.jsonl and checkpoints are the same bits every time on the same data and GPU
+model.
+
 Not supported (the command exits with a message): radam and ranger, --use_amp, more than one
 GPU.
 """
@@ -83,7 +90,19 @@ def build_parser():
                     help="fp32 (as the reference) or tf32 tensor-core convolutions")
     ap.add_argument("--log_every", type=int, default=10, help="steps between JSON log lines")
     ap.add_argument("--num_workers", type=int, default=4, help="host data-loader workers")
+    ap.add_argument("--deterministic", default=False, action="store_true",
+                    help="bit-reproducible steps: torch.use_deterministic_algorithms(True)")
+    ap.add_argument("--seed", type=int, default=None,
+                    help="seed of the initialisation, the shuffle and the workers' jitter draws")
     return ap
+
+
+def set_deterministic():
+    """torch.use_deterministic_algorithms(True), with the cuBLAS workspace setting it asks for
+    (read when cuBLAS initialises, so set before the first CUDA call), and no cuDNN autotuning."""
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+    torch.use_deterministic_algorithms(True)
+    torch.backends.cudnn.benchmark = False
 
 
 def check_supported(a):
@@ -297,16 +316,20 @@ def build_datasets(a):
 def main(argv=None):
     a = build_parser().parse_args(argv)
     check_supported(a)
+    if a.deterministic:
+        set_deterministic()
     if not torch.cuda.is_available():
         raise SystemExit("training needs a CUDA GPU")
     device = "cuda:0"
     train_set, val_set = build_datasets(a)
+    if a.seed is not None:
+        torch.manual_seed(a.seed)
     model = build_model(a, device)
     print("number of parameters : %.2f M" % (sum(p.numel() for p in model.parameters()
                                                   if p.requires_grad) / 1e6))
     trainer = Trainer(a, model, device)
     t0 = time.time()
-    kept = trainer.fit(train_data.loader(train_set, a.batch_size, True, a.num_workers),
+    kept = trainer.fit(train_data.loader(train_set, a.batch_size, True, a.num_workers, seed=a.seed),
                        train_data.loader(val_set, a.batch_size, False, a.num_workers),
                        os.path.join("logs", a.exp_name, "metrics.jsonl"),
                        os.path.join("ckpts", a.exp_name))

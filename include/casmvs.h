@@ -315,6 +315,36 @@ int casmvs_regress_bwd(const float* logits, const float* depth_values, int dv_is
                        const float* grad_depth, float* grad_logits, int B, int D, int h, int w,
                        void* stream);
 
+/* ---- deterministic backward: the same bits for the same inputs, shapes and device model ------
+ * casmvs_warp_cost_bwd_det: what casmvs_warp_cost_bwd computes, with no float atomics.  A
+ *   contribution pass records every bilinear tap's destination texel, weight and coefficient; a
+ *   stable radix sort groups them by destination; each texel then adds its contributions in
+ *   contribution order.  The reference view's gradient is summed over all D planes by one
+ *   thread.  grad_feats is WRITTEN (no zeroing needed).  Same arguments and dims as
+ *   casmvs_warp_cost_bwd, plus `workspace` (256-byte aligned) of at least
+ *   casmvs_warp_cost_bwd_det_workspace_bytes(B, V, C, D, h, w) bytes: 4 (C + 20) bytes per
+ *   (batch item, plane, pixel, source view) plus the sort's temporary storage (0 = dims out of
+ *   range).  feats and grad_feats need 16-byte alignment.
+ * casmvs_conv3d_wgrad_det: what casmvs_conv3d_wgrad computes; each voxel chunk stores its
+ *   [27][Ca][Cb] partial to the workspace and a second kernel adds the chunks in chunk order.
+ *   The chunking depends on B * Do * ho * wo only.  grad_w is WRITTEN.  workspace: at least
+ *   casmvs_conv3d_wgrad_det_workspace_bytes(B, Ca, Cb, Do, ho, wo) bytes.
+ * casmvs_upsample2x_bilinear_bwd: grad_x (N,C,h,w) of y = bilinear upsample to (2h, 2w) with
+ *   align_corners=True, given grad_y (N,C,2h,2w); both CASMVS_NCHW or both CASMVS_NHWC
+ *   (`layout`).  Each input element gathers its output pixels in a fixed order with ATen's
+ *   weights.  grad_x is WRITTEN. */
+size_t casmvs_warp_cost_bwd_det_workspace_bytes(int B, int V, int C, int D, int h, int w);
+int casmvs_warp_cost_bwd_det(const float* feats, const float* proj, const float* depth_values,
+                             const float* grad_cost, float* grad_feats, int B, int V, int C,
+                             int D, int h, int w, int num_groups, void* workspace,
+                             size_t workspace_bytes, void* stream);
+size_t casmvs_conv3d_wgrad_det_workspace_bytes(int B, int Ca, int Cb, int Do, int ho, int wo);
+int casmvs_conv3d_wgrad_det(const float* x, const float* grad_y, float* grad_w, int B, int Ca,
+                            int Cb, int Di, int hi, int wi, int Do, int ho, int wo, int stride,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int casmvs_upsample2x_bilinear_bwd(const float* grad_y, float* grad_x, int N, int C, int h, int w,
+                                   int layout, void* stream);
+
 /* ---- training loss and depth metrics (reference losses.py, metrics.py) ----------------------
  * Per level l < levels (<= 4): pred[l], gt[l] (B,h_l,w_l) float32, mask[l] (B,h_l,w_l) uint8
  * (bool; nonzero = valid); hw is a HOST array (levels,2) of (h_l, w_l); pred / gt / mask /
