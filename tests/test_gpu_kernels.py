@@ -329,8 +329,9 @@ def test_regress_index_exact_given_identical_prob(golden, D):
 
 
 def test_regress_register_path_bit_identical(tmp_path):
-    """The D = 8/32/48 register-resident K3 path performs the generic path's operations in the
-    generic path's order: a child process with CASMVS_K3_REG=0 must reproduce it bit for bit."""
+    """The default K3 kernels -- the register-resident kernel at D = 8, the plane-parallel
+    kernel at D = 32 and 48 -- perform the generic kernel's operations in the generic kernel's
+    order: a child process with CASMVS_K3_REG=0 must reproduce them bit for bit."""
     import subprocess, sys
     code = (
         "import sys, torch\n"
