@@ -5,7 +5,7 @@ device is not a H100 (sm_90a) GPU the import / call fails loudly.
 """
 import ctypes
 import os
-from ctypes import c_char_p, c_double, c_float, c_int, c_size_t, c_uint64, c_void_p, POINTER
+from ctypes import c_char_p, c_double, c_float, c_int, c_longlong, c_size_t, c_uint64, c_void_p, POINTER
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libcasmvs.so")
@@ -104,7 +104,10 @@ SIGNATURES = {
     "casmvs_pcd_capped_nn": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                      POINTER(c_double), c_double, POINTER(c_int), POINTER(c_double),
                                      POINTER(c_double), c_double, c_void_p, c_void_p]),
-    "casmvs_nchw_to_nhwc":(c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
+    "casmvs_view_scores_workspace_bytes": (c_size_t, [c_int, c_int, c_longlong]),
+    "casmvs_view_scores_fwd": (c_int, [c_void_p] * 4 + [c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                                          c_void_p]),
+    "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
 }
 

@@ -14,6 +14,11 @@ over the three test layouts eval.py reads (--dataset_name):
     blendedmvs  BlendedMVSTestScan  datasets/blendedmvs.py; <root>/<scan>/{cams, blended_images,
                                     rendered_depth_maps}, scan lists in <root>/..
 
+and over a scene of the user's own, reconstructed by COLMAP and undistorted:
+
+    colmap      ColmapScan          <root>/images, <root>/sparse/{cameras,images,points3D}.{bin,txt};
+                                    view selection and depth ranges computed here (colmap.py)
+
 Everything between decoding the images and writing the PLY stays on the GPU.  DTU images are
 decoded and resized on the host per use, as the reference does, uploaded as bytes and normalised
 by casmvs_normalize_u8_fwd.  Tanks and BlendedMVS scans decode each view once into SceneImages,
@@ -25,6 +30,8 @@ proba_XXXX.pfm are written as well).
     python -m casmvsnet_pl_b200.eval_pipeline --dataset_name tanks --split intermediate --root_dir TNT
     python -m casmvsnet_pl_b200.eval_pipeline --dataset_name blendedmvs --split val \
         --root_dir BlendedMVS/dataset_low_res --img_wh 768 576
+    python -m casmvsnet_pl_b200.eval_pipeline --dataset_name colmap --root_dir my_capture/dense \
+        --ckpt ckpt.ckpt --img_wh 1152 864 [--depth_interval 192]
 """
 from __future__ import annotations
 
@@ -305,12 +312,72 @@ class BlendedMVSTestScan(_CachedScan):
         return float(np.float32(self.depth_min[ref])), self.depth_interval[ref]
 
 
+class ColmapScan(_CachedScan):
+    """A scene reconstructed by COLMAP, in the workspace `colmap image_undistorter` writes:
+
+        <root>/images/<name>, <root>/sparse/{cameras,images,points3D}.{bin,txt}
+
+    Views are numbered 0..n-1 in sorted image-name order.  Each view's sources are the N_SRC
+    views with the best positive view-selection score (colmap.py; the scores are computed on the
+    GPU by casmvs_view_scores_fwd).  A view is not a reference view when it has fewer than
+    n_views - 1 sources or fewer than 20 observed points in front of it; `skipped` maps those to
+    the reason.  A reference view's depth range is [0.75 q(0.01), 1.25 q(0.99)] of the depths of
+    its observed points and its depth interval that range / n_depths_arg.  Intrinsics are the
+    full-resolution K of the view's own camera, scaled to img_wh like Tanks'.
+    With `out_dir`, the run is recorded in <out_dir>/<scan>: cams/{vid:08d}_cam.txt for every
+    view (MVSNet format: extrinsic, full-resolution intrinsic, `depth_min interval n_depths
+    depth_max`, nan for a view with no point in front of it), pair.txt with the reference views
+    and their scored sources, and view_names.txt (view id -> image name)."""
+
+    def __init__(self, root_dir, scan=None, img_wh=(1152, 864), n_views=5, n_depths_arg=192.0,
+                 levels=3, host_images=False, out_dir=None, device="cuda:0", log=print):
+        from . import colmap
+        assert img_wh[0] % 32 == 0 and img_wh[1] % 32 == 0, "img_wh must both be multiples of 32!"
+        self.root_dir = root_dir
+        self.scan = scan or os.path.basename(os.path.normpath(os.path.abspath(root_dir)))
+        self.img_wh, self.n_views, self.host_images = tuple(img_wh), n_views, host_images
+        sc = self.scene = colmap.load_scene(root_dir)
+        if len(sc) == 0:
+            raise ValueError(f"{root_dir}: the COLMAP model has no registered images")
+        scores = colmap.view_scores(sc.centres, sc.xyz, sc.track_ptr, sc.track_img, device)
+        count, q = colmap.depth_stats(sc.E, sc.xyz, sc.track_ptr, sc.track_img, device)
+        self.scores = scores.cpu().numpy()
+        sources, refs, self.skipped, dmin, dmax = colmap.assemble(self.scores, count, q, n_views)
+        self.metas = [(r, [s for s, _ in sources[r]]) for r in refs]
+        E32, K32 = sc.E.astype(np.float32), sc.K.astype(np.float32)
+        self.proj_mats = {v: io.pyramid_proj_mats(K32[v], E32[v], levels, self.img_wh,
+                                                  tuple(int(x) for x in sc.wh[v]))
+                          for v in range(len(sc))}
+        self.depth_min, self.depth_interval, self.depth_max = {}, {}, {}
+        for v in range(len(sc)):            # NaN for a view with no point in front of it
+            self.depth_min[v] = float(np.float32(dmin[v]))
+            self.depth_interval[v] = float(np.float32((dmax[v] - dmin[v]) / n_depths_arg))
+            self.depth_max[v] = float(dmax[v])
+        for v, why in sorted(self.skipped.items()):
+            log(f"{self.scan}: view {v} ({sc.names[v]}) is not a reference view: {why}")
+        if out_dir:
+            d = os.path.join(out_dir, self.scan)
+            os.makedirs(d, exist_ok=True)
+            colmap.write_cams(os.path.join(d, "cams"), E32, K32,
+                              {v: (self.depth_min[v], self.depth_interval[v], self.depth_max[v])
+                               for v in range(len(sc))}, n_depths_arg)
+            colmap.write_pair(os.path.join(d, "pair.txt"), [(r, sources[r]) for r in refs])
+            colmap.write_view_names(os.path.join(d, "view_names.txt"), sc.names)
+
+    def image_path(self, vid):
+        return os.path.join(self.root_dir, "images", self.scene.names[vid])
+
+    def depth_range(self, ref, depth_interval):
+        # the divisor was applied at construction (n_depths_arg)
+        return self.depth_min[ref], self.depth_interval[ref]
+
+
 @torch.no_grad()
 def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
              dtu_gt=None, dtu_seed=0, save_visual=False):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
-    `scan` is a DTUTestScan, TanksTestScan or BlendedMVSTestScan; each gives the depth range of
+    `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
     and thresholded confidence JPEGs of eval.py:230-239 are written too.
     With `dtu_gt` (a DTU ground-truth directory) the fused cloud is also scored by
@@ -350,6 +417,10 @@ def open_scans(a):
     if a.dataset_name == "dtu":
         yield DTUTestScan(a.root_dir, a.scan, tuple(a.img_wh), a.n_views)
         return
+    if a.dataset_name == "colmap":
+        yield ColmapScan(a.root_dir, a.scan or None, tuple(a.img_wh), a.n_views, a.depth_interval,
+                         out_dir=a.out_dir)
+        return
     if a.dataset_name == "tanks":
         for s in [a.scan] if a.scan else list(TanksTestScan.SCANS[a.split]):
             yield TanksTestScan(a.root_dir, a.split, s, tuple(a.img_wh), a.n_views)
@@ -368,21 +439,32 @@ def load_checkpoint(model, path):
     return model
 
 
-def main(argv=None):
+DEFAULT_DEPTH_INTERVAL = {"dtu": 2.65, "tanks": 2.65, "blendedmvs": 2.65, "colmap": 192.0}
+
+
+def parse_args(argv=None):
+    """The command line, with --depth_interval resolved per data set (DEFAULT_DEPTH_INTERVAL:
+    2.65 as eval.py has it for dtu, tanks and blendedmvs; 192 = 48 x 4 for colmap, so that the
+    coarsest stage's 48 planes at interval ratio 4 span a view's depth range exactly) and the
+    output directory (default results/<dataset_name>) in `out_dir`."""
     ap = argparse.ArgumentParser()
     ap.add_argument("--root_dir", required=True)
-    ap.add_argument("--dataset_name", default="dtu", choices=["dtu", "tanks", "blendedmvs"])
+    ap.add_argument("--dataset_name", default="dtu", choices=["dtu", "tanks", "blendedmvs", "colmap"])
     ap.add_argument("--split", default="test",
-                    help="tanks: intermediate | advanced; blendedmvs: train | val | all; dtu: unused")
-    ap.add_argument("--scan", default="", help="one scan (default: every scan of the split; dtu needs it)")
+                    help="tanks: intermediate | advanced; blendedmvs: train | val | all; "
+                         "dtu, colmap: unused")
+    ap.add_argument("--scan", default="", help="one scan (default: every scan of the split; dtu "
+                                               "needs it; colmap: the name of the root directory)")
     ap.add_argument("--ckpt", default="")
     ap.add_argument("--img_wh", nargs=2, type=int, default=[1152, 864])
     ap.add_argument("--n_views", type=int, default=5)
     ap.add_argument("--n_depths", nargs="+", type=int, default=[8, 32, 48])
     ap.add_argument("--interval_ratios", nargs="+", type=float, default=[1.0, 2.0, 4.0])
     ap.add_argument("--num_groups", type=int, default=1)
-    ap.add_argument("--depth_interval", type=float, default=2.65,
-                    help="dtu: the depth interval; tanks: no effect; blendedmvs: divides each view's depth range")
+    ap.add_argument("--depth_interval", type=float, default=None,
+                    help="dtu: the depth interval (default 2.65); tanks: no effect; blendedmvs: "
+                         "divides each view's depth range (default 2.65); colmap: the same "
+                         "(default 192)")
     ap.add_argument("--conf", type=float, default=0.999)
     ap.add_argument("--min_geo_consistent", type=int, default=5)
     ap.add_argument("--max_ref_views", type=int, default=400)
@@ -393,6 +475,14 @@ def main(argv=None):
     ap.add_argument("--dtu_gt", default=None, help="DTU ground-truth directory: score the fused cloud")
     ap.add_argument("--dtu_seed", type=int, default=0)
     a = ap.parse_args(argv)
+    if a.depth_interval is None:
+        a.depth_interval = DEFAULT_DEPTH_INTERVAL[a.dataset_name]
+    a.out_dir = a.out or os.path.join("results", a.dataset_name)
+    return a
+
+
+def main(argv=None):
+    a = parse_args(argv)
     if a.dtu_gt is not None and a.dataset_name != "dtu":
         raise SystemExit("--dtu_gt applies to dtu only")
     if a.dataset_name == "dtu" and not a.scan:
@@ -400,7 +490,7 @@ def main(argv=None):
     splits = {"tanks": TanksTestScan.SCANS, "blendedmvs": BlendedMVSTestScan.SPLITS}.get(a.dataset_name)
     if splits is not None and a.split not in splits:
         raise SystemExit(f"--split must be one of {sorted(splits)} for {a.dataset_name}")
-    out_dir = a.out or os.path.join("results", a.dataset_name)
+    out_dir = a.out_dir
     from . import ABN
     from .models.mvsnet import CascadeMVSNet
     model = CascadeMVSNet(n_depths=a.n_depths, interval_ratios=a.interval_ratios,

@@ -15,6 +15,10 @@ the native size for timing); each view's source list holds its neighbours on the
 `n_few`, every n_few-th BlendedMVS reference view lists only 2 valid sources, so readers with
 n_views > 2 skip it (blendedmvs.py:51-54), and is no other view's source.
 
+make_colmap writes the same arc of cameras as an undistorted COLMAP workspace (images/ and a
+sparse/ model of points on a known surface, binary and / or text) for eval_pipeline's colmap
+reader; sparse_tracks makes bare sparse models of any size for the view-selection kernel.
+
     python -m casmvsnet_pl_b200.synth_scenes --kind tanks --root TNT --n_views 150 --image_wh 1920 1080
 """
 from __future__ import annotations
@@ -181,6 +185,101 @@ def make_dtu_train(root, scan="scan1", refs=(0, 1, 2), n_src=5, depth=650.0, see
         with open(os.path.join(root, "lists", f"{split}.txt"), "w") as f:
             f.write(scan + "\n")
     return root
+
+
+def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=0, n_single=20,
+                 n_dup=20):
+    """The arc cameras of the other layouts as a COLMAP model (colmap.ColmapModel) looking at a
+    known surface, z = depth + 0.05 depth sin(3x / depth) cos(2y / depth) in world coordinates,
+    which every optical axis meets at depth `depth` (the cameras sit on a circle of that radius
+    around (0, 0, depth) and look at its centre).  Even views use a PINHOLE camera of `image_wh`,
+    odd views a SIMPLE_PINHOLE camera 1.25 times larger.  Image ids are shuffled against the
+    sorted image names.  A point's track is every view it projects into with z > 0; the first
+    n_single tracks of length > 1 are cut to one view and n_dup others list their first view
+    twice."""
+    from . import colmap
+    rng = np.random.default_rng(seed)
+    W, H = image_wh
+    W2, H2 = int(round(W * 1.25)), int(round(H * 1.25))
+    cams = {1: ("PINHOLE", W, H, np.array([1.1 * W, 1.1 * W * 1.01, W / 2, H / 2])),
+            2: ("SIMPLE_PINHOLE", W2, H2, np.array([1.1 * W2, W2 / 2, H2 / 2]))}
+    ids = rng.permutation(n_views) + 1
+    images, Es, Ks, whs = {}, [], [], []
+    for v in range(n_views):
+        t = np.deg2rad(2.0 * (v - n_views / 2))
+        R = np.array([[np.cos(t), 0, np.sin(t)], [0, 1, 0], [-np.sin(t), 0, np.cos(t)]])
+        tv = np.array([-depth * np.sin(t), 0, depth * (1 - np.cos(t))])
+        cid = 1 if v % 2 == 0 else 2
+        images[int(ids[v])] = (colmap.rotmat_to_qvec(R), tv, cid, f"view_{v:03d}.jpg")
+        E = np.eye(4)
+        E[:3, :3], E[:3, 3] = R, tv
+        name, w, h, prm = cams[cid]
+        Es.append(E)
+        Ks.append(colmap.intrinsics(name, prm))
+        whs.append((w, h))
+    x = rng.uniform(-0.5, 0.5, n_points) * depth
+    y = rng.uniform(-0.3, 0.3, n_points) * depth
+    xyz = np.stack([x, y, depth + 0.05 * depth * np.sin(3 * x / depth) * np.cos(2 * y / depth)], 1)
+    tracks = []
+    for p in xyz:
+        tr = []
+        for v in range(n_views):
+            q = Ks[v] @ (Es[v][:3, :3] @ p + Es[v][:3, 3])
+            if q[2] > 0 and 0 <= q[0] / q[2] < whs[v][0] and 0 <= q[1] / q[2] < whs[v][1]:
+                tr.append(int(ids[v]))
+        tracks.append(tr)
+    long_ = [k for k, tr in enumerate(tracks) if len(tr) > 1]
+    for k in long_[:n_single]:
+        tracks[k] = tracks[k][:1]
+    for k in long_[n_single:n_single + n_dup]:
+        tracks[k] = tracks[k] + tracks[k][:1]
+    keep = [k for k, tr in enumerate(tracks) if tr]
+    ptr = np.zeros(len(keep) + 1, np.int64)
+    np.cumsum([len(tracks[k]) for k in keep], out=ptr[1:])
+    img = np.array([i for k in keep for i in tracks[k]], np.int64)
+    return colmap.ColmapModel(cams, images, 1 + 3 * np.arange(len(keep)), xyz[keep], ptr, img)
+
+
+def sparse_tracks(n_img=300, n_pts=500_000, track_len=(3, 11), seed=0):
+    """A seeded sparse reconstruction for view selection alone, as arrays: centres (n_img,3) on
+    a circle of radius 10 around the origin, points (n_pts,3) near the origin, and tracks in CSR
+    form (track_ptr (n_pts+1,) int64, track_img int32) of distinct images, lengths uniform in
+    track_len (inclusive), each a random subset of a window of neighbouring images.  The
+    defaults are the size of a Tanks and Temples scene (mean track 7)."""
+    rng = np.random.default_rng(seed)
+    a = np.linspace(0, 2 * np.pi, n_img, endpoint=False)
+    centres = np.stack([10 * np.cos(a), 10 * np.sin(a), rng.uniform(-1, 1, n_img)], 1)
+    xyz = rng.normal(0, 2, (n_pts, 3))
+    lens = rng.integers(track_len[0], track_len[1] + 1, n_pts)
+    ptr = np.zeros(n_pts + 1, np.int64)
+    np.cumsum(lens, out=ptr[1:])
+    win = min(n_img, max(2 * track_len[1], 16))
+    img = np.empty(ptr[-1], np.int32)
+    first = rng.integers(0, n_img, n_pts)
+    for L in np.unique(lens):
+        sel = np.nonzero(lens == L)[0]
+        pick = np.argsort(rng.random((len(sel), win)), 1)[:, :L]    # L distinct offsets per point
+        img[(ptr[sel][:, None] + np.arange(L)).ravel()] = ((first[sel][:, None] + pick) % n_img).ravel()
+    return centres, xyz, ptr, img
+
+
+def make_colmap(root, n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=0,
+                fmt="bin", **kw):
+    """An undistorted COLMAP workspace: <root>/images/view_XXX.jpg at each view's camera size and
+    the model of colmap_model under <root>/sparse, in binary ("bin"), text ("txt") or both
+    formats ("both"; the reader prefers the binary one).  Returns the model."""
+    from PIL import Image
+
+    from . import colmap
+    model = colmap_model(n_views, image_wh, depth, n_points, seed, **kw)
+    rng = np.random.default_rng(seed + 1)
+    os.makedirs(os.path.join(root, "images"), exist_ok=True)
+    for q, t, cid, name in model.images.values():
+        _, w, h, _ = model.cameras[cid]
+        Image.fromarray(_image(rng, w, h)).save(os.path.join(root, "images", name), quality=92)
+    for f in (("bin", "txt") if fmt == "both" else (fmt,)):
+        colmap.write_model(os.path.join(root, "sparse"), model, f)
+    return model
 
 
 def main(argv=None):

@@ -463,6 +463,29 @@ int casmvs_pcd_capped_nn(const float* queries, int nq, const float* targets,
                          const int* super_dims3, const double* box_lo3, const double* box_hi3,
                          double cap, double* dist, void* stream);
 
+/* ---- view selection of a sparse reconstruction (casmvsnet_pl_b200/colmap.py) ---------------
+ * casmvs_view_scores_fwd: the MVSNet paper's (section 4.1) view-selection scores, in double:
+ *   scores[i][j] = sum over the points p that both images i and j see of G(theta_ij(p)),
+ *   theta_ij(p) = degrees(acos(clamp(dot(unit(c_i - p), unit(c_j - p)), -1, 1))),
+ *   G(theta) = exp(-(theta - 5)^2 / 2) for theta <= 5, exp(-(theta - 5)^2 / 200) else;
+ *   a point on a camera centre contributes 0.  scores (n_img, n_img) is WRITTEN, symmetric, 0 on
+ *   the diagonal.  centres (n_img,3) and points (n_pts,3) row-major doubles; the tracks in CSR
+ *   form: point p is seen by track_img[track_ptr[p] .. track_ptr[p+1]) (int64 offsets, int32
+ *   image ids).  The images of one track must be distinct; a pair with an id outside
+ *   [0, n_img) contributes nothing.  n_img <= 65535.
+ *   Deterministic: each score is added in ascending point order (pairs are expanded, stably
+ *   radix-sorted by image pair and summed run by run), so the result is the same bits on every
+ *   call and for every workspace size.  The pairs are processed in chunks of at most
+ *   max_chunk_pairs entries (default 2^22); the chunk is the largest the workspace holds.
+ *   The call synchronises `stream` once, to read the number of pairs (not graph-capturable).
+ *   No points or fewer than two images: scores is zeroed, no kernel runs, workspace may be NULL.
+ * casmvs_view_scores_workspace_bytes: the workspace (256-byte aligned) for chunks of at most
+ *   max_chunk_pairs pairs (<= 0: the default, the fastest); 0 when none is needed. */
+size_t casmvs_view_scores_workspace_bytes(int n_img, int n_pts, long long max_chunk_pairs);
+int casmvs_view_scores_fwd(const double* centres, const double* points, const long long* track_ptr,
+                           const int* track_img, int n_img, int n_pts, double* scores,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- layout helpers ------------------------------------------------------ */
 /* (N,C,S) -> (N,S,C) and back, S = product of spatial dims. */
 int casmvs_nchw_to_nhwc(const float* in, float* out, int N, int C, size_t S, void* stream);
