@@ -14,6 +14,7 @@ NCHW, NHWC = 0, 1
 ROUND_TF32 = 256
 KEEP_FP32_OUT = 256      # OR-ed into conv3d precision
 BLOCKED = 512            # OR-ed into costreg precision / warp_cost_ladder round_tf32
+FUSED_TAIL = 1024        # OR-ed into costreg precision: conv11 + prob in one kernel, u11 not kept
 FP32, TF32 = 0, 1
 CONV, CONV_TRANSPOSE, CONV_PLANAR = 0, 1, 2
 PRECISIONS = {"fp32": FP32, "tf32": TF32}
@@ -49,6 +50,10 @@ SIGNATURES = {
     "casmvs_costreg_blocked_supported": (c_int, [c_int, c_int]),
     "casmvs_costreg_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                    c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "casmvs_costreg_tail_supported": (c_int, [c_int, c_int]),
+    "casmvs_costreg_layer_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                         c_int, c_int, c_int, c_void_p, c_size_t, c_int,
+                                         c_void_p]),
     "casmvs_regress_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "casmvs_depth_hypotheses_fwd": (c_int, [c_void_p, c_int, c_float, c_float, c_void_p,

@@ -27,6 +27,8 @@ int conv3d_direct(const float* x, const float* wpk, const float* scale, const fl
 ConvLauncher conv3d_tma_find(int Cin, int Cout, int kind, int stride);
 // conv3d_tma2.cu (wgmma + TMA producer, persistent): stride-2 and transposed layers
 ConvLauncher conv3d_tma2_find(int Cin, int Cout, int kind, int stride, bool skip);
+// conv3d_tail.cu: conv11 + prob in one kernel, by (u9 channels, skip channels, output channels)
+TailLauncher conv3d_tail_find(int cin, int cskip, int cout);
 
 static ConvLauncher tensor_core_launcher(int Cin, int Cout, int kind, int stride, bool skip) {
   if (ConvLauncher run = conv3d_tma_find(Cin, Cout, kind, stride)) return run;
@@ -177,18 +179,30 @@ extern "C" int casmvs_costreg_blocked_supported(int Cin, int precision) {
   return 1;
 }
 
+extern "C" int casmvs_costreg_tail_supported(int Cin, int precision) {
+  // conv11 (u9: 16 channels, skip c0: 8) + prob (1 output channel), on blocked activations
+  return casmvs_costreg_blocked_supported(Cin, precision) && conv3d_tail_find(16, 8, 1) ? 1 : 0;
+}
+
+// The driver of casmvs_costreg_fwd (only < 0: the whole stack) and casmvs_costreg_layer_fwd
+// (only = a layer, or 11: the fused conv11 + prob kernel).
 // x and the activations in the workspace are read in 16-byte vectors (the workspace offsets are
 // multiples of 256 B); the prob head writes the logits one float at a time.
-extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* logits, int B,
-                                  int Cin, int D, int h, int w, int precision, void* workspace,
-                                  size_t workspace_bytes, void* stream) {
+static int costreg_run(const float* x, const float* params, float* logits, int B, int Cin, int D,
+                       int h, int w, int precision, void* workspace, size_t workspace_bytes,
+                       void* stream, int only) {
   CASMVS_REQUIRE_ALIGNED("costreg", x, 16);
   CASMVS_REQUIRE_ALIGNED("costreg", workspace, 16);
   CASMVS_REQUIRE_ALIGNED("costreg", logits, 4);
   CASMVS_REQUIRE(x && params && logits, "costreg: null pointer");
   const bool blocked_in = (precision & CASMVS_BLOCKED) != 0;
-  precision &= ~CASMVS_BLOCKED;
+  const bool fuse_tail = (precision & CASMVS_FUSED_TAIL) != 0 || only == 11;
+  precision &= ~(CASMVS_BLOCKED | CASMVS_FUSED_TAIL);
   const bool blocked = casmvs_costreg_blocked_supported(Cin, precision);
+  // u11 is never stored: the logits come from u9 and c0 in one kernel
+  const bool tail = fuse_tail && casmvs_costreg_tail_supported(Cin, precision);
+  CASMVS_REQUIRE(only != 11 || tail, "costreg: no fused conv11 + prob kernel for Cin=%d, "
+                 "precision %d", Cin, precision);
   CASMVS_REQUIRE(!blocked_in || blocked,
                  "costreg: a blocked input needs the TF32 precision and a Cin whose conv0 a "
                  "tensor-core kernel covers (8, 16 or 32; got Cin=%d)", Cin);
@@ -228,9 +242,11 @@ extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* lo
   const int blk = blocked ? kLayoutXBlocked | kLayoutYBlocked : 0;
   int rc;
 #define LAYER(i, in, skip, out, d_, h_, w_, sl, lay)                                              \
-  rc = conv_layer(in, W[i], SC[i], SH[i], sl, skip, out, B, L[i].cin, L[i].cout, d_, h_, w_,     \
-                  L[i].kind, L[i].stride, precision, lay, stream);                                \
-  if (rc) return rc;
+  if (only < 0 || only == i) {                                                                   \
+    rc = conv_layer(in, W[i], SC[i], SH[i], sl, skip, out, B, L[i].cin, L[i].cout, d_, h_, w_,   \
+                    L[i].kind, L[i].stride, precision, lay, stream);                              \
+    if (rc) return rc;                                                                            \
+  }
   LAYER(0, x, nullptr, c0, D, h, w, slope,
         (blk & kLayoutYBlocked) | (blocked_in ? kLayoutXBlocked : 0))
   LAYER(1, c0, nullptr, c1, D, h, w, slope, blk)
@@ -241,8 +257,28 @@ extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* lo
   LAYER(6, c5, nullptr, c6, D / 8, h / 8, w / 8, slope, blk)
   LAYER(7, c6, c4, u7, D / 8, h / 8, w / 8, slope, blk)     // conv4 + conv7(x)   mvsnet.py:97
   LAYER(8, u7, c2, u9, D / 4, h / 4, w / 4, slope, blk)     // conv2 + conv9(x)   mvsnet.py:99
+  if (tail) {                                               // conv11 + prob   mvsnet.py:101,103
+    const TailArgs a{u9, c0, W[9], SC[9], SH[9], W[10], SC[10], SH[10], logits, slope, B, D, h, w};
+    return conv3d_tail_find(16, 8, 1)(a, as_stream(stream));
+  }
   LAYER(9, u9, c0, u11, D / 2, h / 2, w / 2, slope, blk)    // conv0 + conv11(x)  mvsnet.py:101
   LAYER(10, u11, nullptr, logits, D, h, w, 1.0f, blk & kLayoutXBlocked)   // prob: bias  :103
 #undef LAYER
   return 0;
+}
+
+extern "C" int casmvs_costreg_fwd(const float* x, const float* params, float* logits, int B,
+                                  int Cin, int D, int h, int w, int precision, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return costreg_run(x, params, logits, B, Cin, D, h, w, precision, workspace, workspace_bytes,
+                     stream, -1);
+}
+
+extern "C" int casmvs_costreg_layer_fwd(const float* x, const float* params, float* logits, int B,
+                                        int Cin, int D, int h, int w, int precision,
+                                        void* workspace, size_t workspace_bytes, int layer,
+                                        void* stream) {
+  CASMVS_REQUIRE(layer >= 0 && layer <= 11, "costreg_layer: layer %d out of range", layer);
+  return costreg_run(x, params, logits, B, Cin, D, h, w, precision & ~CASMVS_FUSED_TAIL,
+                     workspace, workspace_bytes, stream, layer);
 }

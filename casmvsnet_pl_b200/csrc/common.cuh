@@ -37,6 +37,17 @@ struct ConvArgs {
 };
 using ConvLauncher = int (*)(const ConvArgs& a, cudaStream_t st);
 
+// CostRegNet's conv11 + prob as one kernel (conv3d_tail.cu), blocked activations only.
+struct TailArgs {
+  const float *u9, *c0;                  // (B,4,D/2,h/2,w/2,4), (B,2,D,h,w,4)
+  const float *w11, *scale11, *shift11;  // conv11: packed weights, folded norm
+  const float *wp, *scalep, *shiftp;     // prob: packed weights, scale (1) and bias
+  float* logits;                         // (B,D,h,w)
+  float slope;                           // conv11's LeakyReLU slope
+  int B, D, h, w;                        // full resolution, multiples of 8
+};
+using TailLauncher = int (*)(const TailArgs& a, cudaStream_t st);
+
 // call after every kernel launch: counts it and converts launch errors
 inline int after_launch(const char* what) {
   g_launches.fetch_add(1, std::memory_order_relaxed);

@@ -1,0 +1,389 @@
+// K2 tail — CostRegNet's conv11 (transposed 16 -> 8, + the c0 skip) and prob head (8 -> 1) as
+// one kernel: the logits are computed from u9 and c0, and the full-resolution u11 volume lives
+// only in shared memory.  sm_90a, wgmma tf32, fp32 accumulators in registers.
+//
+// Replaces (reference): conv0 + conv11(x) and prob(x), models/mvsnet.py:101,103.
+//
+// Bit-identical to conv3d_tma2_kernel<MODE_T, 16, 8> followed by conv3d_tma_kernel<8, 8, *,
+// false>: every u11 value is made by the same wgmma (m64n96k8, same B image, same tap / k8
+// order, same accumulator roll) and the same epilogue (scale/shift, LeakyReLU, + c0, tf32
+// rounding), every logit by the same nine m64n24k8 per u11 slice and the same rolling window.
+//
+// Work item: a prob output tile of 8(w) x 16(h) voxels (tc::kTileW x kTileH) times a chunk of
+// output slices [d0, d1), d0 and d1 even.  Its prob GEMM reads u11 over the 18 x 10 halo region
+// of slices d0-1 .. d1; those u11 voxels come from the u9 voxels of an 11 x 6 region (output
+// 2j + p reads input j and j + 1), u9 slices d0/2-1 .. d1/2.
+//   * Producer warp: per u9 slice ("step") one TMA load per u9 channel quad of the 11 x 6 brick,
+//     and the c0 skip bricks ([18][10][4], the stride-1 kernel's box) of the two u11 slices the
+//     step completes.  Out-of-range voxels are zero-filled by the TMA unit.
+//   * Warpgroup 0 (conv11): the u9 brick is stored row after row, 6 voxels each, so GEMM row m
+//     is u9 voxel m of the flattened region and 8 consecutive rows are one 128-byte core matrix:
+//     M = 64 covers the 60 voxels the region needs.  Tap (sh, sw) is the view shifted by
+//     6 sh + sw voxels; rows whose shifted view wraps into the next brick row only feed u11
+//     voxels outside the 18 x 10 region, which are never stored.  After step s the accumulator
+//     holds u11 slices 2s-1 (classes pd = 1) and 2s (pd = 0): their epilogue writes the u11
+//     bricks of a ring in shared memory, with u11 voxels outside the volume set to zero (prob's
+//     zero padding).
+//   * Warpgroup 1 (prob): per u11 slice, the stride-1 GW = 8 GEMM for both 64-row halves of the
+//     tile, then the epilogue of the output slice it completed (logits, fp32).
+#include "common.cuh"
+#include "tc_common.cuh"
+#include "tma_common.cuh"
+
+namespace casmvs {
+
+// conv3d_tma.cu / conv3d_tma2.cu: the operand images of prob and conv11, shared through the
+// image cache with the unfused layers
+int conv3d_tma_prob_image(const float* wpk, cudaStream_t st, tc::ImageRef* ir);
+int conv3d_tma2_conv11_image(const float* wpk, cudaStream_t st, tc::ImageRef* ir);
+
+namespace tail {
+
+using namespace tc;
+using tma::mbar_expect_tx;
+using tma::tma_load_5d;
+
+struct Params {
+  const float* img11;    // conv11 B image (conv3d_tma2 MODE_T, CIN 16, COUT 8)
+  const float* imgp;     // prob B image (conv3d_tma stride-1, CIN 8, GW 8)
+  const float *scale11, *shift11, *scalep, *shiftp;
+  float* logits;         // (B,D,H,W)
+  float slope;           // conv11's LeakyReLU slope
+  int B, D, H, W;        // full resolution: c0, u11, logits
+  int tiles_w, tiles_h, nchunks, dchunk;
+};
+
+constexpr int kU9W = 6, kU9H = 11;                                  // u9 brick columns, rows
+constexpr int kU9Data = kU9H * kU9W * 16;
+constexpr int kU9Bytes = (kU9Data + 127) / 128 * 128;
+constexpr int kBrickData = kHaloH * kHaloW * 16;                    // c0 / u11 brick, one quad
+constexpr int kBrickBytes = (kBrickData + 127) / 128 * 128;
+constexpr int kSliceBytes = 2 * kBrickBytes;                        // 8 channels of one slice
+constexpr int kInBytes = 4 * kU9Bytes + 2 * kSliceBytes;            // u9 slice + 2 c0 slices
+constexpr int IN_SLOTS = 3, U_SLOTS = 4;
+constexpr int kW11Bytes = 4 * 16 * 96 * 4;                          // [tap][cq][12 COUT][4]
+constexpr int kWpBytes = 9 * 8 * 24 * 4;                            // [kh][kw][cq][3 GW][4]
+constexpr int kInOff = 0;
+constexpr int kUOff = kInOff + IN_SLOTS * kInBytes;
+constexpr int kW11Off = kUOff + U_SLOTS * kSliceBytes;
+constexpr int kWpOff = kW11Off + kW11Bytes;
+constexpr int kParamOff = kWpOff + kWpBytes;                        // scale11, shift11, prob
+constexpr int kBarOff = kParamOff + 4 * 8 * 4;
+// barriers: in_full[4] @0, in_empty[4] @32, u_full[4] @64, u_empty[4] @96, w11 @128, wp @136
+constexpr int kTotal = kBarOff + 192 + 1024;                        // + alignment slack
+static_assert(IN_SLOTS <= 4 && U_SLOTS <= 4, "barrier slots");
+static_assert(kInBytes % 128 == 0 && kSliceBytes % 128 == 0, "128-byte aligned slots");
+
+// two CTAs per SM (registers <= 112, 2 x 105 KB of shared memory)
+__global__ void __launch_bounds__(kConvThreads, 2)
+conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
+                   const __grid_constant__ CUtensorMap c0map, const Params p) {
+  extern __shared__ unsigned char smem_raw[];
+  const uint32_t s_raw = smem_u32(smem_raw);
+  const uint32_t s_base = (s_raw + 1023u) & ~1023u;
+  unsigned char* smem = smem_raw + (s_base - s_raw);
+  const uint32_t s_in = s_base + kInOff, s_u = s_base + kUOff, s_w11 = s_base + kW11Off,
+                 s_wp = s_base + kWpOff, s_bar = s_base + kBarOff;
+  float* s_param = reinterpret_cast<float*>(smem + kParamOff);
+  const uint32_t in_full = s_bar, in_empty = s_bar + 32, u_full = s_bar + 64,
+                 u_empty = s_bar + 96, bar_w11 = s_bar + 128, bar_wp = s_bar + 136;
+  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const int total_items = p.B * p.nchunks * p.tiles_h * p.tiles_w;
+
+  // ---- one-time setup ----
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < IN_SLOTS; ++i) {
+      mbar_init(in_full + 8 * i, 1);
+      mbar_init(in_empty + 8 * i, 128);
+    }
+    for (int i = 0; i < U_SLOTS; ++i) {
+      mbar_init(u_full + 8 * i, 128);
+      mbar_init(u_empty + 8 * i, 128);
+    }
+    mbar_init(bar_w11, 1);
+    mbar_init(bar_wp, 1);
+    fence_barrier_init();
+  }
+  if (threadIdx.x < 8) {
+    const int i = threadIdx.x;
+    s_param[i] = __ldg(p.scale11 + i);
+    s_param[8 + i] = __ldg(p.shift11 + i);
+    s_param[16 + i] = i < 1 ? __ldg(p.scalep) : 0.f;           // prob: Cout = 1 of GW = 8
+    s_param[24 + i] = i < 1 ? __ldg(p.shiftp) : 0.f;
+  }
+  // The TMA loads never write the tail of a u9 brick (voxels 66 .. 71), but the shifted views of
+  // GEMM rows 59 .. 63 read it, times the zero weight rows of the classes a tap does not reach:
+  // it must hold finite values, or 0 x NaN would reach u11 voxels of the region.
+  for (int i = threadIdx.x; i < IN_SLOTS * 4 * (kU9Bytes - kU9Data) / 16; i += kConvThreads) {
+    const int per = (kU9Bytes - kU9Data) / 16, brick = i / per;
+    *reinterpret_cast<float4*>(smem + kInOff + (brick / 4) * kInBytes + (brick % 4) * kU9Bytes +
+                               kU9Data + (i % per) * 16) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  fence_proxy_async();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    tma::load_image_bulk(s_w11, p.img11, kW11Bytes, bar_w11);
+    tma::load_image_bulk(s_wp, p.imgp, kWpBytes, bar_wp);
+  }
+
+  // nothing above depends on the previous kernel of the stream (see tma_common.cuh)
+  tma::pdl_trigger();
+  tma::pdl_wait();
+  bool w_ready = false;                             // consumers: weight image has landed
+  uint32_t gin = 0, gu = 0;                         // steps / u11 slices before this item
+  const int wl = warp & 3;
+  for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x) {
+    int item = item0;
+    const int tw = item % p.tiles_w; item /= p.tiles_w;
+    const int th = item % p.tiles_h; item /= p.tiles_h;
+    const int ck = item % p.nchunks;
+    const int b = item / p.nchunks;
+    const int w0 = tw * kTileW, h0 = th * kTileH;
+    const int d0 = ck * p.dchunk, d1 = min(p.D, d0 + p.dchunk);
+    const int nd = d1 - d0;                         // even
+    const int nsteps = nd / 2 + 2;                  // u9 slices d0/2-1 .. d1/2
+    const int s0 = d0 / 2 - 1;
+
+    if (warp == kProdWarp) {
+      // ============ producer: 4 u9 loads per step, + 2 x 2 c0 loads after the first ============
+      if (lane == 0) {
+        for (int st = 0; st < nsteps; ++st) {
+          const uint32_t g = gin + st;
+          const int slot = g % IN_SLOTS;
+          if (g >= (uint32_t)IN_SLOTS) mbar_wait(in_empty + 8 * slot, ((g / IN_SLOTS) - 1) & 1);
+          const uint32_t dst = s_in + slot * kInBytes;
+          mbar_expect_tx(in_full + 8 * slot, 4 * kU9Data + (st > 0 ? 4 * kBrickData : 0));
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const tma::Coords5 k =
+                tma::brick_coords(true, 1, 4, q, w0 / 2 - 1, h0 / 2 - 1, s0 + st, b);
+            tma_load_5d(dst + q * kU9Bytes, &u9map, in_full + 8 * slot, k.c[0], k.c[1], k.c[2],
+                        k.c[3], k.c[4]);
+          }
+          if (st > 0) {                             // the first step's u11 slices are not used
+#pragma unroll
+            for (int k2 = 0; k2 < 2; ++k2) {
+#pragma unroll
+              for (int q = 0; q < 2; ++q) {
+                const tma::Coords5 k = tma::brick_coords(true, 1, 2, q, w0 - 1, h0 - 1,
+                                                         2 * (s0 + st) - 1 + k2, b);
+                tma_load_5d(dst + 4 * kU9Bytes + k2 * kSliceBytes + q * kBrickBytes, &c0map,
+                            in_full + 8 * slot, k.c[0], k.c[1], k.c[2], k.c[3], k.c[4]);
+              }
+            }
+          }
+        }
+      }
+      __syncwarp();
+    } else if (warp < 4) {
+      // ===================== warpgroup 0: conv11 into the u11 ring =====================
+      constexpr uint32_t a_lbo = kU9Bytes, a_sbo = 128;          // next quad; next 8 voxels
+      constexpr uint32_t b_lbo = 96 * 16, b_sbo = 128;
+      const uint64_t a_desc0 = make_desc(s_in, a_lbo, a_sbo);
+      const uint64_t b_desc0 = make_desc(s_w11, b_lbo, b_sbo);
+      // [kd=0 block of group s-1 | kd=1 block of group s | kd=2 block of group s], as in
+      // conv3d_tma2's MODE_T (each block: 4 classes x 8 channels)
+      float acc[48];
+#pragma unroll
+      for (int i = 0; i < 48; ++i) acc[i] = 0.f;
+      // This thread's 8 column pairs of a block (for_each_pair order: class j, row half h)
+      // hold channels c, c + 1 of u9 voxel m = 16 wl + lane/4 + 8h, class (ph, pw) = j: output
+      // voxel (2 jr + ph - 1, 2 jc + pw - 1) of the 18 x 10 region, jr, jc = m / 6, m % 6.
+      // Same slots in both blocks and every step: offsets in a brick and which are in the region
+      // are fixed; which are inside the volume is fixed per item.
+      const int c = 2 * (lane & 3);
+      const float sc0 = s_param[c], sc1 = s_param[c + 1];
+      const float sh0 = s_param[8 + c], sh1 = s_param[8 + c + 1];
+      uint32_t off[8];
+      uint32_t rmask = 0, vmask = 0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int j = i >> 1, m = 16 * wl + (lane >> 2) + 8 * (i & 1);
+        const int jr = m / kU9W, jc = m - kU9W * jr;
+        const int hh = 2 * jr + (j >> 1) - 1, ww = 2 * jc + (j & 1) - 1;
+        const int oh = h0 - 1 + hh, ow = w0 - 1 + ww;
+        const bool in = hh >= 0 && hh < kHaloH && ww >= 0 && ww < kHaloW;
+        rmask |= (in ? 1u : 0u) << i;
+        vmask |= (in && oh >= 0 && oh < p.H && ow >= 0 && ow < p.W ? 1u : 0u) << i;
+        off[i] = in ? (c >> 2) * kBrickBytes + (hh * kHaloW + ww) * 16 + (c & 3) * 4 : 0;
+      }
+      for (int st = 0; st < nsteps; ++st) {
+        const uint32_t g = gin + st;
+        const int slot = g % IN_SLOTS;
+        mbar_wait(in_full + 8 * slot, (g / IN_SLOTS) & 1);
+        if (!w_ready) { mbar_wait(bar_w11, 0); w_ready = true; }
+        const uint64_t a_s = a_desc0 + ((slot * kInBytes) >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 4; ++tap) {
+          const int sh = tap >> 1, sw = tap & 1;
+#pragma unroll
+          for (int k8 = 0; k8 < 2; ++k8) {
+            const uint32_t a_off = (2 * k8 * kU9Bytes + (sh * kU9W + sw) * 16) >> 4;
+            const uint32_t b_off = (tap * (16 * 96 * 4) + k8 * 2 * 96 * 16) >> 4;
+            wgmma_tf32<96>(acc, a_s + a_off, b_desc0 + b_off);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        // blocks 0 and 1 are complete: u11 slices 2s-1 (pd = 1) and 2s (pd = 0).  Copied out
+        // before the per-thread stores (no accumulator register on a divergent path).
+        float done[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) done[i] = acc[i];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          acc[i] = acc[32 + i];
+          acc[16 + i] = 0.f;
+          acc[32 + i] = 0.f;
+        }
+        if (st > 0) {
+          const unsigned char* c0s = smem + (s_in - s_base) + slot * kInBytes + 4 * kU9Bytes;
+          const uint32_t u0 = gu + 2 * (st - 1);
+#pragma unroll
+          for (int k2 = 0; k2 < 2; ++k2) {
+            const uint32_t u = u0 + k2;
+            const int us = u % U_SLOTS;
+            if (u >= (uint32_t)U_SLOTS) mbar_wait(u_empty + 8 * us, ((u / U_SLOTS) - 1) & 1);
+            const int od = 2 * (s0 + st) - 1 + k2;
+            // zero outside the volume (prob's zero padding)
+            const uint32_t live = od >= 0 && od < p.D ? vmask : 0u;
+            const unsigned char* skip = c0s + k2 * kSliceBytes;
+            unsigned char* dst = smem + (s_u - s_base) + us * kSliceBytes;
+            float2 s2[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+              s2[i] = (live >> i) & 1 ? *reinterpret_cast<const float2*>(skip + off[i])
+                                      : make_float2(0.f, 0.f);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              // conv3d_tma2's store2, with the skip from the c0 brick
+              const float a0 = done[16 * k2 + 4 * (i >> 1) + 2 * (i & 1)];
+              const float a1 = done[16 * k2 + 4 * (i >> 1) + 2 * (i & 1) + 1];
+              float v0 = fmaf(a0, sc0, sh0);
+              float v1 = fmaf(a1, sc1, sh1);
+              v0 = v0 >= 0.f ? v0 : v0 * p.slope;
+              v1 = v1 >= 0.f ? v1 : v1 * p.slope;
+              v0 += s2[i].x; v1 += s2[i].y;
+              const float2 v = (live >> i) & 1 ? make_float2(to_tf32(v0), to_tf32(v1))
+                                                : make_float2(0.f, 0.f);
+              if ((rmask >> i) & 1) *reinterpret_cast<float2*>(dst + off[i]) = v;
+            }
+          }
+          fence_proxy_async();                      // generic-proxy writes -> prob's wgmma
+          mbar_arrive(u_full + 8 * (u0 % U_SLOTS));
+          mbar_arrive(u_full + 8 * ((u0 + 1) % U_SLOTS));
+        }
+        mbar_arrive(in_empty + 8 * slot);           // this thread's reads of the slot are done
+      }
+    } else {
+      // ============ warpgroup 1: prob, both 64-row halves of the tile, per u11 slice ============
+      constexpr uint32_t a_lbo = kBrickBytes, a_sbo = kHaloW * 16;
+      constexpr uint32_t b_lbo = 3 * 8 * 16, b_sbo = 128;
+      const uint64_t a_desc0 = make_desc(s_u, a_lbo, a_sbo);
+      const uint64_t b_desc0 = make_desc(s_wp, b_lbo, b_sbo);
+      // column groups 0, 1, 2 = output slices k-2, k-1, k of u11 slice d0-1+k (conv3d_tma.cu)
+      float acc0[12], acc1[12];
+#pragma unroll
+      for (int i = 0; i < 12; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+      auto store_logits = [&](const float* src, int half, int od) {
+        if ((lane & 3) != 0) return;                // column 0: the only output channel
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = 64 * half + 16 * wl + (lane >> 2) + 8 * h;
+          const int oh = h0 + (m >> 3), ow = w0 + (m & 7);
+          if (oh >= p.H || ow >= p.W) continue;
+          // conv3d_tma's store_slice with Cout = 1, slope 1 (identity) and fp32 output
+          p.logits[(((size_t)b * p.D + od) * p.H + oh) * p.W + ow] =
+              fmaf(src[2 * h], s_param[16], s_param[24]);
+        }
+      };
+      for (int k = 0; k < nd + 2; ++k) {
+        const uint32_t u = gu + k;
+        const int us = u % U_SLOTS;
+        mbar_wait(u_full + 8 * us, (u / U_SLOTS) & 1);
+        if (!w_ready) { mbar_wait(bar_wp, 0); w_ready = true; }
+        const uint64_t a_s = a_desc0 + ((us * kSliceBytes) >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int khw = 0; khw < 9; ++khw) {
+          const int kh = khw / 3, kw = khw % 3;
+          const uint32_t a_off = ((kh * kHaloW + kw) * 16) >> 4;
+          const uint32_t b_off = (khw * (8 * 3 * 8 * 4)) >> 4;
+          wgmma_tf32<24>(acc0, a_s + a_off, b_desc0 + b_off);
+          wgmma_tf32<24>(acc1, a_s + a_off + ((8 * a_sbo) >> 4), b_desc0 + b_off);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        mbar_arrive(u_empty + 8 * us);
+        float done0[4], done1[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { done0[i] = acc0[i]; done1[i] = acc1[i]; }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { acc0[i] = acc0[i + 4]; acc1[i] = acc1[i + 4]; }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { acc0[8 + i] = 0.f; acc1[8 + i] = 0.f; }
+        if (k >= 2) {
+          store_logits(done0, 0, d0 + k - 2);
+          store_logits(done1, 1, d0 + k - 2);
+        }
+      }
+    }
+    gin += nsteps;
+    gu += nd + 2;
+  }
+}
+
+static int launch_tail(const TailArgs& a, cudaStream_t st) {
+  static_assert(kTotal <= 227 * 1024, "shared memory budget");
+  auto kfn = conv3d_tail_kernel;
+  static std::atomic<bool> attr_set[kMaxDevices];
+  if (int rc = opt_in_smem(kfn, kTotal, attr_set, "conv3d_tail")) return rc;
+  Params p;
+  p.scale11 = a.scale11; p.shift11 = a.shift11; p.scalep = a.scalep; p.shiftp = a.shiftp;
+  p.logits = a.logits; p.slope = a.slope;
+  p.B = a.B; p.D = a.D; p.H = a.h; p.W = a.w;
+  p.tiles_w = (a.w + kTileW - 1) / kTileW;
+  p.tiles_h = (a.h + kTileH - 1) / kTileH;
+  // input_map returns a per-thread copy that the next call overwrites
+  const CUtensorMap* m9 = tma::input_map(a.u9, a.B, a.D / 2, a.h / 2, a.w / 2, 16, 4, kU9W, kU9H,
+                                         1, true);
+  if (!m9) return -2;
+  const CUtensorMap u9map = *m9;
+  const CUtensorMap* m0 = tma::input_map(a.c0, a.B, a.D, a.h, a.w, 8, 4, kHaloW, kHaloH, 1, true);
+  if (!m0) return -2;
+  const CUtensorMap c0map = *m0;
+  ImageRef i11, ip;
+  if (int rc = conv3d_tma2_conv11_image(a.w11, st, &i11)) return rc;
+  if (int rc = conv3d_tma_prob_image(a.wp, st, &ip)) return rc;
+  p.img11 = i11.img; p.imgp = ip.img;
+  const int per_sm = tma::resident_per_sm(kfn, kConvThreads, kTotal);
+  const long resident = (long)num_sms() * per_sm;
+  const long cols = (long)p.B * p.tiles_w * p.tiles_h;
+  // an item of 2 dc u9 slices walks 2 dc + 2 u11 slices (the prob halo) and dc + 2 u9 slices
+  p.dchunk = 2 * tma::pick_dchunk(p.D / 2, 16, cols, resident, 2, 3);
+  p.nchunks = (p.D + p.dchunk - 1) / p.dchunk;
+  const long items = cols * p.nchunks;
+  const long gx = items < resident ? items : resident;
+  tma::launch_pdl(i11.settled && ip.settled, kfn, dim3((unsigned)gx), kConvThreads, kTotal, st,
+                  u9map, c0map, p);
+  return after_launch("conv3d_tail");
+}
+
+// Coverage: (u9 channels, skip channels, output channels) -- CostRegNet's conv11 + prob for
+// every input width, since neither depends on the stage's Cin.
+struct Shape {
+  int cin, cskip, cout;
+  TailLauncher run;
+};
+static const Shape kShapes[] = {{16, 8, 1, launch_tail}};
+
+}  // namespace tail
+
+TailLauncher conv3d_tail_find(int cin, int cskip, int cout) {
+  for (const tail::Shape& s : tail::kShapes)
+    if (s.cin == cin && s.cskip == cskip && s.cout == cout) return s.run;
+  return nullptr;
+}
+
+}  // namespace casmvs

@@ -360,6 +360,21 @@ const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, 
 }
 
 
+// The B operand image of a layer (nco chunks of GW columns, `cout` of them used), from the
+// per-process cache or built on `st` on a miss.
+template <int CIN, int GW>
+static int stride1_image(const float* wpk, int cout, int cout_total, int nco, cudaStream_t st,
+                         ImageRef* ir) {
+  constexpr int kWBytes = Smem<CIN, GW, 1>::kWBytes;
+  *ir = image_cache_get(wpk, 1000 + CIN * 100 + GW, (size_t)kWBytes * nco, st);
+  if (!ir->img) return -2;
+  if (!ir->hit) {
+    if (int rc = build_stride1_image(wpk, ir->img, CIN, GW, cout, cout_total, st)) return rc;
+    image_cache_built(ir->img, st);
+  }
+  return 0;
+}
+
 // One CTA computes GW output columns (Cout <= GW, or a GW-channel slice of a wider Cout).
 template <int CIN, int GW, int SLOTS, bool PLANAR>
 static int launch(const ConvArgs& a, cudaStream_t st) {
@@ -389,12 +404,8 @@ static int launch(const ConvArgs& a, cudaStream_t st) {
   if (dchunk_env > 0 && dchunk_env <= cap) dchunk = dchunk_env < p.D ? dchunk_env : p.D;
   p.dchunk = dchunk;
   p.nchunks = (p.D + dchunk - 1) / dchunk;
-  const ImageRef ir = image_cache_get(a.wpk, 1000 + CIN * 100 + GW, (size_t)S::kWBytes * nco, st);
-  if (!ir.img) return -2;
-  if (!ir.hit) {
-    if (int rc = build_stride1_image(a.wpk, ir.img, CIN, GW, p.Cout, p.cout_total, st)) return rc;
-    image_cache_built(ir.img, st);
-  }
+  ImageRef ir;
+  if (int rc = stride1_image<CIN, GW>(a.wpk, p.Cout, p.cout_total, nco, st, &ir)) return rc;
   p.bimg = ir.img;
   const long items = (long)p.B * p.nchunks * p.tiles_h * p.tiles_w;
   int resident = num_sms() * per_sm / nco;
@@ -427,6 +438,10 @@ ConvLauncher conv3d_tma_find(int Cin, int Cout, int kind, int stride) {
     if (s.cin == Cin && s.cout_lo <= Cout && Cout <= s.cout_hi)
       return kind == CASMVS_CONV_PLANAR ? s.planar : s.conv;
   return nullptr;
+}
+
+int conv3d_tma_prob_image(const float* wpk, cudaStream_t st, tc::ImageRef* ir) {
+  return tma::stride1_image<8, 8>(wpk, 1, 1, 1, st, ir);
 }
 
 }  // namespace casmvs

@@ -429,6 +429,25 @@ __global__ void build_image_p5_kernel(const float* __restrict__ wt, float* __res
   }
 }
 
+// The B operand image of a layer (all its COUT-channel chunks), from the per-process cache or
+// built on `st` on a miss.
+template <int MODE, int CIN, int COUT>
+static int tma2_image(const float* wpk, int cout_total, cudaStream_t st, ImageRef* ir) {
+  using C = Cfg<MODE, CIN, COUT>;
+  *ir = image_cache_get(wpk, 2000 + MODE * 10000 + CIN * 100 + COUT,
+                        (size_t)C::kWBytes * (cout_total / COUT), st);
+  if (!ir->img) return -2;
+  if (!ir->hit) {
+    if constexpr (MODE == MODE_P5)
+      build_image_p5_kernel<CIN, COUT><<<32, 256, 0, st>>>(wpk, ir->img);
+    else
+      build_image_tma2_kernel<MODE, CIN, COUT><<<64, 256, 0, st>>>(wpk, ir->img, cout_total);
+    if (int rc = after_launch("conv3d_tma2/build_image")) return rc;
+    image_cache_built(ir->img, st);
+  }
+  return 0;
+}
+
 // MODE_S2 / MODE_P5: output = (in - 1) / 2 + 1 along H and W (and D for MODE_S2); MODE_T:
 // output = 2x input.  A CTA computes a COUT-channel slice of a.Cout.
 template <int MODE, int CIN, int COUT>
@@ -470,19 +489,9 @@ static int launch2(const ConvArgs& a, cudaStream_t st) {
   p.dchunk = dchunk;
   p.nchunks = (Dm + dchunk - 1) / dchunk;
   const long items = cols * p.nchunks;
-  const ImageRef ir = image_cache_get(a.wpk, 2000 + MODE * 10000 + CIN * 100 + COUT,
-                                      (size_t)C::kWBytes * nco, st);
-  float* img = ir.img;
-  if (!img) return -2;
-  if (!ir.hit) {
-    if constexpr (MODE == MODE_P5)
-      build_image_p5_kernel<CIN, COUT><<<32, 256, 0, st>>>(a.wpk, img);
-    else
-      build_image_tma2_kernel<MODE, CIN, COUT><<<64, 256, 0, st>>>(a.wpk, img, p.Cout);
-    if (int rc = after_launch("conv3d_tma2/build_image")) return rc;
-    image_cache_built(img, st);
-  }
-  p.bimg = img;
+  ImageRef ir;
+  if (int rc = tma2_image<MODE, CIN, COUT>(a.wpk, p.Cout, st, &ir)) return rc;
+  p.bimg = ir.img;
   long resident = (long)num_sms() * per_sm / nco;
   if (resident < 1) resident = 1;
   const long gx = items < resident ? items : resident;
@@ -513,6 +522,10 @@ ConvLauncher conv3d_tma2_find(int Cin, int Cout, int kind, int stride, bool skip
   for (const tma2::Shape& s : tma2::kShapes)
     if (s.kind == kind && s.cin == Cin && s.cout == Cout && (s.skip || !skip)) return s.run;
   return nullptr;
+}
+
+int conv3d_tma2_conv11_image(const float* wpk, cudaStream_t st, tc::ImageRef* ir) {
+  return tma2::tma2_image<tma2::MODE_T, 16, 8>(wpk, 8, st, ir);
 }
 
 }  // namespace casmvs

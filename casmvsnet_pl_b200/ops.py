@@ -13,7 +13,7 @@ import math
 import torch
 
 from . import _lib
-from ._lib import (BLOCKED, CONV, CONV_PLANAR, CONV_TRANSPOSE, FP32, KEEP_FP32_OUT, NCHW, NHWC, PRECISIONS, TF32,  # noqa: F401
+from ._lib import (BLOCKED, CONV, CONV_PLANAR, CONV_TRANSPOSE, FP32, FUSED_TAIL, KEEP_FP32_OUT, NCHW, NHWC, PRECISIONS, TF32,  # noqa: F401
                    check)
 
 _checked_devices = set()
@@ -235,10 +235,12 @@ def costreg_blocked_supported(cin, precision=TF32):
 
 
 @_on_tensor_device
-def costreg(x, params, cin, precision=FP32, blocked=False):
+def costreg(x, params, cin, precision=FP32, blocked=False, fused_tail=True):
     """Whole CostRegNet.  x logical (B,Cin,D,h,w) -> logits (B,D,h,w).  blocked=True (TF32
     only, where costreg_blocked_supported): x is a contiguous (B,Cin/4,D,h,w,4) tensor, e.g. from
-    warp_cost_ladder(blocked=True)."""
+    warp_cost_ladder(blocked=True).  The workspace is private, so by default conv11 and the prob
+    head run as one kernel where the library has it (casmvs_costreg_tail_supported);
+    fused_tail=False runs them as two layers (the same logits)."""
     _require_cuda(x, params)
     _no_grad_only(x)
     if blocked:
@@ -252,6 +254,8 @@ def costreg(x, params, cin, precision=FP32, blocked=False):
         xs = volume_storage(x)
         B, D, h, w, c = xs.shape
         assert c == cin
+    if fused_tail:
+        precision |= FUSED_TAIL
     lib = _lib.load()
     ws_bytes = lib.casmvs_costreg_workspace_bytes(B, cin, D, h, w)
     ws = torch.empty(ws_bytes // 4, device=x.device, dtype=torch.float32)

@@ -64,6 +64,12 @@ enum casmvs_precision {
  * OR-ed into casmvs_warp_cost_ladder_fwd's round_tf32: write the cost volume blocked. */
 #define CASMVS_BLOCKED 512
 
+/* OR-ed into casmvs_costreg_fwd's precision: the caller does not read the workspace after the
+ * call.  Where casmvs_costreg_tail_supported, conv11 and the prob head then run as one kernel
+ * that computes the logits from u9 and c0 (the same logits, bit for bit), and u11 is never
+ * stored.  Without it every activation c0 .. u11 is left in the workspace. */
+#define CASMVS_FUSED_TAIL 1024
+
 enum casmvs_conv_kind {
   CASMVS_CONV = 0,           /* Conv3d(k=3, pad=1, stride 1|2)   modules.py:26      */
   CASMVS_CONV_TRANSPOSE = 1, /* ConvTranspose3d(k=3,s=2,p=1,op=1) mvsnet.py:75,80,85 */
@@ -184,6 +190,16 @@ int casmvs_costreg_blocked_supported(int Cin, int precision);
 int casmvs_costreg_fwd(const float* x, const float* params, float* logits,
                        int B, int Cin, int D, int h, int w, int precision,
                        void* workspace, size_t workspace_bytes, void* stream);
+/* 1 when casmvs_costreg_fwd with CASMVS_FUSED_TAIL runs conv11 + prob as one kernel: where
+ * casmvs_costreg_blocked_supported (the kernel reads and writes blocked activations). */
+int casmvs_costreg_tail_supported(int Cin, int precision);
+/* One step of casmvs_costreg_fwd, with its arguments (CASMVS_FUSED_TAIL ignored), for timing the
+ * layers one at a time: layer 0 .. 10 runs that layer on the activations a full call leaves in
+ * the workspace; layer 11 runs the fused conv11 + prob kernel (u9, c0 -> logits), where
+ * casmvs_costreg_tail_supported. */
+int casmvs_costreg_layer_fwd(const float* x, const float* params, float* logits,
+                             int B, int Cin, int D, int h, int w, int precision,
+                             void* workspace, size_t workspace_bytes, int layer, void* stream);
 
 /* ---- K3: softmax over D + depth regression + index + confidence --------
  * Replaces F.softmax + depth_regression (models/mvsnet.py:174-177,
