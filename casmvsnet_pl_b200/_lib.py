@@ -26,6 +26,7 @@ SIGNATURES = {
     "casmvs_device_check": (c_int, [c_int]),
     "casmvs_launch_count": (c_uint64, []),
     "casmvs_fallback_count": (c_uint64, []),
+    "casmvs_conv3d_tensor_core": (c_int, [c_int] * 5),
     "casmvs_release_weight_images": (c_int, [c_void_p, c_size_t]),
     "casmvs_weight_cache_generation": (c_uint64, []),
     "casmvs_weight_image_count": (c_int, [c_void_p, c_size_t]),

@@ -25,7 +25,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib, ops
-from .ops import CONV, CONV_TRANSPOSE, FP32, NCHW, NHWC, _ptr, _stream, check
+from .ops import CONV, CONV_TRANSPOSE, FP32, NCHW, NHWC, TF32, _ptr, _stream, check
 
 
 def deterministic():
@@ -74,13 +74,32 @@ class WarpCostFn(torch.autograd.Function):
         return gf.permute(0, 1, 4, 2, 3), None, None, None
 
 
+def _tf32_operand(x, cin, cout, kind, stride, precision):
+    """The activation operand as the layer's kernel should read it.  A tensor-core kernel reads
+    only the top 19 bits of an fp32 value, which biases every product toward zero by about
+    2^-11 of its size.  The inference path stores its activations TF32-rounded for that reason;
+    here the torch norm-act output, the cost volume and the gradients are full fp32.  So where a
+    tensor-core kernel runs, x is RNA-rounded into a new buffer (x itself may be the previous
+    layer's activation, or a gradient autograd also sends to a skip branch).  A TF32-exact value
+    is unchanged.  The CUDA-core fallback multiplies fp32 operands exactly and reads x as is."""
+    if (precision & 0xff) != TF32 or not ops.conv3d_tensor_core(cin, cout, kind, stride):
+        return x
+    r = _dense_ndhwc(x).clone()
+    B, D, h, w, C = r.shape
+    ops.bias_lrelu_(r.view(B * D, h, w, C).permute(0, 3, 1, 2), torch.zeros(C, device=r.device),
+                    1.0, round_tf32=True)
+    return ops.as_volume_view(r)
+
+
 def _raw_conv(x, weight_torch, kind, stride, precision):
+    """-> (y, the operand the kernel read: x, or x rounded to TF32 by _tf32_operand)."""
     cin, cout = (weight_torch.shape[1], weight_torch.shape[0]) if kind == CONV else \
         (weight_torch.shape[0], weight_torch.shape[1])
+    x = _tf32_operand(x, cin, cout, kind, stride, precision)
     wp = ops.pack_conv3d_weight(weight_torch, kind)
     y = ops.conv3d(x, wp, cin, cout, None, None, 1.0, None, kind, stride, precision)
     ops.release_weight_images(wp)          # one-shot weights: do not let operand images pile up
-    return y
+    return y, x
 
 
 class Conv3dFn(torch.autograd.Function):
@@ -88,8 +107,9 @@ class Conv3dFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, kind, stride, precision):
-        xd, wd = x.detach(), weight.detach()
-        y = _raw_conv(xd, wd, kind, stride, precision)
+        wd = weight.detach()
+        # the weight gradient takes the operand the kernel read: the function it computed
+        y, xd = _raw_conv(x.detach(), wd, kind, stride, precision)
         ctx.save_for_backward(xd, wd)
         ctx.cfg = (kind, stride, precision)
         return y
@@ -113,14 +133,14 @@ class Conv3dFn(torch.autograd.Function):
                     pad = 4 - cout % 4
                     g_in = ops.as_volume_view(torch.nn.functional.pad(gyd, (0, pad)))
                     wt = torch.nn.functional.pad(wt, (0, 0, 0, 0, 0, 0, 0, pad))
-                gx = _raw_conv(g_in, wt, CONV, 1, precision)
+                gx, _ = _raw_conv(g_in, wt, CONV, 1, precision)
             elif kind == CONV:
                 # conv(k3,s2,p1) on even dims: its adjoint is ConvTranspose3d(k3,s2,p1,op1) with
                 # the SAME weight tensor read as (in = Cout, out = Cin)
-                gx = _raw_conv(gy_l, w, CONV_TRANSPOSE, 2, precision)
+                gx, _ = _raw_conv(gy_l, w, CONV_TRANSPOSE, 2, precision)
             else:
                 # adjoint of the transposed conv: Conv3d(k3,s2,p1), weight read as (out=Cin, in=Cout)
-                gx = _raw_conv(gy_l, w, CONV, 2, precision)
+                gx, _ = _raw_conv(gy_l, w, CONV, 2, precision)
         if ctx.needs_input_grad[1]:
             with torch.cuda.device(x.device):
                 if kind == CONV:

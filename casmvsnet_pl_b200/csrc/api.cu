@@ -59,6 +59,10 @@ extern "C" uint64_t casmvs_launch_count(void) { return g_launches.load(); }
 
 extern "C" uint64_t casmvs_fallback_count(void) { return g_fallbacks.load(); }
 
+extern "C" int casmvs_conv3d_tensor_core(int Cin, int Cout, int kind, int stride, int has_skip) {
+  return tensor_core_launcher(Cin, Cout, kind, stride, has_skip != 0) ? 1 : 0;
+}
+
 extern "C" int casmvs_device_check(int device) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);

@@ -218,6 +218,12 @@ def conv3d(x, w_packed, cin, cout, scale=None, shift=None, slope=1.0, skip=None,
     return as_volume_view(y)
 
 
+def conv3d_tensor_core(cin, cout, kind, stride, skip=False):
+    """True when conv3d in the TF32 precision runs this layer on a tensor-core kernel, False
+    when it falls back to the CUDA cores (casmvs_fallback_count)."""
+    return bool(_lib.load().casmvs_conv3d_tensor_core(cin, cout, kind, stride, int(skip)))
+
+
 def costreg_layer_info(cin, layer):
     lib = _lib.load()
     ci, co, kind, stride = (ctypes.c_int() for _ in range(4))

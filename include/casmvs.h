@@ -93,6 +93,11 @@ uint64_t casmvs_launch_count(void);
  * reference architecture at every BASELINE configuration; bench.py and the full-size tests
  * assert that. */
 uint64_t casmvs_fallback_count(void);
+/* 1 when a CASMVS_TF32 casmvs_conv3d_fwd of this layer runs on a tensor-core kernel, 0 when it
+ * falls back to the CUDA cores.  A tensor-core kernel reads only the top 19 bits of each fp32
+ * activation (it truncates), so a caller whose activations are not TF32-rounded rounds them
+ * first where this is 1.  Host-only: no device is touched. */
+int casmvs_conv3d_tensor_core(int Cin, int Cout, int kind, int stride, int has_skip);
 
 /* ---- K1: fused homography warp + bilinear sample + cost reduction ------
  * Replaces homo_warp (models/modules.py:52-92) called V-1 times plus the

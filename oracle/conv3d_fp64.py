@@ -106,6 +106,36 @@ def conv3d_ref(x, w, kind, stride=1):
     return y
 
 
+def dgrad_ref(gy, w, kind, stride, in_dims):
+    """Float64 data gradient of the raw layer: the vector-Jacobian product of conv3d_ref with
+    packed w at an input of dims in_dims = (D, h, w), applied to gy (B, Do, ho, wo, Cout), by
+    torch.autograd in float64 -> (B, D, h, w, Cin).  No flipped, transposed or padded weight is
+    built by hand, so a mistake in such a construction elsewhere cannot cancel here.  The map
+    is linear, so dgrad_ref(|gy|, |w|) is the magnitude of the per-element bound."""
+    gy = gy.to(torch.float64)
+    w = w.to(device=gy.device, dtype=torch.float64)
+    x = gy.new_zeros(gy.shape[0], *in_dims, w.shape[-2], requires_grad=True)
+    with torch.enable_grad():
+        y = conv3d_ref(x, w, kind, stride)
+        assert y.shape == gy.shape, (y.shape, gy.shape)
+        (gx,) = torch.autograd.grad(y, x, gy)
+    return gx
+
+
+def operand_bias(y, y64):
+    """sum (y - y64) sign(y64) / sum |y64|: the mean relative error of y in the direction of
+    y64.  About 0 where the operands were rounded to nearest; about -2^-11 (toward zero) where
+    the low 13 mantissa bits of a non-TF32 operand were dropped."""
+    y = y.to(device=y64.device, dtype=torch.float64)
+    return float(((y - y64) * torch.sign(y64)).sum() / y64.abs().sum().clamp_min(TINY))
+
+
+def tf32_trunc(t):
+    """A float32 tensor with its low 13 mantissa bits cleared (round toward zero to TF32)."""
+    assert t.dtype == torch.float32
+    return (t.contiguous().view(torch.int32) & ~0x1FFF).view(torch.float32)
+
+
 def epilogue(acc, scale=None, shift=None, slope=1.0, skip=None):
     """lrelu(scale * acc + shift, slope) + skip, float64, per output channel (last dim)."""
     v = acc

@@ -53,6 +53,24 @@ def test_host_side_queries_without_gpu():
     assert up["kind"] == _lib.CONV_TRANSPOSE and (up["cin"], up["cout"]) == (64, 32)
 
 
+def test_tensor_core_coverage_query_without_gpu():
+    """ops.conv3d_tensor_core: every CostRegNet forward layer and the training adjoints that have
+    a wgmma kernel say True; the adjoints that fall back (prob: 4 -> 8 after padding, the middle
+    level's conv0: 8 -> 16), stride 2 with a skip, and Cin % 8 != 0 say False."""
+    from casmvsnet_pl_b200 import ops
+    C, T = ops.CONV, ops.CONV_TRANSPOSE
+    for cin in (8, 16, 32):
+        assert ops.conv3d_tensor_core(cin, 8, C, 1)
+    for args in ((8, 16, C, 2), (16, 16, C, 1), (16, 32, C, 2), (32, 32, C, 1), (32, 64, C, 2),
+                 (64, 64, C, 1), (64, 32, T, 2), (32, 16, T, 2), (16, 8, T, 2), (8, 1, C, 1),
+                 (16, 8, C, 1), (32, 16, C, 1), (8, 32, C, 1)):
+        assert ops.conv3d_tensor_core(*args), args
+    for args in ((4, 8, C, 1), (8, 16, C, 1), (12, 8, C, 1), (16, 8, C, 2)):
+        assert not ops.conv3d_tensor_core(*args), args
+    assert not ops.conv3d_tensor_core(8, 16, C, 2, skip=True)
+    assert ops.conv3d_tensor_core(64, 32, T, 2, skip=True)
+
+
 def test_errors_are_reported_not_thrown():
     """bad arguments -> negative status + message (no GPU needed: validation is first)."""
     from casmvsnet_pl_b200 import _lib

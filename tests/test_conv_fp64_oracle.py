@@ -8,6 +8,7 @@ import torch.nn.functional as F
 
 from oracle import conv3d_fp64 as R
 import test_gpu_conv_fp64 as G
+import test_gpu_train_step_fp64 as T
 
 torch.set_default_dtype(torch.float32)
 
@@ -221,3 +222,167 @@ def test_flags_cout_chunk_scale_shift_swapped(kind, stride, cin):
     ok, _ = R.bound_excess(bad.float(), y64, A, G.EPS_CEIL_FP32, 0.0,
                            R.epilogue_magnitude(y64, shift))
     assert not ok
+
+
+# ------------------------------------------------------------------------------- data gradient
+DGRAD_SHAPES = [   # kind, stride, cin, cout of the forward layer, input dims
+    (R.CONV, 1, 8, 12, (4, 6, 8)), (R.CONV, 1, 8, 1, (3, 5, 7)), (R.CONV, 1, 4, 4, (1, 2, 3)),
+    (R.CONV, 2, 8, 12, (4, 6, 8)), (R.CONV, 2, 4, 8, (5, 7, 9)), (R.CONV, 2, 4, 1, (2, 3, 4)),
+    (R.CONV_TRANSPOSE, 2, 8, 4, (2, 3, 4)), (R.CONV_TRANSPOSE, 2, 4, 1, (3, 2, 5)),
+]
+
+
+def _torch_weight(g, kind, cin, cout, scale=1.0):
+    shape = (cout, cin, 3, 3, 3) if kind == R.CONV else (cin, cout, 3, 3, 3)
+    return torch.randn(*shape, generator=g, dtype=torch.float64) * scale
+
+
+@pytest.mark.parametrize("kind,stride,cin,cout,dims", DGRAD_SHAPES)
+def test_dgrad_ref_matches_torch_autograd(kind, stride, cin, cout, dims):
+    g = torch.Generator().manual_seed(kind * 100 + stride * 10 + cout + sum(dims))
+    x = torch.randn(2, cin, *dims, generator=g, dtype=torch.float64, requires_grad=True)
+    w = _torch_weight(g, kind, cin, cout)
+    y = F.conv3d(x, w, None, stride, 1) if kind == R.CONV else F.conv_transpose3d(x, w, None, 2, 1, 1)
+    gy = torch.randn(y.shape, generator=g, dtype=torch.float64)
+    (want,) = torch.autograd.grad(y, x, gy)
+    w64 = R.pack_weight(w, kind)
+    got = R.dgrad_ref(_cl(gy), w64, kind, stride, dims)
+    assert got.shape == _cl(want).shape
+    assert _rel(got, _cl(want)) < 1e-12
+    A = R.dgrad_ref(_cl(gy).abs(), w64.abs(), kind, stride, dims)
+    assert (got.abs() <= A * (1 + 1e-12)).all()
+
+
+def test_operand_bias_and_truncation():
+    g = torch.Generator().manual_seed(2)
+    y64 = torch.randn(4, 5, 6, 7, 8, generator=g, dtype=torch.float64)
+    assert R.operand_bias(y64, y64) == 0.0
+    assert abs(R.operand_bias(y64 * (1 - 2.0 ** -11), y64) + 2.0 ** -11) < 1e-15
+    x = torch.randn(100000, generator=g) * 1e3
+    t = R.tf32_trunc(x)
+    assert torch.equal(t.view(torch.int32) & 0x1FFF, torch.zeros_like(t, dtype=torch.int32))
+    assert (t.abs() <= x.abs()).all() and ((x.double() - t.double()).abs() < 2.0 ** -10 * x.double().abs()).all()
+    assert R.operand_bias(t, x.double()) < -2.0 ** -12                 # toward zero, ~0.73 * 2^-11
+    assert abs(R.operand_bias(R.tf32_rna(x), x.double())) < 2.0 ** -16  # to nearest: unbiased
+
+
+def _adjoint_fp32(gy, w, kind, stride, tf32, defect=None, slice_d=None):
+    """fp32 restatement of autograd.Conv3dFn's data gradient.  The adjoint layer is built from the
+    torch weight w the way Conv3dFn builds it (stride 1: flip the taps, swap the channels, pad a
+    Cout = 1 head to 4 zero channels; stride 2: the same weight read as the transposed layer, and
+    back), then applied to gy (B, Do, ho, wo, Cout) by conv3d_ref.  In tf32 both operands are
+    RNA-rounded and the output is stored TF32-rounded, as the tensor-core kernels do.  defect:
+    'unflipped', 'no_transpose', 'tap' (tap 4 of the adjoint dropped on output slice slice_d),
+    'pad_values' (the prob head's padding channels filled with copies instead of zeros), 'trunc'
+    (gy truncated to TF32 instead of rounded)."""
+    gy, w = gy.float(), w.float()
+    if tf32:
+        gy = R.tf32_trunc(gy) if defect == "trunc" else R.tf32_rna(gy)
+        w = R.tf32_rna(w)
+    if kind == R.CONV and stride == 1:
+        wt = w if defect == "unflipped" else w.flip(2, 3, 4)
+        if defect != "no_transpose":
+            wt = wt.transpose(0, 1)                                # (Cin, Cout, 3, 3, 3)
+        pad = -gy.shape[-1] % 4
+        if pad and defect == "pad_values":
+            gy = torch.cat([gy] + [gy[..., :1]] * pad, -1)
+            wt = torch.cat([wt] + [wt[:, :1]] * pad, 1)
+        elif pad:
+            gy = F.pad(gy, (0, pad))
+            wt = F.pad(wt, (0, 0, 0, 0, 0, 0, 0, pad))
+        wa, k, s = R.pack_weight(wt, R.CONV), R.CONV, 1
+    elif kind == R.CONV:
+        wa, k, s = R.pack_weight(w, R.CONV_TRANSPOSE), R.CONV_TRANSPOSE, 2
+    else:
+        wa, k, s = R.pack_weight(w, R.CONV), R.CONV, 2
+    out = R.conv3d_ref(gy, wa, k, s)
+    if defect == "tap":
+        wd = wa.clone()
+        wd[4] = 0                                  # (kd, kh, kw) = (0, 1, 1): reaches odd slices too
+        out[:, slice_d] = R.conv3d_ref(gy, wd, k, s)[:, slice_d]
+    out = out.float()
+    return R.tf32_rna(out) if tf32 else out
+
+
+def _dgrad_case(kind, stride, cin, cout, dims, seed):
+    """A layer's torch weight and an fp32 output gradient that is not TF32-exact (as the norm-act
+    backward produces it), with the float64 data gradient and its magnitude for both precisions."""
+    g = torch.Generator().manual_seed(seed)
+    w = _torch_weight(g, kind, cin, cout, (27 * cin) ** -0.5).float()
+    gy = torch.randn(2, *R.out_dims(kind, stride, *dims), cout, generator=g)
+    assert not T._is_tf32(gy)
+    ref = {}
+    for tf32 in (False, True):
+        w64 = R.pack_weight(R.tf32_rna(w) if tf32 else w, kind)
+        ref[tf32] = (R.dgrad_ref(gy, w64, kind, stride, dims),
+                     R.dgrad_ref(gy.abs(), w64.abs(), kind, stride, dims))
+    return w, gy, ref
+
+
+def _report(got, ref, kind, stride, tf32):
+    """T.conv_report of an adjoint restatement, as the GPU test runs it on a recorded call."""
+    want, A = ref[tf32]
+    kernel = ("tma" if kind == R.CONV and stride == 1 else "tma2") if tf32 else "direct"
+    return T.conv_report(got, want, A, kernel, R.R_TF32 if tf32 else 0.0,
+                         T.R_OP if tf32 else 0.0)
+
+
+@pytest.mark.parametrize("kind,stride,cin,cout,dims", [
+    (R.CONV, 1, 16, 8, (4, 12, 10)), (R.CONV, 1, 8, 1, (4, 12, 10)), (R.CONV, 2, 8, 16, (4, 12, 10)),
+    (R.CONV_TRANSPOSE, 2, 16, 8, (2, 6, 5))])
+def test_clean_adjoint_restatement_passes(kind, stride, cin, cout, dims):
+    w, gy, ref = _dgrad_case(kind, stride, cin, cout, dims, 21)
+    for tf32 in (False, True):
+        ok, bias_ok, worst, need, bias = _report(_adjoint_fp32(gy, w, kind, stride, tf32), ref,
+                                                 kind, stride, tf32)
+        assert ok and bias_ok, (tf32, worst, bias)
+
+
+def _assert_located(worst, got, ref, tf32):
+    """The report points at a voxel whose error really is outside the bound."""
+    want, A = ref[tf32]
+    at = worst["at"]
+    assert worst["got"] == float(got[at]) and worst["want"] == float(want[at])
+    assert abs(worst["got"] - worst["want"]) > (T.EPS["tma"] + T.R_OP) * float(A[at])
+
+
+@pytest.mark.parametrize("tf32", [False, True])
+@pytest.mark.parametrize("defect,layer", [
+    ("unflipped", (R.CONV, 1, 16, 8, (4, 12, 10))),
+    ("no_transpose", (R.CONV, 1, 16, 16, (4, 12, 10))),
+    ("pad_values", (R.CONV, 1, 8, 1, (4, 12, 10))),
+])
+def test_flags_wrong_adjoint_weight(defect, layer, tf32):
+    kind, stride, cin, cout, dims = layer
+    w, gy, ref = _dgrad_case(kind, stride, cin, cout, dims, 22)
+    got = _adjoint_fp32(gy, w, kind, stride, tf32, defect)
+    ok, _, worst, need, _ = _report(got, ref, kind, stride, tf32)
+    assert not ok, (defect, need)
+    _assert_located(worst, got, ref, tf32)
+
+
+@pytest.mark.parametrize("tf32", [False, True])
+@pytest.mark.parametrize("kind,stride,cin,cout,dims", [
+    (R.CONV, 1, 16, 8, (6, 12, 10)), (R.CONV, 2, 8, 16, (6, 12, 10)),
+    (R.CONV_TRANSPOSE, 2, 16, 8, (5, 6, 5))])
+def test_flags_one_adjoint_tap_dropped_on_one_slice(kind, stride, cin, cout, dims, tf32):
+    w, gy, ref = _dgrad_case(kind, stride, cin, cout, dims, 23)
+    d = 3
+    got = _adjoint_fp32(gy, w, kind, stride, tf32, "tap", slice_d=d)
+    ok, _, worst, _, _ = _report(got, ref, kind, stride, tf32)
+    assert not ok and worst["slice"] == d
+    _assert_located(worst, got, ref, tf32)
+
+
+@pytest.mark.parametrize("kind,stride,cin,cout,dims", [
+    (R.CONV, 1, 16, 8, (4, 12, 10)), (R.CONV, 2, 8, 16, (4, 12, 10)),
+    (R.CONV_TRANSPOSE, 2, 16, 8, (2, 6, 5))])
+def test_flags_truncated_operand_by_its_bias(kind, stride, cin, cout, dims):
+    """An operand truncated to TF32 stays within the per-element bound (its error is below an ulp
+    of TF32) but not within the bias check, which names its size and direction."""
+    w, gy, ref = _dgrad_case(kind, stride, cin, cout, dims, 24)
+    ok, bias_ok, _, _, bias = _report(_adjoint_fp32(gy, w, kind, stride, True, "trunc"), ref,
+                                      kind, stride, True)
+    assert not bias_ok and bias < -4 * T.BIAS_MAX, bias
+    _, bias_ok, _, _, bias = _report(_adjoint_fp32(gy, w, kind, stride, True), ref, kind, stride, True)
+    assert bias_ok and abs(bias) < T.BIAS_MAX / 4, bias
