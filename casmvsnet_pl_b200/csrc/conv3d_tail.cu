@@ -40,8 +40,7 @@ int conv3d_tma2_conv11_image(const float* wpk, cudaStream_t st, tc::ImageRef* ir
 namespace tail {
 
 using namespace tc;
-using tma::mbar_expect_tx;
-using tma::tma_load_5d;
+using namespace tma;
 
 struct Params {
   const float* img11;    // conv11 B image (conv3d_tma2 MODE_T, CIN 16, COUT 8)
@@ -50,7 +49,7 @@ struct Params {
   float* logits;         // (B,D,H,W)
   float slope;           // conv11's LeakyReLU slope
   int B, D, H, W;        // full resolution: c0, u11, logits
-  int tiles_w, tiles_h, nchunks, dchunk;
+  Work work;             // prob output tiles; dchunk even
 };
 
 constexpr int kU9W = 6, kU9H = 11;                                  // u9 brick columns, rows
@@ -79,27 +78,22 @@ __global__ void __launch_bounds__(kConvThreads, 2)
 conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
                    const __grid_constant__ CUtensorMap c0map, const Params p) {
   extern __shared__ unsigned char smem_raw[];
-  const uint32_t s_raw = smem_u32(smem_raw);
-  const uint32_t s_base = (s_raw + 1023u) & ~1023u;
-  unsigned char* smem = smem_raw + (s_base - s_raw);
+  unsigned char* smem;
+  const uint32_t s_base = smem_align_1024(smem_raw, &smem);
   const uint32_t s_in = s_base + kInOff, s_u = s_base + kUOff, s_w11 = s_base + kW11Off,
                  s_wp = s_base + kWpOff, s_bar = s_base + kBarOff;
   float* s_param = reinterpret_cast<float*>(smem + kParamOff);
-  const uint32_t in_full = s_bar, in_empty = s_bar + 32, u_full = s_bar + 64,
-                 u_empty = s_bar + 96, bar_w11 = s_bar + 128, bar_wp = s_bar + 136;
+  // u9 / c0 input slots, filled by TMA; u11 slices, written by warpgroup 0 and read by warpgroup 1
+  const Ring<IN_SLOTS> in_ring{s_bar, s_bar + 32};
+  const Ring<U_SLOTS> u_ring{s_bar + 64, s_bar + 96};
+  const uint32_t bar_w11 = s_bar + 128, bar_wp = s_bar + 136;
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int total_items = p.B * p.nchunks * p.tiles_h * p.tiles_w;
+  const int total_items = p.B * p.work.nchunks * p.work.tiles_h * p.work.tiles_w;
 
   // ---- one-time setup ----
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < IN_SLOTS; ++i) {
-      mbar_init(in_full + 8 * i, 1);
-      mbar_init(in_empty + 8 * i, 128);
-    }
-    for (int i = 0; i < U_SLOTS; ++i) {
-      mbar_init(u_full + 8 * i, 128);
-      mbar_init(u_empty + 8 * i, 128);
-    }
+  if (threadIdx.x == 0) {                           // thread 0 initialises every barrier
+    for (int t = 0; t < 2 * IN_SLOTS; ++t) in_ring.init(t, 1, 128);
+    for (int t = 0; t < 2 * U_SLOTS; ++t) u_ring.init(t, 128, 128);
     mbar_init(bar_w11, 1);
     mbar_init(bar_wp, 1);
     fence_barrier_init();
@@ -119,27 +113,15 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
     *reinterpret_cast<float4*>(smem + kInOff + (brick / 4) * kInBytes + (brick % 4) * kU9Bytes +
                                kU9Data + (i % per) * 16) = make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  fence_proxy_async();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    tma::load_image_bulk(s_w11, p.img11, kW11Bytes, bar_w11);
-    tma::load_image_bulk(s_wp, p.imgp, kWpBytes, bar_wp);
-  }
-
-  // nothing above depends on the previous kernel of the stream (see tma_common.cuh)
-  tma::pdl_trigger();
-  tma::pdl_wait();
+  end_prologue(ImageCopy{s_w11, p.img11, kW11Bytes, bar_w11},
+               ImageCopy{s_wp, p.imgp, kWpBytes, bar_wp});
   bool w_ready = false;                             // consumers: weight image has landed
   uint32_t gin = 0, gu = 0;                         // steps / u11 slices before this item
   const int wl = warp & 3;
-  for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x) {
-    int item = item0;
-    const int tw = item % p.tiles_w; item /= p.tiles_w;
-    const int th = item % p.tiles_h; item /= p.tiles_h;
-    const int ck = item % p.nchunks;
-    const int b = item / p.nchunks;
-    const int w0 = tw * kTileW, h0 = th * kTileH;
-    const int d0 = ck * p.dchunk, d1 = min(p.D, d0 + p.dchunk);
+  for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    const Item t = decode_item(item, p.work);
+    const int b = t.b, h0 = t.h0, w0 = t.w0;
+    const int d0 = t.chunk * p.work.dchunk, d1 = min(p.D, d0 + p.work.dchunk);
     const int nd = d1 - d0;                         // even
     const int nsteps = nd / 2 + 2;                  // u9 slices d0/2-1 .. d1/2
     const int s0 = d0 / 2 - 1;
@@ -149,26 +131,22 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
       if (lane == 0) {
         for (int st = 0; st < nsteps; ++st) {
           const uint32_t g = gin + st;
-          const int slot = g % IN_SLOTS;
-          if (g >= (uint32_t)IN_SLOTS) mbar_wait(in_empty + 8 * slot, ((g / IN_SLOTS) - 1) & 1);
-          const uint32_t dst = s_in + slot * kInBytes;
-          mbar_expect_tx(in_full + 8 * slot, 4 * kU9Data + (st > 0 ? 4 * kBrickData : 0));
+          const uint32_t dst = s_in + in_ring.acquire(g) * kInBytes, full = in_ring.full_bar(g);
+          mbar_expect_tx(full, 4 * kU9Data + (st > 0 ? 4 * kBrickData : 0));
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            const tma::Coords5 k =
-                tma::brick_coords(true, 1, 4, q, w0 / 2 - 1, h0 / 2 - 1, s0 + st, b);
-            tma_load_5d(dst + q * kU9Bytes, &u9map, in_full + 8 * slot, k.c[0], k.c[1], k.c[2],
-                        k.c[3], k.c[4]);
+            const Coords5 k = brick_coords(true, 1, 4, q, w0 / 2 - 1, h0 / 2 - 1, s0 + st, b);
+            tma_load_5d(dst + q * kU9Bytes, &u9map, full, k.c[0], k.c[1], k.c[2], k.c[3], k.c[4]);
           }
           if (st > 0) {                             // the first step's u11 slices are not used
 #pragma unroll
             for (int k2 = 0; k2 < 2; ++k2) {
 #pragma unroll
               for (int q = 0; q < 2; ++q) {
-                const tma::Coords5 k = tma::brick_coords(true, 1, 2, q, w0 - 1, h0 - 1,
-                                                         2 * (s0 + st) - 1 + k2, b);
-                tma_load_5d(dst + 4 * kU9Bytes + k2 * kSliceBytes + q * kBrickBytes, &c0map,
-                            in_full + 8 * slot, k.c[0], k.c[1], k.c[2], k.c[3], k.c[4]);
+                const Coords5 k =
+                    brick_coords(true, 1, 2, q, w0 - 1, h0 - 1, 2 * (s0 + st) - 1 + k2, b);
+                tma_load_5d(dst + 4 * kU9Bytes + k2 * kSliceBytes + q * kBrickBytes, &c0map, full,
+                            k.c[0], k.c[1], k.c[2], k.c[3], k.c[4]);
               }
             }
           }
@@ -209,8 +187,7 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
       }
       for (int st = 0; st < nsteps; ++st) {
         const uint32_t g = gin + st;
-        const int slot = g % IN_SLOTS;
-        mbar_wait(in_full + 8 * slot, (g / IN_SLOTS) & 1);
+        const int slot = in_ring.wait(g);
         if (!w_ready) { mbar_wait(bar_w11, 0); w_ready = true; }
         const uint64_t a_s = a_desc0 + ((slot * kInBytes) >> 4);
         wgmma_fence();
@@ -242,9 +219,7 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
           const uint32_t u0 = gu + 2 * (st - 1);
 #pragma unroll
           for (int k2 = 0; k2 < 2; ++k2) {
-            const uint32_t u = u0 + k2;
-            const int us = u % U_SLOTS;
-            if (u >= (uint32_t)U_SLOTS) mbar_wait(u_empty + 8 * us, ((u / U_SLOTS) - 1) & 1);
+            const int us = u_ring.acquire(u0 + k2);
             const int od = 2 * (s0 + st) - 1 + k2;
             // zero outside the volume (prob's zero padding)
             const uint32_t live = od >= 0 && od < p.D ? vmask : 0u;
@@ -271,10 +246,10 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
             }
           }
           fence_proxy_async();                      // generic-proxy writes -> prob's wgmma
-          mbar_arrive(u_full + 8 * (u0 % U_SLOTS));
-          mbar_arrive(u_full + 8 * ((u0 + 1) % U_SLOTS));
+          u_ring.publish(u0);
+          u_ring.publish(u0 + 1);
         }
-        mbar_arrive(in_empty + 8 * slot);           // this thread's reads of the slot are done
+        in_ring.release(g);                         // this thread's reads of the slot are done
       }
     } else {
       // ============ warpgroup 1: prob, both 64-row halves of the tile, per u11 slice ============
@@ -300,8 +275,7 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
       };
       for (int k = 0; k < nd + 2; ++k) {
         const uint32_t u = gu + k;
-        const int us = u % U_SLOTS;
-        mbar_wait(u_full + 8 * us, (u / U_SLOTS) & 1);
+        const int us = u_ring.wait(u);
         if (!w_ready) { mbar_wait(bar_wp, 0); w_ready = true; }
         const uint64_t a_s = a_desc0 + ((us * kSliceBytes) >> 4);
         wgmma_fence();
@@ -315,7 +289,7 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
         }
         wgmma_commit();
         wgmma_wait_all();
-        mbar_arrive(u_empty + 8 * us);
+        u_ring.release(u);
         float done0[4], done1[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) { done0[i] = acc0[i]; done1[i] = acc1[i]; }
@@ -343,30 +317,23 @@ static int launch_tail(const TailArgs& a, cudaStream_t st) {
   p.scale11 = a.scale11; p.shift11 = a.shift11; p.scalep = a.scalep; p.shiftp = a.shiftp;
   p.logits = a.logits; p.slope = a.slope;
   p.B = a.B; p.D = a.D; p.H = a.h; p.W = a.w;
-  p.tiles_w = (a.w + kTileW - 1) / kTileW;
-  p.tiles_h = (a.h + kTileH - 1) / kTileH;
-  // input_map returns a per-thread copy that the next call overwrites
-  const CUtensorMap* m9 = tma::input_map(a.u9, a.B, a.D / 2, a.h / 2, a.w / 2, 16, 4, kU9W, kU9H,
-                                         1, true);
-  if (!m9) return -2;
-  const CUtensorMap u9map = *m9;
-  const CUtensorMap* m0 = tma::input_map(a.c0, a.B, a.D, a.h, a.w, 8, 4, kHaloW, kHaloH, 1, true);
-  if (!m0) return -2;
-  const CUtensorMap c0map = *m0;
+  p.work.tiles_w = (a.w + kTileW - 1) / kTileW;
+  p.work.tiles_h = (a.h + kTileH - 1) / kTileH;
+  CUtensorMap u9map, c0map;
+  if (int rc = input_map(&u9map, a.u9, a.B, a.D / 2, a.h / 2, a.w / 2, 16, kU9W, kU9H, 1, true))
+    return rc;
+  if (int rc = input_map(&c0map, a.c0, a.B, a.D, a.h, a.w, 8, kHaloW, kHaloH, 1, true)) return rc;
   ImageRef i11, ip;
   if (int rc = conv3d_tma2_conv11_image(a.w11, st, &i11)) return rc;
   if (int rc = conv3d_tma_prob_image(a.wp, st, &ip)) return rc;
   p.img11 = i11.img; p.imgp = ip.img;
-  const int per_sm = tma::resident_per_sm(kfn, kConvThreads, kTotal);
-  const long resident = (long)num_sms() * per_sm;
-  const long cols = (long)p.B * p.tiles_w * p.tiles_h;
-  // an item of 2 dc u9 slices walks 2 dc + 2 u11 slices (the prob halo) and dc + 2 u9 slices
-  p.dchunk = 2 * tma::pick_dchunk(p.D / 2, 16, cols, resident, 2, 3);
-  p.nchunks = (p.D + p.dchunk - 1) / p.dchunk;
-  const long items = cols * p.nchunks;
-  const long gx = items < resident ? items : resident;
-  tma::launch_pdl(i11.settled && ip.settled, kfn, dim3((unsigned)gx), kConvThreads, kTotal, st,
-                  u9map, c0map, p);
+  // chunks of dc u9 slices: an item walks dc + 2 u9 slices and 2 dc + 2 u11 slices (the prob
+  // halo), and covers 2 dc output slices
+  const Sizing z = size_persistent(kfn, kTotal, 1, (long)p.B * p.work.tiles_w * p.work.tiles_h,
+                                   p.D / 2, 16, 2, 3);
+  p.work.dchunk = 2 * z.dchunk;
+  p.work.nchunks = z.nchunks;
+  launch_pdl(i11.settled && ip.settled, kfn, z.grid, kConvThreads, kTotal, st, u9map, c0map, p);
   return after_launch("conv3d_tail");
 }
 

@@ -29,6 +29,7 @@
 
 #include "common.cuh"
 #include "tc_common.cuh"
+#include <string.h>
 #include <mutex>
 
 #include "tma_common.cuh"
@@ -48,9 +49,8 @@ struct Params {
   float slope;
   int B, D, H, W, Cout;   // Cout = channels handled by one CTA (<= GW)
   int cout_total;         // channel count of the output tensor; blockIdx.y selects the chunk
-  int tiles_w, tiles_h, nchunks, dchunk;
+  Work work;
   int round_out;        // round the stored activations to tf32 (unbiased next-layer operand)
-  int planar;           // 1x3x3 kernel: input slice s feeds output slice s only (kd = 1)
   int x_blocked;        // x stored blocked by channel quads (input_map); else channels-last
   int y_blocked;        // y and skip stored blocked by channel quads; else channels-last
 };
@@ -112,37 +112,27 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   using S = Smem<CIN, GW, SLOTS_>;
   constexpr int SLOTS = S::SLOTS;
   extern __shared__ unsigned char smem_raw[];
-  const uint32_t s_raw = smem_u32(smem_raw);
-  const uint32_t s_base = (s_raw + 1023u) & ~1023u;
-  unsigned char* smem = smem_raw + (s_base - s_raw);
+  unsigned char* smem;
+  const uint32_t s_base = smem_align_1024(smem_raw, &smem);
   const uint32_t s_ring = s_base + S::kRingOff, s_w = s_base + S::kWOff,
                  s_bar = s_base + S::kBarOff;
   float* s_param = reinterpret_cast<float*>(smem + S::kParamOff);
-  const uint32_t bar_full = s_bar, bar_empty = s_bar + 64, bar_w = s_bar + 128;
+  const Ring<SLOTS> ring{s_bar, s_bar + 64};
+  const uint32_t bar_w = s_bar + 128;
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int total_items = p.B * p.nchunks * p.tiles_h * p.tiles_w;
+  const int total_items = p.B * p.work.nchunks * p.work.tiles_h * p.work.tiles_w;
 
   // ---- one-time setup ----
   {
     const int t = threadIdx.x;
-    if (t < SLOTS) mbar_init(bar_full + 8 * t, 1);
-    else if (t < 2 * SLOTS) mbar_init(bar_empty + 8 * (t - SLOTS), kConsumerThreads);
-    else if (t == 2 * SLOTS) mbar_init(bar_w, 1);
+    ring.init(t, 1, kConsumerThreads);
+    if (t == 2 * SLOTS) mbar_init(bar_w, 1);
     if (t <= 2 * SLOTS) fence_barrier_init();
   }
   const int co_base = blockIdx.y * p.Cout;
-  for (int i = threadIdx.x; i < GW; i += kConvThreads) {
-    s_param[i] = (i < p.Cout) ? (p.scale ? __ldg(p.scale + co_base + i) : 1.f) : 0.f;
-    s_param[GW + i] = (i < p.Cout) ? (p.shift ? __ldg(p.shift + co_base + i) : 0.f) : 0.f;
-  }
-  fence_proxy_async();
-  __syncthreads();
-  if (threadIdx.x == 0) load_image_bulk(s_w, p.bimg + (size_t)blockIdx.y * (S::kWBytes / 4), S::kWBytes, bar_w);
-
-  // nothing above depends on the previous kernel of the stream (see tma_common.cuh)
-  tma::pdl_trigger();
-  tma::pdl_wait();
+  stage_scale_shift<GW>(s_param, p.scale, p.shift, co_base, p.Cout);
+  end_prologue(ImageCopy{s_w, p.bimg + (size_t)blockIdx.y * (S::kWBytes / 4), S::kWBytes, bar_w});
   bool w_ready = false;                             // consumers: weight image has landed
   uint32_t gs = 0;                                  // slices processed before this item (all roles)
   // consumers: the accumulator, column groups 0, 1, 2 = output slices it-2, it-1, it (planar:
@@ -155,14 +145,10 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   int pend_od = -1, pend_b = 0, pend_h0 = 0, pend_w0 = 0;
   const int wg = warp >> 2, wl = warp & 3;
   const int row0 = 64 * wg;                         // consumers: first GEMM row of the warpgroup
-  for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x) {
-    int item = item0;
-    const int tw = item % p.tiles_w; item /= p.tiles_w;
-    const int th = item % p.tiles_h; item /= p.tiles_h;
-    const int ck = item % p.nchunks;
-    const int b = item / p.nchunks;
-    const int w0 = tw * kTileW, h0 = th * kTileH;
-    const int d0 = ck * p.dchunk, d1 = min(p.D, d0 + p.dchunk);
+  for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    const Item t = decode_item(item, p.work);
+    const int b = t.b, h0 = t.h0, w0 = t.w0;
+    const int d0 = t.chunk * p.work.dchunk, d1 = min(p.D, d0 + p.work.dchunk);
     const int nd = d1 - d0;
     const int halo = PLANAR ? 0 : 1;
     const int nslices = nd + 2 * halo;              // input slices d0-halo .. d1-1+halo
@@ -172,16 +158,14 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
       if (lane == 0) {
         for (int it = 0; it < nslices; ++it) {
           const uint32_t g = gs + it;
-          const int slot = g % SLOTS;
-          if (g >= (uint32_t)SLOTS) mbar_wait(bar_empty + 8 * slot, ((g / SLOTS) - 1) & 1);
-          const uint32_t dst = s_ring + slot * S::kSlotBytes;
-          mbar_expect_tx(bar_full + 8 * slot, S::CQ * S::kBrickData);
+          const uint32_t dst = s_ring + ring.acquire(g) * S::kSlotBytes, full = ring.full_bar(g);
+          mbar_expect_tx(full, S::CQ * S::kBrickData);
 #pragma unroll
           for (int q = 0; q < S::CQ; ++q) {
             const Coords5 k = brick_coords(!PLANAR && p.x_blocked, 1, S::CQ, q, w0 - 1, h0 - 1,
                                            d0 - halo + it, b);
-            tma_load_5d(dst + q * S::kBrickBytes, &xmap, bar_full + 8 * slot, k.c[0], k.c[1],
-                        k.c[2], k.c[3], k.c[4]);
+            tma_load_5d(dst + q * S::kBrickBytes, &xmap, full, k.c[0], k.c[1], k.c[2], k.c[3],
+                        k.c[4]);
           }
         }
       }
@@ -195,9 +179,9 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
       const uint64_t b_desc0 = make_desc(s_w, b_lbo, b_sbo);
       for (int it = 0; it < nslices; ++it) {
         const uint32_t g = gs + it;
-        mbar_wait(bar_full + 8 * (g % SLOTS), (g / SLOTS) & 1);
+        const int slot = ring.wait(g);
         if (!w_ready) { mbar_wait(bar_w, 0); w_ready = true; }
-        const uint64_t a_s = a_desc0 + (((g % SLOTS) * S::kSlotBytes) >> 4);
+        const uint64_t a_s = a_desc0 + ((slot * S::kSlotBytes) >> 4);
         wgmma_fence();
 #pragma unroll
         for (int khw = 0; khw < 9; ++khw) {
@@ -219,7 +203,7 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
           store_slice<GW, 0, PLANAR>(done, p, s_param, pend_b, pend_od, pend_h0, pend_w0, row0, wl,
                                      lane, co_base);
         wgmma_wait_all();
-        mbar_arrive(bar_empty + 8 * (g % SLOTS));   // this thread's reads of the slot are done
+        ring.release(g);                            // this thread's reads of the slot are done
         // output slice of column group 0: `it` when planar, else it - 2 (complete after its
         // third input slice).  Group 0 is copied out before the (per-thread) stores so that no
         // accumulator register is touched on a divergent path: that would make ptxas serialize
@@ -250,129 +234,95 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
 
 // ---- host side ----
 
-static PFN_cuTensorMapEncodeTiled_v12000 encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
+int encode_map(const MapDesc& d, CUtensorMap* out) {
+  static_assert(sizeof(MapDesc) == 128, "MapDesc is compared bytewise: no padding");
+  static const PFN_cuTensorMapEncodeTiled_v12000 enc = [] {
     void* ptr = nullptr;
     cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) ==
-            cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr);
+    return cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) ==
+                   cudaSuccess && q == cudaDriverEntryPointSuccess
+               ? reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr)
+               : nullptr;
+  }();
+  struct Entry { MapDesc d; CUtensorMap map; };
+  static Entry memo[128];
+  static int memo_n = 0, memo_next = 0;
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  for (int i = 0; i < memo_n; ++i) {
+    if (memcmp(&memo[i].d, &d, sizeof(MapDesc)) == 0) {
+      *out = memo[i].map;
+      return 0;
+    }
   }
-  return fn;
-}
-
-// Generic tiled-map encoder for other kernels of the library (K1's feature boxes): fp32
-// elements, rank <= 5, zero fill out of bounds.  0 on success.
-int encode_tiled(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                 const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) {
-  auto enc = encode_fn();
   if (!enc) { set_error("tma: cuTensorMapEncodeTiled is not available"); return -2; }
-  cuuint64_t gdim[5], gstr[4];
-  cuuint32_t bx[5], es[5];
-  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  const CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
-                                                      : CU_TENSOR_MAP_SWIZZLE_NONE;
-  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank,
-                         const_cast<void*>(base), gdim, gstr, bx, es,
+  const CUtensorMapSwizzle sw = d.swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                : d.swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                : d.swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                                        : CU_TENSOR_MAP_SWIZZLE_NONE;
+  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)d.rank,
+                         const_cast<void*>(d.base), d.dims, d.strides_bytes, d.box, d.elem_strides,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("tma: cuTensorMapEncodeTiled failed (%d), rank %d", (int)r, rank);
+    set_error("tma: cuTensorMapEncodeTiled failed (%d), rank %d, dims %llu %llu %llu %llu %llu",
+              (int)r, d.rank, (unsigned long long)d.dims[0], (unsigned long long)d.dims[1],
+              (unsigned long long)d.dims[2], (unsigned long long)d.dims[3],
+              (unsigned long long)d.dims[4]);
     return -2;
   }
+  memo[memo_next] = Entry{d, *out};
+  memo_next = (memo_next + 1) % 128;
+  if (memo_n < 128) ++memo_n;
   return 0;
 }
 
-// Tensor maps are pure functions of (pointer, shape, box): memoised, since inference calls
-// every layer with the same workspace pointers each step.
-struct MapEntry { const void* x; int B, D, H, W, C, CB, bw, bh, sw, blk; CUtensorMap map; };
-static MapEntry g_maps[128];
-static int g_maps_n = 0, g_maps_next = 0;
-static std::mutex g_maps_mu;
-
-const CUtensorMap* input_map(const float* x, int B, int D, int H, int W, int C, int CB, int box_w,
-                             int box_h, int stride_w, bool blocked) {
-  // the returned map is a per-thread copy: ring slots may be recycled by other threads
-  static thread_local CUtensorMap t_ret;
-  const int blk = blocked ? 1 : 0;
-  std::lock_guard<std::mutex> lock(g_maps_mu);
-  for (int i = 0; i < g_maps_n; ++i) {
-    const MapEntry& e = g_maps[i];
-    if (e.x == x && e.B == B && e.D == D && e.H == H && e.W == W && e.C == C && e.CB == CB &&
-        e.bw == box_w && e.bh == box_h && e.sw == stride_w && e.blk == blk) {
-      t_ret = e.map;
-      return &t_ret;
-    }
-  }
-  auto enc = encode_fn();
-  if (!enc) { set_error("conv3d_tma: cuTensorMapEncodeTiled is not available"); return nullptr; }
-  MapEntry& e = g_maps[g_maps_next];
-  g_maps_next = (g_maps_next + 1) % 128;
-  if (g_maps_n < 128) ++g_maps_n;
-  const cuuint64_t vox = (cuuint64_t)D * H * W;      // voxels per channel plane
-  // channels-last (B,D,H,W,C) as {C, W, H, D, B}, box {CB, box_w, box_h, 1, 1}
-  cuuint64_t gdim[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)B};
-  cuuint64_t gstr[4] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4,
-                        vox * C * 4};
-  cuuint32_t box[5] = {(cuuint32_t)CB, (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1};
-  cuuint32_t estr[5] = {1, (cuuint32_t)stride_w, 1, 1, 1};
-  if (blocked && stride_w == 1) {
-    // blocked (B,C/4,D,H,W,4) as {4W, H, D, C/4, B}: the quad folded into the inner dimension,
-    // box {4 box_w, box_h, 1, 1, 1}: one brick row is 16 box_w contiguous bytes
-    const cuuint64_t d2[5] = {4 * (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)C / 4,
-                              (cuuint64_t)B};
-    const cuuint64_t s2[4] = {(cuuint64_t)W * 16, (cuuint64_t)H * W * 16, vox * 16, vox * C * 4};
-    const cuuint32_t b2[5] = {4 * (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1, 1};
-    for (int i = 0; i < 5; ++i) { gdim[i] = d2[i]; box[i] = b2[i]; estr[i] = 1; }
-    for (int i = 0; i < 4; ++i) gstr[i] = s2[i];
-  } else if (blocked) {
-    // blocked, W walked with element stride 2: {4, W, H, D, C/4 * B}, box {4, box_w, box_h, 1, 1}
-    const cuuint64_t d2[5] = {4, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D,
-                              (cuuint64_t)C / 4 * B};
-    const cuuint64_t s2[4] = {16, (cuuint64_t)W * 16, (cuuint64_t)H * W * 16, vox * 16};
-    for (int i = 0; i < 5; ++i) gdim[i] = d2[i];
-    for (int i = 0; i < 4; ++i) gstr[i] = s2[i];
-    box[0] = 4;
-  }
-  const CUtensorMapSwizzle sw = CB * 4 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                : CB * 4 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                : CB * 4 == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
-                                               : CU_TENSOR_MAP_SWIZZLE_NONE;
-  const CUresult r = enc(&e.map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(x), gdim,
-                         gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    e.x = nullptr;
-    set_error("conv3d_tma: cuTensorMapEncodeTiled failed (%d) for C=%d W=%d H=%d D=%d B=%d",
-              (int)r, C, W, H, D, B);
-    return nullptr;
-  }
-  e.x = x; e.B = B; e.D = D; e.H = H; e.W = W; e.C = C; e.CB = CB; e.bw = box_w; e.bh = box_h;
-  e.sw = stride_w; e.blk = blk;
-  t_ret = e.map;
-  return &t_ret;
+int input_map(CUtensorMap* out, const float* x, int B, int D, int H, int W, int C, int box_w,
+              int box_h, int stride_w, bool blocked) {
+  const uint64_t c = C, w = W, h = H, dp = D, b = B, vox = dp * h * w;
+  const uint32_t bw = box_w, bh = box_h, sw = stride_w;
+  const MapDesc d =
+      !blocked        ? MapDesc{x, 5, 0, {c, w, h, dp, b}, {4 * c, 4 * c * w, 4 * c * w * h, 4 * c * vox},
+                                {4, bw, bh, 1, 1}, {1, sw, 1, 1, 1}}
+      : stride_w == 1 ? MapDesc{x, 5, 0, {4 * w, h, dp, c / 4, b}, {16 * w, 16 * w * h, 16 * vox, 4 * c * vox},
+                                {4 * bw, bh, 1, 1, 1}, {1, 1, 1, 1, 1}}
+                      : MapDesc{x, 5, 0, {4, w, h, dp, c / 4 * b}, {16, 16 * w, 16 * w * h, 16 * vox},
+                                {4, bw, bh, 1, 1}, {1, sw, 1, 1, 1}};
+  return encode_map(d, out);
 }
 
+// B operand image of the stride-1 kernels: [chunk][kh][kw][CIN/4][3*GW][4], column group g
+// holds the weights of kd = 2 - g, tf32-rounded (to nearest), zero rows for co >= chunk.  One
+// image per Cout chunk (chunk = blockIdx.y of the conv kernel), `chunk` channels each.
+__global__ void build_image_kernel(const float* __restrict__ wpk, float* __restrict__ img,
+                                   int CIN, int GW, int chunk, int cout_total) {
+  const int CQ = CIN / 4;
+  const int per = 9 * CIN * 3 * GW;
+  const int total = per * (cout_total / chunk);
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
+    const int ck = t / per, i = t - ck * per;
+    const int j = i & 3;
+    const int n = (i >> 2) % (3 * GW);
+    const int r = (i >> 2) / (3 * GW);    // (kh*3+kw)*CQ + cq
+    const int cq = r % CQ, khw = r / CQ;
+    const int g = n / GW, co = n % GW;
+    const int kd = 2 - g;
+    const int ci = cq * 4 + j;
+    float v = 0.f;
+    if (co < chunk)
+      v = to_tf32(__ldg(wpk + ((size_t)(kd * 9 + khw) * CIN + ci) * cout_total + ck * chunk + co));
+    img[t] = v;
+  }
+}
 
-// The B operand image of a layer (nco chunks of GW columns, `cout` of them used), from the
-// per-process cache or built on `st` on a miss.
+// The B operand image of a layer (nco chunks of GW columns, `cout` of them used).
 template <int CIN, int GW>
 static int stride1_image(const float* wpk, int cout, int cout_total, int nco, cudaStream_t st,
                          ImageRef* ir) {
-  constexpr int kWBytes = Smem<CIN, GW, 1>::kWBytes;
-  *ir = image_cache_get(wpk, 1000 + CIN * 100 + GW, (size_t)kWBytes * nco, st);
-  if (!ir->img) return -2;
-  if (!ir->hit) {
-    if (int rc = build_stride1_image(wpk, ir->img, CIN, GW, cout, cout_total, st)) return rc;
-    image_cache_built(ir->img, st);
-  }
-  return 0;
+  return cached_image(wpk, 1000 + CIN * 100 + GW, (size_t)Smem<CIN, GW, 1>::kWBytes * nco, st, ir,
+                      "conv3d_tma/build_image", [&](float* img) {
+                        build_image_kernel<<<64, 256, 0, st>>>(wpk, img, CIN, GW, cout, cout_total);
+                      });
 }
 
 // One CTA computes GW output columns (Cout <= GW, or a GW-channel slice of a wider Cout).
@@ -387,31 +337,23 @@ static int launch(const ConvArgs& a, cudaStream_t st) {
   p.scale = a.scale; p.shift = a.shift; p.skip = a.skip; p.y = a.y;
   p.slope = a.slope; p.B = a.B; p.D = a.D; p.H = a.h; p.W = a.w;
   p.Cout = a.Cout < GW ? a.Cout : GW; p.cout_total = a.Cout;
-  p.tiles_w = (a.w + tc::kTileW - 1) / tc::kTileW;
-  p.tiles_h = (a.h + tc::kTileH - 1) / tc::kTileH;
-  p.planar = PLANAR ? 1 : 0;
+  p.work.tiles_w = (a.w + tc::kTileW - 1) / tc::kTileW;
+  p.work.tiles_h = (a.h + tc::kTileH - 1) / tc::kTileH;
   p.x_blocked = (a.layout & kLayoutXBlocked) ? 1 : 0;
   p.y_blocked = (a.layout & kLayoutYBlocked) ? 1 : 0;
   p.round_out = a.round_out;
-  const CUtensorMap* map = input_map(a.x, p.B, p.D, p.H, p.W, CIN, 4, kHaloW, kHaloH, 1, p.x_blocked);
-  if (!map) return -2;
-  const int per_sm = resident_per_sm(kfn, kConvThreads, S::kTotal);
+  CUtensorMap map;
+  if (int rc = input_map(&map, a.x, p.B, p.D, p.H, p.W, CIN, kHaloW, kHaloH, 1, p.x_blocked))
+    return rc;
   const int nco = p.cout_total / p.Cout;
-  const int cap = 32;
-  const long cols = (long)p.B * p.tiles_w * p.tiles_h;
-  int dchunk = pick_dchunk(p.D, cap, cols, (long)num_sms() * per_sm / nco, 1, p.planar ? 0 : 2);
-  const int dchunk_env = switches().tma_dchunk;
-  if (dchunk_env > 0 && dchunk_env <= cap) dchunk = dchunk_env < p.D ? dchunk_env : p.D;
-  p.dchunk = dchunk;
-  p.nchunks = (p.D + dchunk - 1) / dchunk;
+  const Sizing z = size_persistent(kfn, S::kTotal, nco, (long)p.B * p.work.tiles_w * p.work.tiles_h,
+                                   p.D, 32, 1, PLANAR ? 0 : 2);
+  p.work.dchunk = z.dchunk;
+  p.work.nchunks = z.nchunks;
   ImageRef ir;
   if (int rc = stride1_image<CIN, GW>(a.wpk, p.Cout, p.cout_total, nco, st, &ir)) return rc;
   p.bimg = ir.img;
-  const long items = (long)p.B * p.nchunks * p.tiles_h * p.tiles_w;
-  int resident = num_sms() * per_sm / nco;
-  if (resident < 1) resident = 1;
-  const long gx = items < resident ? items : resident;
-  launch_pdl(ir.settled, kfn, dim3((unsigned)gx, (unsigned)nco), kConvThreads, S::kTotal, st, *map, p);
+  launch_pdl(ir.settled, kfn, z.grid, kConvThreads, S::kTotal, st, map, p);
   return after_launch("conv3d_tma");
 }
 

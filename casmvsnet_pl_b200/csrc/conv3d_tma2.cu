@@ -41,8 +41,7 @@ namespace casmvs {
 namespace tma2 {
 
 using namespace casmvs::tc;
-using casmvs::tma::mbar_expect_tx;
-using casmvs::tma::tma_load_5d;
+using namespace casmvs::tma;
 
 enum { MODE_S2 = 0, MODE_T = 1, MODE_P5 = 2 };
 
@@ -55,7 +54,7 @@ struct Params {
   float slope;
   int B, Di, Hi, Wi, Do, Ho, Wo, Cout;     // Cout = channel count of the output tensor;
                                            // a CTA handles the COUT-channel chunk blockIdx.y
-  int tiles_w, tiles_h, nchunks, dchunk;   // tiles over the M space (output for S2, input for T)
+  tma::Work work;       // tiles over the M space (output for S2 and P5, input for T)
   int round_out;
   int x_blocked;       // x stored blocked by channel quads (tma::input_map); else channels-last
   int y_blocked;       // y and skip stored blocked by channel quads; else channels-last
@@ -94,48 +93,34 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   constexpr int BW = C::BW, GW = C::GW, BROWS = C::BROWS;
   constexpr int SLOTS = C::SLOTS;
   extern __shared__ unsigned char smem_raw[];
-  const uint32_t s_raw = smem_u32(smem_raw);
-  const uint32_t s_base = (s_raw + 1023u) & ~1023u;
-  unsigned char* smem = smem_raw + (s_base - s_raw);
+  unsigned char* smem;
+  const uint32_t s_base = smem_align_1024(smem_raw, &smem);
   const uint32_t s_ring = s_base + C::kRingOff, s_w = s_base + C::kWOff,
                  s_bar = s_base + C::kBarOff;
   float* s_param = reinterpret_cast<float*>(smem + C::kParamOff);
-  const uint32_t bar_full = s_bar, bar_empty = s_bar + 64, bar_w = s_bar + 128;
+  const Ring<SLOTS> ring{s_bar, s_bar + 64};
+  const uint32_t bar_w = s_bar + 128;
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int total_items = p.B * p.nchunks * p.tiles_h * p.tiles_w;
+  const int total_items = p.B * p.work.nchunks * p.work.tiles_h * p.work.tiles_w;
   const int Dm = MODE == MODE_T ? p.Di : p.Do;               // M-space depth
 
   // ---- one-time setup ----
   {
     const int t = threadIdx.x;
-    if (t < SLOTS) mbar_init(bar_full + 8 * t, 1);
-    else if (t < 2 * SLOTS) mbar_init(bar_empty + 8 * (t - SLOTS), kConsumerThreads);
-    else if (t == 2 * SLOTS) mbar_init(bar_w, 1);
+    ring.init(t, 1, kConsumerThreads);
+    if (t == 2 * SLOTS) mbar_init(bar_w, 1);
     if (t <= 2 * SLOTS) fence_barrier_init();
   }
   const int co_base = blockIdx.y * COUT;
-  for (int i = threadIdx.x; i < 32; i += kConvThreads) {
-    s_param[i] = (i < COUT) ? (p.scale ? __ldg(p.scale + co_base + i) : 1.f) : 0.f;
-    s_param[32 + i] = (i < COUT) ? (p.shift ? __ldg(p.shift + co_base + i) : 0.f) : 0.f;
-  }
-  fence_proxy_async();
-  __syncthreads();
-  if (threadIdx.x == 0) tma::load_image_bulk(s_w, p.bimg + (size_t)blockIdx.y * (C::kWBytes / 4), C::kWBytes, bar_w);
-
-  // nothing above depends on the previous kernel of the stream (see tma_common.cuh)
-  tma::pdl_trigger();
-  tma::pdl_wait();
+  stage_scale_shift<32>(s_param, p.scale, p.shift, co_base, COUT);
+  end_prologue(ImageCopy{s_w, p.bimg + (size_t)blockIdx.y * (C::kWBytes / 4), C::kWBytes, bar_w});
   bool w_ready = false;                             // consumers: weight image has landed
   uint32_t gs = 0;                                  // slices processed before this item
-  for (int item0 = blockIdx.x; item0 < total_items; item0 += gridDim.x) {
-    // ---- work item: (b, chunk of groups along depth, tile_h, tile_w) over the M space ----
-    int item = item0;
-    const int tw = item % p.tiles_w; item /= p.tiles_w;
-    const int th = item % p.tiles_h; item /= p.tiles_h;
-    const int ck = item % p.nchunks;
-    const int b = item / p.nchunks;
-    const int w0 = tw * kTileW, h0 = th * kTileH;            // M-space origin of the tile
-    const int g0 = ck * p.dchunk, g1 = min(Dm, g0 + p.dchunk);
+  for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    // work item: (b, chunk of groups along depth, M-space origin of the tile)
+    const Item t = decode_item(item, p.work);
+    const int b = t.b, h0 = t.h0, w0 = t.w0;
+    const int g0 = t.chunk * p.work.dchunk, g1 = min(Dm, g0 + p.work.dchunk);
     const int ng = g1 - g0;                                  // output groups of this item
     // input slices walked: S2: s = 2*g0-1 .. 2*g1-1  (2*ng+1);  T: s = g0 .. g1  (ng+1)
     // P5: s = g0 .. g1-1 (every image is its own group)
@@ -147,10 +132,8 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
       if (lane == 0) {
         for (int it = 0; it < nslices; ++it) {
           const uint32_t g = gs + it;
-          const int slot = g % SLOTS;
-          if (g >= (uint32_t)SLOTS) mbar_wait(bar_empty + 8 * slot, ((g / SLOTS) - 1) & 1);
-          const uint32_t dst = s_ring + slot * C::kSlotBytes;
-          mbar_expect_tx(bar_full + 8 * slot, C::NPL * C::kPlaneData);
+          const uint32_t dst = s_ring + ring.acquire(g) * C::kSlotBytes, full = ring.full_bar(g);
+          mbar_expect_tx(full, C::NPL * C::kPlaneData);
 #pragma unroll
           for (int pl = 0; pl < C::NPL; ++pl) {
             // plane pl = PAR * (channel quad) + column parity
@@ -161,8 +144,8 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
             const tma::Coords5 k = tma::brick_coords(MODE != MODE_P5 && p.x_blocked,
                                                      MODE == MODE_T ? 1 : 2, C::CQ,
                                                      q, wc, hc, s_first + it, b);
-            tma_load_5d(dst + pl * C::kPlaneBytes, &xmap, bar_full + 8 * slot, k.c[0], k.c[1],
-                        k.c[2], k.c[3], k.c[4]);
+            tma_load_5d(dst + pl * C::kPlaneBytes, &xmap, full, k.c[0], k.c[1], k.c[2], k.c[3],
+                        k.c[4]);
           }
         }
       }
@@ -316,9 +299,9 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
 
       for (int it = 0; it < nslices; ++it) {
         const uint32_t g = gs + it;
-        mbar_wait(bar_full + 8 * (g % SLOTS), (g / SLOTS) & 1);
+        const int slot = ring.wait(g);
         if (!w_ready) { mbar_wait(bar_w, 0); w_ready = true; }
-        const uint64_t a_s = a_desc0 + (((g % SLOTS) * C::kSlotBytes) >> 4);
+        const uint64_t a_s = a_desc0 + ((slot * C::kSlotBytes) >> 4);
         if constexpr (MODE == MODE_S2) {
           // B rows [W(kd=1) | W(kd=2) | W(kd=0)]
           if ((it & 1) == 0) issue(std::integral_constant<int, 2 * GW>{}, a_s, GW);  // kd=2 -> a-1, kd=0 -> a
@@ -330,7 +313,7 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
         } else {
           issue(std::integral_constant<int, 12 * COUT>{}, a_s, 0);
         }
-        mbar_arrive(bar_empty + 8 * (g % SLOTS));   // this thread's reads of the slot are done
+        ring.release(g);                            // this thread's reads of the slot are done
         if constexpr (MODE == MODE_S2) {
           if ((it & 1) == 0) {
             // even walk index it = 2a: group a-1 is complete (its kd = 2 slice was this one)
@@ -429,23 +412,19 @@ __global__ void build_image_p5_kernel(const float* __restrict__ wt, float* __res
   }
 }
 
-// The B operand image of a layer (all its COUT-channel chunks), from the per-process cache or
-// built on `st` on a miss.
+// The B operand image of a layer (all its COUT-channel chunks).
 template <int MODE, int CIN, int COUT>
 static int tma2_image(const float* wpk, int cout_total, cudaStream_t st, ImageRef* ir) {
   using C = Cfg<MODE, CIN, COUT>;
-  *ir = image_cache_get(wpk, 2000 + MODE * 10000 + CIN * 100 + COUT,
-                        (size_t)C::kWBytes * (cout_total / COUT), st);
-  if (!ir->img) return -2;
-  if (!ir->hit) {
-    if constexpr (MODE == MODE_P5)
-      build_image_p5_kernel<CIN, COUT><<<32, 256, 0, st>>>(wpk, ir->img);
-    else
-      build_image_tma2_kernel<MODE, CIN, COUT><<<64, 256, 0, st>>>(wpk, ir->img, cout_total);
-    if (int rc = after_launch("conv3d_tma2/build_image")) return rc;
-    image_cache_built(ir->img, st);
-  }
-  return 0;
+  return cached_image(wpk, 2000 + MODE * 10000 + CIN * 100 + COUT,
+                      (size_t)C::kWBytes * (cout_total / COUT), st, ir, "conv3d_tma2/build_image",
+                      [&](float* img) {
+                        if constexpr (MODE == MODE_P5)
+                          build_image_p5_kernel<CIN, COUT><<<32, 256, 0, st>>>(wpk, img);
+                        else
+                          build_image_tma2_kernel<MODE, CIN, COUT><<<64, 256, 0, st>>>(wpk, img,
+                                                                                       cout_total);
+                      });
 }
 
 // MODE_S2 / MODE_P5: output = (in - 1) / 2 + 1 along H and W (and D for MODE_S2); MODE_T:
@@ -468,34 +447,28 @@ static int launch2(const ConvArgs& a, cudaStream_t st) {
   p.y_blocked = (a.layout & kLayoutYBlocked) ? 1 : 0;
   // S2: box {4, 17 traversed -> 9 loaded, 33, 1, 1} walking W with stride 2; T: {4, 9, 17}
   // P5: box {4, 19 traversed -> 10 loaded, 35, 1, 1} walking W with stride 2
-  const CUtensorMap* map =
-      MODE == MODE_S2   ? tma::input_map(a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 17, C::BR, 2,
+  CUtensorMap map;
+  const int rc =
+      MODE == MODE_S2   ? tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 17, C::BR, 2,
                                          p.x_blocked)
-      : MODE == MODE_P5 ? tma::input_map(a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, 19, C::BR, 2)
-                        : tma::input_map(a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 4, C::BW, C::BR, 1,
+      : MODE == MODE_P5 ? tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 19, C::BR, 2)
+                        : tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, C::BW, C::BR, 1,
                                          p.x_blocked);
-  if (!map) return -2;
-  const int per_sm = tma::resident_per_sm(kfn, kConvThreads, C::kTotal);
+  if (rc) return rc;
   const int Dm = MODE == MODE_T ? p.Di : p.Do;
   const int Hm = MODE == MODE_T ? p.Hi : p.Ho, Wm = MODE == MODE_T ? p.Wi : p.Wo;
-  p.tiles_w = (Wm + kTileW - 1) / kTileW;
-  p.tiles_h = (Hm + kTileH - 1) / kTileH;
+  p.work.tiles_w = (Wm + kTileW - 1) / kTileW;
+  p.work.tiles_h = (Hm + kTileH - 1) / kTileH;
   const int nco = p.Cout / COUT;
-  const int cap = 32;
-  const long cols = (long)p.B * p.tiles_w * p.tiles_h;
-  const int dchunk = tma::pick_dchunk(Dm, cap, cols, (long)num_sms() * per_sm / nco,
-                                      MODE == MODE_S2 ? 2 : 1,
-                                      MODE == MODE_S2 ? 1 : MODE == MODE_T ? 1 : 0);
-  p.dchunk = dchunk;
-  p.nchunks = (Dm + dchunk - 1) / dchunk;
-  const long items = cols * p.nchunks;
+  const tma::Sizing z = tma::size_persistent(
+      kfn, C::kTotal, nco, (long)p.B * p.work.tiles_w * p.work.tiles_h, Dm, 32,
+      MODE == MODE_S2 ? 2 : 1, MODE == MODE_S2 ? 1 : MODE == MODE_T ? 1 : 0);
+  p.work.dchunk = z.dchunk;
+  p.work.nchunks = z.nchunks;
   ImageRef ir;
   if (int rc = tma2_image<MODE, CIN, COUT>(a.wpk, p.Cout, st, &ir)) return rc;
   p.bimg = ir.img;
-  long resident = (long)num_sms() * per_sm / nco;
-  if (resident < 1) resident = 1;
-  const long gx = items < resident ? items : resident;
-  tma::launch_pdl(ir.settled, kfn, dim3((unsigned)gx, (unsigned)nco), kConvThreads, C::kTotal, st, *map, p);
+  tma::launch_pdl(ir.settled, kfn, z.grid, kConvThreads, C::kTotal, st, map, p);
   return after_launch("conv3d_tma2");
 }
 

@@ -166,10 +166,21 @@ __device__ __forceinline__ float to_tf32(float x) {
 struct ImageRef { float* img; bool hit; bool settled; };
 ImageRef image_cache_get(const void* wpk, int tag, size_t bytes, cudaStream_t st);
 void image_cache_built(const float* img, cudaStream_t st);
-// B operand image of the stride-1 kernels: [chunk][kh][kw][CIN/4][3*GW][4], tf32-rounded,
-// column group g holds the weights of kd = 2 - g (weight_image.cu)
-int build_stride1_image(const float* wpk, float* img, int CIN, int GW, int chunk, int cout_total,
-                        cudaStream_t st);
+
+// The image of (wpk, tag, bytes) from the cache, or built on a miss: build(img) launches the
+// builder kernel on `st`.  0, or < 0 with the casmvs error set.
+template <typename Build>
+inline int cached_image(const void* wpk, int tag, size_t bytes, cudaStream_t st, ImageRef* ir,
+                        const char* what, Build build) {
+  *ir = image_cache_get(wpk, tag, bytes, st);
+  if (!ir->img) return -2;
+  if (!ir->hit) {
+    build(ir->img);
+    if (int rc = after_launch(what)) return rc;
+    image_cache_built(ir->img, st);
+  }
+  return 0;
+}
 
 }  // namespace tc
 }  // namespace casmvs

@@ -27,8 +27,6 @@
 // (tile, run), hypotheses once, the cost volume is written once, 32 bytes per thread as two 16-byte stores.
 #include <limits.h>
 
-#include <mutex>
-
 #include "k1_common.cuh"
 #include "tma_common.cuh"
 
@@ -434,31 +432,14 @@ warp_var_smem_pg_kernel(const __grid_constant__ CUtensorMap fmap, const float* _
 }
 
 // ---- host side -------------------------------------------------------------------------------
-struct MapEntry { const void* p; int BV, h, w, C, BW, BH; CUtensorMap map; };
-static MapEntry g_maps[32];
-static int g_maps_n = 0, g_maps_next = 0;
-static std::mutex g_maps_mu;
-
-static bool feature_map(CUtensorMap* out, const float* feats, int BV, int h, int w, int C, int BW,
-                        int BH) {
-  std::lock_guard<std::mutex> lock(g_maps_mu);
-  for (int i = 0; i < g_maps_n; ++i) {
-    const MapEntry& e = g_maps[i];
-    if (e.p == feats && e.BV == BV && e.h == h && e.w == w && e.C == C && e.BW == BW && e.BH == BH) {
-      *out = e.map;
-      return true;
-    }
-  }
-  const uint64_t dims[4] = {(uint64_t)C, (uint64_t)w, (uint64_t)h, (uint64_t)BV};
-  const uint64_t str[3] = {(uint64_t)C * 4, (uint64_t)w * C * 4, (uint64_t)h * w * C * 4};
-  const uint32_t box[4] = {(uint32_t)C, (uint32_t)BW, (uint32_t)BH, 1};
-  MapEntry e{feats, BV, h, w, C, BW, BH, {}};
-  if (tma::encode_tiled(&e.map, feats, 4, dims, str, box, C * 4)) return false;
-  g_maps[g_maps_next] = e;
-  g_maps_next = (g_maps_next + 1) % 32;
-  if (g_maps_n < 32) ++g_maps_n;
-  *out = e.map;
-  return true;
+// The features (BV, h, w, C) as {C, w, h, BV}, box {C, BW, BH, 1}, swizzle C*4 bytes.
+static int feature_map(CUtensorMap* out, const float* feats, int BV, int h, int w, int C, int BW,
+                       int BH) {
+  const uint64_t c = C, x = w, y = h, n = BV;
+  const uint32_t bw = BW, bh = BH, bc = C;
+  const tma::MapDesc d{feats, 4, C * 4, {c, x, y, n, 0}, {4 * c, 4 * c * x, 4 * c * x * y, 0},
+                       {bc, bw, bh, 1, 0}, {1, 1, 1, 1, 0}};
+  return tma::encode_map(d, out);
 }
 
 // One launcher for both kernels: NSRC source views, TW x TH pixel tiles.  PG > 0 launches the
@@ -484,7 +465,7 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   static std::atomic<bool> attr_set[2][kMaxDevices];
   if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[blocked ? 1 : 0], "warp_cost")) return rc;
   CUtensorMap map;
-  if (!feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return -2;
+  if (int rc = feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return rc;
   // depth runs: long enough to amortise the staging (a box is re-used by every plane of the
   // run), short enough to keep the sweep inside the margin and >= ~4 CTAs per SM in flight
   const int tiles_x = (w + TW - 1) / TW, tiles_y = (h + TH - 1) / TH;

@@ -1,5 +1,4 @@
-// Tensor-core operand ("weight image") cache shared by the tensor-core convolution kernels, and the
-// image builder of the stride-1 kernel (conv3d_tma.cu).
+// Tensor-core operand ("weight image") cache shared by the tensor-core convolution kernels.
 //
 // The kernels read their B operand from a UMMA-ready image built once per layer from the
 // caller's packed weights ([27][Cin][Cout], casmvs_pack_conv3d_weights).  Images are cached by
@@ -22,35 +21,6 @@
 
 namespace casmvs {
 namespace tc {
-
-// [kh][kw][cq][n = g*GW + co][4], g = 2 - kd; tf32-rounded (to nearest); zero rows for co >= Cout
-// One image per Cout chunk (chunk = blockIdx.y of the conv kernel), `chunk` channels each.
-__global__ void build_image_kernel(const float* __restrict__ wpk, float* __restrict__ img,
-                                   int CIN, int GW, int chunk, int cout_total) {
-  const int CQ = CIN / 4;
-  const int per = 9 * CIN * 3 * GW;
-  const int total = per * (cout_total / chunk);
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
-    const int ck = t / per, i = t - ck * per;
-    const int j = i & 3;
-    const int n = (i >> 2) % (3 * GW);
-    const int r = (i >> 2) / (3 * GW);    // (kh*3+kw)*CQ + cq
-    const int cq = r % CQ, khw = r / CQ;
-    const int g = n / GW, co = n % GW;
-    const int kd = 2 - g;
-    const int ci = cq * 4 + j;
-    float v = 0.f;
-    if (co < chunk)
-      v = to_tf32(__ldg(wpk + ((size_t)(kd * 9 + khw) * CIN + ci) * cout_total + ck * chunk + co));
-    img[t] = v;
-  }
-}
-
-int build_stride1_image(const float* wpk, float* img, int CIN, int GW, int chunk, int cout_total,
-                        cudaStream_t st) {
-  build_image_kernel<<<64, 256, 0, st>>>(wpk, img, CIN, GW, chunk, cout_total);
-  return after_launch("conv3d_tma/build_image");
-}
 
 struct CacheEntry {
   const void* key;
