@@ -113,6 +113,15 @@ SIGNATURES = {
     "casmvs_view_scores_workspace_bytes": (c_size_t, [c_int, c_int, c_longlong]),
     "casmvs_view_scores_fwd": (c_int, [c_void_p] * 4 + [c_int, c_int, c_void_p, c_void_p, c_size_t,
                                                           c_void_p]),
+    "casmvs_mesh_brick_keys": (c_int, [c_void_p, c_int, c_float, c_float, c_void_p, c_void_p,
+                                       c_void_p]),
+    "casmvs_mesh_brick_neighbors": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_mesh_integrate": (c_int, [c_void_p, c_int, c_float, c_float, c_void_p, c_void_p,
+                                      POINTER(c_float), c_int, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]),
+    "casmvs_mesh_count": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
+    "casmvs_mesh_vertices": (c_int, [c_void_p, c_void_p, c_int, c_float] + [c_void_p] * 7),
+    "casmvs_mesh_faces": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
     "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
 }

@@ -31,7 +31,10 @@ proba_XXXX.pfm are written as well).
     python -m casmvsnet_pl_b200.eval_pipeline --dataset_name blendedmvs --split val \
         --root_dir BlendedMVS/dataset_low_res --img_wh 768 576
     python -m casmvsnet_pl_b200.eval_pipeline --dataset_name colmap --root_dir my_capture/dense \
-        --ckpt ckpt.ckpt --img_wh 1152 864 [--depth_interval 192]
+        --ckpt ckpt.ckpt --img_wh 1152 864 [--depth_interval 192] [--mesh [--mesh_voxel S]]
+
+--mesh also fuses each scan's filtered depth maps into a TSDF volume on the GPU and writes the
+marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes changes.
 """
 from __future__ import annotations
 
@@ -375,14 +378,17 @@ class ColmapScan(_CachedScan):
 @torch.no_grad()
 def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
-             dtu_gt=None, dtu_seed=0, save_visual=False):
+             dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
     and thresholded confidence JPEGs of eval.py:230-239 are written too.
     With `dtu_gt` (a DTU ground-truth directory) the fused cloud is also scored by
     dtu_eval.evaluate_scan from the device tensors, the scores are written next to the PLY as
-    <ply>_scores.json when ply_path is given, and (xyz, rgb, scores) is returned."""
+    <ply>_scores.json when ply_path is given, and (xyz, rgb, scores) is returned.
+    With `mesh_path`, the masked refined depth maps are also fused into a TSDF volume and the
+    marching-cubes mesh is written there as a PLY (mesh.py; voxel size `mesh_voxel`, default
+    mesh.default_voxel_size); the other outputs are unchanged."""
     depths, probas = {}, {}
     writer = io.DepthWriter(depth_dir) if depth_dir else None
     for ref, imgs, pm in scan.views(device):
@@ -397,10 +403,24 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
                 io.save_visual(depth_dir, scan.scan, ref, d, p, conf)
     images = scan.fusion_images(list(depths), device)
     proj0 = {v: scan.proj_mats[v][0].numpy() for v in scan.proj_mats}     # finest level (eval.py:108)
+    fused = [] if mesh_path else None
     xyz, rgb = fusion.fuse_scan(scan.metas, depths, probas, images, proj0, conf, min_geo_consistent,
-                                skip, max_ref_views)
+                                skip, max_ref_views, collect=fused)
     if ply_path:
         fusion.write_ply(ply_path, xyz, rgb)
+    if mesh_path:
+        from . import mesh
+        if not fused:
+            raise ValueError(f"{scan.scan}: no reference view was fused, nothing to mesh")
+        verts, colours, faces, st = mesh.mesh_views([f["points"] for f in fused],
+                                                    [f["depth"] for f in fused],
+                                                    [f["image"] for f in fused],
+                                                    [f["P"] for f in fused], mesh_voxel)
+        del fused
+        mesh.write_mesh_ply(mesh_path, verts, colours, faces)
+        log(f"{scan.scan}: mesh at voxel {st['voxel']:.6g}: {st['bricks']} bricks, {st['voxels']} "
+            f"voxels, {st['vertices']} vertices, {st['triangles']} triangles, {st['dropped']} "
+            "points dropped")
     if dtu_gt is None:
         return xyz, rgb
     from . import dtu_eval
@@ -474,7 +494,14 @@ def parse_args(argv=None):
     ap.add_argument("--out", default=None, help="output directory (default results/<dataset_name>)")
     ap.add_argument("--dtu_gt", default=None, help="DTU ground-truth directory: score the fused cloud")
     ap.add_argument("--dtu_seed", type=int, default=0)
+    ap.add_argument("--mesh", action="store_true",
+                    help="also write a TSDF / marching-cubes mesh of each scan to <out>/mesh/<scan>.ply")
+    ap.add_argument("--mesh_voxel", type=float, default=None,
+                    help="voxel size of --mesh in world units (default: 2 x the median pixel "
+                         "footprint at the views' median depth)")
     a = ap.parse_args(argv)
+    if a.mesh_voxel is not None and not a.mesh_voxel > 0:
+        ap.error("--mesh_voxel must be > 0")
     if a.depth_interval is None:
         a.depth_interval = DEFAULT_DEPTH_INTERVAL[a.dataset_name]
     a.out_dir = a.out or os.path.join("results", a.dataset_name)
@@ -499,11 +526,15 @@ def main(argv=None):
         load_checkpoint(model, a.ckpt)
     model = model.eval().cuda()
     os.makedirs(os.path.join(out_dir, "points"), exist_ok=True)
+    if a.mesh:
+        os.makedirs(os.path.join(out_dir, "mesh"), exist_ok=True)
     for scan in open_scans(a):
         out = run_scan(model, scan, a.depth_interval, a.conf, a.min_geo_consistent, a.skip,
                        a.max_ref_views, depth_dir=os.path.join(out_dir, "depth"),
                        ply_path=os.path.join(out_dir, "points", f"{scan.scan}.ply"), dtu_gt=a.dtu_gt,
-                       dtu_seed=a.dtu_seed, save_visual=a.save_visual)
+                       dtu_seed=a.dtu_seed, save_visual=a.save_visual,
+                       mesh_path=os.path.join(out_dir, "mesh", f"{scan.scan}.ply") if a.mesh else None,
+                       mesh_voxel=a.mesh_voxel)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

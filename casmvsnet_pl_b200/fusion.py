@@ -83,13 +83,16 @@ def refine_ref_view(depth_ref, P_world2ref, depth_srcs, P_world2srcs, image_ref=
 
 
 def fuse_scan(metas, depths, probas, images, proj_mats, conf=0.999, min_geo_consistent=5, skip=1,
-              max_ref_views=400):
+              max_ref_views=400, collect=None):
     """The scan loop of eval.py:245-330.  metas: [(ref_vid, [src_vids])] in pair-file order;
     depths[vid] (H,W), probas[vid] (H/4,W/4), images[vid] (H,W,3) float32 RGB CUDA tensors;
     proj_mats[vid] (4,4) finest-level world->pixel.  Like the reference, a view that has been a
     reference view is used in its REFINED form (depth averaged over consistent views, colours
     rounded to uint8 as its PNG round trip does) by later reference views, and a source view's
-    raw depth is cached on first use.  Returns (xyz (N,3) float32, rgb (N,3) uint8) on the GPU."""
+    raw depth is cached on first use.  Returns (xyz (N,3) float32, rgb (N,3) uint8) on the GPU.
+    With `collect` (a list), one dict per fused reference view is appended to it, in order, for
+    meshing: depth (H,W) = refined depth where mask_final else 0, image = image_refined (H,W,3),
+    P (4,4) and points = the world points of every masked pixel (not thinned by `skip`)."""
     image_refined, depth_refined = {}, {}
     vs, cs = [], []
     for ref_vid, src_vids in metas[:max_ref_views]:
@@ -121,6 +124,10 @@ def fuse_scan(metas, depths, probas, images, proj_mats, conf=0.999, min_geo_cons
         m = r["mask_final"]
         vs.append(r["points"][m][::skip])
         cs.append(r["image_refined"][m][::skip])
+        if collect is not None:
+            collect.append(dict(depth=torch.where(m, r["depth_refined"], 0.0),
+                                image=r["image_refined"], P=np.asarray(proj_mats[ref_vid], np.float32),
+                                points=vs[-1] if skip == 1 else r["points"][m]))
     if not vs:
         dev = next(iter(depths.values())).device
         return torch.zeros(0, 3, device=dev), torch.zeros(0, 3, device=dev, dtype=torch.uint8)

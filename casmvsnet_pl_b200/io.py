@@ -146,6 +146,57 @@ def read_ply(filename):
     return out
 
 
+def read_mesh_ply(filename):
+    """A binary little-endian triangle-mesh PLY (as mesh.write_mesh_ply writes it: a vertex
+    element of scalar properties with x, y, z and red, green, blue, then `element face` with
+    `property list uchar int|uint vertex_indices` of triangles) -> (verts (N,3) float32,
+    colours (N,3) uint8, faces (M,3) int32).  Anything else raises ValueError."""
+    with open(filename, "rb") as f:
+        if f.readline().rstrip(b"\r\n") != b"ply":
+            raise ValueError(f"{filename}: not a PLY file")
+        fmt, elements = None, []
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{filename}: PLY header has no end_header")
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = " ".join(tok[1:])
+            elif tok[0] == "element" and len(tok) == 3:
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property" and elements:
+                elements[-1][2].append(tok[1:])
+            else:
+                raise ValueError(f"{filename}: malformed PLY header line {line!r}")
+        if fmt != "binary_little_endian 1.0":
+            raise ValueError(f"{filename}: mesh PLY must be binary_little_endian 1.0, got {fmt}")
+        if [e[0] for e in elements] != ["vertex", "face"]:
+            raise ValueError(f"{filename}: a mesh PLY holds a vertex and then a face element")
+        (_, nv, vprops), (_, nf, fprops) = elements
+        if any(len(p) != 2 or p[0] not in _PLY_TYPES for p in vprops):
+            raise ValueError(f"{filename}: vertex properties must be scalars")
+        vdt = np.dtype([(p[1], "<" + _PLY_TYPES[p[0]]) for p in vprops])
+        if (len(fprops) != 1 or fprops[0][:3] not in (["list", "uchar", "int"], ["list", "uchar", "uint"])
+                or fprops[0][3:] != ["vertex_indices"]):
+            raise ValueError(f"{filename}: faces must be `property list uchar int vertex_indices`")
+        v = np.frombuffer(f.read(nv * vdt.itemsize), dtype=vdt)
+        fdt = np.dtype([("n", "u1"), ("i", "<" + _PLY_TYPES[fprops[0][2]], (3,))])
+        fr = np.frombuffer(f.read(nf * fdt.itemsize), dtype=fdt)
+    if len(v) != nv or len(fr) != nf:
+        raise ValueError(f"{filename}: truncated mesh PLY")
+    if nf and (fr["n"] != 3).any():
+        raise ValueError(f"{filename}: only triangle faces are read")
+    verts = np.stack([v["x"], v["y"], v["z"]], axis=1).astype(np.float32).reshape(-1, 3)
+    names = v.dtype.names
+    colours = (np.stack([v["red"], v["green"], v["blue"]], axis=1).astype(np.uint8)
+               if all(c in names for c in ("red", "green", "blue")) else np.zeros((nv, 3), np.uint8))
+    return verts, colours.reshape(-1, 3), fr["i"].astype(np.int32).reshape(-1, 3)
+
+
 # ------------------------------------------------------------------------------ cameras
 def read_cam_file(filename):
     """MVSNet cam.txt -> (intrinsics (3,3) f32, extrinsics (4,4) f32, depth_min float).

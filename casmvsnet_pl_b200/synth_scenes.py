@@ -18,6 +18,7 @@ n_views > 2 skip it (blendedmvs.py:51-54), and is no other view's source.
 make_colmap writes the same arc of cameras as an undistorted COLMAP workspace (images/ and a
 sparse/ model of points on a known surface, binary and / or text) for eval_pipeline's colmap
 reader; sparse_tracks makes bare sparse models of any size for the view-selection kernel.
+sphere_scene renders analytic depth maps and colours of a sphere (on a plane) for meshing.
 
     python -m casmvsnet_pl_b200.synth_scenes --kind tanks --root TNT --n_views 150 --image_wh 1920 1080
 """
@@ -27,6 +28,7 @@ import argparse
 import os
 
 import numpy as np
+import torch
 
 from . import io
 
@@ -280,6 +282,71 @@ def make_colmap(root, n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, 
     for f in (("bin", "txt") if fmt == "both" else (fmt,)):
         colmap.write_model(os.path.join(root, "sparse"), model, f)
     return model
+
+
+def _look_at(centre, target):
+    """World -> camera rotation (rows x, y, z) of a camera at `centre` looking at `target`, image
+    y pointing down (world z up)."""
+    z = target - centre
+    z /= np.linalg.norm(z)
+    up = np.array([0.0, 0.0, 1.0]) if abs(z[2]) < 0.99 else np.array([0.0, 1.0, 0.0])
+    x = np.cross(-up, z)
+    x /= np.linalg.norm(x)
+    return np.stack([x, np.cross(z, x), z])
+
+
+def sphere_scene(n_views, image_wh, seed=0, radius=1.0, plane=True, device="cpu"):
+    """Analytic depth maps for meshing: a sphere of `radius` at the origin, resting on the square
+    |x|, |y| <= 3 radius of the plane z = -radius when `plane`.  With the plane, the cameras sit on
+    the upper hemisphere (elevation 15..60 degrees), else all around (a Fibonacci sphere), 3.5 to
+    4.5 radii from the origin, aimed at a point near it (seeded jitter).  f = 0.9 W, principal
+    point at the image centre.  Pixels that see nothing have depth 0.  Returns a list of dicts
+    per view: depth (H,W) float32 (z-depth), image (H,W,3) float32 colours 0..255 from the surface
+    position, P (4,4) float32 numpy world -> pixel, points (N,3) float32 of the pixels with depth;
+    tensors on `device` (computed in float64)."""
+    rng = np.random.default_rng(seed)
+    W, H = image_wh
+    K = np.array([[0.9 * W, 0, W / 2], [0, 0.9 * W, H / 2], [0, 0, 1]], dtype=np.float64)
+    f64 = dict(dtype=torch.float64, device=device)
+    ys, xs = torch.meshgrid(torch.arange(H, **f64), torch.arange(W, **f64), indexing="ij")
+    rays_cam = torch.stack([(xs - K[0, 2]) / K[0, 0], (ys - K[1, 2]) / K[1, 1], torch.ones_like(xs)], -1)
+    views = []
+    for i in range(n_views):
+        if plane:
+            el, az = np.radians(rng.uniform(15, 60)), 2 * np.pi * (i + rng.uniform(0, 0.5)) / n_views
+        else:                                   # Fibonacci sphere
+            el = np.arcsin(1 - 2 * (i + 0.5) / n_views)
+            az = i * np.pi * (3 - np.sqrt(5)) + rng.uniform(0, 0.1)
+        dist = radius * rng.uniform(3.5, 4.5)
+        C = dist * np.array([np.cos(el) * np.cos(az), np.cos(el) * np.sin(az), np.sin(el)])
+        R = _look_at(C, rng.uniform(-0.1, 0.1, 3) * radius)
+        d = rays_cam @ torch.as_tensor(R, **f64)         # world directions, camera z component 1
+        o = torch.as_tensor(C, **f64)
+        # sphere: |o + s d|^2 = r^2, nearest root
+        a, b, c = (d * d).sum(-1), 2 * (d @ o), float(o @ o) - radius ** 2
+        disc = b * b - 4 * a * c
+        s_sph = torch.where(disc >= 0, (-b - torch.sqrt(disc.clamp(min=0))) / (2 * a), torch.inf)
+        s_sph = torch.where(s_sph > 0, s_sph, torch.inf)
+        s = s_sph
+        if plane:
+            s_pl = (-radius - o[2]) / d[..., 2]
+            p = o + s_pl[..., None] * d
+            ok = (s_pl > 0) & (p[..., 0].abs() <= 3 * radius) & (p[..., 1].abs() <= 3 * radius)
+            s = torch.minimum(s, torch.where(ok, s_pl, torch.inf))
+        hit = torch.isfinite(s)
+        X = o + torch.where(hit, s, 0.0)[..., None] * d
+        on_sph = hit & (s == s_sph)
+        u = X / radius
+        check = ((torch.floor(2 * u[..., 0]) + torch.floor(2 * u[..., 1])) % 2) * 120 + 60
+        rgb = torch.stack([torch.where(on_sph, 128 + 100 * u[..., 0], check),
+                           torch.where(on_sph, 128 + 100 * u[..., 1], check),
+                           torch.where(on_sph, 128 + 100 * u[..., 2], 0.5 * check)], -1)
+        P = np.eye(4)
+        P[:3, :3], P[:3, 3] = K @ R, K @ (-R @ C)
+        views.append(dict(depth=torch.where(hit, s, 0.0).float(),
+                          image=torch.where(hit[..., None], rgb, 0.0).float(),
+                          P=P.astype(np.float32), points=X[hit].float()))
+    return views
 
 
 def main(argv=None):

@@ -507,6 +507,60 @@ int casmvs_view_scores_fwd(const double* centres, const double* points, const lo
                            const int* track_img, int n_img, int n_pts, double* scores,
                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- TSDF fusion and marching cubes (casmvsnet_pl_b200/mesh.py) -----------------------------
+ * A sparse volume of bricks of 8^3 voxels; voxel ijk is centred at ijk * voxel (world units).
+ * Brick (bx,by,bz) has key ((bx + 2^20) << 42) | ((by + 2^20) << 21) | (bz + 2^20), valid for
+ * -2^20 <= b <= 2^20 - 2.  `keys` is the sorted, unique key list of the allocated bricks (nb
+ * entries, nb <= 2^31 / 1536); voxel v = 512 * brick + (lz * 8 + ly) * 8 + lx, local lx = i - 8 bx.
+ * Per voxel: tsdf (nb*512) f32, weight (nb*512) f32 (a view count), color (nb*512,3) f32.
+ * casmvs_mesh_brick_keys: for each of n points (n,3) f32, the 8 keys (n,8) int64 of the bricks
+ *   holding voxel centres in the cube of half-size trunc around it, per axis indices
+ *   ceil((p - trunc)/voxel) .. floor((p + trunc)/voxel) (float, rounded division); a point
+ *   spanning fewer than 2 bricks on an axis repeats the lower one.  NaN points and points whose
+ *   bricks leave the packable range get INT64_MAX 8 times and add 1 to *dropped (device u64,
+ *   not zeroed here).  voxel <= trunc <= 4 voxel.
+ * casmvs_mesh_brick_neighbors: nbr (nb,7) int32, nbr[b][dx + 2dy + 4dz - 1] = index of brick
+ *   b + (dx,dy,dz) for (dx,dy,dz) in {0,1}^3 \ 0, by binary search; -1 if not allocated.
+ * casmvs_mesh_integrate: Curless & Levoy's projective TSDF of n_views masked depth maps (H,W) f32
+ *   (0 = no depth) with colours image (H,W,3) f32, in view order; depth / image are HOST arrays
+ *   of device pointers, proj a HOST array (n_views,4,4) f32 of world -> pixel matrices P.  Every
+ *   voxel centre X and view, with every float operation rounded to nearest, no contraction:
+ *     z  = ((P20 X + P21 Y) + P22 Z) + P23, likewise uz (row 0) and vz (row 1); skip unless z > 0
+ *     px = floor(uz / z + 0.5), py = floor(vz / z + 0.5); skip outside the image or if D = 0
+ *     sdf = D - z; skip unless sdf >= -trunc;  t = min(1, sdf / trunc)
+ *     tsdf = (tsdf * w + t) / (w + 1);  color_c = (color_c * w + image_c) / (w + 1);  w = w + 1
+ *   One thread per voxel, views batched 8 per launch: deterministic, no atomics.  The volume is
+ *   not cleared: start from zeros.
+ * Marching cubes over the cells (lower corner v, corners v + {0,1}^3) whose 8 corners are
+ * allocated with weight > 0; a corner is inside when tsdf < 0; the case table is
+ * csrc/mc_table.h (generated, see casmvsnet_pl_b200/mc_table.py).  Voxel v owns the edges
+ * e = 3v + axis from v to v + unit(axis).
+ * casmvs_mesh_count: cases (nb*512) u8 and tri_count (nb*512) int32 per cell (0 when not meshed);
+ *   edge_used (nb*512*3) int32 = 1 for the crossing edges of meshed cells, else 0 (zeroed here).
+ * casmvs_mesh_vertices: with edge_scan = inclusive scan of edge_used, the vertex of used edge q is
+ *   number edge_scan[q] - 1: along the axis, t = s0 / (s0 - s1) of the end values in double,
+ *   position (index + t) * voxel in double rounded once to f32 (other axes index * voxel);
+ *   colour c0 + t (c1 - c0) in double, rint (half even), clamped to 0..255.  verts (N,3) f32,
+ *   vcolor (N,3) u8.
+ * casmvs_mesh_faces: with tri_scan = inclusive scan of tri_count, the triangles of cell v in table
+ *   order from row tri_scan[v] - tri_count[v] of faces (M,3) int32 (vertex numbers); counter-
+ *   clockwise seen from outside (the normal points from tsdf < 0 towards tsdf >= 0).
+ * Empty volumes (nb = 0) launch nothing. */
+int casmvs_mesh_brick_keys(const float* points, int n, float voxel, float trunc, long long* keys,
+                           unsigned long long* dropped, void* stream);
+int casmvs_mesh_brick_neighbors(const long long* keys, int nb, int* nbr, void* stream);
+int casmvs_mesh_integrate(const long long* keys, int nb, float voxel, float trunc,
+                          const float* const* depth, const float* const* image, const float* proj,
+                          int n_views, int H, int W, float* tsdf, float* weight, float* color,
+                          void* stream);
+int casmvs_mesh_count(const int* nbr, int nb, const float* tsdf, const float* weight,
+                      unsigned char* cases, int* tri_count, int* edge_used, void* stream);
+int casmvs_mesh_vertices(const long long* keys, const int* nbr, int nb, float voxel,
+                         const float* tsdf, const float* color, const int* edge_used,
+                         const int* edge_scan, float* verts, unsigned char* vcolor, void* stream);
+int casmvs_mesh_faces(const int* nbr, int nb, const unsigned char* cases, const int* tri_count,
+                      const int* tri_scan, const int* edge_scan, int* faces, void* stream);
+
 /* ---- layout helpers ------------------------------------------------------ */
 /* (N,C,S) -> (N,S,C) and back, S = product of spatial dims. */
 int casmvs_nchw_to_nhwc(const float* in, float* out, int N, int C, size_t S, void* stream);
