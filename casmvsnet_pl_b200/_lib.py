@@ -122,6 +122,12 @@ SIGNATURES = {
     "casmvs_mesh_count": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
     "casmvs_mesh_vertices": (c_int, [c_void_p, c_void_p, c_int, c_float] + [c_void_p] * 7),
     "casmvs_mesh_faces": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
+    "casmvs_render_points_fwd": (c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
+                                         c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_render_mesh_workspace_bytes": (c_size_t, [c_int]),
+    "casmvs_render_mesh_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, POINTER(c_float),
+                                       POINTER(c_float), c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                       c_void_p, c_void_p, c_void_p]),
     "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
 }

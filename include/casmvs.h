@@ -561,6 +561,44 @@ int casmvs_mesh_vertices(const long long* keys, const int* nbr, int nb, float vo
 int casmvs_mesh_faces(const int* nbr, int nb, const unsigned char* cases, const int* tri_count,
                       const int* tri_scan, const int* edge_scan, int* faces, void* stream);
 
+/* ---- headless rendering of clouds and meshes (casmvsnet_pl_b200/render.py) -----------------
+ * P is a HOST array of 16 floats, row-major, world -> pixel (rows 0..2 used): every float
+ * operation below is rounded to nearest, no contraction, in the order written.
+ *   w = ((P20 X + P21 Y) + P22 Z) + P23, likewise x (row 0) and y (row 1); u = x / w, v = y / w.
+ * A vertex or point is drawn only when X, Y, Z, w, u, v are finite and w > 0; there is no near-
+ * plane clipping, so a triangle with one vertex at w <= 0 is skipped whole.  Pixel (px, py) has
+ * its centre at the integers (px, py), row-major.  zbuf (H*W) u64 is caller-provided and filled
+ * here: each covered pixel takes atomicMin of key = (float bits of w) << 32 | primitive index, so
+ * the nearest primitive wins and an exact depth tie goes to the lower index (deterministic).
+ * image (H,W,3) u8 gets the winner's colour or the background (128, 128, 255); depth (H,W) f32
+ * the winner's w, 0 where nothing is drawn.  1 <= W, H <= 16384.
+ * casmvs_render_points_fwd: xyz (n,3) f32, rgb (n,3) u8, n < 2^32.  A point of size s (1..64)
+ *   covers the pixel centres in [u - s/2, u + s/2) x [v - s/2, v + s/2): px from
+ *   ceil(u - s/2) to ceil(u + s/2) - 1, likewise py.
+ * casmvs_render_mesh_fwd: verts (n_vertices,3) f32, colours (n_vertices,3) u8, faces (n_faces,3)
+ *   int32; eye a HOST array of 3 floats (the camera centre).  Both windings are drawn.  Face t is
+ *   skipped unless its area a = e(u0,v0, u1,v1, u2,v2) != 0, with
+ *     e(ax,ay, bx,by, px,py) = (bx - ax)(py - ay) - (by - ay)(px - ax).
+ *   It covers pixel (px, py) of its box [ceil(min u), floor(max u)] x [ceil(min v), floor(max v)]
+ *   when e0 = e(1,2,p), e1 = e(2,0,p), e2 = e(0,1,p) are all >= 0 or all <= 0; then
+ *     q_k = e_k / w_k, den = (q0 + q1) + q2, depth = ((e0 + e1) + e2) / den (drawn if > 0, finite)
+ *     colour_c = floor((((q0 c0 + q1 c1) + q2 c2) / den) * shade + 0.5), clamped to 0..255,
+ *     shade = 0.3 + 0.7 min(1, |n.d| / (sqrt(n.n) sqrt(d.d))) (0.3 when the divisor is 0),
+ *     n = (x1 - x0) x (x2 - x0), d = ((x0 + x1) + x2) / 3 - eye, dots summed ((a0 + a1) + a2).
+ *   A face index outside [0, n_vertices) is caught on the device: nothing is read through it and
+ *   the call fails.  The call synchronises `stream` once, to read that flag.  Boxes up to 8x8
+ *   pixels are rasterised by one thread per face, larger ones by a CTA each.
+ * casmvs_render_mesh_workspace_bytes: the workspace (4-byte aligned) for n_faces faces. */
+int casmvs_render_points_fwd(const float* xyz, const unsigned char* rgb, long long n, const float* P,
+                             int W, int H, int point_size, unsigned long long* zbuf,
+                             unsigned char* image, float* depth, void* stream);
+size_t casmvs_render_mesh_workspace_bytes(int n_faces);
+int casmvs_render_mesh_fwd(const float* verts, const unsigned char* colours, int n_vertices,
+                           const int* faces, int n_faces, const float* P, const float* eye, int W,
+                           int H, unsigned long long* zbuf, void* workspace,
+                           size_t workspace_bytes, unsigned char* image, float* depth,
+                           void* stream);
+
 /* ---- layout helpers ------------------------------------------------------ */
 /* (N,C,S) -> (N,S,C) and back, S = product of spatial dims. */
 int casmvs_nchw_to_nhwc(const float* in, float* out, int N, int C, size_t S, void* stream);
