@@ -110,6 +110,20 @@ SIGNATURES = {
     "casmvs_pcd_capped_nn": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                      POINTER(c_double), c_double, POINTER(c_int), POINTER(c_double),
                                      POINTER(c_double), c_double, c_void_p, c_void_p]),
+    "casmvs_pcd_capped_nn_index": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                           c_void_p, POINTER(c_double), c_double, POINTER(c_int),
+                                           POINTER(c_double), POINTER(c_double), c_double,
+                                           c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_tnt_crop_blocks": (c_int, [c_int]),
+    "casmvs_tnt_transform_crop": (c_int, [c_void_p, c_int, POINTER(c_double), c_int, c_double,
+                                          c_double, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                          c_void_p]),
+    "casmvs_tnt_compact": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                   c_void_p]),
+    "casmvs_tnt_voxel_mean": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_tnt_icp_workspace_bytes": (c_size_t, [c_int]),
+    "casmvs_tnt_icp_moments": (c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_double),
+                                       c_void_p, c_void_p, c_size_t, c_void_p]),
     "casmvs_view_scores_workspace_bytes": (c_size_t, [c_int, c_int, c_longlong]),
     "casmvs_view_scores_fwd": (c_int, [c_void_p] * 4 + [c_int, c_int, c_void_p, c_void_p, c_size_t,
                                                           c_void_p]),

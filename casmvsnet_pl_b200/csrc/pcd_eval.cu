@@ -174,34 +174,59 @@ __device__ __forceinline__ double box_d2(const double q[3], double bx, double by
   return d2;
 }
 
+// kIndex == false is the DTU search (casmvs_pcd_capped_nn).  kIndex == true also returns the
+// original index of the nearest target (tgt_index maps the key-sorted targets back): it evaluates
+// the distance with explicit round-to-nearest intrinsics in the same order, breaks an exact tie
+// towards the lower original index and prunes only boxes strictly farther than the best distance,
+// so that a tied target in another cell is still visited.
+template <bool kIndex>
 __device__ __forceinline__ void scan_super(const NNGrid& G, const double q[3], int sx, int sy,
                                            int sz, const int* __restrict__ super_begin,
                                            const int64_t* __restrict__ cell_keys,
                                            const int* __restrict__ cell_start,
-                                           const float* __restrict__ tgt, double& best2) {
+                                           const float* __restrict__ tgt,
+                                           const int64_t* __restrict__ tgt_index, double& best2,
+                                           int64_t& best_i) {
   const int s = (sx * G.S[1] + sy) * G.S[2] + sz;
   const int c0 = __ldg(super_begin + s), c1 = __ldg(super_begin + s + 1);
   if (c0 == c1) return;
   const double bx = G.org[0] + sx * G.hs, by = G.org[1] + sy * G.hs, bz = G.org[2] + sz * G.hs;
-  if (box_d2(q, bx, by, bz, G.hs) >= best2) return;
+  const double sd2 = box_d2(q, bx, by, bz, G.hs);
+  if (kIndex ? sd2 > best2 : sd2 >= best2) return;
   for (int c = c0; c < c1; ++c) {
     const int l = (int)(__ldg(cell_keys + c) & 511);
-    if (box_d2(q, bx + (l >> 6) * G.h, by + ((l >> 3) & 7) * G.h, bz + (l & 7) * G.h, G.h) >= best2)
-      continue;
+    const double cd2 = box_d2(q, bx + (l >> 6) * G.h, by + ((l >> 3) & 7) * G.h, bz + (l & 7) * G.h, G.h);
+    if (kIndex ? cd2 > best2 : cd2 >= best2) continue;
     for (int t = __ldg(cell_start + c), e = __ldg(cell_start + c + 1); t < e; ++t) {
-      const double dx = (double)__ldg(tgt + 3 * (size_t)t) - q[0];
-      const double dy = (double)__ldg(tgt + 3 * (size_t)t + 1) - q[1];
-      const double dz = (double)__ldg(tgt + 3 * (size_t)t + 2) - q[2];
-      best2 = fmin(best2, dx * dx + dy * dy + dz * dz);
+      if constexpr (kIndex) {
+        const double dx = __dsub_rn((double)__ldg(tgt + 3 * (size_t)t), q[0]);
+        const double dy = __dsub_rn((double)__ldg(tgt + 3 * (size_t)t + 1), q[1]);
+        const double dz = __dsub_rn((double)__ldg(tgt + 3 * (size_t)t + 2), q[2]);
+        const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+        if (d2 <= best2) {
+          const int64_t id = __ldg(tgt_index + t);
+          if (d2 < best2 || id < best_i) {
+            best2 = d2;
+            best_i = id;
+          }
+        }
+      } else {
+        const double dx = (double)__ldg(tgt + 3 * (size_t)t) - q[0];
+        const double dy = (double)__ldg(tgt + 3 * (size_t)t + 1) - q[1];
+        const double dz = (double)__ldg(tgt + 3 * (size_t)t + 2) - q[2];
+        best2 = fmin(best2, dx * dx + dy * dy + dz * dz);
+      }
     }
   }
 }
 
-__global__ void __launch_bounds__(128)
+template <bool kIndex>
+__global__ void __launch_bounds__(128, kIndex ? 8 : 0)
 pcd_capped_nn_kernel(const __grid_constant__ NNGrid G, const float* __restrict__ qry, int nq,
                      const float* __restrict__ tgt, const int64_t* __restrict__ cell_keys,
                      const int* __restrict__ cell_start, const int* __restrict__ super_begin,
-                     double* __restrict__ dist) {
+                     const int64_t* __restrict__ tgt_index, double* __restrict__ dist,
+                     int64_t* __restrict__ index) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nq) return;
   const double q[3] = {(double)__ldg(qry + 3 * (size_t)i), (double)__ldg(qry + 3 * (size_t)i + 1),
@@ -211,6 +236,7 @@ pcd_capped_nn_kernel(const __grid_constant__ NNGrid G, const float* __restrict__
   for (int a = 0; a < 3; ++a) inside = inside && q[a] >= G.lo[a] && q[a] < G.hi[a];
   if (!inside || super_begin == nullptr) {       // outside every block, or no target at all
     dist[i] = G.cap;
+    if (kIndex) index[i] = -1;
     return;
   }
   // the target grid spans the block grid widened by the cap, so an inside query is in it
@@ -219,11 +245,12 @@ pcd_capped_nn_kernel(const __grid_constant__ NNGrid G, const float* __restrict__
   for (int a = 0; a < 3; ++a)
     c[a] = min(max((int)floor((q[a] - G.org[a]) / G.hs), 0), G.S[a] - 1);
   double best2 = G.cap2;
+  int64_t best_i = INT64_MAX;
   const int rmax = max(G.S[0], max(G.S[1], G.S[2]));
   for (int R = 0; R <= rmax; ++R) {
     // every cell of ring R is at least (R - 1) super edges away along one axis
     const double lb = (R - 1) * G.hs - 1e-6;
-    if (R >= 2 && lb * lb >= best2) break;
+    if (R >= 2 && (kIndex ? lb * lb > best2 : lb * lb >= best2)) break;
     const int x0 = max(c[0] - R, 0), x1 = min(c[0] + R, G.S[0] - 1);
     const int y0 = max(c[1] - R, 0), y1 = min(c[1] + R, G.S[1] - 1);
     for (int x = x0; x <= x1; ++x) {
@@ -233,17 +260,21 @@ pcd_capped_nn_kernel(const __grid_constant__ NNGrid G, const float* __restrict__
         if (face) {
           const int z0 = max(c[2] - R, 0), z1 = min(c[2] + R, G.S[2] - 1);
           for (int z = z0; z <= z1; ++z)
-            scan_super(G, q, x, y, z, super_begin, cell_keys, cell_start, tgt, best2);
+            scan_super<kIndex>(G, q, x, y, z, super_begin, cell_keys, cell_start, tgt, tgt_index,
+                               best2, best_i);
         } else {
           if (c[2] - R >= 0)
-            scan_super(G, q, x, y, c[2] - R, super_begin, cell_keys, cell_start, tgt, best2);
+            scan_super<kIndex>(G, q, x, y, c[2] - R, super_begin, cell_keys, cell_start, tgt,
+                               tgt_index, best2, best_i);
           if (R > 0 && c[2] + R < G.S[2])
-            scan_super(G, q, x, y, c[2] + R, super_begin, cell_keys, cell_start, tgt, best2);
+            scan_super<kIndex>(G, q, x, y, c[2] + R, super_begin, cell_keys, cell_start, tgt,
+                               tgt_index, best2, best_i);
         }
       }
     }
   }
   dist[i] = best2 < G.cap2 ? sqrt(best2) : G.cap;
+  if (kIndex) index[i] = best2 < G.cap2 ? best_i : -1;
 }
 
 }  // namespace casmvs
@@ -319,35 +350,66 @@ extern "C" int casmvs_pcd_thin_round(const float* points, const int* rank, const
   return after_launch("pcd_thin_remove");
 }
 
-extern "C" int casmvs_pcd_capped_nn(const float* queries, int nq, const float* targets,
-                                    const int64_t* cell_keys, const int* cell_start, int ncells,
-                                    const int* super_begin, const double* origin3, double h,
-                                    const int* super_dims3, const double* box_lo3,
-                                    const double* box_hi3, double cap, double* dist,
-                                    void* stream) {
-  CASMVS_REQUIRE(nq >= 0 && ncells >= 0, "pcd_capped_nn: bad sizes");
-  CASMVS_REQUIRE(origin3 && super_dims3 && box_lo3 && box_hi3, "pcd_capped_nn: null host array");
-  CASMVS_REQUIRE(h > 0.0 && cap > 0.0, "pcd_capped_nn: h and cap must be > 0");
-  CASMVS_REQUIRE(nq == 0 || (queries && dist), "pcd_capped_nn: null pointer");
+static int capped_nn_launch(const char* what, const float* queries, int nq, const float* targets,
+                            const int64_t* cell_keys, const int* cell_start, int ncells,
+                            const int* super_begin, const double* origin3, double h,
+                            const int* super_dims3, const double* box_lo3, const double* box_hi3,
+                            double cap, const int64_t* target_index, double* dist, int64_t* index,
+                            void* stream) {
+  CASMVS_REQUIRE(nq >= 0 && ncells >= 0, "%s: bad sizes", what);
+  CASMVS_REQUIRE(origin3 && super_dims3 && box_lo3 && box_hi3, "%s: null host array", what);
+  CASMVS_REQUIRE(h > 0.0 && cap > 0.0, "%s: h and cap must be > 0", what);
+  CASMVS_REQUIRE(nq == 0 || (queries && dist), "%s: null pointer", what);
   CASMVS_REQUIRE(ncells == 0 || (targets && cell_keys && cell_start && super_begin),
-                 "pcd_capped_nn: null target pointer");
+                 "%s: null target pointer", what);
   NNGrid G;
   size_t nsuper = 1;
   for (int a = 0; a < 3; ++a) {
-    CASMVS_REQUIRE(super_dims3[a] > 0 && super_dims3[a] < (1 << 17), "pcd_capped_nn: bad super dims");
+    CASMVS_REQUIRE(super_dims3[a] > 0 && super_dims3[a] < (1 << 17), "%s: bad super dims", what);
     nsuper *= (size_t)super_dims3[a];
     G.org[a] = origin3[a];
     G.S[a] = super_dims3[a];
     G.lo[a] = box_lo3[a];
     G.hi[a] = box_hi3[a];
   }
-  CASMVS_REQUIRE(nsuper < (1u << 31), "pcd_capped_nn: too many super cells");
+  CASMVS_REQUIRE(nsuper < (1u << 31), "%s: too many super cells", what);
   G.h = h;
   G.hs = 8.0 * h;
   G.cap = cap;
   G.cap2 = cap * cap;
   if (nq == 0) return 0;
-  pcd_capped_nn_kernel<<<(nq + 127) / 128, 128, 0, as_stream(stream)>>>(
-      G, queries, nq, targets, cell_keys, cell_start, ncells ? super_begin : nullptr, dist);
-  return after_launch("pcd_capped_nn");
+  const int* sb = ncells ? super_begin : nullptr;
+  if (index) {
+    pcd_capped_nn_kernel<true><<<(nq + 127) / 128, 128, 0, as_stream(stream)>>>(
+        G, queries, nq, targets, cell_keys, cell_start, sb, target_index, dist, index);
+  } else {
+    pcd_capped_nn_kernel<false><<<(nq + 127) / 128, 128, 0, as_stream(stream)>>>(
+        G, queries, nq, targets, cell_keys, cell_start, sb, nullptr, dist, nullptr);
+  }
+  return after_launch(what);
+}
+
+extern "C" int casmvs_pcd_capped_nn(const float* queries, int nq, const float* targets,
+                                    const int64_t* cell_keys, const int* cell_start, int ncells,
+                                    const int* super_begin, const double* origin3, double h,
+                                    const int* super_dims3, const double* box_lo3,
+                                    const double* box_hi3, double cap, double* dist,
+                                    void* stream) {
+  return capped_nn_launch("pcd_capped_nn", queries, nq, targets, cell_keys, cell_start, ncells,
+                          super_begin, origin3, h, super_dims3, box_lo3, box_hi3, cap, nullptr,
+                          dist, nullptr, stream);
+}
+
+extern "C" int casmvs_pcd_capped_nn_index(const float* queries, int nq, const float* targets,
+                                          const int64_t* cell_keys, const int* cell_start,
+                                          int ncells, const int* super_begin,
+                                          const double* origin3, double h, const int* super_dims3,
+                                          const double* box_lo3, const double* box_hi3, double cap,
+                                          const int64_t* target_index, double* dist,
+                                          int64_t* index, void* stream) {
+  CASMVS_REQUIRE(nq == 0 || index, "pcd_capped_nn_index: null index pointer");
+  CASMVS_REQUIRE(ncells == 0 || target_index, "pcd_capped_nn_index: null target_index pointer");
+  return capped_nn_launch("pcd_capped_nn_index", queries, nq, targets, cell_keys, cell_start,
+                          ncells, super_begin, origin3, h, super_dims3, box_lo3, box_hi3, cap,
+                          target_index, dist, index, stream);
 }

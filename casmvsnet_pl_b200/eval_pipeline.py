@@ -378,7 +378,8 @@ class ColmapScan(_CachedScan):
 @torch.no_grad()
 def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
-             dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print):
+             dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
+             tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -388,7 +389,11 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     <ply>_scores.json when ply_path is given, and (xyz, rgb, scores) is returned.
     With `mesh_path`, the masked refined depth maps are also fused into a TSDF volume and the
     marching-cubes mesh is written there as a PLY (mesh.py; voxel size `mesh_voxel`, default
-    mesh.default_voxel_size); the other outputs are unchanged."""
+    mesh.default_voxel_size); the other outputs are unchanged.
+    With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
+    cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
+    recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
+    is given, and (xyz, rgb, scores) is returned."""
     depths, probas = {}, {}
     writer = io.DepthWriter(depth_dir) if depth_dir else None
     for ref, imgs, pm in scan.views(device):
@@ -421,6 +426,13 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         log(f"{scan.scan}: mesh at voxel {st['voxel']:.6g}: {st['bricks']} bricks, {st['voxels']} "
             f"voxels, {st['vertices']} vertices, {st['triangles']} triangles, {st['dropped']} "
             "points dropped")
+    if tnt_gt is not None:
+        from . import tnt_eval
+        scores = tnt_eval.evaluate_scene(xyz, run_dir, tnt_gt, scan.scan, tnt_tau, tnt_seed,
+                                         images=tnt_images)
+        if ply_path:
+            tnt_eval.write_json(os.path.splitext(ply_path)[0] + "_tnt.json", scores)
+        return xyz, rgb, scores
     if dtu_gt is None:
         return xyz, rgb
     from . import dtu_eval
@@ -494,6 +506,14 @@ def parse_args(argv=None):
     ap.add_argument("--out", default=None, help="output directory (default results/<dataset_name>)")
     ap.add_argument("--dtu_gt", default=None, help="DTU ground-truth directory: score the fused cloud")
     ap.add_argument("--dtu_seed", type=int, default=0)
+    ap.add_argument("--tnt_gt", default=None,
+                    help="colmap: Tanks and Temples ground-truth directory holding <gt>/<scan>/: "
+                         "score the fused cloud (points/<scan>_tnt.json)")
+    ap.add_argument("--tnt_images", default=None,
+                    help="with --tnt_gt: the complete image directory, to pair cameras by name")
+    ap.add_argument("--tnt_tau", type=float, default=None,
+                    help="with --tnt_gt: tau for a scene outside the seven training scenes")
+    ap.add_argument("--tnt_seed", type=int, default=0)
     ap.add_argument("--mesh", action="store_true",
                     help="also write a TSDF / marching-cubes mesh of each scan to <out>/mesh/<scan>.ply")
     ap.add_argument("--mesh_voxel", type=float, default=None,
@@ -512,6 +532,8 @@ def main(argv=None):
     a = parse_args(argv)
     if a.dtu_gt is not None and a.dataset_name != "dtu":
         raise SystemExit("--dtu_gt applies to dtu only")
+    if a.tnt_gt is not None and a.dataset_name != "colmap":
+        raise SystemExit("--tnt_gt applies to colmap only")
     if a.dataset_name == "dtu" and not a.scan:
         raise SystemExit("--scan is required for dtu")
     splits = {"tanks": TanksTestScan.SCANS, "blendedmvs": BlendedMVSTestScan.SPLITS}.get(a.dataset_name)
@@ -529,15 +551,22 @@ def main(argv=None):
     if a.mesh:
         os.makedirs(os.path.join(out_dir, "mesh"), exist_ok=True)
     for scan in open_scans(a):
+        tnt = {}
+        if a.tnt_gt is not None:
+            tnt = dict(tnt_gt=a.tnt_gt, tnt_images=a.tnt_images, tnt_tau=a.tnt_tau,
+                       tnt_seed=a.tnt_seed, run_dir=os.path.join(out_dir, scan.scan))
         out = run_scan(model, scan, a.depth_interval, a.conf, a.min_geo_consistent, a.skip,
                        a.max_ref_views, depth_dir=os.path.join(out_dir, "depth"),
                        ply_path=os.path.join(out_dir, "points", f"{scan.scan}.ply"), dtu_gt=a.dtu_gt,
                        dtu_seed=a.dtu_seed, save_visual=a.save_visual,
                        mesh_path=os.path.join(out_dir, "mesh", f"{scan.scan}.ply") if a.mesh else None,
-                       mesh_voxel=a.mesh_voxel)
+                       mesh_voxel=a.mesh_voxel, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt
+            print(_fmt(out[2]))
+        if a.tnt_gt is not None:
+            from .tnt_eval import _fmt
             print(_fmt(out[2]))
 
 

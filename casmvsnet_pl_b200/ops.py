@@ -672,3 +672,108 @@ def pcd_capped_nn(queries, targets, cell_keys, cell_start, super_begin, origin, 
         (ctypes.c_int * 3)(*map(int, super_dims)), d3(*map(float, box_lo)), d3(*map(float, box_hi)),
         float(cap), _ptr(dist), _stream()), "pcd_capped_nn")
     return dist
+
+
+@_on_tensor_device
+def pcd_capped_nn_index(queries, targets, cell_keys, cell_start, super_begin, origin, h, super_dims,
+                        box_lo, box_hi, cap, target_index):
+    """pcd_capped_nn that also returns the original index (target_index of the key-sorted
+    target, int64) of the nearest target, -1 where none lies strictly closer than cap
+    (casmvs_pcd_capped_nn_index): -> (dist float64, index int64)."""
+    q = _points("queries", queries)
+    t = _points("targets", targets)
+    _require_cuda_typed(queries=(q, torch.float32), targets=(t, torch.float32),
+                        cell_keys=(cell_keys, torch.int64), cell_start=(cell_start, torch.int32),
+                        super_begin=(super_begin, torch.int32),
+                        target_index=(target_index, torch.int64))
+    ncells = cell_keys.shape[0]
+    if cell_start.shape[0] != ncells + 1 or super_begin.shape[0] != math.prod(int(v) for v in super_dims) + 1:
+        raise _lib.CasMVSError("cell_start / super_begin sizes do not match the grid")
+    if target_index.shape != (t.shape[0],):
+        raise _lib.CasMVSError("target_index must hold one index per target")
+    dist = torch.empty(q.shape[0], device=q.device, dtype=torch.float64)
+    index = torch.empty(q.shape[0], device=q.device, dtype=torch.int64)
+    d3 = ctypes.c_double * 3
+    check(_lib.load().casmvs_pcd_capped_nn_index(
+        _ptr(q), q.shape[0], _ptr(t), _ptr(cell_keys.contiguous()), _ptr(cell_start.contiguous()),
+        ncells, _ptr(super_begin.contiguous()), d3(*map(float, origin)), float(h),
+        (ctypes.c_int * 3)(*map(int, super_dims)), d3(*map(float, box_lo)), d3(*map(float, box_hi)),
+        float(cap), _ptr(target_index.contiguous()), _ptr(dist), _ptr(index), _stream()),
+          "pcd_capped_nn_index")
+    return dist, index
+
+
+# ------------------------------------------------------------------ Tanks and Temples scoring
+@_on_tensor_device
+def tnt_transform_crop(points, T=None, crop=None):
+    """float32(T p) of every point of an (N,3) float32 cloud (casmvs_tnt_transform_crop; T a 4x4
+    or None for the points as they are).  With crop = (axis, axis_min, axis_max, polygon (m,2)
+    float64 CUDA tensor of (u, v) vertices) -> the transformed points inside the crop volume in
+    input order and their input indices (int64); without -> the transformed points."""
+    pts = _points("points", points)
+    _require_cuda_typed(points=(pts, torch.float32))
+    n = pts.shape[0]
+    lib = _lib.load()
+    out = torch.empty_like(pts)
+    Tp = None
+    if T is not None:
+        rows = torch.as_tensor(T, dtype=torch.float64).reshape(4, 4)[:3].reshape(-1).tolist()
+        Tp = (ctypes.c_double * 12)(*rows)
+    if crop is None:
+        check(lib.casmvs_tnt_transform_crop(_ptr(pts), n, Tp, -1, 0.0, 0.0, None, 0, _ptr(out),
+                                            None, None, _stream()), "tnt_transform_crop")
+        return out
+    axis, amin, amax, poly = crop
+    _require_cuda_typed(points=(pts, torch.float32), polygon=(poly, torch.float64))
+    poly = poly.contiguous()
+    if poly.dim() != 2 or poly.shape[1] != 2:
+        raise _lib.CasMVSError("polygon must be an (m,2) tensor")
+    nb = lib.casmvs_tnt_crop_blocks(n)
+    mask = torch.empty(n, device=pts.device, dtype=torch.uint8)
+    counts = torch.empty(max(nb, 1), device=pts.device, dtype=torch.int32)
+    check(lib.casmvs_tnt_transform_crop(_ptr(pts), n, Tp, int(axis), float(amin), float(amax),
+                                        _ptr(poly), poly.shape[0], _ptr(out), _ptr(mask),
+                                        _ptr(counts), _stream()), "tnt_transform_crop")
+    offsets = torch.zeros(max(nb, 1) + 1, device=pts.device, dtype=torch.int64)
+    torch.cumsum(counts[:nb], 0, out=offsets[1:nb + 1])
+    kept = int(offsets[nb].item()) if nb else 0
+    res = torch.empty((kept, 3), device=pts.device, dtype=torch.float32)
+    idx = torch.empty(kept, device=pts.device, dtype=torch.int64)
+    check(lib.casmvs_tnt_compact(_ptr(out), _ptr(mask), n, _ptr(offsets), _ptr(res), _ptr(idx),
+                                 _stream()), "tnt_compact")
+    return res, idx
+
+
+@_on_tensor_device
+def tnt_voxel_mean(points, order, voxel_start):
+    """float32 mean of each voxel's points order[voxel_start[v]:voxel_start[v+1]], summed in double
+    in that order (casmvs_tnt_voxel_mean)."""
+    pts = _points("points", points)
+    _require_cuda_typed(points=(pts, torch.float32), order=(order, torch.int64),
+                        voxel_start=(voxel_start, torch.int32))
+    nv = voxel_start.shape[0] - 1
+    out = torch.empty((max(nv, 0), 3), device=pts.device, dtype=torch.float32)
+    check(_lib.load().casmvs_tnt_voxel_mean(_ptr(pts), _ptr(order.contiguous()),
+                                            _ptr(voxel_start.contiguous()), max(nv, 0), _ptr(out),
+                                            _stream()), "tnt_voxel_mean")
+    return out
+
+
+@_on_tensor_device
+def tnt_icp_moments(src, tgt, index, origin):
+    """The 18 float64 correspondence moments of casmvs_tnt_icp_moments (device tensor):
+    count, sum d^2, sum s', sum t', sum |s'|^2, sum t' s'^T (row-major) about `origin`."""
+    s = _points("src", src)
+    t = _points("tgt", tgt)
+    _require_cuda_typed(src=(s, torch.float32), tgt=(t, torch.float32), index=(index, torch.int64))
+    if index.shape != (s.shape[0],):
+        raise _lib.CasMVSError("index must hold one entry per source point")
+    lib = _lib.load()
+    n = s.shape[0]
+    nbytes = lib.casmvs_tnt_icp_workspace_bytes(n)
+    ws = torch.empty(nbytes // 8, device=s.device, dtype=torch.float64)
+    out = torch.empty(18, device=s.device, dtype=torch.float64)
+    check(lib.casmvs_tnt_icp_moments(_ptr(s), n, _ptr(t), _ptr(index.contiguous()),
+                                     (ctypes.c_double * 3)(*map(float, origin)), _ptr(out), _ptr(ws),
+                                     nbytes, _stream()), "tnt_icp_moments")
+    return out

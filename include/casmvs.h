@@ -483,6 +483,50 @@ int casmvs_pcd_capped_nn(const float* queries, int nq, const float* targets,
                          const int* super_begin, const double* origin3, double h,
                          const int* super_dims3, const double* box_lo3, const double* box_hi3,
                          double cap, double* dist, void* stream);
+/* casmvs_pcd_capped_nn_index: casmvs_pcd_capped_nn that also writes index[i], the original index
+ *   (target_index[k] of the key-sorted target k) of the nearest target, or -1 with dist = cap
+ *   when no target lies strictly closer than cap.  d^2 = (dx*dx + dy*dy) + dz*dz, dx = t - q, in
+ *   double from the float32 coordinates with every operation rounded to nearest (no
+ *   contraction); dist = sqrt(d^2).  An exact tie goes to the lower original index. */
+int casmvs_pcd_capped_nn_index(const float* queries, int nq, const float* targets,
+                               const int64_t* cell_keys, const int* cell_start, int ncells,
+                               const int* super_begin, const double* origin3, double h,
+                               const int* super_dims3, const double* box_lo3,
+                               const double* box_hi3, double cap, const int64_t* target_index,
+                               double* dist, int64_t* index, void* stream);
+
+/* ---- Tanks and Temples scoring (casmvsnet_pl_b200/tnt_eval.py) ------------------------------
+ * Every double operation below is rounded to nearest, no contraction, in the order written.
+ * casmvs_tnt_transform_crop: out[i] = p_i, or with T (a HOST array of 12 doubles, rows 0..2 of a
+ *   4x4, row-major) out[i].r = float32(((T_r0 x + T_r1 y) + T_r2 z) + T_r3) in double.  With axis
+ *   0, 1 or 2 (the crop's orthogonal axis; -1 = no crop) it also writes mask[i] = 1 when out[i]
+ *   lies in the crop volume (Open3D's CropInPolygon, in double): axis_min <= p[axis] <= axis_max
+ *   and, with (u, v) = (y, z), (x, z) or (x, y), an odd number of polygon edges (i, j = i+1 mod m)
+ *   with (P_i.u < p.u <= P_j.u) or (P_j.u < p.u <= P_i.u) whose node
+ *   P_i.v + ((p.u - P_i.u) / (P_j.u - P_i.u)) * (P_j.v - P_i.v) is < p.v.  polygon is (m,2)
+ *   doubles (u, v) on the DEVICE.  block_counts (casmvs_tnt_crop_blocks(n) ints) gets the kept
+ *   points of each block of the launch.
+ * casmvs_tnt_compact: the points with mask[i] != 0 in input order, given block_offsets, the int64
+ *   exclusive scan of block_counts; out_index (optional) gets their input indices.
+ * casmvs_tnt_voxel_mean: out[v] = float32(sum / count) of the points order[voxel_start[v]] ..
+ *   order[voxel_start[v+1] - 1], summed per axis in double in that order.
+ * casmvs_tnt_icp_moments: with s = src[i], t = tgt[index[i]] over the i with index[i] >= 0,
+ *   s' = s - origin, t' = t - origin: moments (18 doubles, DEVICE) = count, sum |t - s|^2, sum s'
+ *   (3), sum t' (3), sum |s'|^2, sum t'_a s'_b (3x3 row-major).  The sums are the same bits on
+ *   every call: a grid fixed by n, a fixed reduction tree, no atomics.  origin3 is a HOST array. */
+int casmvs_tnt_crop_blocks(int n);
+int casmvs_tnt_transform_crop(const float* points, int n, const double* T, int axis,
+                              double axis_min, double axis_max, const double* polygon,
+                              int n_polygon, float* out, unsigned char* mask, int* block_counts,
+                              void* stream);
+int casmvs_tnt_compact(const float* points, const unsigned char* mask, int n,
+                       const int64_t* block_offsets, float* out, int64_t* out_index, void* stream);
+int casmvs_tnt_voxel_mean(const float* points, const int64_t* order, const int* voxel_start,
+                          int n_voxels, float* out, void* stream);
+size_t casmvs_tnt_icp_workspace_bytes(int n);
+int casmvs_tnt_icp_moments(const float* src, int n, const float* tgt, const int64_t* index,
+                           const double* origin3, double* moments, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* ---- view selection of a sparse reconstruction (casmvsnet_pl_b200/colmap.py) ---------------
  * casmvs_view_scores_fwd: the MVSNet paper's (section 4.1) view-selection scores, in double:
