@@ -83,6 +83,8 @@ SIGNATURES = {
                                                                           c_void_p, c_void_p, c_int,
                                                                           c_void_p]),
     "casmvs_resize_u8_linear_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3),
+    "casmvs_undistort_u8_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [POINTER(c_double),
+                                                                         POINTER(c_double), c_void_p]),
     "casmvs_warp_cost_bwd": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
     "casmvs_conv3d_wgrad": (c_int, [c_void_p] * 3 + [c_int] * 10 + [c_void_p]),
     "casmvs_regress_bwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),

@@ -1,16 +1,23 @@
 """Scenes reconstructed with COLMAP, as the input of eval_pipeline --dataset_name colmap.
 
-The input is the workspace `colmap image_undistorter` writes:
+The input is the workspace `colmap image_undistorter` writes, or a `colmap mapper` project:
 
-    <root>/images/<name>                          the undistorted images
-    <root>/sparse/{cameras,images,points3D}.bin   (or .txt) the model
+    <root>/images/<name>                          the images (or any directory: --image_dir)
+    <root>/sparse/{cameras,images,points3D}.bin   (or .txt; or under <root>/sparse/0) the model
 
 Conversion, in order:
 
-  read_model         the model in COLMAP's binary or text format (host).  Only the undistorted
-                     camera models PINHOLE and SIMPLE_PINHOLE are accepted.  Everything the files
+  read_model         the model in COLMAP's binary or text format (host).  By default only the
+                     undistorted camera models PINHOLE and SIMPLE_PINHOLE are accepted;
+                     distorted=True also admits the seven DISTORTED_MODELS.  Everything the files
                      supply is validated before anything reaches the GPU: finite poses, intrinsics
-                     and points, and tracks that name registered images.
+                     and points, tracks that name registered images, and for a distorted camera
+                     its undistorted camera (undistorted_camera).
+  undistorted_camera the PINHOLE camera a distorted one is resampled to (README, "Your own
+                     scene"): the border pixels undistorted by Newton's method in float64, the
+                     scales of the largest centred box they enclose clipped to [0.2, 2], the size
+                     and principal point scaled by them.  The images are undistorted on the GPU
+                     as they are read (io.undistort_u8, csrc/undistort.cu).
   load_scene         views 0..n-1 in sorted image-name order: full-resolution K, world->camera
                      E = [R(q) | t], camera centre c = -R^T t, tracks in CSR form over view ids
                      (an image listed twice in one track counts once).
@@ -45,6 +52,14 @@ CAMERA_MODELS = {0: ("SIMPLE_PINHOLE", 3), 1: ("PINHOLE", 4), 2: ("SIMPLE_RADIAL
                  9: ("RADIAL_FISHEYE", 5), 10: ("THIN_PRISM_FISHEYE", 12)}
 MODEL_IDS = {name: (i, n) for i, (name, n) in CAMERA_MODELS.items()}
 SUPPORTED_MODELS = ("PINHOLE", "SIMPLE_PINHOLE")
+DISTORTED_MODELS = ("SIMPLE_RADIAL", "RADIAL", "OPENCV", "FULL_OPENCV", "SIMPLE_RADIAL_FISHEYE",
+                    "RADIAL_FISHEYE", "OPENCV_FISHEYE")
+FISHEYE_MODELS = ("SIMPLE_RADIAL_FISHEYE", "RADIAL_FISHEYE", "OPENCV_FISHEYE")
+SINGLE_FOCAL_MODELS = ("SIMPLE_PINHOLE", "SIMPLE_RADIAL", "RADIAL", "SIMPLE_RADIAL_FISHEYE",
+                       "RADIAL_FISHEYE")
+UNDISTORT_SCALES = (0.2, 2.0)       # min_scale, max_scale of the undistorted camera
+NEWTON_ITERS = 100
+NEWTON_TOL_PX = 1e-9                # round-trip residual a border pixel must reach
 
 N_SRC = 10                 # sources listed per view
 MIN_FRONT_POINTS = 20      # a reference view needs this many observed points in front of it
@@ -174,17 +189,18 @@ def _lines(path, keep_empty=False):
 
 
 def find_sparse_dir(root):
-    """The model directory of an undistorted workspace: <root>/sparse, or <root> itself."""
-    for d in (os.path.join(root, "sparse"), root):
+    """The model directory: <root>/sparse (an undistorted workspace), <root> itself, or
+    <root>/sparse/0 (where `colmap mapper` writes its first model)."""
+    for d in (os.path.join(root, "sparse"), root, os.path.join(root, "sparse", "0")):
         for ext in (".bin", ".txt"):
             if os.path.isfile(os.path.join(d, "cameras" + ext)):
                 return d
     raise FileNotFoundError(f"no COLMAP model (cameras.bin / cameras.txt) under {root}/sparse")
 
 
-def read_model(sparse_dir, ext=None):
+def read_model(sparse_dir, ext=None, distorted=False):
     """cameras, images and points3D of a COLMAP model, binary (.bin, preferred when both exist)
-    or text (.txt), validated (check_model)."""
+    or text (.txt), validated (check_model; `distorted` admits the DISTORTED_MODELS)."""
     if ext is None:
         ext = ".bin" if os.path.isfile(os.path.join(sparse_dir, "cameras.bin")) else ".txt"
     p = lambda name: os.path.join(sparse_dir, name + ext)      # noqa: E731
@@ -194,19 +210,26 @@ def read_model(sparse_dir, ext=None):
     else:
         model = ColmapModel(_read_cameras_txt(p("cameras")), _read_images_txt(p("images")),
                             *_read_points_txt(p("points3D")))
-    check_model(model)
+    check_model(model, distorted)
     return model
 
 
-def check_model(model):
+def check_model(model, distorted=False):
     """Raises ValueError unless every camera is PINHOLE or SIMPLE_PINHOLE with finite positive
-    focal lengths and a positive size, every image has a finite pose with a nonzero quaternion and
-    an existing camera, every point is finite and every track entry names a registered image."""
+    focal lengths and a positive size (or, with `distorted`, one of DISTORTED_MODELS that
+    undistorted_camera accepts), every image has a finite pose with a nonzero quaternion and an
+    existing camera, every point is finite and every track entry names a registered image."""
     for cid, (name, w, h, params) in model.cameras.items():
         if name not in SUPPORTED_MODELS:
-            raise ValueError(f"camera {cid} uses the {name} model; only undistorted PINHOLE and "
-                             "SIMPLE_PINHOLE cameras are supported: run `colmap image_undistorter` "
-                             "on the reconstruction first")
+            if not distorted:
+                raise ValueError(f"camera {cid} uses the {name} model; only undistorted PINHOLE and "
+                                 "SIMPLE_PINHOLE cameras are supported: run `colmap image_undistorter` "
+                                 "on the reconstruction first")
+            if name not in DISTORTED_MODELS:
+                raise ValueError(f"camera {cid} uses the {name} model, which is not supported; the "
+                                 "supported models are " + ", ".join(SUPPORTED_MODELS + DISTORTED_MODELS))
+            undistorted_camera(cid, name, w, h, params)
+            continue
         if w <= 0 or h <= 0 or not np.all(np.isfinite(params)) or np.any(params[:1] <= 0):
             raise ValueError(f"camera {cid}: bad size or parameters")
     for iid, (q, t, cid, name) in model.images.items():
@@ -315,10 +338,118 @@ def intrinsics(name, params):
     return np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1.0]])
 
 
+def split_params(name, params):
+    """COLMAP camera parameters -> (fx, fy, cx, cy, distortion coefficients in COLMAP's order)."""
+    p = [float(x) for x in params]
+    if name in SINGLE_FOCAL_MODELS:
+        return p[0], p[0], p[1], p[2], p[3:]
+    return p[0], p[1], p[2], p[3], p[4:]
+
+
+def distortion(name, k, u, v):
+    """COLMAP's forward distortion (du, dv) of normalised points (u, v) (float64 arrays) for the
+    coefficients k of model `name`; the distorted pixel is (fx (u + du) + cx, fy (v + dv) + cy)."""
+    k = list(k) + [0.0] * 8
+    u2, v2, uv = u * u, v * v, u * v
+    r2 = u2 + v2
+    if name in FISHEYE_MODELS:
+        r = np.sqrt(r2)
+        th = np.arctan(r)
+        t2 = th * th
+        thd = th * ((((1.0 + k[0] * t2) + k[1] * t2 ** 2) + k[2] * t2 ** 3) + k[3] * t2 ** 4)
+        rs = np.where(r > 0, r, 1.0)
+        return np.where(r > 0, u * thd / rs - u, 0.0), np.where(r > 0, v * thd / rs - v, 0.0)
+    if name in ("SIMPLE_RADIAL", "RADIAL"):
+        rad = k[0] * r2 + k[1] * r2 * r2
+        return u * rad, v * rad
+    p1, p2 = k[2], k[3]
+    tu, tv = 2 * p1 * uv + p2 * (r2 + 2 * u2), 2 * p2 * uv + p1 * (r2 + 2 * v2)
+    if name == "OPENCV":
+        rad = k[0] * r2 + k[1] * r2 * r2
+        return u * rad + tu, v * rad + tv
+    if name == "FULL_OPENCV":
+        r4, r6 = r2 * r2, r2 * r2 * r2
+        rad = (1 + k[0] * r2 + k[1] * r4 + k[4] * r6) / (1 + k[5] * r2 + k[6] * r4 + k[7] * r6)
+        return u * rad + tu - u, v * rad + tv - v
+    raise ValueError(f"no distortion for the {name} model")
+
+
+def _undistort_normalised(name, k, ud, vd):
+    """(u, v) with (u, v) + distortion(u, v) = (ud, vd): Newton's method from (ud, vd) with a
+    central-difference Jacobian, at most NEWTON_ITERS steps."""
+    u, v = ud.copy(), vd.copy()
+    for _ in range(NEWTON_ITERS):
+        du, dv = distortion(name, k, u, v)
+        eu, ev = u + du - ud, v + dv - vd
+        hu, hv = 1e-6 * np.maximum(1.0, np.abs(u)), 1e-6 * np.maximum(1.0, np.abs(v))
+        up, um = distortion(name, k, u + hu, v), distortion(name, k, u - hu, v)
+        vp, vm = distortion(name, k, u, v + hv), distortion(name, k, u, v - hv)
+        a, c = 1 + (up[0] - um[0]) / (2 * hu), (up[1] - um[1]) / (2 * hu)
+        b, d = (vp[0] - vm[0]) / (2 * hv), 1 + (vp[1] - vm[1]) / (2 * hv)
+        det = a * d - b * c
+        su, sv = (d * eu - b * ev) / det, (a * ev - c * eu) / det
+        u, v = u - su, v - sv
+        if np.all(np.abs(su) <= 1e-15 * np.maximum(1.0, np.abs(u))) and \
+                np.all(np.abs(sv) <= 1e-15 * np.maximum(1.0, np.abs(v))):
+            break
+    return u, v
+
+
+def undistorted_camera(cid, name, w, h, params):
+    """The PINHOLE camera a distorted camera `cid` is resampled to -> (W', H', [fx, fy, cx', cy']).
+
+    Modelled on COLMAP's undistorter with blank_pixels = 0, min_scale = 0.2, max_scale = 2: the
+    pixel centres of the four borders are undistorted (Newton, float64) and mapped back with the
+    camera's own fx, fy, cx, cy; sx = min((cx - max_left X) / (cx - 0.5), (min_right X - cx) /
+    (W - 0.5 - cx)), sy likewise in y, each clipped to [0.2, 2]; W' = max(2, round(sx W)),
+    H' = max(2, round(sy H)), cx' = cx (W' / W), cy' = cy (H' / H); fx and fy are kept.
+    Raises ValueError naming the camera when a parameter is not finite, a focal length is not
+    positive, the size is below 2 x 2, the principal point is not inside the pixel-centre box, a
+    border pixel does not round-trip within NEWTON_TOL_PX or a ratio is not positive."""
+    def refuse(why):
+        raise ValueError(f"camera {cid} ({name}, {w}x{h}): {why}")
+    params = np.asarray(params, np.float64)
+    if not np.all(np.isfinite(params)):
+        refuse("a parameter is not finite")
+    fx, fy, cx, cy, k = split_params(name, params)
+    if not (fx > 0 and fy > 0):
+        refuse("the focal length is not positive")
+    if w < 2 or h < 2:
+        refuse("the size is below 2 x 2")
+    if not (0.5 < cx < w - 0.5 and 0.5 < cy < h - 0.5):
+        refuse(f"the principal point ({cx!r}, {cy!r}) is not inside the pixel-centre box")
+    xs, ys = np.arange(w) + 0.5, np.arange(h) + 0.5
+    bx = np.concatenate([np.full(h, 0.5), np.full(h, w - 0.5), xs, xs])
+    by = np.concatenate([ys, ys, np.full(w, 0.5), np.full(w, h - 0.5)])
+    with np.errstate(all="ignore"):                 # a diverging point ends as inf / NaN
+        u, v = _undistort_normalised(name, k, (bx - cx) / fx, (by - cy) / fy)
+        du, dv = distortion(name, k, u, v)
+        res = np.maximum(np.abs(fx * (u + du) + cx - bx), np.abs(fy * (v + dv) + cy - by))
+    if not np.all(res <= NEWTON_TOL_PX):
+        i = int(np.argmax(np.where(res <= NEWTON_TOL_PX, 0, 1)))
+        refuse(f"the undistortion of border pixel ({bx[i]}, {by[i]}) does not converge "
+               f"(residual {res[i]:.3g} px)")
+    X, Y = fx * u + cx, fy * v + cy
+    left, right, top, bottom = X[:h], X[h:2 * h], Y[2 * h:2 * h + w], Y[2 * h + w:]
+    ratios = ((cx - left.max()) / (cx - 0.5), (right.min() - cx) / (w - 0.5 - cx),
+              (cy - top.max()) / (cy - 0.5), (bottom.min() - cy) / (h - 0.5 - cy))
+    if not all(r > 0 for r in ratios):
+        refuse(f"a scale ratio is not positive {tuple(float(r) for r in ratios)}")
+    lo, hi = UNDISTORT_SCALES
+    sx = min(max(min(ratios[0], ratios[1]), lo), hi)
+    sy = min(max(min(ratios[2], ratios[3]), lo), hi)
+    w2, h2 = max(2, int(np.floor(sx * w + 0.5))), max(2, int(np.floor(sy * h + 0.5)))
+    return w2, h2, np.array([fx, fy, cx * (w2 / w), cy * (h2 / h)])
+
+
 class Scene:
     """A validated model indexed by view id (sorted image names): names [n], K (n,3,3) and
     E (n,4,4) float64, wh (n,2) camera sizes, centres (n,3), xyz (N,3), and the tracks over view
-    ids in CSR form, track_ptr (N+1,) int64 / track_img (nnz,) int32, duplicates removed."""
+    ids in CSR form, track_ptr (N+1,) int64 / track_img (nnz,) int32, duplicates removed.
+    K and wh are the camera the depth maps are computed in: the view's own for a PINHOLE or
+    SIMPLE_PINHOLE camera, else its undistorted camera (undistorted_camera).  src_cameras[v] is
+    the view's camera as the model has it, (model id, w, h, params), and distorted (n,) bool marks
+    the views whose images must be undistorted."""
 
     def __init__(self, model):
         order = sorted(model.images, key=lambda i: model.images[i][3])
@@ -326,13 +457,24 @@ class Scene:
         n = len(order)
         self.K, self.E = np.zeros((n, 3, 3)), np.tile(np.eye(4), (n, 1, 1))
         self.wh = np.zeros((n, 2), np.int64)
+        self.src_cameras, self.distorted = [], np.zeros(n, bool)
+        undistorted = {}
         for v, iid in enumerate(order):
             q, t, cid, _ = model.images[iid]
             name, w, h, params = model.cameras[cid]
-            self.K[v] = intrinsics(name, params)
+            self.src_cameras.append((MODEL_IDS[name][0], w, h, np.asarray(params, np.float64)))
+            if name in SUPPORTED_MODELS:
+                self.K[v] = intrinsics(name, params)
+                self.wh[v] = (w, h)
+            else:
+                if cid not in undistorted:
+                    undistorted[cid] = undistorted_camera(cid, name, w, h, params)
+                w2, h2, pinhole = undistorted[cid]
+                self.K[v] = intrinsics("PINHOLE", pinhole)
+                self.wh[v] = (w2, h2)
+                self.distorted[v] = True
             self.E[v, :3, :3] = qvec_to_rotmat(q)
             self.E[v, :3, 3] = t
-            self.wh[v] = (w, h)
         self.centres = -np.einsum("nji,nj->ni", self.E[:, :3, :3], self.E[:, :3, 3])
         self.xyz = model.xyz
         ids = np.array(order, np.int64)
@@ -354,7 +496,7 @@ class Scene:
 
 
 def load_scene(root):
-    return Scene(read_model(find_sparse_dir(root)))
+    return Scene(read_model(find_sparse_dir(root), distorted=True))
 
 
 def view_scores(centres, xyz, track_ptr, track_img, device="cuda:0", max_chunk_pairs=0):

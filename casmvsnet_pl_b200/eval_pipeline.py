@@ -14,10 +14,12 @@ over the three test layouts eval.py reads (--dataset_name):
     blendedmvs  BlendedMVSTestScan  datasets/blendedmvs.py; <root>/<scan>/{cams, blended_images,
                                     rendered_depth_maps}, scan lists in <root>/..
 
-and over a scene of the user's own, reconstructed by COLMAP and undistorted:
+and over a scene of the user's own, reconstructed by COLMAP:
 
-    colmap      ColmapScan          <root>/images, <root>/sparse/{cameras,images,points3D}.{bin,txt};
-                                    view selection and depth ranges computed here (colmap.py)
+    colmap      ColmapScan          <root>/images (or --image_dir), <root>/sparse[/0]/{cameras,
+                                    images,points3D}.{bin,txt}; view selection and depth ranges
+                                    computed here (colmap.py); views of a distorted camera are
+                                    undistorted on the GPU as they are read (io.undistort_u8)
 
 Everything between decoding the images and writing the PLY stays on the GPU.  DTU images are
 decoded and resized on the host per use, as the reference does, uploaded as bytes and normalised
@@ -32,6 +34,8 @@ proba_XXXX.pfm are written as well).
         --root_dir BlendedMVS/dataset_low_res --img_wh 768 576
     python -m casmvsnet_pl_b200.eval_pipeline --dataset_name colmap --root_dir my_capture/dense \
         --ckpt ckpt.ckpt --img_wh 1152 864 [--depth_interval 192] [--mesh [--mesh_voxel S]]
+    python -m casmvsnet_pl_b200.eval_pipeline --dataset_name colmap --root_dir my_capture \
+        --image_dir my_capture/photos --ckpt ckpt.ckpt     (a `colmap mapper` project, sparse/0)
 
 --mesh also fuses each scan's filtered depth maps into a TSDF volume on the GPU and writes the
 marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes changes.
@@ -121,17 +125,32 @@ class SceneImages:
     `fus` (n,h,w,3) uint8 RGB = cv2.imread + cv2.resize(INTER_LINEAR) (the fusion colours).
     Decoding runs in a small host thread pool while the device resizes the views already
     uploaded (io.resize_u8_pil / io.resize_u8_linear, byte-identical to Pillow / cv2).  A view
-    is decoded once instead of once per reference view it takes part in, plus once for fusion."""
+    is decoded once instead of once per reference view it takes part in, plus once for fusion.
+    `cameras` {view: (src_cam, dst_cam)} (io.undistort_u8's camera pair) names the views of a
+    distorted camera: both decodes of such a view must be the camera's size, and are undistorted
+    to its pinhole camera in one call before they are resized."""
 
-    def __init__(self, paths, img_wh, device, workers=4):
+    def __init__(self, paths, img_wh, device, workers=4, cameras=None):
         from concurrent.futures import ThreadPoolExecutor
         self.index = {v: i for i, v in enumerate(paths)}
+        cameras = cameras or {}
         w, h = img_wh
         n = len(self.index)
         self.net = torch.empty(n, h, w, 3, dtype=torch.uint8, device=device)
         self.fus = torch.empty(n, h, w, 3, dtype=torch.uint8, device=device)
         with ThreadPoolExecutor(max(1, workers)) as ex:
-            for i, (pil, bgr) in enumerate(ex.map(_decode_pil_cv2, paths.values())):
+            for i, (v, (pil, bgr)) in enumerate(zip(paths, ex.map(_decode_pil_cv2, paths.values()))):
+                if v in cameras:
+                    src, dst = cameras[v]
+                    for img in (pil, bgr):
+                        if img.shape[:2] != (src[2], src[1]):
+                            raise ValueError(f"{paths[v]}: the image is {img.shape[1]}x{img.shape[0]}, "
+                                             f"its camera {src[1]}x{src[2]}")
+                    both = torch.from_numpy(np.stack([pil, bgr])).pin_memory()
+                    und = io.undistort_u8(both.to(device, non_blocking=True), src, dst)
+                    io.resize_u8_pil(und[0:1], img_wh, out=self.net[i:i + 1])
+                    io.resize_u8_linear(und[1:2], img_wh, out=self.fus[i:i + 1])
+                    continue
                 io.resize_u8_pil(torch.from_numpy(pil).pin_memory().to(device, non_blocking=True)[None],
                                  img_wh, out=self.net[i:i + 1])
                 io.resize_u8_linear(torch.from_numpy(bgr).pin_memory().to(device, non_blocking=True)[None],
@@ -152,12 +171,13 @@ class _CachedScan:
     on the host each time it is used, as the reference does (its PIL / cv2 route, kept as the
     reference the device route is tested and timed against)."""
     host_images = False
+    camera_pairs = None          # SceneImages' `cameras`: views to undistort
     _images = None
 
     def _image_cache(self, device):
         if self._images is None:
             self._images = SceneImages({v: self.image_path(v) for v in self.proj_mats}, self.img_wh,
-                                       device)
+                                       device, cameras=self.camera_pairs)
         return self._images
 
     def views(self, device):
@@ -316,9 +336,16 @@ class BlendedMVSTestScan(_CachedScan):
 
 
 class ColmapScan(_CachedScan):
-    """A scene reconstructed by COLMAP, in the workspace `colmap image_undistorter` writes:
+    """A scene reconstructed by COLMAP, in the workspace `colmap image_undistorter` writes or as
+    a `colmap mapper` project:
 
-        <root>/images/<name>, <root>/sparse/{cameras,images,points3D}.{bin,txt}
+        <image_dir>/<name> (default <root>/images),
+        <root>/sparse/{cameras,images,points3D}.{bin,txt} (or <root>/sparse/0/...)
+
+    A view of a distorted camera (colmap.DISTORTED_MODELS) is computed in its undistorted
+    PINHOLE camera (colmap.undistorted_camera): K, the projections and the written cams are that
+    camera's, and its images are undistorted on the GPU as SceneImages reads them.  The host
+    route (host_images=True) has no undistortion and refuses such a scene.
 
     Views are numbered 0..n-1 in sorted image-name order.  Each view's sources are the N_SRC
     views with the best positive view-selection score (colmap.py; the scores are computed on the
@@ -326,22 +353,34 @@ class ColmapScan(_CachedScan):
     n_views - 1 sources or fewer than 20 observed points in front of it; `skipped` maps those to
     the reason.  A reference view's depth range is [0.75 q(0.01), 1.25 q(0.99)] of the depths of
     its observed points and its depth interval that range / n_depths_arg.  Intrinsics are the
-    full-resolution K of the view's own camera, scaled to img_wh like Tanks'.
+    full-resolution K of the view's (undistorted) camera, scaled to img_wh like Tanks'.
     With `out_dir`, the run is recorded in <out_dir>/<scan>: cams/{vid:08d}_cam.txt for every
     view (MVSNet format: extrinsic, full-resolution intrinsic, `depth_min interval n_depths
     depth_max`, nan for a view with no point in front of it), pair.txt with the reference views
     and their scored sources, and view_names.txt (view id -> image name)."""
 
     def __init__(self, root_dir, scan=None, img_wh=(1152, 864), n_views=5, n_depths_arg=192.0,
-                 levels=3, host_images=False, out_dir=None, device="cuda:0", log=print):
+                 levels=3, host_images=False, out_dir=None, device="cuda:0", log=print,
+                 image_dir=None):
         from . import colmap
         assert img_wh[0] % 32 == 0 and img_wh[1] % 32 == 0, "img_wh must both be multiples of 32!"
         self.root_dir = root_dir
+        self.image_dir = image_dir or os.path.join(root_dir, "images")
         self.scan = scan or os.path.basename(os.path.normpath(os.path.abspath(root_dir)))
         self.img_wh, self.n_views, self.host_images = tuple(img_wh), n_views, host_images
         sc = self.scene = colmap.load_scene(root_dir)
         if len(sc) == 0:
             raise ValueError(f"{root_dir}: the COLMAP model has no registered images")
+        if sc.distorted.any():
+            if host_images:
+                v = int(np.argmax(sc.distorted))
+                raise ValueError(f"{root_dir}: view {v} ({sc.names[v]}) has a distorted camera "
+                                 f"({colmap.CAMERA_MODELS[sc.src_cameras[v][0]][0]}); the host "
+                                 "image route (host_images=True) has no undistortion")
+            self.camera_pairs = {
+                int(v): (sc.src_cameras[v], (int(sc.wh[v, 0]), int(sc.wh[v, 1]),
+                                             sc.K[v][[0, 1, 0, 1], [0, 1, 2, 2]]))
+                for v in np.nonzero(sc.distorted)[0]}
         scores = colmap.view_scores(sc.centres, sc.xyz, sc.track_ptr, sc.track_img, device)
         count, q = colmap.depth_stats(sc.E, sc.xyz, sc.track_ptr, sc.track_img, device)
         self.scores = scores.cpu().numpy()
@@ -368,7 +407,7 @@ class ColmapScan(_CachedScan):
             colmap.write_view_names(os.path.join(d, "view_names.txt"), sc.names)
 
     def image_path(self, vid):
-        return os.path.join(self.root_dir, "images", self.scene.names[vid])
+        return os.path.join(self.image_dir, self.scene.names[vid])
 
     def depth_range(self, ref, depth_interval):
         # the divisor was applied at construction (n_depths_arg)
@@ -451,7 +490,7 @@ def open_scans(a):
         return
     if a.dataset_name == "colmap":
         yield ColmapScan(a.root_dir, a.scan or None, tuple(a.img_wh), a.n_views, a.depth_interval,
-                         out_dir=a.out_dir)
+                         out_dir=a.out_dir, image_dir=a.image_dir)
         return
     if a.dataset_name == "tanks":
         for s in [a.scan] if a.scan else list(TanksTestScan.SCANS[a.split]):
@@ -487,6 +526,8 @@ def parse_args(argv=None):
                          "dtu, colmap: unused")
     ap.add_argument("--scan", default="", help="one scan (default: every scan of the split; dtu "
                                                "needs it; colmap: the name of the root directory)")
+    ap.add_argument("--image_dir", default=None,
+                    help="colmap: the directory holding the model's images (default <root_dir>/images)")
     ap.add_argument("--ckpt", default="")
     ap.add_argument("--img_wh", nargs=2, type=int, default=[1152, 864])
     ap.add_argument("--n_views", type=int, default=5)
@@ -534,6 +575,8 @@ def main(argv=None):
         raise SystemExit("--dtu_gt applies to dtu only")
     if a.tnt_gt is not None and a.dataset_name != "colmap":
         raise SystemExit("--tnt_gt applies to colmap only")
+    if a.image_dir is not None and a.dataset_name != "colmap":
+        raise SystemExit("--image_dir applies to colmap only")
     if a.dataset_name == "dtu" and not a.scan:
         raise SystemExit("--scan is required for dtu")
     splits = {"tanks": TanksTestScan.SCANS, "blendedmvs": BlendedMVSTestScan.SPLITS}.get(a.dataset_name)

@@ -443,6 +443,41 @@ def resize_u8_linear(images, wh, out=None):
     return out
 
 
+def undistort_u8(images, src_cam, dst_cam, out=None):
+    """uint8 (N,H,W,3) CUDA images of one distorted COLMAP camera -> (N,OH,OW,3) uint8 in its
+    undistorted PINHOLE camera (casmvs_undistort_u8_fwd).  src_cam = (model id, W, H, params)
+    as colmap.Scene.src_cameras holds it; dst_cam = (OW, OH, [fx, fy, cx, cy]) as
+    colmap.undistorted_camera returns it.  The images must be W x H."""
+    import ctypes
+
+    from . import _lib
+    t = _check_u8_images(images, "undistort_u8")
+    N, H, W, _ = t.shape
+    model, sw, sh, sp = src_cam
+    OW, OH, dp = dst_cam
+    if (int(sw), int(sh)) != (W, H):
+        raise _lib.CasMVSError(f"undistort_u8: the images are {W}x{H}, the camera {sw}x{sh}")
+    OW, OH = int(OW), int(OH)
+    if OW <= 0 or OH <= 0:
+        raise _lib.CasMVSError(f"undistort_u8: bad size {(OW, OH)}")
+    from .colmap import CAMERA_MODELS
+    if int(model) in CAMERA_MODELS and len(sp) != CAMERA_MODELS[int(model)][1]:
+        raise _lib.CasMVSError(f"undistort_u8: {CAMERA_MODELS[int(model)][0]} takes "
+                               f"{CAMERA_MODELS[int(model)][1]} parameters, got {len(sp)}")
+    if len(dp) != 4:
+        raise _lib.CasMVSError("undistort_u8: the undistorted camera is (fx, fy, cx, cy)")
+    if out is None:
+        out = torch.empty(N, OH, OW, 3, device=t.device, dtype=torch.uint8)
+    src = (ctypes.c_double * len(sp))(*[float(x) for x in sp])
+    dst = (ctypes.c_double * 4)(*[float(x) for x in dp])
+    with torch.cuda.device(t.device):
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        _lib.check(_lib.load().casmvs_undistort_u8_fwd(
+            ctypes.c_void_p(t.data_ptr()), ctypes.c_void_p(out.data_ptr()), N, H, W, OH, OW,
+            int(model), src, dst, st), "undistort_u8")
+    return out
+
+
 def save_visual(depth_dir, scan, vid, depth, proba, conf):
     """eval.py:230-239: JET-coloured depth (min over positive depths .. max, to uint8) and the
     confidence mask proba > conf as JPEGs next to the PFMs."""

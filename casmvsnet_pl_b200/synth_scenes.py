@@ -17,7 +17,8 @@ n_views > 2 skip it (blendedmvs.py:51-54), and is no other view's source.
 
 make_colmap writes the same arc of cameras as an undistorted COLMAP workspace (images/ and a
 sparse/ model of points on a known surface, binary and / or text) for eval_pipeline's colmap
-reader; sparse_tracks makes bare sparse models of any size for the view-selection kernel.
+reader, or with distorted cameras and / or as a `colmap mapper` project (sparse/0); sparse_tracks
+makes bare sparse models of any size for the view-selection kernel.
 sphere_scene renders analytic depth maps and colours of a sphere (on a plane) for meshing.
 
     python -m casmvsnet_pl_b200.synth_scenes --kind tanks --root TNT --n_views 150 --image_wh 1920 1080
@@ -189,8 +190,23 @@ def make_dtu_train(root, scan="scan1", refs=(0, 1, 2), n_src=5, depth=650.0, see
     return root
 
 
+def _distorted(cam, model, coeffs):
+    """A PINHOLE / SIMPLE_PINHOLE camera as `model` with the same fx, fy, cx, cy and `coeffs`."""
+    from . import colmap
+    name, w, h, prm = cam
+    fx, fy, cx, cy, _ = colmap.split_params(name, prm)
+    single = model in colmap.SINGLE_FOCAL_MODELS
+    if single and fx != fy:
+        raise ValueError(f"{model} has one focal length; the {name} camera has fx {fx} != fy {fy}")
+    params = ([fx] if single else [fx, fy]) + [cx, cy] + [float(c) for c in coeffs]
+    if len(params) != colmap.MODEL_IDS[model][1]:
+        raise ValueError(f"{model} takes {colmap.MODEL_IDS[model][1] - (3 if single else 4)} "
+                         f"coefficients, got {len(coeffs)}")
+    return (model, w, h, np.array(params))
+
+
 def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=0, n_single=20,
-                 n_dup=20):
+                 n_dup=20, distortion=None, ext="jpg"):
     """The arc cameras of the other layouts as a COLMAP model (colmap.ColmapModel) looking at a
     known surface, z = depth + 0.05 depth sin(3x / depth) cos(2y / depth) in world coordinates,
     which every optical axis meets at depth `depth` (the cameras sit on a circle of that radius
@@ -198,7 +214,9 @@ def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=
     odd views a SIMPLE_PINHOLE camera 1.25 times larger.  Image ids are shuffled against the
     sorted image names.  A point's track is every view it projects into with z > 0; the first
     n_single tracks of length > 1 are cut to one view and n_dup others list their first view
-    twice."""
+    twice.  `distortion`, (model, coefficients) or {camera id: (model, coefficients)}, turns
+    both cameras (or the ones named) into that COLMAP model with the same fx, fy, cx and cy
+    (tracks as without it); `ext` is the image names' extension."""
     from . import colmap
     rng = np.random.default_rng(seed)
     W, H = image_wh
@@ -212,7 +230,7 @@ def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=
         R = np.array([[np.cos(t), 0, np.sin(t)], [0, 1, 0], [-np.sin(t), 0, np.cos(t)]])
         tv = np.array([-depth * np.sin(t), 0, depth * (1 - np.cos(t))])
         cid = 1 if v % 2 == 0 else 2
-        images[int(ids[v])] = (colmap.rotmat_to_qvec(R), tv, cid, f"view_{v:03d}.jpg")
+        images[int(ids[v])] = (colmap.rotmat_to_qvec(R), tv, cid, f"view_{v:03d}.{ext}")
         E = np.eye(4)
         E[:3, :3], E[:3, 3] = R, tv
         name, w, h, prm = cams[cid]
@@ -239,6 +257,10 @@ def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=
     ptr = np.zeros(len(keep) + 1, np.int64)
     np.cumsum([len(tracks[k]) for k in keep], out=ptr[1:])
     img = np.array([i for k in keep for i in tracks[k]], np.int64)
+    if distortion is not None:
+        per_cam = distortion if isinstance(distortion, dict) else {cid: distortion for cid in cams}
+        for cid, (model, coeffs) in per_cam.items():
+            cams[cid] = _distorted(cams[cid], model, coeffs)
     return colmap.ColmapModel(cams, images, 1 + 3 * np.arange(len(keep)), xyz[keep], ptr, img)
 
 
@@ -266,21 +288,29 @@ def sparse_tracks(n_img=300, n_pts=500_000, track_len=(3, 11), seed=0):
 
 
 def make_colmap(root, n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=0,
-                fmt="bin", **kw):
+                fmt="bin", layout="undistorted", image_ext="jpg", image_dir=None, **kw):
     """An undistorted COLMAP workspace: <root>/images/view_XXX.jpg at each view's camera size and
     the model of colmap_model under <root>/sparse, in binary ("bin"), text ("txt") or both
-    formats ("both"; the reader prefers the binary one).  Returns the model."""
+    formats ("both"; the reader prefers the binary one).  layout="mapper" puts the model under
+    <root>/sparse/0 as `colmap mapper` does; image_ext="png" writes lossless images (the same
+    bytes from every decoder); image_dir replaces <root>/images; `distortion` (colmap_model)
+    makes the cameras distorted.  Returns the model."""
     from PIL import Image
 
     from . import colmap
-    model = colmap_model(n_views, image_wh, depth, n_points, seed, **kw)
+    if layout not in ("undistorted", "mapper") or image_ext not in ("jpg", "png"):
+        raise ValueError(f"unknown layout {layout!r} or image extension {image_ext!r}")
+    model = colmap_model(n_views, image_wh, depth, n_points, seed, ext=image_ext, **kw)
     rng = np.random.default_rng(seed + 1)
-    os.makedirs(os.path.join(root, "images"), exist_ok=True)
+    image_dir = image_dir or os.path.join(root, "images")
+    os.makedirs(image_dir, exist_ok=True)
     for q, t, cid, name in model.images.values():
         _, w, h, _ = model.cameras[cid]
-        Image.fromarray(_image(rng, w, h)).save(os.path.join(root, "images", name), quality=92)
+        opts = {"quality": 92} if image_ext == "jpg" else {}
+        Image.fromarray(_image(rng, w, h)).save(os.path.join(image_dir, name), **opts)
+    sparse = os.path.join(root, "sparse", "0") if layout == "mapper" else os.path.join(root, "sparse")
     for f in (("bin", "txt") if fmt == "both" else (fmt,)):
-        colmap.write_model(os.path.join(root, "sparse"), model, f)
+        colmap.write_model(sparse, model, f)
     return model
 
 

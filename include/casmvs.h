@@ -424,6 +424,20 @@ int casmvs_resize_u8_pil_fwd(const uint8_t* images, uint8_t* out, uint8_t* tmp, 
 int casmvs_resize_u8_linear_fwd(const uint8_t* images, uint8_t* out, int N, int H, int W, int OH,
                                 int OW, const int* xtab, const int* ytab, void* stream);
 
+/* Undistortion of distorted COLMAP views (casmvsnet_pl_b200/colmap.py undistorted_camera):
+ * images (N,H,W,3) uint8 of one source camera -> out (N,OH,OW,3) uint8 in its undistorted
+ * PINHOLE camera.  model: COLMAP's model id (0-6, 8, 9; FOV and THIN_PRISM_FISHEYE are refused);
+ * src_params: HOST array of the model's parameters in COLMAP's order; dst_params: HOST array
+ * (fx, fy, cx, cy) of the undistorted camera.  Both are copied into the launch, not to the device.
+ * Per output pixel, in float64 with every operation rounded separately: u = (x + 0.5 - cx') / fx',
+ * v likewise, COLMAP's forward distortion and projection to (X, Y), sx = X - 0.5, sy = Y - 0.5;
+ * 0 when either lies more than 1e-6 outside [0, W-1] / [0, H-1], else the bilinear sample at
+ * the clamped point, rounded by floor(s + 0.5).  The map is computed once per output pixel and
+ * applied to all N images.  H, W >= 2. */
+int casmvs_undistort_u8_fwd(const uint8_t* images, uint8_t* out, int N, int H, int W, int OH,
+                            int OW, int model, const double* src_params, const double* dst_params,
+                            void* stream);
+
 /* ---- geometric-consistency filter + refinement + back-projection (SURVEY.md 8 f-3) ------
  * One reference view of eval.py:262-318 on the device; replaces xy_ref2src / xy_src2ref /
  * check_geo_consistency (eval.py:113-182, numba + cv2.remap on the CPU).  For every reference
