@@ -122,23 +122,6 @@ inline int opt_in_smem(K kfn, int bytes, std::atomic<bool> (&done)[kMaxDevices],
   return 0;
 }
 
-// Division of a work-item index by a launch constant without the ~30-instruction runtime
-// division: q = umulhi(n, m), m = floor(2^32 / d) + 1, exact while n * d < 2^32 (the host
-// checks that with fastdiv_ok before it launches).
-struct FastDiv {
-  uint32_t d, m;
-};
-inline FastDiv make_fastdiv(uint32_t d) {
-  return FastDiv{d, d > 1 ? (uint32_t)((1ull << 32) / d) + 1u : 0u};
-}
-inline bool fastdiv_ok(uint64_t n_max, uint32_t d) { return n_max * d < (1ull << 32); }
-// n -> n / d, with the remainder in r
-__device__ __forceinline__ uint32_t fastdivmod(uint32_t n, const FastDiv f, uint32_t& r) {
-  const uint32_t q = f.d > 1 ? __umulhi(n, f.m) : n;
-  r = n - q * f.d;
-  return q;
-}
-
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }

@@ -209,34 +209,3 @@ def test_new_entry_points_validate_arguments():
     rc = lib.casmvs_conv2d_rgb8_fwd(None, one, one, 0.01, one, 1, 32, 32, 0, None)
     assert rc < 0 and b"null" in lib.casmvs_last_error()
     assert lib.casmvs_conv2d_rgb8_fwd(one, one, one, 0.01, one, 0, 32, 32, 0, None) == 0   # empty batch
-
-
-def test_work_item_magic_division_is_exact_in_its_range():
-    """The persistent conv kernels decompose a work-item index with q = umulhi(n, m),
-    m = floor(2^32 / d) + 1 (common.cuh: make_fastdiv / fastdivmod) and the host only launches when
-    items * max_divisor < 2^32 (fastdiv_ok).  Restated here in integer arithmetic: the quotient is
-    exact for every n with n * d < 2^32, at the divisors and item counts of the BASELINE shapes
-    and at the edge of the range."""
-    import random
-    rnd = random.Random(0)
-
-    def fastdiv(n, d):
-        if d <= 1:
-            return n
-        m = ((1 << 32) // d + 1) & 0xFFFFFFFF
-        return (n * m) >> 32
-
-    divisors = [1, 2, 3, 5, 7, 11, 16, 22, 30, 39, 64, 128, 216, 264, 1000, 4097, 65535]
-    for d in divisors:
-        top = ((1 << 32) - 1) // d                       # largest n with n * d < 2^32
-        samples = {0, 1, d - 1, d, d + 1, top, top - 1, top // 2}
-        samples |= {rnd.randrange(0, top + 1) for _ in range(2000)}
-        samples |= {k * d + r for k in (top // d, top // d - 1, 12345 % (top // d + 1)) for r in (0, d - 1)
-                    if 0 <= k * d + r <= top}
-        for n in samples:
-            if n < 0:
-                continue
-            assert fastdiv(n, d) == n // d, (n, d)
-    # cfg5 (1920x1056, D = 64): tile columns x rows x chunks of the Cout <= 8 kernel stay in range
-    items = 64 * 264 * 64
-    assert items * 264 < (1 << 32)
