@@ -18,6 +18,7 @@ FUSED_TAIL = 1024        # OR-ed into costreg precision: conv11 + prob in one ke
 FP32, TF32 = 0, 1
 CONV, CONV_TRANSPOSE, CONV_PLANAR = 0, 1, 2
 PRECISIONS = {"fp32": FP32, "tf32": TF32}
+VISUAL_WORKSPACE_BYTES = 4096   # casmvs_visual_panels
 
 # name -> (restype, argtypes); must list every symbol include/casmvs.h declares
 SIGNATURES = {
@@ -144,6 +145,7 @@ SIGNATURES = {
     "casmvs_render_mesh_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, POINTER(c_float),
                                        POINTER(c_float), c_int, c_int, c_void_p, c_void_p, c_size_t,
                                        c_void_p, c_void_p, c_void_p]),
+    "casmvs_visual_panels": (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
 }

@@ -28,6 +28,16 @@ for the reference's MVSSystem:
   * checkpoints in Lightning's layout, ckpts/<exp_name>/_ckpt_epoch_{e}.ckpt, keeping the 5
     best by val/acc_2mm.
 
+TensorBoard (--tensorboard): the original's log as well, under logs/<exp_name>/tensorboard/.
+Every metrics.jsonl record goes there too, each key but epoch, step and checkpoint as a scalar
+of that name at the record's step; and at batch 0 of every training epoch and of every
+validation pass the 4-panel image train/image_GT_pred_prob / val/image_GT_pred_prob (reference
+image, depth_gt, depth_pred * mask, confidence * mask; visual.py), drawn on the GPU from the
+step's own forward and copied to the host once.  The training image is logged at the number of
+steps completed before its step, the validation one at the current step, as Lightning numbers
+them.  A run without the flag writes the same files as before, and with it the same
+metrics.jsonl and checkpoints.
+
 Reproducible runs: --deterministic turns on torch.use_deterministic_algorithms (Lightning's
 Trainer(deterministic=True)); the backward then runs the library's deterministic kernels and
 cuDNN's heuristically chosen deterministic algorithms.  --seed N seeds the model's
@@ -94,6 +104,9 @@ def build_parser():
                     help="bit-reproducible steps: torch.use_deterministic_algorithms(True)")
     ap.add_argument("--seed", type=int, default=None,
                     help="seed of the initialisation, the shuffle and the workers' jitter draws")
+    # absent from the namespace unless given, so that a run without it parses as before
+    ap.add_argument("--tensorboard", action="store_true", default=argparse.SUPPRESS,
+                    help="also log to TensorBoard under logs/<exp_name>/tensorboard/")
     return ap
 
 
@@ -246,15 +259,34 @@ class Trainer:
         self.optimizer = get_optimizer(a, model)
         self.scheduler = get_scheduler(a, self.optimizer)
         self.global_step = 0
+        self.tb = None                  # a SummaryWriter while fit() logs to TensorBoard
 
     def forward(self, s):
         return self.model(s["imgs"], s["proj_mats"], s["init_depth_min"], s["depth_interval"])
 
-    def train_step(self, s):
-        """One optimiser step on a device sample -> (loss, metrics) device tensors."""
+    def log_panel(self, tag, s, results, step):
+        """The TensorBoard image of sample 0: reference image, depth_gt, depth_pred * mask and
+        confidence * mask (the original train.py:107-114), one device -> host copy."""
+        from .visual import training_panel
+        with torch.no_grad():
+            panel = training_panel(s["imgs"][0, 0], s["depths"]["level_0"][0],
+                                   results["depth_0"][0].detach(),
+                                   results["confidence_0"][0].detach(), s["masks"]["level_0"][0])
+        self.tb.add_image(tag, panel.cpu().numpy(), step, dataformats="HWC")
+
+    def log_scalars(self, rec):
+        for k, v in rec.items():
+            if k not in ("epoch", "step", "checkpoint"):
+                self.tb.add_scalar(k, v, rec["step"])
+
+    def train_step(self, s, log_panel=False):
+        """One optimiser step on a device sample -> (loss, metrics) device tensors.  With
+        log_panel, the step's forward also goes to TensorBoard as train/image_GT_pred_prob."""
         self.model.train()
         results = self.forward(s)
         loss, metrics = sl1_loss_and_metrics(results, s["depths"], s["masks"], self.a.levels)
+        if log_panel:
+            self.log_panel("train/image_GT_pred_prob", s, results, self.global_step)
         self.optimizer.zero_grad(set_to_none=True)
         loss.backward()
         self.optimizer.step()
@@ -268,9 +300,12 @@ class Trainer:
         loss_sum = torch.zeros((), device=self.device, dtype=torch.float64)
         msum = torch.zeros(5, device=self.device, dtype=torch.float64)
         n = 0
-        for batch in batches:
+        for i, batch in enumerate(batches):
             s = train_data.to_device(batch, self.device)
-            loss, metrics = sl1_loss_and_metrics(self.forward(s), s["depths"], s["masks"], self.a.levels)
+            results = self.forward(s)
+            if i == 0 and self.tb is not None:
+                self.log_panel("val/image_GT_pred_prob", s, results, self.global_step)
+            loss, metrics = sl1_loss_and_metrics(results, s["depths"], s["masks"], self.a.levels)
             loss_sum += loss
             msum += metrics
             n += 1
@@ -282,25 +317,42 @@ class Trainer:
         a = self.a
         os.makedirs(os.path.dirname(log_path) or ".", exist_ok=True)
         keep = TopKCheckpoints(ckpt_dir, 5)
+        if getattr(a, "tensorboard", False):
+            from torch.utils.tensorboard import SummaryWriter
+            self.tb = SummaryWriter(os.path.join(os.path.dirname(log_path), "tensorboard"))
+        try:
+            self._fit(train_loader, val_loader, log_path, keep)
+        finally:
+            if self.tb is not None:
+                self.tb.close()
+                self.tb = None
+        return keep.kept
+
+    def _fit(self, train_loader, val_loader, log_path, keep):
+        a = self.a
         with open(log_path, "a") as log:
             for epoch in range(a.num_epochs):
-                for batch in train_loader:
+                for i, batch in enumerate(train_loader):
                     lr = get_learning_rate(self.optimizer)
-                    loss, m = self.train_step(train_data.to_device(batch, self.device))
+                    loss, m = self.train_step(train_data.to_device(batch, self.device),
+                                              log_panel=i == 0 and self.tb is not None)
                     if self.global_step % a.log_every == 0 or self.global_step == 1:
                         vals = torch.cat([loss.view(1), m[:4] / m[4]]).tolist()
                         rec = {"epoch": epoch, "step": self.global_step, "lr": lr, "train/loss": vals[0]}
                         rec.update({f"train/{k}": v for k, v in zip(METRIC_NAMES, vals[1:])})
-                        log.write(json.dumps(rec) + "\n")
-                        log.flush()
+                        self._record(log, rec)
                 val = self.validate(val_loader)
                 path = keep(self.model, epoch, self.global_step, val["val/acc_2mm"])
-                log.write(json.dumps({"epoch": epoch, "step": self.global_step, **val,
-                                      "checkpoint": path}) + "\n")
-                log.flush()
+                self._record(log, {"epoch": epoch, "step": self.global_step, **val,
+                                   "checkpoint": path})
                 print(f"epoch {epoch}: " + ", ".join(f"{k} {v:.4f}" for k, v in val.items()))
                 self.scheduler.step()
-        return keep.kept
+
+    def _record(self, log, rec):
+        log.write(json.dumps(rec) + "\n")
+        log.flush()
+        if self.tb is not None:
+            self.log_scalars(rec)
 
 
 def build_datasets(a):

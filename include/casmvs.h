@@ -657,6 +657,23 @@ int casmvs_render_mesh_fwd(const float* verts, const unsigned char* colours, int
                            size_t workspace_bytes, unsigned char* image, float* depth,
                            void* stream);
 
+/* ---- training panels (csrc/visual.cu; utils/visualization.py, train.py:107-114) ---------
+ * The original's TensorBoard image strip as uint8 (H, n*W, 3), n = the number of non-NULL panel
+ * inputs, panels left to right in the order img, depth_gt, depth_pred, conf:
+ *   img (3,H,W) f32, normalised as the data readers leave it -> un-normalised RGB;
+ *   depth_gt (H,W) f32 -> visualize_depth(depth_gt);
+ *   depth_pred (H,W) f32 -> visualize_depth(depth_pred * mask);
+ *   conf (H,W) f32 -> visualize_prob(conf * mask).
+ * mask (H,W) u8 (nonzero = valid) may be NULL: all valid.  The bytes equal the original's chain
+ * (cv2 colour maps with blue and red swapped, numpy's wrapping float -> uint8 cast); a depth map
+ * with no positive value is drawn in the colour of grey level 0, where the original raises.
+ * workspace: CASMVS_VISUAL_WORKSPACE_BYTES, 16-byte aligned, needed with a depth panel; nothing
+ * is read from it before the call writes it.  H * W < 2^31. */
+#define CASMVS_VISUAL_WORKSPACE_BYTES 4096
+int casmvs_visual_panels(const float* img, const float* depth_gt, const float* depth_pred,
+                         const float* conf, const unsigned char* mask, int H, int W,
+                         unsigned char* out, void* workspace, void* stream);
+
 /* ---- layout helpers ------------------------------------------------------ */
 /* (N,C,S) -> (N,S,C) and back, S = product of spatial dims. */
 int casmvs_nchw_to_nhwc(const float* in, float* out, int N, int C, size_t S, void* stream);
