@@ -51,6 +51,19 @@ import torch
 
 from . import fusion, io
 
+# --num_groups values (eval_pipeline and train.py): the group-wise correlation splits the
+# 8 / 16 / 32 feature channels of every stage into this many groups
+NUM_GROUPS = (1, 2, 4, 8)
+
+
+def depth_count(text):
+    """argparse type of --n_depths: CostRegNet halves the depth three times and back, so each
+    stage's plane count must be a positive multiple of 8."""
+    n = int(text)
+    if n <= 0 or n % 8:
+        raise argparse.ArgumentTypeError(f"{text} is not a positive multiple of 8")
+    return n
+
 
 def read_image_rgb_u8(path, img_wh):
     """cv2.imread + cv2.resize(INTER_LINEAR) + BGR->RGB (eval.py:76-79, 267-268) -> (H,W,3) uint8.
@@ -531,9 +544,9 @@ def parse_args(argv=None):
     ap.add_argument("--ckpt", default="")
     ap.add_argument("--img_wh", nargs=2, type=int, default=[1152, 864])
     ap.add_argument("--n_views", type=int, default=5)
-    ap.add_argument("--n_depths", nargs="+", type=int, default=[8, 32, 48])
+    ap.add_argument("--n_depths", nargs="+", type=depth_count, default=[8, 32, 48])
     ap.add_argument("--interval_ratios", nargs="+", type=float, default=[1.0, 2.0, 4.0])
-    ap.add_argument("--num_groups", type=int, default=1)
+    ap.add_argument("--num_groups", type=int, default=1, choices=NUM_GROUPS)
     ap.add_argument("--depth_interval", type=float, default=None,
                     help="dtu: the depth interval (default 2.65); tanks: no effect; blendedmvs: "
                          "divides each view's depth range (default 2.65); colmap: the same "

@@ -284,6 +284,28 @@ class CostRegNet(nn.Module):
         for name in self._ORDER[:-1]:
             yield self._layer_tensors(name)[1]
 
+    @property
+    def kernel_channels(self):
+        """conv0's input channels as the kernels take them: in_channels rounded up to a multiple
+        of 4, since every convolution kernel reads channel quads.  A 2-group cost volume gets two
+        zero channels and conv0 two zero weight rows, which leaves the function unchanged; the
+        module's own conv0 keeps the reference's shape, so checkpoints load as they are."""
+        return -(-self.in_channels // 4) * 4
+
+    def _pad_channels(self, x):
+        """logical (B,in_channels,D,h,w) -> (B,kernel_channels,D,h,w), zero channels appended,
+        channels-last storage; differentiable (the gradient of the pad is dropped)."""
+        pad = self.kernel_channels - self.in_channels
+        if pad == 0:
+            return x
+        return ops.as_volume_view(F.pad(ops.volume_storage(x), (0, pad)))
+
+    def _conv0_weight(self):
+        """conv0's (8, in_channels, 3, 3, 3) weight with zero input rows up to kernel_channels."""
+        w = self.conv0.conv.weight
+        pad = self.kernel_channels - self.in_channels
+        return F.pad(w, (0, 0, 0, 0, 0, 0, 0, pad)) if pad else w
+
     def packed_params(self):
         """Device blob for casmvs_costreg_fwd (layout: casmvs_costreg_layer_info)."""
         key = tuple((t.data_ptr(), t._version) for t in
@@ -293,12 +315,14 @@ class CostRegNet(nn.Module):
         dev = self.prob.weight.device
         if self._blob is not None:
             ops.release_weight_images(self._blob)     # the old blob's operand images die with it
-        n = ops._lib.load().casmvs_costreg_param_floats(self.in_channels)
+        n = ops._lib.load().casmvs_costreg_param_floats(self.kernel_channels)
         blob = torch.empty(n, device=dev, dtype=torch.float32)
         ops.release_weight_images(blob)     # a recycled address must not hit stale operand images
         for i, name in enumerate(self._ORDER):
-            info = ops.costreg_layer_info(self.in_channels, i)
+            info = ops.costreg_layer_info(self.kernel_channels, i)
             w, bn, bias = self._layer_tensors(name)
+            if i == 0:
+                w = self._conv0_weight()
             wp = ops.pack_conv3d_weight(w, info["kind"])
             blob[info["w_off"]:info["w_off"] + wp.numel()] = wp
             co = info["cout"]
@@ -319,13 +343,14 @@ class CostRegNet(nn.Module):
         from .. import autograd as AG
         prec = ops.PRECISIONS[self.precision]
 
-        def cbr(m, t, stride=1):
-            return m.bn(AG.conv3d(t, m.conv.weight, ops.CONV, stride, prec))
+        def cbr(m, t, stride=1, weight=None):
+            w = m.conv.weight if weight is None else weight
+            return m.bn(AG.conv3d(t, w, ops.CONV, stride, prec))
 
         def up(m, t):
             return m[1](AG.conv3d(t, m[0].weight, ops.CONV_TRANSPOSE, 2, prec))
 
-        conv0 = cbr(self.conv0, x)
+        conv0 = cbr(self.conv0, self._pad_channels(x), weight=self._conv0_weight())
         conv2 = cbr(self.conv2, cbr(self.conv1, conv0, 2))
         conv4 = cbr(self.conv4, cbr(self.conv3, conv2, 2))
         x = cbr(self.conv6, cbr(self.conv5, conv4, 2))
@@ -347,13 +372,13 @@ class CostRegNet(nn.Module):
                                         any(p.requires_grad for p in self.parameters())):
             return self._forward_autograd(x)
         self._check_inference()
-        logits = ops.costreg(x, self.packed_params(), self.in_channels,
+        logits = ops.costreg(self._pad_channels(x), self.packed_params(), self.kernel_channels,
                              ops.PRECISIONS[self.precision])
         return logits.unsqueeze(1)                                   # (B,1,D,h,w)
 
     def blocked_supported(self):
         """forward_blocked applies: tf32, and the tensor-core kernels cover every layer."""
-        return self.precision == "tf32" and ops.costreg_blocked_supported(self.in_channels)
+        return self.precision == "tf32" and ops.costreg_blocked_supported(self.kernel_channels)
 
     def forward_blocked(self, x):
         """Inference in the tf32 precision from the (B,Cin/4,D,h,w,4) cost volume of
@@ -362,7 +387,7 @@ class CostRegNet(nn.Module):
         if not self.blocked_supported():
             raise ops._lib.CasMVSError("CostRegNet.forward_blocked needs the tf32 precision and "
                                        "tensor-core kernels for every layer (in_channels 8, 16, 32)")
-        return ops.costreg(x, self.packed_params(), self.in_channels, ops.TF32, blocked=True)
+        return ops.costreg(x, self.packed_params(), self.kernel_channels, ops.TF32, blocked=True)
 
 
 class CascadeMVSNet(nn.Module):

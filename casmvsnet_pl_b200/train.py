@@ -60,6 +60,7 @@ from torch.optim import SGD, Adam
 from torch.optim.lr_scheduler import CosineAnnealingLR, LambdaLR, LRScheduler, MultiStepLR
 
 from . import train_data
+from .eval_pipeline import NUM_GROUPS, depth_count
 from .losses import sl1_loss_and_metrics
 
 METRIC_NAMES = ("abs_err", "acc_1mm", "acc_2mm", "acc_4mm")
@@ -75,9 +76,9 @@ def build_parser():
     ap.add_argument("--n_views", type=int, default=3)
     ap.add_argument("--levels", type=int, default=3, choices=[3])
     ap.add_argument("--depth_interval", type=float, default=2.65)
-    ap.add_argument("--n_depths", nargs="+", type=int, default=[8, 32, 48])
+    ap.add_argument("--n_depths", nargs="+", type=depth_count, default=[8, 32, 48])
     ap.add_argument("--interval_ratios", nargs="+", type=float, default=[1.0, 2.0, 4.0])
-    ap.add_argument("--num_groups", type=int, default=1, choices=[1, 2, 4, 8])
+    ap.add_argument("--num_groups", type=int, default=1, choices=NUM_GROUPS)
     ap.add_argument("--loss_type", type=str, default="sl1", choices=["sl1"])
     ap.add_argument("--batch_size", type=int, default=1)
     ap.add_argument("--num_epochs", type=int, default=16)

@@ -64,37 +64,50 @@ def costreg_layers(params, cin):
     return out
 
 
-def check_costreg_elements(tag, x, ws, logits, layers, B, D, h, w, elements):
+def check_costreg_elements(tag, x, ws, logits, layers, B, D, h, w, elements, blocked=True,
+                           kernels=None, tf32=True):
     """Check every layer of batch elements `elements` of a casmvs_costreg_fwd call: x the blocked
     input (B, Cin/4, D, h, w, 4), ws the workspace it left (blocked activations at the offsets
     the driver slices it at), logits (B, D, h, w).  The float64 reference of element b is
-    computed from element b's activations alone."""
+    computed from element b's activations alone.
+
+    blocked=False: x and the activations are channels-last (B, D, h, w, C), as the driver leaves
+    them where some layer has no tensor-core kernel or in the fp32 precision.  kernels: the eps
+    family of each layer's kernel (default: the wgmma kernel of its stride).  tf32=False: the
+    fp32 precision, whose stores and inputs are not TF32-rounded.  -> {family: worst eps needed}."""
     n = B * D * h * w
-    blocked, off = {"x": x}, 0
+    acts, off = {"x": x}, 0
     for name, c, s in CONV_T._ACTS:
         size = c * n // s ** 3
-        blocked[name] = ws[off:off + size].view(B, c // 4, D // s, h // s, w // s, 4)
+        dims = (D // s, h // s, w // s)
+        buf = ws[off:off + size]
+        acts[name] = buf.view(B, c // 4, *dims, 4) if blocked else buf.view(B, *dims, c)
         off += size
     assert (off + 64) == ws.numel()         # every float but the 64-float alignment slack
 
     def element(name, b):
         if name == "logits":
             return logits[b:b + 1].unsqueeze(-1)
-        return R.from_blocked(blocked[name][b:b + 1])
+        return R.from_blocked(acts[name][b:b + 1]) if blocked else acts[name][b:b + 1]
 
+    worst = {}
     for b in elements:
         for i, L in enumerate(layers):
             xin = element(CONV_T._IN[i], b)
-            assert CONV_T._is_tf32(xin), f"{tag} b={b}: input of layer {i} is not TF32-exact"
+            if tf32:
+                assert CONV_T._is_tf32(xin), f"{tag} b={b}: input of layer {i} is not TF32-exact"
             skip = element(CONV_T._SKIP[i], b) if i in CONV_T._SKIP else None
             slope = 1.0 if i == 10 else CONV_T.SLOPE
             y64, A, extra = layer_fp64(xin, L["w"], L["kind"], L["stride"], L["scale"],
                                        L["shift"], slope, skip)
-            CONV_T._check(f"{tag} b={b} layer {i} ({CONV_T._OUT[i]})",
-                          "tma" if L["stride"] == 1 else "tma2", element(CONV_T._OUT[i], b), y64,
-                          A, R.R_TF32 if L["cout"] > 1 else 0.0, extra)
+            kernel = kernels[i] if kernels else "tma" if L["stride"] == 1 else "tma2"
+            need = CONV_T._check(f"{tag} b={b} layer {i} ({CONV_T._OUT[i]})", kernel,
+                                 element(CONV_T._OUT[i], b), y64, A,
+                                 R.R_TF32 if tf32 and L["cout"] > 1 else 0.0, extra)
+            worst[kernel] = max(worst.get(kernel, 0.0), need)
             del xin, skip, y64, A, extra
     print(f"[fp64] {tag}: checked batch elements {list(elements)} of B={B}")
+    return worst
 
 
 def _blocked_input(seed, cin, B, D, h, w):
@@ -352,12 +365,12 @@ def test_per_element_reference_equals_whole_batch():
 _SMALL = (8, 3, 8, 16, 24)     # Cin, B, D, h, w
 
 
-def _small_net():
-    """A CostRegNet driver call simulated in float64 on the CPU at _SMALL: random layers of the
-    driver's shapes; each activation is its float64 layer, TF32-rounded like the kernels' stores
-    (the logits unrounded), laid out as casmvs_costreg_fwd leaves its workspace.  -> x, acts,
-    layers, with acts channels-last by name."""
-    cin, B, D, h, w = _SMALL
+def _small_net(shape=_SMALL):
+    """A CostRegNet driver call simulated in float64 on the CPU at `shape` (Cin, B, D, h, w):
+    random layers of the driver's shapes; each activation is its float64 layer, TF32-rounded like
+    the kernels' stores (the logits unrounded), laid out as casmvs_costreg_fwd leaves its
+    workspace.  -> x, acts, layers, with acts channels-last by name."""
+    cin, B, D, h, w = shape
     g = torch.Generator().manual_seed(5)
     layers = []
     for i in range(11):
@@ -375,13 +388,15 @@ def _small_net():
     return acts, layers
 
 
-def _pack(acts):
-    """-> blocked x, workspace, logits (B, D, h, w) in casmvs_costreg_fwd's layout."""
-    cin, B, D, h, w = _SMALL
-    ws = torch.cat([R.to_blocked(acts[name]).reshape(-1) for name, _, _ in CONV_T._ACTS] +
+def _pack(acts, shape=_SMALL, blocked=True):
+    """-> x, workspace, logits (B, D, h, w) in casmvs_costreg_fwd's layout: blocked, or with
+    blocked=False channels-last."""
+    cin, B, D, h, w = shape
+    lay = R.to_blocked if blocked else (lambda t: t.contiguous())
+    ws = torch.cat([lay(acts[name]).reshape(-1) for name, _, _ in CONV_T._ACTS] +
                    [torch.full((64,), float("nan"))])
     assert ws.numel() * 4 == _lib.load().casmvs_costreg_workspace_bytes(B, cin, D, h, w)
-    return R.to_blocked(acts["x"]), ws, acts["logits"][..., 0].contiguous()
+    return lay(acts["x"]), ws, acts["logits"][..., 0].contiguous()
 
 
 def _check_small(acts, layers):

@@ -47,6 +47,7 @@ SLOPE = 0.01
 
 
 def _check(tag, kernel, y, y64, A, r, extra=None):
+    """Asserts the bound of R.bound_excess at EPS[kernel]; returns the eps the layer needed."""
     ok, worst = R.bound_excess(y, y64, A, EPS[kernel], r, extra)
     print(f"[fp64] {tag} [{kernel}]: worst err/A {worst['eps_needed']:.3e} "
           f"(eps {EPS[kernel]:.3e}) at (b,d,h,w,c)={worst['at']}")
@@ -54,6 +55,7 @@ def _check(tag, kernel, y, y64, A, r, extra=None):
                 f"(b,d,h,w,c)={worst['at']} h%16={worst['h16']} w%8={worst['w8']} "
                 f"slice={worst['slice']}: got {worst['got']!r}, float64 {worst['want']!r}, "
                 f"A={worst['A']:.4e}, needs eps {worst['eps_needed']:.3e} > {EPS[kernel]:.3e}")
+    return worst["eps_needed"]
 
 
 def _seed(*parts):

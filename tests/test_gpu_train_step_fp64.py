@@ -84,8 +84,8 @@ def _is_tf32(t):
     return bool((t.contiguous().view(torch.int32) & 0x1FFF).eq(0).all())
 
 
-def _sample(B, W, H, seed):
-    imgs, pm, dmin, dint = synth.make_inputs(B=B, V=3, W=W, H=H, seed=seed)
+def _sample(B, W, H, seed, V=3):
+    imgs, pm, dmin, dint = synth.make_inputs(B=B, V=V, W=W, H=H, seed=seed)
     g = torch.Generator().manual_seed(seed + 1)
     depths, masks = {}, {}
     for l in range(3):
@@ -313,6 +313,8 @@ def _expected_fallbacks(tf32, G):
     fb = {(l, "prob", "dgrad") for l in LEVELS}          # Cout = 1: a 4 -> 8 adjoint
     if G == 1:
         fb.add((1, "conv0", "dgrad"))                      # 8 -> 16: no stride-1 kernel
+    if G in (2, 4):                                        # 4 -> 8 (G = 2 zero-padded to 4)
+        fb |= {(l, "conv0", "forward") for l in LEVELS}
     return fb
 
 

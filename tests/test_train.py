@@ -149,6 +149,30 @@ def test_cli_rejects_unsupported(argv, msg):
     assert msg in str(e.value.code)
 
 
+@pytest.mark.parametrize("argv,flag", [(["--n_depths", "8", "32", "44"], "--n_depths"),
+                                       (["--n_depths", "0", "32", "48"], "--n_depths"),
+                                       (["--n_depths", "-8"], "--n_depths"),
+                                       (["--num_groups", "3"], "--num_groups"),
+                                       (["--num_groups", "16"], "--num_groups")])
+def test_cli_refuses_bad_depths_and_groups_at_parsing(argv, flag, capsys):
+    from casmvsnet_pl_b200 import eval_pipeline
+    with pytest.raises(SystemExit) as e:
+        train.build_parser().parse_args(argv)
+    assert e.value.code == 2 and f"argument {flag}" in capsys.readouterr().err
+    with pytest.raises(SystemExit) as e:
+        eval_pipeline.parse_args(["--root_dir", "x"] + argv)
+    assert e.value.code == 2 and f"argument {flag}" in capsys.readouterr().err
+
+
+def test_cli_accepts_the_depths_and_groups_the_network_runs():
+    from casmvsnet_pl_b200 import eval_pipeline
+    for g in (1, 2, 4, 8):
+        argv = ["--num_groups", str(g), "--n_depths", "8", "24", "192"]
+        a = train.build_parser().parse_args(argv)
+        b = eval_pipeline.parse_args(["--root_dir", "x"] + argv)
+        assert a.num_groups == b.num_groups == g and a.n_depths == b.n_depths == [8, 24, 192]
+
+
 def test_top_k_checkpoints_keep_the_best(tmp_path):
     keep = train.TopKCheckpoints(str(tmp_path), k=2)
     m = torch.nn.Linear(1, 1)
