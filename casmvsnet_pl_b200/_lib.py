@@ -139,6 +139,32 @@ SIGNATURES = {
     "casmvs_mesh_count": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
     "casmvs_mesh_vertices": (c_int, [c_void_p, c_void_p, c_int, c_float] + [c_void_p] * 7),
     "casmvs_mesh_faces": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
+    "casmvs_poisson_workspace_bytes": (c_size_t, [c_longlong]),
+    "casmvs_poisson_cell_keys": (c_int, [c_void_p, c_void_p, c_int, c_float] + [c_int] * 4
+                                 + [c_void_p] * 3),
+    "casmvs_poisson_cell_moments": (c_int, [c_void_p, c_void_p, c_int] + [c_double] * 3
+                                    + [c_void_p] * 2),
+    "casmvs_poisson_cell_normals": (c_int, [c_void_p] * 3 + [c_int] * 2 + [c_void_p] * 3),
+    "casmvs_poisson_orient": (c_int, [c_void_p] * 3 + [c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_poisson_splat": (c_int, [c_void_p] * 5 + [c_int, c_float] + [c_int] * 3
+                             + [c_void_p] * 4),
+    "casmvs_poisson_rhs": (c_int, [c_void_p, c_int, c_float] + [c_void_p] * 4),
+    "casmvs_poisson_residual": (c_int, [c_void_p, c_void_p, c_int, c_float] + [c_void_p] * 4),
+    "casmvs_poisson_smooth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_int,
+                                      c_void_p]),
+    "casmvs_poisson_mg_residual": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p,
+                                           c_void_p]),
+    "casmvs_poisson_restrict": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_poisson_prolong_add": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "casmvs_poisson_accumulate": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
+    "casmvs_poisson_iso_sum": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float] + [c_int] * 3
+                               + [c_void_p] * 3),
+    "casmvs_poisson_trim": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "casmvs_poisson_brick_flags": (c_int, [c_void_p] + [c_int] * 10 + [c_void_p] * 2),
+    "casmvs_poisson_fill_bricks": (c_int, [c_void_p, c_int] + [c_void_p] * 3 + [c_int] * 4
+                                   + [c_void_p] * 3),
+    "casmvs_poisson_fill_tsdf": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_double]
+                                 + [c_int] * 4 + [c_void_p] * 2),
     "casmvs_render_points_fwd": (c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
                                          c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "casmvs_render_mesh_workspace_bytes": (c_size_t, [c_int]),

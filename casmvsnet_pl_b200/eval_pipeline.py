@@ -39,6 +39,8 @@ proba_XXXX.pfm are written as well).
 
 --mesh also fuses each scan's filtered depth maps into a TSDF volume on the GPU and writes the
 marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes changes.
+--mesh --mesh_method poisson [--poisson_depth 9] meshes the scan's fused points by Poisson surface
+reconstruction instead (poisson.py).
 """
 from __future__ import annotations
 
@@ -431,7 +433,8 @@ class ColmapScan(_CachedScan):
 def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
-             tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None):
+             tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
+             mesh_method="tsdf", poisson_depth=None):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -441,7 +444,10 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     <ply>_scores.json when ply_path is given, and (xyz, rgb, scores) is returned.
     With `mesh_path`, the masked refined depth maps are also fused into a TSDF volume and the
     marching-cubes mesh is written there as a PLY (mesh.py; voxel size `mesh_voxel`, default
-    mesh.default_voxel_size); the other outputs are unchanged.
+    mesh.default_voxel_size); the other outputs are unchanged.  With mesh_method="poisson" the
+    mesh is instead the Poisson surface (poisson.py, grid depth `poisson_depth`, default 9) of
+    every fused point (not thinned by `skip`), coloured by the refined image at its pixel, its
+    normals oriented toward the reference cameras.
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
@@ -465,7 +471,26 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
                                 skip, max_ref_views, collect=fused)
     if ply_path:
         fusion.write_ply(ply_path, xyz, rgb)
-    if mesh_path:
+    if mesh_path and mesh_method == "poisson":
+        from . import mesh, poisson
+        if not fused:
+            raise ValueError(f"{scan.scan}: no reference view was fused, nothing to mesh")
+        pts = torch.cat([f["points"] for f in fused]).float()
+        cols = torch.cat([f["image"][f["depth"] != 0] for f in fused]).to(torch.uint8)
+        if len(cols) != len(pts):
+            raise ValueError(f"{scan.scan}: the fused depth maps and points disagree")
+        cams = np.stack([-np.linalg.inv(np.asarray(f["P"], np.float64)[:3, :3]) @
+                         np.asarray(f["P"], np.float64)[:3, 3] for f in fused])
+        del fused
+        verts, colours, faces, st = poisson.poisson_mesh(
+            pts, cols, cam_centres=cams,
+            depth=poisson.DEFAULT_DEPTH if poisson_depth is None else poisson_depth, log=log)
+        del pts, cols
+        mesh.write_mesh_ply(mesh_path, verts, colours, faces)
+        log(f"{scan.scan}: poisson mesh at depth {st['depth']} (h {st['h']:.6g}): {st['points']} "
+            f"points ({st['dropped']} dropped), {st['cycles']} cycles, {st['bricks']} bricks, "
+            f"{st['vertices']} vertices, {st['triangles']} triangles")
+    elif mesh_path:
         from . import mesh
         if not fused:
             raise ValueError(f"{scan.scan}: no reference view was fused, nothing to mesh")
@@ -573,9 +598,23 @@ def parse_args(argv=None):
     ap.add_argument("--mesh_voxel", type=float, default=None,
                     help="voxel size of --mesh in world units (default: 2 x the median pixel "
                          "footprint at the views' median depth)")
+    ap.add_argument("--mesh_method", default=None, choices=["tsdf", "poisson"],
+                    help="with --mesh: tsdf (default) fuses the depth maps into a TSDF volume; "
+                         "poisson meshes the fused points by Poisson surface reconstruction")
+    ap.add_argument("--poisson_depth", type=int, default=None,
+                    help="with --mesh_method poisson: the grid depth, 6..10 (default 9)")
     a = ap.parse_args(argv)
     if a.mesh_voxel is not None and not a.mesh_voxel > 0:
         ap.error("--mesh_voxel must be > 0")
+    if a.mesh_method is not None and not a.mesh:
+        ap.error("--mesh_method needs --mesh")
+    if a.mesh_voxel is not None and a.mesh_method == "poisson":
+        ap.error("--mesh_voxel applies to --mesh_method tsdf, not poisson")
+    if a.poisson_depth is not None and a.mesh_method != "poisson":
+        ap.error("--poisson_depth needs --mesh_method poisson")
+    if a.poisson_depth is not None and not 6 <= a.poisson_depth <= 10:
+        ap.error("--poisson_depth must be in 6..10")
+    a.mesh_method = a.mesh_method or "tsdf"
     if a.depth_interval is None:
         a.depth_interval = DEFAULT_DEPTH_INTERVAL[a.dataset_name]
     a.out_dir = a.out or os.path.join("results", a.dataset_name)
@@ -616,7 +655,8 @@ def main(argv=None):
                        ply_path=os.path.join(out_dir, "points", f"{scan.scan}.ply"), dtu_gt=a.dtu_gt,
                        dtu_seed=a.dtu_seed, save_visual=a.save_visual,
                        mesh_path=os.path.join(out_dir, "mesh", f"{scan.scan}.ply") if a.mesh else None,
-                       mesh_voxel=a.mesh_voxel, **tnt)
+                       mesh_voxel=a.mesh_voxel, mesh_method=a.mesh_method,
+                       poisson_depth=a.poisson_depth, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

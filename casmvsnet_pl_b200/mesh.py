@@ -105,11 +105,7 @@ class TSDFVolume:
         return keys.contiguous(), int(dropped.item())
 
     def _check_fits(self, max_bytes):
-        if max_bytes is None:
-            free, total = torch.cuda.mem_get_info(self.device)
-            free += torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
-            max_bytes = free - max(1 << 30, total // 20)         # margin: 1 GiB or 5 %
-        budget = min(max_bytes, MAX_BRICKS * 512 * BYTES_PER_VOXEL)
+        budget = min(device_budget(self.device, max_bytes), MAX_BRICKS * 512 * BYTES_PER_VOXEL)
         need = self.n_voxels * BYTES_PER_VOXEL
         if need <= budget:
             return
@@ -158,32 +154,48 @@ class TSDFVolume:
     def extract(self):
         """Marching cubes -> (verts (N,3) float32, colours (N,3) uint8, faces (M,3) int32) on the
         device, in the same order and bits on every run."""
-        lib = _lib.load()
-        dev, nb, nvox = self.device, self.n_bricks, self.n_voxels
-        i32 = dict(dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            cases = torch.empty(nvox, dtype=torch.uint8, device=dev)
-            tri_count = torch.empty(nvox, **i32)
-            edge_used = torch.empty(nvox * 3, **i32)
-            _lib.check(lib.casmvs_mesh_count(_ptr(self.nbr), nb, _ptr(self.tsdf), _ptr(self.weight),
-                                             _ptr(cases), _ptr(tri_count), _ptr(edge_used),
-                                             _stream()), "mesh_count")
-            edge_scan = torch.cumsum(edge_used, 0, dtype=torch.int32)
-            tri_scan = torch.cumsum(tri_count, 0, dtype=torch.int32)
-            n_verts = int(edge_scan[-1]) if nvox else 0
-            n_faces = int(tri_scan[-1]) if nvox else 0
-            verts = torch.empty(n_verts, 3, dtype=torch.float32, device=dev)
-            colours = torch.empty(n_verts, 3, dtype=torch.uint8, device=dev)
-            faces = torch.empty(n_faces, 3, **i32)
-            if n_faces:
-                _lib.check(lib.casmvs_mesh_vertices(
-                    _ptr(self.keys), _ptr(self.nbr), nb, self.voxel, _ptr(self.tsdf),
-                    _ptr(self.color), _ptr(edge_used), _ptr(edge_scan), _ptr(verts), _ptr(colours),
-                    _stream()), "mesh_vertices")
-                _lib.check(lib.casmvs_mesh_faces(
-                    _ptr(self.nbr), nb, _ptr(cases), _ptr(tri_count), _ptr(tri_scan),
-                    _ptr(edge_scan), _ptr(faces), _stream()), "mesh_faces")
-        return verts, colours, faces
+        with torch.cuda.device(self.device):
+            return extract_bricks(self.keys, self.nbr, self.voxel, self.tsdf, self.weight, self.color)
+
+
+def device_budget(device, max_bytes=None):
+    """The bytes a new volume may take on `device`: `max_bytes`, or by default the free device
+    memory (counting what torch's allocator holds unused) less a margin of 1 GiB or 5 %."""
+    if max_bytes is not None:
+        return max_bytes
+    free, total = torch.cuda.mem_get_info(device)
+    free += torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+    return free - max(1 << 30, total // 20)
+
+
+def extract_bricks(keys, nbr, voxel, tsdf, weight, color):
+    """Marching cubes over a brick volume (keys (nb,) sorted, nbr (nb,7) from
+    casmvs_mesh_brick_neighbors, tsdf / weight (nb*512), color (nb*512,3) float32) on the current
+    device -> (verts (N,3) float32, colours (N,3) uint8, faces (M,3) int32)."""
+    lib = _lib.load()
+    dev, nb = keys.device, int(keys.numel())
+    nvox = nb * 512
+    i32 = dict(dtype=torch.int32, device=dev)
+    cases = torch.empty(nvox, dtype=torch.uint8, device=dev)
+    tri_count = torch.empty(nvox, **i32)
+    edge_used = torch.empty(nvox * 3, **i32)
+    _lib.check(lib.casmvs_mesh_count(_ptr(nbr), nb, _ptr(tsdf), _ptr(weight), _ptr(cases),
+                                     _ptr(tri_count), _ptr(edge_used), _stream()), "mesh_count")
+    edge_scan = torch.cumsum(edge_used, 0, dtype=torch.int32)
+    tri_scan = torch.cumsum(tri_count, 0, dtype=torch.int32)
+    n_verts = int(edge_scan[-1]) if nvox else 0
+    n_faces = int(tri_scan[-1]) if nvox else 0
+    verts = torch.empty(n_verts, 3, dtype=torch.float32, device=dev)
+    colours = torch.empty(n_verts, 3, dtype=torch.uint8, device=dev)
+    faces = torch.empty(n_faces, 3, **i32)
+    if n_faces:
+        _lib.check(lib.casmvs_mesh_vertices(
+            _ptr(keys), _ptr(nbr), nb, voxel, _ptr(tsdf), _ptr(color), _ptr(edge_used),
+            _ptr(edge_scan), _ptr(verts), _ptr(colours), _stream()), "mesh_vertices")
+        _lib.check(lib.casmvs_mesh_faces(
+            _ptr(nbr), nb, _ptr(cases), _ptr(tri_count), _ptr(tri_scan), _ptr(edge_scan),
+            _ptr(faces), _stream()), "mesh_faces")
+    return verts, colours, faces
 
 
 def pixel_footprint(depth, P):

@@ -619,6 +619,94 @@ int casmvs_mesh_vertices(const long long* keys, const int* nbr, int nb, float vo
 int casmvs_mesh_faces(const int* nbr, int nb, const unsigned char* cases, const int* tri_count,
                       const int* tri_scan, const int* edge_scan, int* faces, void* stream);
 
+/* ---- Poisson surface reconstruction (csrc/poisson.cu, casmvsnet_pl_b200/poisson.py) ---------
+ * A dense grid of N^3 nodes (N a power of two, 8..1024), spacing h; local node (x,y,z) is the
+ * global node lo + (x,y,z) at world (lo + x) h; dense fields are flat, index (x N + y) N + z.  A
+ * point p's cell is the node round(p / h) (float division, half to even); its splat corners are
+ * floor(p / h) + {0,1}^3 with float32 weights (wx wy) wz, w = frac or 1 - frac, frac =
+ * p / h - floor(p / h).  No float atomics: every sum has a fixed order.
+ * casmvs_poisson_cell_keys: keys (n) int64 = flat local cell index, INT64_MAX for a point that is
+ *   not finite, lies outside the grid, or (normals != NULL) has a zero-length or non-finite
+ *   normal; unit_normals (n,3) f32 = normals / |normals| computed in double (0 when dropped).
+ * casmvs_poisson_cell_moments: cells are runs of equal keys in the sorted points; cell_start
+ *   (n_cells + 1) int32 offsets.  moments (n_cells,10) f64 = count, sum d, sum d d^T (xx, xy, xz,
+ *   yy, yz, zz), d = p - (cx,cy,cz), summed in point order.
+ * casmvs_poisson_cell_normals: cell_of (N^3) int32 = cell number of a node, -1 if empty; per cell,
+ *   the moments of the 3x3x3 cells around it (x-major order) give the covariance; cell_normals
+ *   (n_cells,3) f64 = unit eigenvector of its smallest eigenvalue (Jacobi, double); cell_ok = 0
+ *   when the block holds < 3 points or lambda_mid <= 1e-10 lambda_max.
+ * casmvs_poisson_orient: normals (n,3) f32 = the point's cell normal (point_cell (n) int32),
+ *   flipped so that n . (C - p) > 0 for the nearest camera centre C of cams (n_cams,3) f64 on the
+ *   device (ties to the lower index; a dot product of 0 keeps the sign).
+ * casmvs_poisson_splat: one thread per node gathers the sorted points of the 27 cells around it:
+ *   V (N^3,3) = sum w n, W (N^3) = sum w, C (N^3,3) = sum w rgb (rgb (n,3) u8, NULL = white),
+ *   summed in double in cell and point order, stored f32.
+ * casmvs_poisson_rhs: b (N^3) f32 = div V by central differences / (2h) at interior nodes, 0 on
+ *   the outer layer; *bb (device f64) = sum of b^2.  workspace: casmvs_poisson_workspace_bytes(N^3).
+ * Multigrid for (sum of the 6 neighbours - 6 x) / h^2 = rhs.  Level l (0 = finest) has n = N >> l
+ * nodes per axis stored, node I at fine node 2^l I.  Level 0 has x = 0 on its outer layer (indices
+ * 0 and N - 1, interior 1..N-2).  A coarse level (l > 0) has x = 0 at index 0 and at index n, fine
+ * index N on every coarse level; node n is not stored and reads as 0, so the interior is 1..n-1.
+ * casmvs_poisson_residual: r (N^3) f32 = b - L chi computed in double from chi (N^3) f64 on level
+ *   0, 0 on the outer layer; *rr (device f64) = sum of r^2 (before rounding).
+ * casmvs_poisson_smooth: `sweeps` red-black Gauss-Seidel sweeps (red: x+y+z even, first) on e
+ *   (n^3) f32 of level `level` with right-hand side r at spacing h; zero_first: start from e = 0.
+ * casmvs_poisson_mg_residual: out = r - L e (f32) at the level's interior nodes, 0 elsewhere.
+ * casmvs_poisson_restrict: coarse (nf/2)^3 = full weighting of fine at coarse interior node I
+ *   (1..nf/2-1; fine 2I + {-1,0,1}^3, weights (1/4,1/2,1/4)^3), 0 elsewhere.
+ * casmvs_poisson_prolong_add: the interior nodes of fine (level fine_level, (2nc)^3) += trilinear
+ *   interpolation of coarse (nc^3), coarse node I at fine 2I, coarse index nc counting as 0.
+ * casmvs_poisson_accumulate: chi (f64) += e (f32).
+ * casmvs_poisson_iso_sum: *sum (device f64) = sum over the points of chi trilinearly interpolated;
+ *   a corner outside the grid counts as chi = 0 (poisson.py's grid keeps every corner inside).
+ * casmvs_poisson_trim: keep (N^3) u8 = 1 where the 5x5x5 box around the node holds W > 0;
+ *   workspace N^3 bytes.
+ * casmvs_poisson_brick_flags: flags (nb_x,nb_y,nb_z) u8 = 1 for the global bricks b0 + (i,j,k)
+ *   (mesh.cu's 8^3 bricks, key floor(global node / 8)) that hold a kept node.
+ * casmvs_poisson_fill_bricks: in mesh.cu's brick layout (keys sorted), weight = 1 and colour =
+ *   box5(C) / box5(W) (sums in double) at kept nodes, weight 0 and colour 0 elsewhere.
+ * casmvs_poisson_fill_tsdf: tsdf = chi - iso (double, rounded once) where weight > 0, else 0.
+ * casmvs_poisson_workspace_bytes: the reduction workspace for n terms. */
+size_t casmvs_poisson_workspace_bytes(long long n);
+int casmvs_poisson_cell_keys(const float* points, const float* normals, int n, float h, int lo_x,
+                             int lo_y, int lo_z, int N, long long* keys, float* unit_normals,
+                             void* stream);
+int casmvs_poisson_cell_moments(const float* points, const int* cell_start, int n_cells, double cx,
+                                double cy, double cz, double* moments, void* stream);
+int casmvs_poisson_cell_normals(const long long* cell_keys, const int* cell_of,
+                                const double* moments, int n_cells, int N, double* cell_normals,
+                                unsigned char* cell_ok, void* stream);
+int casmvs_poisson_orient(const float* points, const int* point_cell, const double* cell_normals,
+                          int n, const double* cams, int n_cams, float* normals, void* stream);
+int casmvs_poisson_splat(const float* points, const float* normals, const unsigned char* rgb,
+                         const int* cell_start, const int* cell_of, int N, float h, int lo_x,
+                         int lo_y, int lo_z, float* V, float* W, float* C, void* stream);
+int casmvs_poisson_rhs(const float* V, int N, float h, float* b, double* workspace, double* bb,
+                       void* stream);
+int casmvs_poisson_residual(const double* chi, const float* b, int N, float h, float* r,
+                            double* workspace, double* rr, void* stream);
+int casmvs_poisson_smooth(float* e, const float* r, int n, int level, float h, int sweeps,
+                          int zero_first, void* stream);
+int casmvs_poisson_mg_residual(const float* e, const float* r, int n, int level, float h,
+                               float* out, void* stream);
+int casmvs_poisson_restrict(const float* fine, int nf, float* coarse, void* stream);
+int casmvs_poisson_prolong_add(const float* coarse, int nc, float* fine, int fine_level,
+                               void* stream);
+int casmvs_poisson_accumulate(double* chi, const float* e, int N, void* stream);
+int casmvs_poisson_iso_sum(const double* chi, const float* points, int n, int N, float h, int lo_x,
+                           int lo_y, int lo_z, double* workspace, double* sum, void* stream);
+int casmvs_poisson_trim(const float* W, int N, unsigned char* keep, unsigned char* workspace,
+                        void* stream);
+int casmvs_poisson_brick_flags(const unsigned char* keep, int N, int lo_x, int lo_y, int lo_z,
+                               int b0_x, int b0_y, int b0_z, int nb_x, int nb_y, int nb_z,
+                               unsigned char* flags, void* stream);
+int casmvs_poisson_fill_bricks(const long long* keys, int nb, const unsigned char* keep,
+                               const float* W, const float* C, int N, int lo_x, int lo_y, int lo_z,
+                               float* weight, float* color, void* stream);
+int casmvs_poisson_fill_tsdf(const long long* keys, int nb, const float* weight, const double* chi,
+                             double iso, int N, int lo_x, int lo_y, int lo_z, float* tsdf,
+                             void* stream);
+
 /* ---- headless rendering of clouds and meshes (casmvsnet_pl_b200/render.py) -----------------
  * P is a HOST array of 16 floats, row-major, world -> pixel (rows 0..2 used): every float
  * operation below is rounded to nearest, no contraction, in the order written.
