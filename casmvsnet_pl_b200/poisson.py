@@ -145,28 +145,29 @@ def _vcycle(l, sizes, hs, e, rhs, tmp):
 
 
 def _solve(b, bb, N, h, ws):
-    """V(2,2) multigrid for L chi = b -> (chi (N^3) float64, cycles, ||r|| / ||b||).  chi and the
-    residual are kept in double on the finest level; each cycle solves for the correction in
-    float32."""
+    """V(2,2) multigrid for L chi = b -> (chi (N^3) float64, cycles, ||r|| / ||b|| before each
+    cycle and at the end (cycles + 1 values)).  chi and the residual are kept in double on the
+    finest level; each cycle solves for the correction in float32."""
     lib, st, dev = _lib.load(), _stream(), b.device
     sizes = [N >> l for l in range(0, 32) if (N >> l) >= COARSEST]
     f32 = dict(dtype=torch.float32, device=dev)
     chi = torch.zeros(N ** 3, dtype=torch.float64, device=dev)
     bn = math.sqrt(bb)
     if bn == 0:
-        return chi, 0, 0.0
+        return chi, 0, [0.0]
     rhs = [torch.empty(n ** 3, **f32) for n in sizes]
     e = [torch.empty(n ** 3, **f32) for n in sizes]
     tmp = [torch.empty(n ** 3, **f32) for n in sizes[:-1]]
     hs = [float(np.float32(h * (1 << l))) for l in range(len(sizes))]
     rr = torch.zeros(1, dtype=torch.float64, device=dev)
     cycles = 0
+    ratios = []
     while True:
         _lib.check(lib.casmvs_poisson_residual(_ptr(chi), _ptr(b), N, h, _ptr(rhs[0]), _ptr(ws),
                                                _ptr(rr), st), "poisson_residual")
-        ratio = math.sqrt(float(rr.item())) / bn
-        if ratio <= TOL or cycles == MAX_CYCLES:
-            return chi, cycles, ratio
+        ratios.append(math.sqrt(float(rr.item())) / bn)
+        if ratios[-1] <= TOL or cycles == MAX_CYCLES:
+            return chi, cycles, ratios
         _vcycle(0, sizes, hs, e, rhs, tmp)
         _lib.check(lib.casmvs_poisson_accumulate(_ptr(chi), _ptr(e[0]), N, st), "poisson_accumulate")
         cycles += 1
@@ -178,7 +179,8 @@ def poisson_mesh(xyz, rgb=None, normals=None, cam_centres=None, depth=DEFAULT_DE
     (None: white) and either normals (n,3) float32 (normalised; zero-length ones are dropped) or
     the camera centres cam_centres (k,3) that estimated normals are oriented toward.
     -> (verts (V,3) float32, colours (V,3) uint8, faces (F,3) int32 on the device, stats dict:
-    h, N, depth, points, dropped, cycles, residual, iso, bricks, vertices, triangles).
+    h, N, depth, points, dropped, cycles, residual, ratios (||r|| / ||b|| before each cycle and
+    at the end), iso, bricks, vertices, triangles).
     Raises ValueError for a depth outside 6..10, a cloud without a finite point or with zero
     extent, or neither normals nor cameras; CasMVSError when the grid, or once they are known the
     grid and the mesh bricks, would not fit in free device memory (or `max_bytes`), naming the
@@ -307,7 +309,8 @@ def poisson_mesh(xyz, rgb=None, normals=None, cam_centres=None, depth=DEFAULT_DE
         del keepn, W, C
         mark("trim_bricks")
         # solve, iso level, field
-        chi, cycles, ratio = _solve(b, float(bb.item()), N, h, ws)
+        chi, cycles, ratios = _solve(b, float(bb.item()), N, h, ws)
+        ratio = ratios[-1]
         del b, ws
         ws_p = torch.empty(max(1, lib.casmvs_poisson_workspace_bytes(n_kept) // 8),
                            dtype=torch.float64, device=dev)
@@ -329,7 +332,8 @@ def poisson_mesh(xyz, rgb=None, normals=None, cam_centres=None, depth=DEFAULT_DE
         log(f"poisson: the multigrid solve stopped after {cycles} cycles at residual ratio "
             f"{ratio:.3g} (> {TOL:g}); the mesh is from the unconverged field")
     stats = dict(h=h, N=N, depth=depth, points=n_kept, dropped=dropped, cycles=cycles,
-                 residual=ratio, iso=iso, bricks=nb, vertices=len(verts), triangles=len(faces))
+                 residual=ratio, ratios=ratios, iso=iso, bricks=nb, vertices=len(verts),
+                 triangles=len(faces))
     return verts, colours, faces, stats
 
 
