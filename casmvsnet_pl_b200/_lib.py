@@ -165,6 +165,21 @@ SIGNATURES = {
                                    + [c_void_p] * 3),
     "casmvs_poisson_fill_tsdf": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_double]
                                  + [c_int] * 4 + [c_void_p] * 2),
+    "casmvs_poisson_screen_keys": (c_int, [c_void_p, c_int, c_float] + [c_int] * 4
+                                   + [c_void_p] * 2),
+    "casmvs_poisson_screen_moments": (c_int, [c_void_p] * 3 + [c_int, c_float] + [c_int] * 3
+                                      + [c_void_p] * 2),
+    "casmvs_poisson_screen_coarsen": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                              c_void_p, c_void_p]),
+    "casmvs_poisson_screen_rhs": (c_int, [c_void_p] * 4 + [c_int, c_double] + [c_void_p] * 4),
+    "casmvs_poisson_screen_stencil": (c_int, [c_void_p, c_int] + [c_void_p] * 3
+                                      + [c_int, c_void_p, c_void_p, c_void_p]),
+    "casmvs_poisson_screen_residual": (c_int, [c_void_p] * 5 + [c_int, c_float, c_double]
+                                       + [c_void_p] * 4),
+    "casmvs_poisson_screen_mg_residual": (c_int, [c_void_p] * 5 + [c_int, c_int, c_float, c_double]
+                                          + [c_void_p] * 2),
+    "casmvs_poisson_screen_smooth": (c_int, [c_void_p] * 5 + [c_int, c_int, c_float, c_double,
+                                                              c_int, c_int, c_void_p]),
     "casmvs_render_points_fwd": (c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
                                          c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "casmvs_render_mesh_workspace_bytes": (c_size_t, [c_int]),

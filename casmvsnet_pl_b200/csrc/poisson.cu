@@ -574,6 +574,386 @@ poisson_fill_tsdf_kernel(const long long* __restrict__ keys, int nb, const float
   tsdf[v] = f;
 }
 
+// ---------------------------------------------------------------------------- screening
+// A point's splat cell is its floor corner c; per cell, mom[27] = sum over its points of
+// Fx^a Fy^b Fz^c (index 9a + 3b + c), F the float32 fraction.  Per axis, w(0) = 1 - F and
+// w(1) = F, so w(d) w(e) and w(d) are polynomials in F with the coefficients below, and every
+// S = sum phi_i phi_j and Phi = sum phi_i of the cell is a fixed combination of its moments.
+// mask[node] bit d (d = 4 dx + 2 dy + dz) is set when cell node - d holds points; map[cell] is
+// the cell's row in mom.
+__device__ __forceinline__ double pair_coef(int d, int e, int k) {
+  if (d != e) return k == 0 ? 0.0 : (k == 1 ? 1.0 : -1.0);
+  return d ? (k == 2 ? 1.0 : 0.0) : (k == 0 ? 1.0 : (k == 1 ? -2.0 : 1.0));
+}
+
+// S[e] = sum_p phi_d(p) phi_e(p) over one cell, for corner d and its 8 corners e (x-major):
+// contract the moments over z, then y, then x
+__device__ __forceinline__ void cell_row(const double* __restrict__ m, int dx, int dy, int dz,
+                                         double (&S)[8]) {
+  double tz[2][9];
+#pragma unroll
+  for (int ez = 0; ez < 2; ++ez)
+#pragma unroll
+    for (int ab = 0; ab < 9; ++ab) {
+      double s = 0.0;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s += pair_coef(dz, ez, c) * __ldg(m + ab * 3 + c);
+      tz[ez][ab] = s;
+    }
+#pragma unroll
+  for (int ey = 0; ey < 2; ++ey)
+#pragma unroll
+    for (int ez = 0; ez < 2; ++ez) {
+      double ty[3];
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        double s = 0.0;
+#pragma unroll
+        for (int b = 0; b < 3; ++b) s += pair_coef(dy, ey, b) * tz[ez][a * 3 + b];
+        ty[a] = s;
+      }
+#pragma unroll
+      for (int ex = 0; ex < 2; ++ex) {
+        double s = 0.0;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) s += pair_coef(dx, ex, a) * ty[a];
+        S[ex * 4 + ey * 2 + ez] = s;
+      }
+    }
+}
+
+// sum_p phi_d(p) over one cell: w(0) = 1 - F, w(1) = F
+__device__ __forceinline__ double cell_phi(const double* __restrict__ m, int dx, int dy, int dz) {
+  double s = 0.0;
+#pragma unroll
+  for (int a = 0; a < 2; ++a)
+#pragma unroll
+    for (int b = 0; b < 2; ++b)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const double w = (dx ? (a ? 1.0 : 0.0) : (a ? -1.0 : 1.0)) *
+                         (dy ? (b ? 1.0 : 0.0) : (b ? -1.0 : 1.0)) *
+                         (dz ? (c ? 1.0 : 0.0) : (c ? -1.0 : 1.0));
+        if (w != 0.0) s += w * __ldg(m + a * 9 + b * 3 + c);
+      }
+  return s;
+}
+
+// splat-cell key of each point: flat floor(p / h) - lo, kPoissonKeyNone when the cell leaves
+// 0..N-2 on an axis (its corners would leave the grid)
+__global__ void __launch_bounds__(256)
+poisson_screen_keys_kernel(const float* __restrict__ pts, int n, float h, int lx, int ly, int lz,
+                           int N, long long* __restrict__ keys) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  float fr;
+  const int cx = point_axis(pts, j, 0, h, lx, fr), cy = point_axis(pts, j, 1, h, ly, fr),
+            cz = point_axis(pts, j, 2, h, lz, fr);
+  const bool ok = cx >= 0 && cy >= 0 && cz >= 0 && cx < N - 1 && cy < N - 1 && cz < N - 1;
+  keys[j] = ok ? ((long long)cx * N + cy) * N + cz : kPoissonKeyNone;
+}
+
+// one thread per cell: the 27 moments of its points (order[start[c]..start[c+1]]) in order
+__global__ void __launch_bounds__(128)
+poisson_screen_moments_kernel(const float* __restrict__ pts, const int* __restrict__ order,
+                              const int* __restrict__ start, int nc, float h, int lx, int ly,
+                              int lz, double* __restrict__ mom) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= nc) return;
+  double m[27];
+#pragma unroll
+  for (int k = 0; k < 27; ++k) m[k] = 0.0;
+  for (int q = __ldg(start + c); q < __ldg(start + c + 1); ++q) {
+    const size_t j = (size_t)__ldg(order + q);
+    float f[3];
+    point_axis(pts, j, 0, h, lx, f[0]);
+    point_axis(pts, j, 1, h, ly, f[1]);
+    point_axis(pts, j, 2, h, lz, f[2]);
+    const double px[3] = {1.0, (double)f[0], (double)f[0] * f[0]};
+    const double py[3] = {1.0, (double)f[1], (double)f[1] * f[1]};
+    const double pz[3] = {1.0, (double)f[2], (double)f[2] * f[2]};
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int b = 0; b < 3; ++b) {
+        const double ab = px[a] * py[b];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) m[a * 9 + b * 3 + k] += ab * pz[k];
+      }
+  }
+#pragma unroll
+  for (int k = 0; k < 27; ++k) mom[(size_t)c * 27 + k] = m[k];
+}
+
+// F' = (m + F) / 2 per axis: coefficient of F^k in F'^kk
+__device__ __forceinline__ double half_coef(int mbit, int kk, int k) {
+  if (kk == 0) return k == 0 ? 1.0 : 0.0;
+  if (kk == 1) return k == 1 ? 0.5 : (k == 0 && mbit ? 0.5 : 0.0);
+  return k == 2 ? 0.25 : (mbit ? (k == 1 ? 0.5 : 0.25) : 0.0);
+}
+
+// one thread per parent cell: the sum over its children m = 0..7 (x-major) of the child
+// moments under F' = (m + F) / 2, each transformed over z, then y, then x
+__global__ void __launch_bounds__(128)
+poisson_screen_coarsen_kernel(const int* __restrict__ cmap, const double* __restrict__ cmom,
+                              int nchild, const long long* __restrict__ pkeys, int np,
+                              double* __restrict__ pmom) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= np) return;
+  const int n = nchild / 2;
+  const long long key = __ldg(pkeys + c);
+  const int X = (int)(key / ((long long)n * n)), Y = (int)((key / n) % n), Z = (int)(key % n);
+  double acc[27];
+#pragma unroll
+  for (int k = 0; k < 27; ++k) acc[k] = 0.0;
+  for (int m = 0; m < 8; ++m) {
+    const int mx = m >> 2, my = (m >> 1) & 1, mz = m & 1;
+    const int k = __ldg(cmap + node(2 * X + mx, 2 * Y + my, 2 * Z + mz, nchild));
+    if (k < 0) continue;
+    const double* M = cmom + (size_t)k * 27;
+    double tz[27], ty[27];
+#pragma unroll
+    for (int ab = 0; ab < 9; ++ab)
+#pragma unroll
+      for (int kk = 0; kk < 3; ++kk) {
+        double s = 0.0;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) s += half_coef(mz, kk, q) * __ldg(M + ab * 3 + q);
+        tz[ab * 3 + kk] = s;
+      }
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int kk = 0; kk < 3; ++kk)
+#pragma unroll
+        for (int q3 = 0; q3 < 3; ++q3) {
+          double s = 0.0;
+#pragma unroll
+          for (int q = 0; q < 3; ++q) s += half_coef(my, kk, q) * tz[a * 9 + q * 3 + q3];
+          ty[a * 9 + kk * 3 + q3] = s;
+        }
+#pragma unroll
+    for (int kk = 0; kk < 3; ++kk)
+#pragma unroll
+      for (int r = 0; r < 9; ++r) {
+        double s = 0.0;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) s += half_coef(mx, kk, q) * ty[q * 9 + r];
+        acc[kk * 9 + r] += s;
+      }
+  }
+#pragma unroll
+  for (int k = 0; k < 27; ++k) pmom[(size_t)c * 27 + k] = acc[k];
+}
+
+// b_s = float32(b - gamma_t Phi) at interior nodes of level 0, 0 on the outer layer; part: b_s^2
+__global__ void __launch_bounds__(kSumThreads)
+poisson_screen_rhs_kernel(const float* __restrict__ b, const unsigned char* __restrict__ mask,
+                          const int* __restrict__ map, const double* __restrict__ mom, int N,
+                          double gamma_t, float* __restrict__ bs, double* __restrict__ part) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  double v = 0.0;
+  if (i < (size_t)N * N * N) {
+    int x, y, z;
+    node_xyz(i, N, x, y, z);
+    float o = 0.f;
+    if (interior(x, y, z, N)) {
+      const unsigned bits = __ldg(mask + i);
+      double phi = 0.0;
+      for (int d = 0; d < 8; ++d) {
+        if (!((bits >> d) & 1u)) continue;
+        const int dx = d >> 2, dy = (d >> 1) & 1, dz = d & 1;
+        const int k = __ldg(map + node(x - dx, y - dy, z - dz, N));
+        phi += cell_phi(mom + (size_t)k * 27, dx, dy, dz);
+      }
+      o = (float)((double)__ldg(b + i) - gamma_t * phi);
+    }
+    bs[i] = o;
+    v = (double)o * o;
+  }
+  const double s = block_sum(v);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+
+// The 27-point stencil of S at each listed node (a node with a set mask bit): st[k], k = 9 (dx+1)
+// + 3 (dy+1) + (dz+1), = sum over the cells d = 0..7 around the node, then their corners t = 0..7,
+// of S entries expanded in double; corners at index n drop.  Written as float32 and/or double.
+__global__ void __launch_bounds__(128)
+poisson_screen_stencil_kernel(const long long* __restrict__ nodes, int ns,
+                              const unsigned char* __restrict__ mask, const int* __restrict__ map,
+                              const double* __restrict__ mom, int n, float* __restrict__ st32,
+                              double* __restrict__ st64) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= ns) return;
+  const size_t i = (size_t)__ldg(nodes + s);
+  int x, y, z;
+  node_xyz(i, n, x, y, z);
+  const unsigned bits = __ldg(mask + i);
+  double acc[27];
+#pragma unroll
+  for (int k = 0; k < 27; ++k) acc[k] = 0.0;
+  for (int d = 0; d < 8; ++d) {
+    if (!((bits >> d) & 1u)) continue;
+    const int dx = d >> 2, dy = (d >> 1) & 1, dz = d & 1;
+    const int cx = x - dx, cy = y - dy, cz = z - dz;
+    double S[8];
+    cell_row(mom + (size_t)__ldg(map + node(cx, cy, cz, n)) * 27, dx, dy, dz, S);
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+      const int tx = t >> 2, ty = (t >> 1) & 1, tz = t & 1;
+      if (cx + tx >= n || cy + ty >= n || cz + tz >= n) continue;
+      acc[(tx - dx + 1) * 9 + (ty - dy + 1) * 3 + (tz - dz + 1)] += S[t];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 27; ++k) {
+    if (st32) st32[(size_t)s * 27 + k] = (float)acc[k];
+    if (st64) st64[(size_t)s * 27 + k] = acc[k];
+  }
+}
+
+// node_xyz for a power-of-two n <= 1024 (n^3 <= 2^30): shifts, no 64-bit division
+__device__ __forceinline__ void node_xyz_pow2(size_t i, int n, int& x, int& y, int& z) {
+  const unsigned u = (unsigned)i, s = __ffs(n) - 1, m = (unsigned)n - 1;
+  z = (int)(u & m);
+  y = (int)((u >> s) & m);
+  x = (int)(u >> (2 * s));
+}
+
+// sum_{k != 13} st[k] e[node + offset k] (k order), a neighbour at index n (unstored) drops; the
+// node is interior, so no offset leaves the grid below
+template <typename T, typename S>
+__device__ __forceinline__ T stencil_off(const T* e, const S* __restrict__ st, int x, int y, int z,
+                                         int n) {
+  T off = T(0);
+#pragma unroll 1
+  for (int k = 0; k < 27; ++k) {
+    const int X = x + k / 9 - 1, Y = y + (k / 3) % 3 - 1, Z = z + k % 3 - 1;
+    if (k == 13 || X >= n || Y >= n || Z >= n) continue;
+    off += (T)__ldg(st + k) * e[node(X, Y, Z, n)];
+  }
+  return off;
+}
+
+// r = b_s - (nbsum(chi) - 6 chi - g S chi) / h^2 at interior nodes of level 0, in double, S the
+// double stencil of the surface nodes (srow[node] its row; mask 0: no screening term)
+__global__ void __launch_bounds__(kSumThreads)
+poisson_screen_residual_kernel(const double* __restrict__ chi, const float* __restrict__ bs,
+                               const unsigned char* __restrict__ mask, const int* __restrict__ srow,
+                               const double* __restrict__ st, int N, float h, double g,
+                               float* __restrict__ r, double* __restrict__ part) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  double v = 0.0;
+  if (i < (size_t)N * N * N) {
+    int x, y, z;
+    node_xyz_pow2(i, N, x, y, z);
+    double ri = 0.0;
+    if (interior(x, y, z, N)) {
+      const double hh = (double)h * h;
+      double a = nbsum(chi, i, N) - 6.0 * chi[i];
+      if (__ldg(mask + i)) {
+        const double* s = st + (size_t)__ldg(srow + i) * 27;
+        a -= g * (__ldg(s + 13) * chi[i] + stencil_off(chi, s, x, y, z, N));
+      }
+      ri = (double)__ldg(bs + i) - a / hh;
+    }
+    r[i] = (float)ri;
+    v = ri * ri;
+  }
+  const double s = block_sum(v);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+
+// out = r - (nbsum(e) - 6 e - gl (S e)) / h2 in float32 at the level's interior nodes, 0 elsewhere
+__global__ void __launch_bounds__(256)
+poisson_screen_mg_residual_kernel(const float* __restrict__ e, const float* __restrict__ r,
+                                  const unsigned char* __restrict__ mask,
+                                  const int* __restrict__ srow, const float* __restrict__ st,
+                                  int n, int level, float h2, float gl, float* __restrict__ out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)n * n * n) return;
+  int x, y, z;
+  node_xyz_pow2(i, n, x, y, z);
+  float o = 0.f;
+  if (level_interior(x, y, z, n, level)) {
+    float a = level_nbsum(e, i, x, y, z, n) - 6.f * __ldg(e + i);
+    if (__ldg(mask + i)) {
+      const float* s = st + (size_t)__ldg(srow + i) * 27;
+      a -= gl * (__ldg(s + 13) * __ldg(e + i) + stencil_off(e, s, x, y, z, n));
+    }
+    o = __ldg(r + i) - a / h2;
+  }
+  out[i] = o;
+}
+
+// neighbour sum without __restrict__: the line smoother reads values its block wrote
+__device__ __forceinline__ float plain_nbsum(const float* e, size_t i, int x, int y, int z, int n) {
+  const size_t sx = (size_t)n * n, sy = n;
+  const float zx = x + 1 < n ? e[i + sx] : 0.f, zy = y + 1 < n ? e[i + sy] : 0.f,
+              zz = z + 1 < n ? e[i + 1] : 0.f;
+  return ((((e[i - sx] + zx) + e[i - sy]) + zy) + e[i - 1]) + zz;
+}
+
+// e = (nbsum - h2 r - gl off) / (6 + gl S_ii), float32; mask 0: (nbsum - h2 r) / 6
+__device__ __forceinline__ float screen_update(const float* e, float ri, unsigned bits,
+                                               const int* __restrict__ srow,
+                                               const float* __restrict__ st, size_t i, int x,
+                                               int y, int z, int n, float h2, float gl) {
+  const float nb = plain_nbsum(e, i, x, y, z, n);
+  if (!bits) return (nb - h2 * ri) / 6.f;
+  const float* s = st + (size_t)__ldg(srow + i) * 27;
+  return (nb - h2 * ri - gl * stencil_off(e, s, x, y, z, n)) / (6.f + gl * __ldg(s + 13));
+}
+
+// Colours 2j and 2j + 1 of an 8-colour sweep (colour = 4 (x&1) + 2 (y&1) + (z&1)): one block per
+// z-line (x, y) with 2 (x&1) + (y&1) = j, thread t owning z = 2t and 2t + 1.  The even nodes
+// update first; after the barrier the odd nodes read them.  Lines of one (x, y) parity share no
+// cell and no neighbour, so this is Gauss-Seidel in the colour order.
+__global__ void __launch_bounds__(512)
+poisson_screen_smooth_lines_kernel(float* e, const float* __restrict__ r,
+                                   const unsigned char* __restrict__ mask,
+                                   const int* __restrict__ srow, const float* __restrict__ st,
+                                   int n, int level, float h2, float gl, int j) {
+  const int m = n / 2;
+  const int sm = __ffs(m) - 1;                         // m = n / 2 is a power of two
+  const int x = 2 * (int)(blockIdx.x >> sm) + (j >> 1), y = 2 * (int)(blockIdx.x & (m - 1)) + (j & 1);
+  const int top = level ? n : n - 1;
+  const bool line_in = x > 0 && y > 0 && x < top && y < top;
+#pragma unroll
+  for (int cz = 0; cz < 2; ++cz) {
+    const int z = 2 * (int)threadIdx.x + cz;
+    if (line_in && z > 0 && z < top) {
+      const size_t i = node(x, y, z, n);
+      e[i] = screen_update(e, __ldg(r + i), __ldg(mask + i), srow, st, i, x, y, z, n, h2, gl);
+    }
+    __syncthreads();
+  }
+}
+
+// The coarsest grid (n^3 <= 512 nodes) in one block: e = 0, then `sweeps` 8-colour sweeps.
+__global__ void __launch_bounds__(512)
+poisson_screen_smooth_coarse_kernel(float* __restrict__ e, const float* __restrict__ r,
+                                    const unsigned char* __restrict__ mask,
+                                    const int* __restrict__ srow, const float* __restrict__ st,
+                                    int n, int level, float h2, float gl, int sweeps) {
+  __shared__ float se[512];
+  const int i = threadIdx.x, nn = n * n * n;
+  int x = 0, y = 0, z = 0;
+  if (i < nn) node_xyz(i, n, x, y, z);
+  const bool in = i < nn && level_interior(x, y, z, n, level);
+  const float ri = in ? r[i] : 0.f;
+  const unsigned bits = in ? mask[i] : 0u;
+  const int mine = 4 * (x & 1) + 2 * (y & 1) + (z & 1);
+  if (i < nn) se[i] = 0.f;
+  __syncthreads();
+  for (int s = 0; s < sweeps; ++s)
+    for (int colour = 0; colour < 8; ++colour) {
+      if (in && mine == colour) se[i] = screen_update(se, ri, bits, srow, st, i, x, y, z, n, h2, gl);
+      __syncthreads();
+    }
+  if (i < nn) e[i] = se[i];
+}
+
 inline int finish_sum(double* part, int nparts, double* out, cudaStream_t st, const char* what) {
   poisson_sum_partials_kernel<<<1, 1024, 0, st>>>(part, nparts, out);
   return after_launch(what);
@@ -802,4 +1182,132 @@ extern "C" int casmvs_poisson_fill_tsdf(const long long* keys, int nb, const flo
   poisson_fill_tsdf_kernel<<<pblocks((size_t)nb * 512), 256, 0, as_stream(stream)>>>(
       keys, nb, weight, chi, iso, N, lo_x, lo_y, lo_z, tsdf);
   return after_launch("poisson_fill_tsdf");
+}
+
+extern "C" int casmvs_poisson_screen_keys(const float* points, int n, float h, int lo_x, int lo_y,
+                                          int lo_z, int N, long long* keys, void* stream) {
+  CASMVS_REQUIRE(n >= 0, "poisson_screen_keys: n < 0");
+  CASMVS_REQUIRE(h > 0.f, "poisson_screen_keys: h must be > 0");
+  POISSON_GRID("poisson_screen_keys", N);
+  if (n == 0) return 0;
+  CASMVS_REQUIRE(points && keys, "poisson_screen_keys: null pointer");
+  poisson_screen_keys_kernel<<<pblocks(n), 256, 0, as_stream(stream)>>>(points, n, h, lo_x, lo_y,
+                                                                        lo_z, N, keys);
+  return after_launch("poisson_screen_keys");
+}
+
+extern "C" int casmvs_poisson_screen_moments(const float* points, const int* order,
+                                             const int* cell_start, int n_cells, float h, int lo_x,
+                                             int lo_y, int lo_z, double* moments, void* stream) {
+  CASMVS_REQUIRE(n_cells >= 0, "poisson_screen_moments: n_cells < 0");
+  CASMVS_REQUIRE(h > 0.f, "poisson_screen_moments: h must be > 0");
+  if (n_cells == 0) return 0;
+  CASMVS_REQUIRE(points && order && cell_start && moments, "poisson_screen_moments: null pointer");
+  poisson_screen_moments_kernel<<<(n_cells + 127) / 128, 128, 0, as_stream(stream)>>>(
+      points, order, cell_start, n_cells, h, lo_x, lo_y, lo_z, moments);
+  return after_launch("poisson_screen_moments");
+}
+
+extern "C" int casmvs_poisson_screen_coarsen(const int* child_map, const double* child_moments,
+                                             int n_child, const long long* parent_keys,
+                                             int n_parents, double* parent_moments, void* stream) {
+  POISSON_GRID("poisson_screen_coarsen", n_child);
+  CASMVS_REQUIRE(n_child >= 16, "poisson_screen_coarsen: the child grid needs >= 16 nodes per axis");
+  CASMVS_REQUIRE(n_parents >= 0, "poisson_screen_coarsen: n_parents < 0");
+  if (n_parents == 0) return 0;
+  CASMVS_REQUIRE(child_map && child_moments && parent_keys && parent_moments,
+                 "poisson_screen_coarsen: null pointer");
+  poisson_screen_coarsen_kernel<<<(n_parents + 127) / 128, 128, 0, as_stream(stream)>>>(
+      child_map, child_moments, n_child, parent_keys, n_parents, parent_moments);
+  return after_launch("poisson_screen_coarsen");
+}
+
+extern "C" int casmvs_poisson_screen_rhs(const float* b, const unsigned char* mask, const int* map,
+                                         const double* moments, int N, double gamma_t, float* b_s,
+                                         double* workspace, double* bb, void* stream) {
+  POISSON_GRID("poisson_screen_rhs", N);
+  CASMVS_REQUIRE(b && mask && map && moments && b_s && workspace && bb,
+                 "poisson_screen_rhs: null pointer");
+  const unsigned nblk = pblocks((size_t)N * N * N);
+  poisson_screen_rhs_kernel<<<nblk, kSumThreads, 0, as_stream(stream)>>>(b, mask, map, moments, N,
+                                                                         gamma_t, b_s, workspace);
+  const int rc = after_launch("poisson_screen_rhs");
+  return rc ? rc : finish_sum(workspace, (int)nblk, bb, as_stream(stream), "poisson_screen_rhs");
+}
+
+extern "C" int casmvs_poisson_screen_stencil(const long long* nodes, int n_nodes,
+                                             const unsigned char* mask, const int* map,
+                                             const double* moments, int n, float* stencil32,
+                                             double* stencil64, void* stream) {
+  POISSON_GRID("poisson_screen_stencil", n);
+  CASMVS_REQUIRE(n_nodes >= 0, "poisson_screen_stencil: n_nodes < 0");
+  if (n_nodes == 0) return 0;
+  CASMVS_REQUIRE(nodes && mask && map && moments && (stencil32 || stencil64),
+                 "poisson_screen_stencil: null pointer");
+  poisson_screen_stencil_kernel<<<(n_nodes + 127) / 128, 128, 0, as_stream(stream)>>>(
+      nodes, n_nodes, mask, map, moments, n, stencil32, stencil64);
+  return after_launch("poisson_screen_stencil");
+}
+
+extern "C" int casmvs_poisson_screen_residual(const double* chi, const float* b_s,
+                                              const unsigned char* mask, const int* srow,
+                                              const double* stencil, int N, float h, double g,
+                                              float* r, double* workspace, double* rr,
+                                              void* stream) {
+  POISSON_GRID("poisson_screen_residual", N);
+  CASMVS_REQUIRE(h > 0.f && g >= 0.0, "poisson_screen_residual: need h > 0 and g >= 0");
+  CASMVS_REQUIRE(chi && b_s && mask && srow && stencil && r && workspace && rr,
+                 "poisson_screen_residual: null pointer");
+  const unsigned nblk = pblocks((size_t)N * N * N);
+  poisson_screen_residual_kernel<<<nblk, kSumThreads, 0, as_stream(stream)>>>(
+      chi, b_s, mask, srow, stencil, N, h, g, r, workspace);
+  const int rc = after_launch("poisson_screen_residual");
+  return rc ? rc : finish_sum(workspace, (int)nblk, rr, as_stream(stream), "poisson_screen_residual");
+}
+
+extern "C" int casmvs_poisson_screen_mg_residual(const float* e, const float* r,
+                                                 const unsigned char* mask, const int* srow,
+                                                 const float* stencil, int n, int level, float h,
+                                                 double g, float* out, void* stream) {
+  POISSON_GRID("poisson_screen_mg_residual", n);
+  CASMVS_REQUIRE(level >= 0, "poisson_screen_mg_residual: level < 0");
+  CASMVS_REQUIRE(h > 0.f && g >= 0.0, "poisson_screen_mg_residual: need h > 0 and g >= 0");
+  CASMVS_REQUIRE(e && r && mask && srow && stencil && out, "poisson_screen_mg_residual: null pointer");
+  poisson_screen_mg_residual_kernel<<<pblocks((size_t)n * n * n), 256, 0, as_stream(stream)>>>(
+      e, r, mask, srow, stencil, n, level, h * h, (float)ldexp(g, -level), out);
+  return after_launch("poisson_screen_mg_residual");
+}
+
+extern "C" int casmvs_poisson_screen_smooth(float* e, const float* r, const unsigned char* mask,
+                                            const int* srow, const float* stencil, int n, int level,
+                                            float h, double g, int sweeps, int zero_first,
+                                            void* stream) {
+  POISSON_GRID("poisson_screen_smooth", n);
+  CASMVS_REQUIRE(level >= 0, "poisson_screen_smooth: level < 0");
+  CASMVS_REQUIRE(h > 0.f && g >= 0.0 && sweeps >= 0,
+                 "poisson_screen_smooth: need h > 0, g >= 0 and sweeps >= 0");
+  CASMVS_REQUIRE(e && r && mask && srow && stencil, "poisson_screen_smooth: null pointer");
+  const float h2 = h * h;
+  const float gl = (float)ldexp(g, -level);         // gamma_l h_l^2 = (gamma / 8^l) (2^l h)^2
+  const size_t nn = (size_t)n * n * n;
+  cudaStream_t st = as_stream(stream);
+  if (zero_first && nn <= 512) {
+    poisson_screen_smooth_coarse_kernel<<<1, 512, 0, st>>>(e, r, mask, srow, stencil, n, level, h2,
+                                                           gl, sweeps);
+    return after_launch("poisson_screen_smooth");
+  }
+  if (zero_first) {
+    cudaError_t err = cudaMemsetAsync(e, 0, nn * sizeof(float), st);
+    CASMVS_REQUIRE(err == cudaSuccess, "poisson_screen_smooth: memset failed: %s",
+                   cudaGetErrorString(err));
+  }
+  const unsigned lines = (unsigned)((n / 2) * (n / 2));
+  for (int s = 0; s < sweeps; ++s)
+    for (int j = 0; j < 4; ++j) {
+      poisson_screen_smooth_lines_kernel<<<lines, n / 2, 0, st>>>(e, r, mask, srow, stencil, n,
+                                                                  level, h2, gl, j);
+      const int rc = after_launch("poisson_screen_smooth");
+      if (rc) return rc;
+    }
+  return 0;
 }

@@ -40,12 +40,13 @@ proba_XXXX.pfm are written as well).
 --mesh also fuses each scan's filtered depth maps into a TSDF volume on the GPU and writes the
 marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes changes.
 --mesh --mesh_method poisson [--poisson_depth 9] meshes the scan's fused points by Poisson surface
-reconstruction instead (poisson.py).
+reconstruction instead (poisson.py); --poisson_point_weight A > 0 screens it.
 """
 from __future__ import annotations
 
 import argparse
 import json
+import math
 import os
 
 import numpy as np
@@ -434,7 +435,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
-             mesh_method="tsdf", poisson_depth=None):
+             mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -447,7 +448,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     mesh.default_voxel_size); the other outputs are unchanged.  With mesh_method="poisson" the
     mesh is instead the Poisson surface (poisson.py, grid depth `poisson_depth`, default 9) of
     every fused point (not thinned by `skip`), coloured by the refined image at its pixel, its
-    normals oriented toward the reference cameras.
+    normals oriented toward the reference cameras, screened with point weight
+    `poisson_point_weight` when it is > 0.
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
@@ -484,7 +486,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         del fused
         verts, colours, faces, st = poisson.poisson_mesh(
             pts, cols, cam_centres=cams,
-            depth=poisson.DEFAULT_DEPTH if poisson_depth is None else poisson_depth, log=log)
+            depth=poisson.DEFAULT_DEPTH if poisson_depth is None else poisson_depth, log=log,
+            point_weight=poisson_point_weight)
         del pts, cols
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         log(f"{scan.scan}: poisson mesh at depth {st['depth']} (h {st['h']:.6g}): {st['points']} "
@@ -603,6 +606,9 @@ def parse_args(argv=None):
                          "poisson meshes the fused points by Poisson surface reconstruction")
     ap.add_argument("--poisson_depth", type=int, default=None,
                     help="with --mesh_method poisson: the grid depth, 6..10 (default 9)")
+    ap.add_argument("--poisson_point_weight", type=float, default=None,
+                    help="with --mesh_method poisson: the screening weight alpha >= 0 that pulls "
+                         "the surface through the points (default 0, unscreened)")
     a = ap.parse_args(argv)
     if a.mesh_voxel is not None and not a.mesh_voxel > 0:
         ap.error("--mesh_voxel must be > 0")
@@ -614,6 +620,11 @@ def parse_args(argv=None):
         ap.error("--poisson_depth needs --mesh_method poisson")
     if a.poisson_depth is not None and not 6 <= a.poisson_depth <= 10:
         ap.error("--poisson_depth must be in 6..10")
+    if a.poisson_point_weight is not None and a.mesh_method != "poisson":
+        ap.error("--poisson_point_weight needs --mesh_method poisson")
+    if a.poisson_point_weight is not None and not (math.isfinite(a.poisson_point_weight)
+                                                   and a.poisson_point_weight >= 0):
+        ap.error("--poisson_point_weight must be a finite number >= 0")
     a.mesh_method = a.mesh_method or "tsdf"
     if a.depth_interval is None:
         a.depth_interval = DEFAULT_DEPTH_INTERVAL[a.dataset_name]
@@ -656,7 +667,8 @@ def main(argv=None):
                        dtu_seed=a.dtu_seed, save_visual=a.save_visual,
                        mesh_path=os.path.join(out_dir, "mesh", f"{scan.scan}.ply") if a.mesh else None,
                        mesh_voxel=a.mesh_voxel, mesh_method=a.mesh_method,
-                       poisson_depth=a.poisson_depth, **tnt)
+                       poisson_depth=a.poisson_depth,
+                       poisson_point_weight=a.poisson_point_weight or 0.0, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

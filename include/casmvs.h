@@ -707,6 +707,59 @@ int casmvs_poisson_fill_tsdf(const long long* keys, int nb, const float* weight,
                              double iso, int N, int lo_x, int lo_y, int lo_z, float* tsdf,
                              void* stream);
 
+/* ---- screened Poisson (the point-weight term; poisson.py's point_weight > 0) ----------------
+ * A point's splat cell is its floor corner floor(p / h) - lo; F its float32 fraction.  Per cell,
+ * moments (n_cells,27) f64 hold sum F_x^a F_y^b F_z^c (index 9a + 3b + c, a,b,c in 0..2).  S_ij =
+ * sum_p phi_i(p) phi_j(p) and Phi_i = sum_p phi_i(p) (phi the trilinear weight, a polynomial in
+ * F) are expanded from them in double.  Level l's cells sit on its grid (coarse node I at fine
+ * node 2^l I); map (n^3) int32 = a cell's row in moments or -1; mask (n^3) u8 bit d (d = 4 dx +
+ * 2 dy + dz) = cell node - d holds points.  g = alpha n_s / n = gamma h^2; level l uses
+ * L_l - (gamma / 8^l) S_l, so its g is g / 2^l.  Boundary rules are those of the multigrid above.
+ * casmvs_poisson_screen_keys: keys (n) int64 = flat splat cell, INT64_MAX when it leaves 0..N-2.
+ * casmvs_poisson_screen_moments: the points order[cell_start[c] .. cell_start[c+1]) of each cell,
+ *   summed in that order.
+ * casmvs_poisson_screen_coarsen: parent cell (parent_keys, flat on the (n_child/2)^3 grid) = sum
+ *   over its children m = 0..7 (x-major, child_map on the n_child^3 grid) of the child moments
+ *   under F' = (m + F) / 2.
+ * casmvs_poisson_screen_rhs: b_s = f32(b - gamma_t Phi) at interior nodes of level 0, 0 on the
+ *   outer layer; *bb = sum of b_s^2.
+ * casmvs_poisson_screen_stencil: for the nodes (n_nodes flat indices, mask != 0) of a level,
+ *   the 27-point stencil of S (k = 9 (dx+1) + 3 (dy+1) + (dz+1)): sum over the cells d = 0..7
+ *   around the node, then their corners, of S expanded from the moments in double; corners at
+ *   index n drop.  stencil32 (n_nodes,27) f32 and/or stencil64 f64 (either may be NULL).
+ *   srow (n^3) int32 = a node's row in the stencil arrays (read only where mask != 0).
+ * casmvs_poisson_screen_residual: r = b_s - (sum of the 6 neighbours - 6 chi - g S chi) / h^2 in
+ *   double on level 0 with the f64 stencil; *rr = sum of r^2 (before rounding).
+ * casmvs_poisson_screen_mg_residual: out = r - (nbsum(e) - 6 e - g_l S e) / h^2 in f32 with the
+ *   f32 stencil (S e summed in k order) at the level's interior nodes; 0 elsewhere.
+ * casmvs_poisson_screen_smooth: `sweeps` 8-colour Gauss-Seidel sweeps, colour 4 (x&1) + 2 (y&1) +
+ *   (z&1) in order 0..7, in f32: e = (nbsum(e) - h^2 r - g_l sum_{k != 13} S_k e_k) /
+ *   (6 + g_l S_13), (nbsum(e) - h^2 r) / 6 where mask = 0; zero_first: start from e = 0 (in one
+ *   block when n^3 <= 512). */
+int casmvs_poisson_screen_keys(const float* points, int n, float h, int lo_x, int lo_y, int lo_z,
+                               int N, long long* keys, void* stream);
+int casmvs_poisson_screen_moments(const float* points, const int* order, const int* cell_start,
+                                  int n_cells, float h, int lo_x, int lo_y, int lo_z,
+                                  double* moments, void* stream);
+int casmvs_poisson_screen_coarsen(const int* child_map, const double* child_moments, int n_child,
+                                  const long long* parent_keys, int n_parents,
+                                  double* parent_moments, void* stream);
+int casmvs_poisson_screen_rhs(const float* b, const unsigned char* mask, const int* map,
+                              const double* moments, int N, double gamma_t, float* b_s,
+                              double* workspace, double* bb, void* stream);
+int casmvs_poisson_screen_stencil(const long long* nodes, int n_nodes, const unsigned char* mask,
+                                  const int* map, const double* moments, int n, float* stencil32,
+                                  double* stencil64, void* stream);
+int casmvs_poisson_screen_residual(const double* chi, const float* b_s, const unsigned char* mask,
+                                   const int* srow, const double* stencil, int N, float h, double g,
+                                   float* r, double* workspace, double* rr, void* stream);
+int casmvs_poisson_screen_mg_residual(const float* e, const float* r, const unsigned char* mask,
+                                      const int* srow, const float* stencil, int n, int level,
+                                      float h, double g, float* out, void* stream);
+int casmvs_poisson_screen_smooth(float* e, const float* r, const unsigned char* mask,
+                                 const int* srow, const float* stencil, int n, int level, float h,
+                                 double g, int sweeps, int zero_first, void* stream);
+
 /* ---- headless rendering of clouds and meshes (casmvsnet_pl_b200/render.py) -----------------
  * P is a HOST array of 16 floats, row-major, world -> pixel (rows 0..2 used): every float
  * operation below is rounded to nearest, no contraction, in the order written.
