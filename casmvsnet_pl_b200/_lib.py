@@ -180,6 +180,17 @@ SIGNATURES = {
                                           + [c_void_p] * 2),
     "casmvs_poisson_screen_smooth": (c_int, [c_void_p] * 5 + [c_int, c_int, c_float, c_double,
                                                               c_int, c_int, c_void_p]),
+    "casmvs_simplify_clean": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_simplify_frozen": (c_int, [c_void_p, c_int] + [c_void_p] * 6),
+    "casmvs_simplify_face_quadrics": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_simplify_vertex_quadrics": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 8),
+    "casmvs_simplify_edge_costs": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 4
+                                   + [c_int, c_void_p, c_int, c_double] + [c_void_p] * 7),
+    "casmvs_simplify_select": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_int]
+                               + [c_void_p] * 6),
+    "casmvs_simplify_collapse": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 6),
+    "casmvs_simplify_remap_faces": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "casmvs_simplify_mark_used": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "casmvs_render_points_fwd": (c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
                                          c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "casmvs_render_mesh_workspace_bytes": (c_size_t, [c_int]),

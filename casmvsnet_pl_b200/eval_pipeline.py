@@ -41,6 +41,8 @@ proba_XXXX.pfm are written as well).
 marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes changes.
 --mesh --mesh_method poisson [--poisson_depth 9] meshes the scan's fused points by Poisson surface
 reconstruction instead (poisson.py); --poisson_point_weight A > 0 screens it.
+--mesh --mesh_faces N decimates either mesh to at most N faces on the GPU before it is written
+(simplify.py).
 """
 from __future__ import annotations
 
@@ -430,12 +432,23 @@ class ColmapScan(_CachedScan):
         return self.depth_min[ref], self.depth_interval[ref]
 
 
+def _simplify(name, verts, colours, faces, mesh_faces, log):
+    """The mesh decimated to `mesh_faces` faces (unchanged when it is None)."""
+    if mesh_faces is None:
+        return verts, colours, faces
+    from . import simplify
+    verts, colours, faces, st = simplify.simplify_mesh(verts, colours, faces, mesh_faces, log=log)
+    log(f"{name}: simplified the mesh from {st['faces_in']} to {st['faces']} faces in "
+        f"{st['rounds']} rounds")
+    return verts, colours, faces
+
+
 @torch.no_grad()
 def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
-             mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0):
+             mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -449,7 +462,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     mesh is instead the Poisson surface (poisson.py, grid depth `poisson_depth`, default 9) of
     every fused point (not thinned by `skip`), coloured by the refined image at its pixel, its
     normals oriented toward the reference cameras, screened with point weight
-    `poisson_point_weight` when it is > 0.
+    `poisson_point_weight` when it is > 0.  With `mesh_faces`, either mesh is decimated to at most
+    that many faces (simplify.py) before it is written.
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
@@ -489,6 +503,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
             depth=poisson.DEFAULT_DEPTH if poisson_depth is None else poisson_depth, log=log,
             point_weight=poisson_point_weight)
         del pts, cols
+        verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         log(f"{scan.scan}: poisson mesh at depth {st['depth']} (h {st['h']:.6g}): {st['points']} "
             f"points ({st['dropped']} dropped), {st['cycles']} cycles, {st['bricks']} bricks, "
@@ -502,6 +517,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
                                                     [f["image"] for f in fused],
                                                     [f["P"] for f in fused], mesh_voxel)
         del fused
+        verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         log(f"{scan.scan}: mesh at voxel {st['voxel']:.6g}: {st['bricks']} bricks, {st['voxels']} "
             f"voxels, {st['vertices']} vertices, {st['triangles']} triangles, {st['dropped']} "
@@ -609,7 +625,14 @@ def parse_args(argv=None):
     ap.add_argument("--poisson_point_weight", type=float, default=None,
                     help="with --mesh_method poisson: the screening weight alpha >= 0 that pulls "
                          "the surface through the points (default 0, unscreened)")
+    ap.add_argument("--mesh_faces", type=int, default=None,
+                    help="with --mesh: simplify the mesh to at most this many faces (>= 1) by "
+                         "quadric edge-collapse decimation before it is written")
     a = ap.parse_args(argv)
+    if a.mesh_faces is not None and not a.mesh:
+        ap.error("--mesh_faces needs --mesh")
+    if a.mesh_faces is not None and a.mesh_faces < 1:
+        ap.error("--mesh_faces must be >= 1")
     if a.mesh_voxel is not None and not a.mesh_voxel > 0:
         ap.error("--mesh_voxel must be > 0")
     if a.mesh_method is not None and not a.mesh:
@@ -668,7 +691,8 @@ def main(argv=None):
                        mesh_path=os.path.join(out_dir, "mesh", f"{scan.scan}.ply") if a.mesh else None,
                        mesh_voxel=a.mesh_voxel, mesh_method=a.mesh_method,
                        poisson_depth=a.poisson_depth,
-                       poisson_point_weight=a.poisson_point_weight or 0.0, **tnt)
+                       poisson_point_weight=a.poisson_point_weight or 0.0,
+                       mesh_faces=a.mesh_faces, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

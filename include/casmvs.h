@@ -760,6 +760,73 @@ int casmvs_poisson_screen_smooth(float* e, const float* r, const unsigned char* 
                                  const int* srow, const float* stencil, int n, int level, float h,
                                  double g, int sweeps, int zero_first, void* stream);
 
+/* ---- quadric edge-collapse decimation (csrc/simplify.cu, casmvsnet_pl_b200/simplify.py) ----
+ * A mesh is verts (V,3) f32, colours (V,3) u8, faces (F,3) int32, 3F < 2^31.  Every double
+ * operation below is rounded to nearest in the order written, with no contraction; sums run in
+ * a fixed order and the only atomics are integer ones, so results are bitwise reproducible.
+ * Corner c = 3 f + k of face f sits at vertex faces[f][k] and owns the edge faces[f][k] --
+ * faces[f][(k+1)%3].  Edges: edge_keys (E) int64 = (a << 32) | b, a < b, sorted and unique,
+ * edge index = rank; corner_edge (3F) int32 = the edge a corner owns; edge_count (E) int32 =
+ * faces on the edge (1 = boundary edge).  CSR: the corners at vertex v are
+ * corners[off[v] .. off[v+1]) (int32), in increasing corner (so face) order.
+ * Plane quadric of unit normal n^ through p0 with weight w: w [n^, -n^.p0][n^, -n^.p0]^T, as the
+ * 10 unique entries (xx, xy, xz, xw, yy, yz, yw, zz, zw, ww), n^ = n / sqrt((nx nx + ny ny) + nz nz).
+ * casmvs_simplify_clean: keep (F) u8 = 0 for a face with a repeated index or with
+ *   n = (p1 - p0) x (p2 - p0) = 0 in double.
+ * casmvs_simplify_frozen: frozen (V) u8 = 1 for a vertex with > 32 faces, on an edge of > 2
+ *   faces, or whose link (an edge p-q per face (v, p, q)) is not connected (not one fan).
+ * casmvs_simplify_face_quadrics: fq (F,10) f64, the plane quadric of n = (p1 - p0) x (p2 - p0)
+ *   through p0 with weight |n| / 2.
+ * casmvs_simplify_vertex_quadrics: Q (V,10) f64 = 0 + the fq of v's faces in face order + the
+ *   quadrics of v's boundary edges in edge order: plane normal (pb - pa) x n_f of the edge's
+ *   face f, through pa, weight 1000 |pb - pa|^2.
+ * casmvs_simplify_edge_costs: deg (V) int32 = distinct neighbours, bnd (V) u8 = on a boundary
+ *   edge (both zeroed and filled here); per edge, Q = Q_a + Q_b, A its upper-left 3x3:
+ *   v = f32(Cramer's solution of A v = -Q[0:3,3]) when |det A| > 1e-12 max|A_ij|^3 and v is
+ *   finite, else the first of a, b, f32((a + b) * 0.5) of least [v,1]^T Q [v,1];
+ *   cost = f32(max(0, [v,1]^T Q [v,1])) (NaN stays NaN), newpos (E,3) f32 = v.
+ *   valid0 (E) u8: cost finite, a and b not frozen, the common neighbours of a and b are
+ *   exactly the opposite vertices of the faces on ab, not (a and b on the boundary and ab
+ *   interior), deg a + deg b - 2 - common >= 3 (2 when a or b is on the boundary), deg c - 1 >= 3
+ *   (2 on the boundary) for every opposite vertex c, faces(a) + faces(b) - faces(ab) <= 32, and
+ *   every face around a or b without both has n_new . n_old > (0.2 |n_new|) |n_old| with the
+ *   moved vertex at v.  key (E) int64 = (float bits of cost << 32) | e when valid0 and (unless
+ *   !has_max_error) cost <= max_error, else INT64_MAX.
+ * casmvs_simplify_select: m1 (V) = least key <= thr over the edges at v (INT64_MAX if none);
+ *   m2 (V) = least m1 over v and the vertices of its faces; sel (E) u8 = key <= thr and
+ *   key == m2[a] == m2[b].  No endpoint of one selected edge is in the 1-ring of another's.
+ * casmvs_simplify_collapse: for the n edges idx (int64): a takes v = newpos[e], Q_a + Q_b and
+ *   colour rint(c_a + t (c_b - c_a)), t = clamp(((v - a).(b - a)) / |b - a|^2, 0, 1) (0 when
+ *   |b - a| = 0), remap[b] = a (remap otherwise as the caller set it).
+ * casmvs_simplify_remap_faces: faces = map[faces] in place; keep (F) u8 = three distinct indices.
+ * casmvs_simplify_mark_used: used (V) int32 = 1 for a vertex of a face, else 0 (zeroed here). */
+int casmvs_simplify_clean(const float* verts, const int* faces, int F, unsigned char* keep,
+                          void* stream);
+int casmvs_simplify_frozen(const int* faces, int V, const int* off, const int* corners,
+                           const int* corner_edge, const int* edge_count, unsigned char* frozen,
+                           void* stream);
+int casmvs_simplify_face_quadrics(const float* verts, const int* faces, int F, double* fq,
+                                  void* stream);
+int casmvs_simplify_vertex_quadrics(const float* verts, const int* faces, int V, const int* off,
+                                    const int* corners, const int* corner_edge,
+                                    const long long* edge_keys, const int* edge_count,
+                                    const double* fq, double* Q, void* stream);
+int casmvs_simplify_edge_costs(const float* verts, const double* Q, const int* faces, int V,
+                               const int* off, const int* corners, const long long* edge_keys,
+                               const int* edge_count, int E, const unsigned char* frozen,
+                               int has_max_error, double max_error, int* deg, unsigned char* bnd,
+                               float* newpos, float* cost, unsigned char* valid0, long long* key,
+                               void* stream);
+int casmvs_simplify_select(const long long* edge_keys, const long long* key, int E, long long thr,
+                           const int* faces, int V, const int* off, const int* corners,
+                           long long* m1, long long* m2, unsigned char* sel, void* stream);
+int casmvs_simplify_collapse(const long long* edge_keys, const long long* idx, int n,
+                             const float* newpos, float* verts, unsigned char* colours, double* Q,
+                             int* remap, void* stream);
+int casmvs_simplify_remap_faces(int* faces, int F, const int* map, unsigned char* keep,
+                                void* stream);
+int casmvs_simplify_mark_used(const int* faces, int F, int V, int* used, void* stream);
+
 /* ---- headless rendering of clouds and meshes (casmvsnet_pl_b200/render.py) -----------------
  * P is a HOST array of 16 floats, row-major, world -> pixel (rows 0..2 used): every float
  * operation below is rounded to nearest, no contraction, in the order written.
