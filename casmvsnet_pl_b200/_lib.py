@@ -197,6 +197,22 @@ SIGNATURES = {
     "casmvs_render_mesh_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, POINTER(c_float),
                                        POINTER(c_float), c_int, c_int, c_void_p, c_void_p, c_size_t,
                                        c_void_p, c_void_p, c_void_p]),
+    "casmvs_render_mesh_keys": (c_int, [c_void_p, c_int, c_void_p, c_int, POINTER(c_float), c_int,
+                                        c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "casmvs_render_textured_mesh_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                                c_void_p, c_int, c_int, POINTER(c_float), c_int,
+                                                c_int, c_void_p, c_void_p, c_size_t, c_void_p,
+                                                c_void_p, c_void_p]),
+    "casmvs_texture_scores": (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(c_float),
+                                      POINTER(c_double), POINTER(c_int), POINTER(c_int),
+                                      POINTER(c_void_p), c_void_p, c_void_p, c_void_p]),
+    "casmvs_texture_smooth": (c_int, [c_void_p] * 3 + [c_int, c_void_p, c_void_p, c_void_p]),
+    "casmvs_texture_charts": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int),
+                                      c_void_p]),
+    "casmvs_texture_rects": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 5),
+    "casmvs_texture_fill": (c_int, [c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p]),
+    "casmvs_texture_uvs": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4
+                           + [c_int, c_void_p, c_void_p, c_void_p]),
     "casmvs_visual_panels": (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),

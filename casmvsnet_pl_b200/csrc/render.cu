@@ -14,35 +14,12 @@
 // Triangles: one thread per triangle projects it and rasterises its screen bounding box when that
 // is at most kSmallBox x kSmallBox pixels; larger boxes go to a list that whole CTAs work through,
 // so a triangle filling the screen does not serialise in one thread.
-#include "common.cuh"
+#include "render_common.cuh"
 
 namespace casmvs {
 
-constexpr unsigned long long kKeyEmpty = ~0ull;
 constexpr int kSmallBox = 8;                  // px per side rasterised by the triangle's thread
 constexpr int kMaxSide = 16384, kMaxPointSize = 64;
-
-struct RenderCam {
-  float P[12];                                // rows 0..2 of the world -> pixel matrix
-  float eye[3];                               // camera centre, for the mesh shade
-};
-
-// ((A0 X + A1 Y) + A2 Z) + A3
-__device__ __forceinline__ float proj_row(const float* A, float X, float Y, float Z) {
-  return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(A[0], X), __fmul_rn(A[1], Y)), __fmul_rn(A[2], Z)),
-                   A[3]);
-}
-
-// World point -> (u, v, w); false unless it is finite with w > 0 and finite u, v.
-__device__ __forceinline__ bool project(const RenderCam& c, float X, float Y, float Z, float& u,
-                                        float& v, float& w) {
-  if (!(isfinite(X) && isfinite(Y) && isfinite(Z))) return false;
-  w = proj_row(c.P + 8, X, Y, Z);
-  if (!(w > 0.f) || !isfinite(w)) return false;
-  u = __fdiv_rn(proj_row(c.P, X, Y, Z), w);
-  v = __fdiv_rn(proj_row(c.P + 4, X, Y, Z), w);
-  return isfinite(u) && isfinite(v);
-}
 
 __device__ __forceinline__ unsigned long long depth_key(float w, unsigned idx) {
   return ((unsigned long long)__float_as_uint(w) << 32) | idx;
@@ -263,6 +240,60 @@ render_mesh_resolve_kernel(const __grid_constant__ RenderCam cam, const float* _
   depth[p] = d;
 }
 
+// Textured resolve: the winner's UV interpolated perspective-correctly (as the colours above),
+// then the page sampled bilinearly with texel centres at i + 0.5 and clamped indices.  Unshaded.
+__global__ void __launch_bounds__(256)
+render_textured_resolve_kernel(const __grid_constant__ RenderCam cam, const float* __restrict__ verts,
+                               int nv, const int* __restrict__ faces, const float* __restrict__ uv,
+                               const int* __restrict__ page, const unsigned char* __restrict__ atlas,
+                               int n_pages, int S, const unsigned long long* __restrict__ zbuf,
+                               int W, int H, unsigned char* __restrict__ image,
+                               float* __restrict__ depth) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= W * H) return;
+  const unsigned long long k = zbuf[p];
+  unsigned char out[3] = {128, 128, 255};
+  float d = 0.f;
+  if (k != kKeyEmpty) {
+    const unsigned t = (unsigned)k;
+    d = __uint_as_float((unsigned)(k >> 32));
+    Tri T;
+    float q[3], den, w;
+    const int pg = __ldg(page + t);
+    if (pg >= 0 && pg < n_pages && setup_tri(cam, verts, nv, faces, t, W, H, T, nullptr) &&
+        tri_depth(T, p % W, p / W, q, den, w)) {
+      const float* c = uv + (size_t)t * 6;
+      const float tu = __fdiv_rn(__fadd_rn(__fadd_rn(__fmul_rn(q[0], __ldg(c)), __fmul_rn(q[1], __ldg(c + 2))),
+                                           __fmul_rn(q[2], __ldg(c + 4))), den);
+      const float tv = __fdiv_rn(__fadd_rn(__fadd_rn(__fmul_rn(q[0], __ldg(c + 1)), __fmul_rn(q[1], __ldg(c + 3))),
+                                           __fmul_rn(q[2], __ldg(c + 5))), den);
+      const float Sf = (float)S;
+      // texel space; clamped to [-1, S] first so that the integer conversion is defined
+      const float x = fminf(fmaxf(__fsub_rn(__fmul_rn(tu, Sf), 0.5f), -1.f), Sf);
+      const float y = fminf(fmaxf(__fsub_rn(__fmul_rn(__fsub_rn(1.f, tv), Sf), 0.5f), -1.f), Sf);
+      const float fx = floorf(x), fy = floorf(y);
+      const float ax = __fsub_rn(x, fx), ay = __fsub_rn(y, fy);
+      const int x0 = min(max((int)fx, 0), S - 1), x1 = min(max((int)fx + 1, 0), S - 1);
+      const int y0 = min(max((int)fy, 0), S - 1), y1 = min(max((int)fy + 1, 0), S - 1);
+      const unsigned char* A = atlas + (size_t)pg * S * S * 3;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const float c00 = (float)__ldg(A + ((size_t)y0 * S + x0) * 3 + ch);
+        const float c10 = (float)__ldg(A + ((size_t)y0 * S + x1) * 3 + ch);
+        const float c01 = (float)__ldg(A + ((size_t)y1 * S + x0) * 3 + ch);
+        const float c11 = (float)__ldg(A + ((size_t)y1 * S + x1) * 3 + ch);
+        const float r0 = __fadd_rn(__fmul_rn(__fsub_rn(1.f, ax), c00), __fmul_rn(ax, c10));
+        const float r1 = __fadd_rn(__fmul_rn(__fsub_rn(1.f, ax), c01), __fmul_rn(ax, c11));
+        const float val = floorf(__fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(1.f, ay), r0),
+                                                     __fmul_rn(ay, r1)), 0.5f));
+        out[ch] = (unsigned char)fminf(255.f, fmaxf(0.f, val));
+      }
+    }
+  }
+  image[(size_t)p * 3] = out[0]; image[(size_t)p * 3 + 1] = out[1]; image[(size_t)p * 3 + 2] = out[2];
+  depth[p] = d;
+}
+
 inline unsigned render_blocks(unsigned long long n) { return (unsigned)((n + 255) / 256); }
 
 inline RenderCam make_cam(const float* P, const float* eye) {
@@ -312,28 +343,12 @@ extern "C" size_t casmvs_render_mesh_workspace_bytes(int n_faces) {
   return n_faces < 0 ? 0 : (size_t)(n_faces + 2) * sizeof(unsigned);
 }
 
-extern "C" int casmvs_render_mesh_fwd(const float* verts, const unsigned char* colours, int n_vertices,
-                                      const int* faces, int n_faces, const float* P, const float* eye,
-                                      int W, int H, unsigned long long* zbuf, void* workspace,
-                                      size_t workspace_bytes, unsigned char* image, float* depth,
-                                      void* stream) {
-  const char* what = "render_mesh_fwd";
-  CASMVS_REQUIRE(n_vertices >= 0 && n_faces >= 0, "%s: negative vertex or face count", what);
-  RENDER_CHECK_SIZE(what, W, H);
-  CASMVS_REQUIRE_ALIGNED(what, verts, 4);
-  CASMVS_REQUIRE_ALIGNED(what, faces, 4);
-  CASMVS_REQUIRE_ALIGNED(what, zbuf, 8);
-  CASMVS_REQUIRE_ALIGNED(what, workspace, 4);
-  CASMVS_REQUIRE_ALIGNED(what, depth, 4);
-  CASMVS_REQUIRE(workspace_bytes >= casmvs_render_mesh_workspace_bytes(n_faces),
-                 "%s: workspace of %zu bytes, need %zu", what, workspace_bytes,
-                 casmvs_render_mesh_workspace_bytes(n_faces));
-  CASMVS_REQUIRE(P && eye && zbuf && workspace && image && depth &&
-                 (n_faces == 0 || (verts && colours && faces)), "%s: null pointer", what);
-  const RenderCam cam = make_cam(P, eye);
-  cudaStream_t st = as_stream(stream);
+// The raster pass of a mesh: zbuf cleared, then every face's covered pixels keyed; the bad-face
+// flag is read back (one synchronise).
+static int raster_mesh(const char* what, const RenderCam& cam, const float* verts, int n_vertices,
+                       const int* faces, int n_faces, int W, int H, unsigned long long* zbuf,
+                       unsigned* ws, cudaStream_t st) {
   const size_t npix = (size_t)W * H;
-  unsigned* ws = static_cast<unsigned*>(workspace);
   cudaError_t e = cudaMemsetAsync(zbuf, 0xff, npix * sizeof(unsigned long long), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(ws, 0, 2 * sizeof(unsigned), st);
   CASMVS_REQUIRE(e == cudaSuccess, "%s: memset failed: %s", what, cudaGetErrorString(e));
@@ -352,7 +367,76 @@ extern "C" int casmvs_render_mesh_fwd(const float* verts, const unsigned char* c
     CASMVS_REQUIRE(e == cudaSuccess, "%s: %s", what, cudaGetErrorString(e));
     CASMVS_REQUIRE(!bad, "%s: a face index lies outside [0, %d)", what, n_vertices);
   }
+  return 0;
+}
+
+#define RENDER_CHECK_MESH(what)                                                              \
+  CASMVS_REQUIRE(n_vertices >= 0 && n_faces >= 0, "%s: negative vertex or face count", what); \
+  RENDER_CHECK_SIZE(what, W, H);                                                              \
+  CASMVS_REQUIRE_ALIGNED(what, verts, 4);                                                     \
+  CASMVS_REQUIRE_ALIGNED(what, faces, 4);                                                     \
+  CASMVS_REQUIRE_ALIGNED(what, zbuf, 8);                                                      \
+  CASMVS_REQUIRE_ALIGNED(what, workspace, 4);                                                 \
+  CASMVS_REQUIRE(workspace_bytes >= casmvs_render_mesh_workspace_bytes(n_faces),              \
+                 "%s: workspace of %zu bytes, need %zu", what, workspace_bytes,               \
+                 casmvs_render_mesh_workspace_bytes(n_faces))
+
+extern "C" int casmvs_render_mesh_fwd(const float* verts, const unsigned char* colours, int n_vertices,
+                                      const int* faces, int n_faces, const float* P, const float* eye,
+                                      int W, int H, unsigned long long* zbuf, void* workspace,
+                                      size_t workspace_bytes, unsigned char* image, float* depth,
+                                      void* stream) {
+  const char* what = "render_mesh_fwd";
+  RENDER_CHECK_MESH(what);
+  CASMVS_REQUIRE_ALIGNED(what, depth, 4);
+  CASMVS_REQUIRE(P && eye && zbuf && workspace && image && depth &&
+                 (n_faces == 0 || (verts && colours && faces)), "%s: null pointer", what);
+  const RenderCam cam = make_cam(P, eye);
+  cudaStream_t st = as_stream(stream);
+  const size_t npix = (size_t)W * H;
+  const int rc = raster_mesh(what, cam, verts, n_vertices, faces, n_faces, W, H, zbuf,
+                             static_cast<unsigned*>(workspace), st);
+  if (rc) return rc;
   render_mesh_resolve_kernel<<<render_blocks(npix), 256, 0, st>>>(cam, verts, colours, n_vertices,
                                                                   faces, zbuf, W, H, image, depth);
+  return after_launch(what);
+}
+
+extern "C" int casmvs_render_mesh_keys(const float* verts, int n_vertices, const int* faces,
+                                       int n_faces, const float* P, int W, int H,
+                                       unsigned long long* zbuf, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  const char* what = "render_mesh_keys";
+  RENDER_CHECK_MESH(what);
+  CASMVS_REQUIRE(P && zbuf && workspace && (n_faces == 0 || (verts && faces)), "%s: null pointer",
+                 what);
+  return raster_mesh(what, make_cam(P, nullptr), verts, n_vertices, faces, n_faces, W, H, zbuf,
+                     static_cast<unsigned*>(workspace), as_stream(stream));
+}
+
+extern "C" int casmvs_render_textured_mesh_fwd(const float* verts, int n_vertices, const int* faces,
+                                               int n_faces, const float* uv, const int* page,
+                                               const unsigned char* atlas, int n_pages, int S,
+                                               const float* P, int W, int H,
+                                               unsigned long long* zbuf, void* workspace,
+                                               size_t workspace_bytes, unsigned char* image,
+                                               float* depth, void* stream) {
+  const char* what = "render_textured_mesh_fwd";
+  RENDER_CHECK_MESH(what);
+  CASMVS_REQUIRE_ALIGNED(what, uv, 4);
+  CASMVS_REQUIRE_ALIGNED(what, page, 4);
+  CASMVS_REQUIRE_ALIGNED(what, depth, 4);
+  CASMVS_REQUIRE(n_pages >= 1 && S >= 1 && S <= kMaxSide, "%s: need n_pages >= 1 and S in 1..%d "
+                 "(got %d, %d)", what, kMaxSide, n_pages, S);
+  CASMVS_REQUIRE(P && zbuf && workspace && image && depth && atlas &&
+                 (n_faces == 0 || (verts && faces && uv && page)), "%s: null pointer", what);
+  const RenderCam cam = make_cam(P, nullptr);
+  cudaStream_t st = as_stream(stream);
+  const size_t npix = (size_t)W * H;
+  const int rc = raster_mesh(what, cam, verts, n_vertices, faces, n_faces, W, H, zbuf,
+                             static_cast<unsigned*>(workspace), st);
+  if (rc) return rc;
+  render_textured_resolve_kernel<<<render_blocks(npix), 256, 0, st>>>(
+      cam, verts, n_vertices, faces, uv, page, atlas, n_pages, S, zbuf, W, H, image, depth);
   return after_launch(what);
 }

@@ -43,6 +43,8 @@ marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes c
 reconstruction instead (poisson.py); --poisson_point_weight A > 0 screens it.
 --mesh --mesh_faces N decimates either mesh to at most N faces on the GPU before it is written
 (simplify.py).
+--mesh --mesh_texture also textures the mesh that is written from the scan's reference-view images
+at --img_wh and writes <out>/mesh/<scan>.obj, .mtl and _<k>.png beside the PLY (texture.py).
 """
 from __future__ import annotations
 
@@ -443,12 +445,25 @@ def _simplify(name, verts, colours, faces, mesh_faces, log):
     return verts, colours, faces
 
 
+def _texture(name, mesh_path, verts, colours, faces, images, proj0, log):
+    """Texture the written mesh from the reference views' images (cast to uint8) and proj0, and
+    write <mesh_path without .ply>.obj / .mtl / _<k>.png."""
+    from . import texture
+    vids = sorted(images)
+    ims = [images[v].to(torch.uint8).contiguous() for v in vids]
+    uv, page, atlas, st = texture.texture_mesh(verts, colours, faces, ims, [proj0[v] for v in vids])
+    texture.write_textured_obj(os.path.splitext(mesh_path)[0] + ".obj", verts, faces, uv, page, atlas)
+    log(f"{name}: textured {st['faces']} faces from {st['views']} views: {st['unseen_faces']} "
+        f"unseen, {st['charts']} charts on {st['pages']} pages ({st['packed_share']:.1%} packed)")
+
+
 @torch.no_grad()
 def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              skip=1, max_ref_views=400, device="cuda:0", depth_dir=None, ply_path=None,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
-             mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None):
+             mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
+             mesh_texture=False):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -463,7 +478,9 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     every fused point (not thinned by `skip`), coloured by the refined image at its pixel, its
     normals oriented toward the reference cameras, screened with point weight
     `poisson_point_weight` when it is > 0.  With `mesh_faces`, either mesh is decimated to at most
-    that many faces (simplify.py) before it is written.
+    that many faces (simplify.py) before it is written.  With `mesh_texture`, the written mesh is
+    also textured from the reference views' images and proj0 (texture.py) and written beside it
+    as an OBJ with its MTL and atlas PNGs.
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
@@ -505,6 +522,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         del pts, cols
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
+        if mesh_texture:
+            _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log)
         log(f"{scan.scan}: poisson mesh at depth {st['depth']} (h {st['h']:.6g}): {st['points']} "
             f"points ({st['dropped']} dropped), {st['cycles']} cycles, {st['bricks']} bricks, "
             f"{st['vertices']} vertices, {st['triangles']} triangles")
@@ -519,6 +538,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         del fused
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
+        if mesh_texture:
+            _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log)
         log(f"{scan.scan}: mesh at voxel {st['voxel']:.6g}: {st['bricks']} bricks, {st['voxels']} "
             f"voxels, {st['vertices']} vertices, {st['triangles']} triangles, {st['dropped']} "
             "points dropped")
@@ -628,7 +649,12 @@ def parse_args(argv=None):
     ap.add_argument("--mesh_faces", type=int, default=None,
                     help="with --mesh: simplify the mesh to at most this many faces (>= 1) by "
                          "quadric edge-collapse decimation before it is written")
+    ap.add_argument("--mesh_texture", action="store_true",
+                    help="with --mesh: also texture the mesh from the reference views and write "
+                         "<out>/mesh/<scan>.obj with its .mtl and atlas PNGs")
     a = ap.parse_args(argv)
+    if a.mesh_texture and not a.mesh:
+        ap.error("--mesh_texture needs --mesh")
     if a.mesh_faces is not None and not a.mesh:
         ap.error("--mesh_faces needs --mesh")
     if a.mesh_faces is not None and a.mesh_faces < 1:
@@ -692,7 +718,7 @@ def main(argv=None):
                        mesh_voxel=a.mesh_voxel, mesh_method=a.mesh_method,
                        poisson_depth=a.poisson_depth,
                        poisson_point_weight=a.poisson_point_weight or 0.0,
-                       mesh_faces=a.mesh_faces, **tnt)
+                       mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

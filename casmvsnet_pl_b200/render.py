@@ -3,6 +3,7 @@ float32 numpy restatement in oracle/render_oracle.py, bit for bit).
 
     image, depth = render_points(xyz, rgb, P, (W, H), point_size=1)
     image, depth = render_mesh(verts, colours, faces, P, (W, H))
+    image, depth = render_textured_mesh(verts, faces, uv, page, atlas, P, (W, H))
 
 take CUDA tensors ((N,3) float32 positions, (N,3) uint8 colours, (M,3) int32 faces) and a 4x4
 world -> pixel matrix P, and return (H,W,3) uint8 and (H,W) float32 camera depth (0 where nothing
@@ -17,7 +18,10 @@ the original project's visualize_ply.py saves (read_viewpoint / write_viewpoint)
 line renders a scan the pipeline wrote:
 
     python -m casmvsnet_pl_b200.render --dataset_name dtu --scan scan9 \\
-        [--use_viewpoint | --save_viewpoint] [--mesh] [--point_size 1] [--out results/dtu]
+        [--use_viewpoint | --save_viewpoint] [--mesh [--textured]] [--point_size 1] [--out results/dtu]
+
+A textured mesh (texture.py) is drawn unshaded: its UV is interpolated perspective-correctly and
+its atlas page sampled bilinearly, texel centres at i + 0.5, indices clamped to the page.
 """
 from __future__ import annotations
 
@@ -128,6 +132,43 @@ def render_mesh(verts, colours, faces, P, wh):
             _ptr(verts), _ptr(colours), len(verts), _ptr(faces), len(faces), _f32p(P), _f32p(eye),
             W, H, _ptr(zbuf), _ptr(ws), ws.numel() * 4, _ptr(image), _ptr(depth), _stream()),
             "render_mesh_fwd")
+    return image, depth
+
+
+def render_textured_mesh(verts, faces, uv, page, atlas, P, wh):
+    """Triangles faces (M,3) int32 over verts (N,3) float32 with per-corner uv (M,3,2) float32,
+    a page (M,) int32 per face and atlas (pages,S,S,3) uint8, CUDA tensors (texture.texture_mesh
+    returns them) -> (image (H,W,3) uint8, depth (H,W) float32) on their device.  The raster
+    pass is render_mesh's; the colour is the page sampled bilinearly at the perspective-correct UV,
+    unshaded (the photographs carry the light)."""
+    verts = _check_cuda("verts", verts, torch.float32, 3)
+    faces = _check_cuda("faces", faces, torch.int32, 3)
+    if not (torch.is_tensor(uv) and uv.is_cuda and uv.dtype == torch.float32
+            and tuple(uv.shape) == (len(faces), 3, 2)):
+        raise ValueError("uv must be a float32 CUDA tensor of shape (M, 3, 2)")
+    if not (torch.is_tensor(page) and page.is_cuda and page.dtype == torch.int32
+            and tuple(page.shape) == (len(faces),)):
+        raise ValueError("page must be an int32 CUDA tensor of shape (M,)")
+    if not (torch.is_tensor(atlas) and atlas.is_cuda and atlas.dtype == torch.uint8
+            and atlas.dim() == 4 and atlas.shape[1] == atlas.shape[2] and atlas.shape[3] == 3
+            and len(atlas) >= 1 and atlas.shape[1] <= MAX_SIDE):
+        raise ValueError(f"atlas must be a uint8 CUDA tensor of shape (pages, S, S, 3), S <= {MAX_SIDE}")
+    if not (verts.device == faces.device == uv.device == page.device == atlas.device):
+        raise ValueError("the mesh, its UVs, pages and atlas must be on one device")
+    if len(page) and not bool(((page >= 0) & (page < len(atlas))).all()):
+        raise ValueError(f"page holds an index outside 0..{len(atlas) - 1}")
+    W, H = _size(wh)
+    P = _matrix(P)
+    uv, page, atlas = uv.contiguous(), page.contiguous(), atlas.contiguous()
+    lib = _lib.load()
+    with torch.cuda.device(verts.device):
+        zbuf, image, depth = _outputs(W, H, verts.device)
+        nbytes = lib.casmvs_render_mesh_workspace_bytes(len(faces))
+        ws = torch.empty((nbytes + 3) // 4, dtype=torch.int32, device=verts.device)
+        _lib.check(lib.casmvs_render_textured_mesh_fwd(
+            _ptr(verts), len(verts), _ptr(faces), len(faces), _ptr(uv), _ptr(page), _ptr(atlas),
+            len(atlas), atlas.shape[1], _f32p(P), W, H, _ptr(zbuf), _ptr(ws), ws.numel() * 4,
+            _ptr(image), _ptr(depth), _stream()), "render_textured_mesh_fwd")
     return image, depth
 
 
@@ -274,9 +315,14 @@ def parse_args(argv=None):
     ap.add_argument("--save_viewpoint", action="store_true",
                     help="write the default view to <out>/viewpoint.json (ignored with --use_viewpoint)")
     ap.add_argument("--mesh", action="store_true", help="render the mesh of eval_pipeline --mesh")
+    ap.add_argument("--textured", action="store_true",
+                    help="with --mesh: draw the textured <out>/mesh/<scan>.obj of eval_pipeline "
+                         "--mesh_texture to <out>/render/<scan>_textured.png")
     ap.add_argument("--point_size", type=int, default=1, help=f"pixels per side, 1..{MAX_POINT_SIZE}")
     ap.add_argument("--out", default=None, help="output directory (default results/<dataset_name>)")
     a = ap.parse_args(argv)
+    if a.textured and not a.mesh:
+        ap.error("--textured needs --mesh")
     if not 1 <= a.point_size <= MAX_POINT_SIZE:
         ap.error(f"--point_size must lie in 1..{MAX_POINT_SIZE}")
     a.out_dir = a.out or os.path.join("results", a.dataset_name)
@@ -305,13 +351,18 @@ def main(argv=None):
     """-> the path of the PNG written."""
     a = parse_args(argv)
     kind = "mesh" if a.mesh else "points"
-    ply = os.path.join(a.out_dir, kind, f"{a.scan}.ply")
+    ply = os.path.join(a.out_dir, kind, f"{a.scan}.obj" if a.textured else f"{a.scan}.ply")
     vp = os.path.join(a.out_dir, "viewpoint.json")
     if not os.path.isfile(ply):
         raise SystemExit(f"{ply}: no such file")
     if a.use_viewpoint and not os.path.isfile(vp):
         raise SystemExit(f"{vp}: no such file (write one with --save_viewpoint)")
-    xyz, rgb, faces = load_scan(ply, a.mesh)
+    if a.textured:
+        from . import texture
+        xyz, faces, uv, page, atlas = texture.read_textured_obj(ply)
+        rgb = None
+    else:
+        xyz, rgb, faces = load_scan(ply, a.mesh)
     if a.use_viewpoint:
         try:
             P, wh = read_viewpoint(vp)
@@ -324,10 +375,18 @@ def main(argv=None):
         if a.save_viewpoint:
             write_viewpoint(vp, K, E, wh)
             print(f"viewpoint saved to {vp}")
-    image, depth = draw(xyz, rgb, faces, P, wh, a.point_size)
+    if a.textured:
+        def cuda(x):
+            return torch.from_numpy(np.ascontiguousarray(x)).to("cuda")
+        image, depth = render_textured_mesh(cuda(xyz), cuda(faces), cuda(uv), cuda(page),
+                                            cuda(atlas), P, wh)
+        image, depth = image.cpu().numpy(), depth.cpu().numpy()
+    else:
+        image, depth = draw(xyz, rgb, faces, P, wh, a.point_size)
     from PIL import Image
     os.makedirs(os.path.join(a.out_dir, "render"), exist_ok=True)
-    png = os.path.join(a.out_dir, "render", f"{a.scan}_mesh.png" if a.mesh else f"{a.scan}.png")
+    png = os.path.join(a.out_dir, "render", f"{a.scan}_textured.png" if a.textured else
+                       f"{a.scan}_mesh.png" if a.mesh else f"{a.scan}.png")
     Image.fromarray(image).save(png)
     what = (f"{len(faces)} triangles" if a.mesh else f"{len(xyz) / 1e6:.2f} M points")
     print(f"{a.scan} contains {what}; {int((depth > 0).sum())} of {wh[0] * wh[1]} pixels drawn "

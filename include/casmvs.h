@@ -865,6 +865,78 @@ int casmvs_render_mesh_fwd(const float* verts, const unsigned char* colours, int
                            size_t workspace_bytes, unsigned char* image, float* depth,
                            void* stream);
 
+/* ---- mesh texturing from the views (csrc/texture.cu, casmvsnet_pl_b200/texture.py) -----------
+ * casmvs_render_mesh_keys: the raster pass of casmvs_render_mesh_fwd alone (same arguments, same
+ *   zbuf bits): the view's visibility buffer.
+ * casmvs_render_textured_mesh_fwd: the raster pass, then per covered pixel the winner t's UV
+ *   tu = (((q0 U0 + q1 U1) + q2 U2) / den), likewise tv, from uv (n_faces,3,2) f32 (corner k of
+ *   face t at uv[t][k]); x = tu S - 0.5, y = (1 - tv) S - 0.5, each clamped to [-1, S];
+ *   i = floor, a = x - floor(x) (likewise y); the four texels (i, i + 1) x (j, j + 1) clamped to
+ *   0..S-1 of page[t] in atlas (n_pages,S,S,3) u8 (row j, column i) give
+ *   c = floor(((1 - ay) ((1 - ax) c00 + ax c10) + ay ((1 - ax) c01 + ax c11)) + 0.5), clamped to
+ *   0..255, per channel.  Unshaded.  depth as render_mesh_fwd.
+ * The texturing rule.  Constants: K = 4 candidates, PAD = 2, MIN_COS = 0.1, DEPTH_TOL = 0.01
+ * (the float 1.01f below), at most 8 views per scores call.  Views are P (4,4) f32 row-major
+ * world -> pixel and the eye (3) f64, the camera centre solved from P in double.
+ * casmvs_texture_scores: for n_views views of one batch (HOST arrays: P n*16 f32, eye n*3 f64,
+ *   wh n*2 int32, view_index n int32, zbufs n DEVICE key buffers of casmvs_render_mesh_keys),
+ *   one thread per face f of corners x0, x1, x2 (f32): n = (x1 - x0) x (x2 - x0) and the centroid
+ *   c = ((x0 + x1) + x2) / 3 in double, c' the same in float32.  f is a candidate in view j when
+ *   n.n > 0; x0, x1, x2 and c' project (render_mesh_fwd's projection); each vertex has
+ *   PAD <= u <= W-1-PAD and PAD <= v <= H-1-PAD; |n.d| >= 0.1 (sqrt(n.n) sqrt(d.d)), d = c - eye,
+ *   dots ((a0 b0 + a1 b1) + a2 b2); and each of the four samples has a non-empty key at pixel
+ *   (rint(u), rint(v)) with w <= f32(depth * 1.01f).  Score = f32(0.5 |(u1-u0)(v2-v0) -
+ *   (v1-v0)(u2-u0)|) in double.  cand_score (F,4) f32 and cand_view (F,4) int32 (-1 = empty, the
+ *   caller's initial state) keep the best 4 by (score desc, view asc) across calls made in view
+ *   order.
+ * casmvs_texture_smooth: one Jacobi round over label_in -> label_out (F) int32.  nbr (F,3) int32
+ *   is the face across the edge of corner k (faces[f][k] -- faces[f][(k+1)%3]) when exactly two
+ *   distinct faces share it, else -1.  f takes L when >= 2 of its nbr held L and L is one of its
+ *   candidates with score >= f32(0.5 * best score); otherwise it keeps label_in[f].
+ * casmvs_texture_charts: comp (F) int32 = the least face index of f's component: faces joined
+ *   across nbr edges with equal labels >= 0 (a face of label -1 is alone).  atomicMin hooking and
+ *   pointer jumping, repeated until a hook round changes nothing (flag: 4 device bytes; *rounds,
+ *   HOST, the hook rounds).  Synchronises stream once per round.
+ * casmvs_texture_rects: rect (F,4) int32, filled here: for a root r, (min x0, min y0, max x1,
+ *   max y1) over its faces of label L >= 0 with x0 = floor(min u) - PAD, x1 = ceil(max u) + PAD
+ *   (v likewise) of the face's corners projected by Ps[L] (Ps (n_views,16) f32, DEVICE);
+ *   (INT_MAX, INT_MAX, INT_MIN, INT_MIN) elsewhere.
+ * charts (n_charts,9) int32 rows: root face, view (-1 = flat), x0, y0, x1, y1, page, ox, oy.
+ * casmvs_texture_fill: atlas (pages,S,S,3) u8, zeroed by the caller; a view chart's
+ *   (x1-x0+1) x (y1-y0+1) texels at (ox, oy) of its page are the bytes of its rectangle in
+ *   images[view] (DEVICE array of (H,W,3) u8 device pointers, wh (n_views,2) int32 DEVICE); a flat
+ *   chart's 4 x 4 texels are the root face's vertex colours' mean, (sum + 1) / 3 per channel
+ *   (round half to even, as a third is never a half).
+ * casmvs_texture_uvs: slot (F) int32 = the chart row of f.  page[f] = its page; corner k of a view
+ *   chart's face: (u, v) projected by Ps[label], uv = f32((((u - x0) + ox) + 0.5) / S),
+ *   f32(1 - (((v - y0) + oy) + 0.5) / S) in double; of a flat face: the texel centres
+ *   (1.5, 1.5), (2.5, 1.5), (1.5, 2.5) of its square, f32((o + c) / S) and f32(1 - (o + c) / S). */
+int casmvs_render_mesh_keys(const float* verts, int n_vertices, const int* faces, int n_faces,
+                            const float* P, int W, int H, unsigned long long* zbuf,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int casmvs_render_textured_mesh_fwd(const float* verts, int n_vertices, const int* faces,
+                                    int n_faces, const float* uv, const int* page,
+                                    const unsigned char* atlas, int n_pages, int S, const float* P,
+                                    int W, int H, unsigned long long* zbuf, void* workspace,
+                                    size_t workspace_bytes, unsigned char* image, float* depth,
+                                    void* stream);
+int casmvs_texture_scores(const float* verts, const int* faces, int F, int n_views, const float* P,
+                          const double* eye, const int* wh, const int* view_index,
+                          unsigned long long* const* zbufs, float* cand_score, int* cand_view,
+                          void* stream);
+int casmvs_texture_smooth(const int* nbr, const float* cand_score, const int* cand_view, int F,
+                          const int* label_in, int* label_out, void* stream);
+int casmvs_texture_charts(const int* nbr, const int* label, int F, int* comp, unsigned* flag,
+                          int* rounds, void* stream);
+int casmvs_texture_rects(const float* verts, const int* faces, int F, const int* label,
+                         const int* comp, const float* Ps, int* rect, void* stream);
+int casmvs_texture_fill(const int* charts, int n_charts, const unsigned long long* images,
+                        const int* wh, const unsigned char* colours, const int* faces, int S,
+                        unsigned char* atlas, void* stream);
+int casmvs_texture_uvs(const float* verts, const int* faces, int F, const int* label,
+                       const int* slot, const int* charts, const float* Ps, int S, float* uv,
+                       int* page, void* stream);
+
 /* ---- training panels (csrc/visual.cu; utils/visualization.py, train.py:107-114) ---------
  * The original's TensorBoard image strip as uint8 (H, n*W, 3), n = the number of non-NULL panel
  * inputs, panels left to right in the order img, depth_gt, depth_pred, conf:
