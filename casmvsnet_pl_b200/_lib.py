@@ -191,6 +191,10 @@ SIGNATURES = {
     "casmvs_simplify_collapse": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 6),
     "casmvs_simplify_remap_faces": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "casmvs_simplify_mark_used": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "casmvs_mesh_sample_count": (c_int, [c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p,
+                                         c_void_p]),
+    "casmvs_mesh_sample_points": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_longlong,
+                                          c_void_p, c_void_p]),
     "casmvs_render_points_fwd": (c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
                                          c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "casmvs_render_mesh_workspace_bytes": (c_size_t, [c_int]),

@@ -21,6 +21,11 @@ order is torch.randperm on the CPU seeded by `seed`, and the same seed and input
 same kept set on every run and every GPU.
 
     python -m casmvsnet_pl_b200.dtu_eval --ply_dir results/dtu/points --gt_dir DTU_GT [--scans 1 4]
+    python -m casmvsnet_pl_b200.dtu_eval --mesh_dir results/dtu/mesh --gt_dir DTU_GT [--error_dir E]
+
+A mesh is scored as the toolbox scores surfaces (BaseEvalMain_web.m:14, representation
+'Surfaces'): its surface is sampled at the thinning distance (mesh_sample.py) and the samples are
+scored like points.  --error_dir writes the distance-coloured clouds of BaseEval2Obj_web.m.
 """
 from __future__ import annotations
 
@@ -286,6 +291,53 @@ def evaluate_scan(points, scan, gt_dir, dst=DST, seed=0, device="cuda:0", return
     return out
 
 
+def evaluate_mesh(mesh, scan, gt_dir, dst=DST, seed=0, device="cuda:0", return_arrays=False):
+    """Scores a mesh of one DTU scan as the DTU toolbox scores surfaces: the surface is sampled
+    at the thinning distance `dst` (mesh_sample.sample_surface) and the samples are scored by
+    evaluate_scan.  `mesh` is (verts (V,3) float32, faces (F,3) int) CUDA tensors or a mesh PLY
+    path.  Returns evaluate_scan's dict plus n_faces, n_samples, spacing and time_s["sample_s"];
+    return_arrays adds the samples."""
+    from . import mesh_sample
+    if isinstance(scan, bool) or not isinstance(scan, (int, np.integer)) or scan < 0:
+        raise ValueError(f"scan must be a DTU scan number, got {scan!r}")
+    if not os.path.isdir(gt_dir):
+        raise FileNotFoundError(gt_dir)
+    verts, faces = mesh_sample.load_mesh(mesh, device)
+    t0 = _sync_time()
+    samples = mesh_sample.sample_surface(verts, faces, dst)
+    t1 = _sync_time()
+    out = evaluate_scan(samples, scan, gt_dir, dst, seed, return_arrays=return_arrays)
+    out.update(n_faces=int(len(faces)), n_samples=int(len(samples)), spacing=float(dst))
+    out["time_s"]["sample_s"] = t1 - t0
+    if return_arrays:
+        out["samples"] = samples
+    return out
+
+
+def error_colours(d, inside):
+    """BaseEval2Obj_web.m's colours of distances d (N,) by a flag (N,) bool: alpha = min(d, 10)/10
+    in double, C = [1 0 0] alpha + [1 1 1] (1 - alpha) where inside, else [0 1 0] alpha +
+    [0 0 1] (1 - alpha), each byte floor(255 C + 0.5) -> (N,3) uint8."""
+    a = (np.minimum(np.asarray(d, np.float64), 10.0) / 10.0)[:, None]
+    inside = np.asarray(inside, bool)[:, None]
+    c_in = np.array([1.0, 0.0, 0.0]) * a + np.array([1.0, 1.0, 1.0]) * (1 - a)
+    c_out = np.array([0.0, 1.0, 0.0]) * a + np.array([0.0, 0.0, 1.0]) * (1 - a)
+    return np.floor(255 * np.where(inside, c_in, c_out) + 0.5).astype(np.uint8)
+
+
+def write_error_clouds(out_dir, scan, data, stl, result):
+    """scan{N}_data2stl.ply (the thinned data points coloured by Ddata and DataInMask) and
+    scan{N}_stl2data.ply (the STL points by Dstl and StlAbovePlane) in the point-PLY layout, from
+    evaluate_scan's return_arrays result; `data` is the scored cloud, `stl` the STL points."""
+    from .fusion import write_ply
+    os.makedirs(out_dir, exist_ok=True)
+    kept = result["kept"].cpu().numpy()
+    for name, pts, d, flag in (("data2stl", data[kept], result["Ddata"], result["data_in_mask"]),
+                               ("stl2data", stl, result["Dstl"], result["stl_above_plane"])):
+        write_ply(os.path.join(out_dir, f"scan{scan}_{name}.ply"), pts,
+                  error_colours(d.cpu().numpy(), flag.cpu().numpy()))
+
+
 def _require_device(dev):
     if dev.type != "cuda" or not torch.cuda.is_available():
         raise _lib.CasMVSError("DTU scoring runs on the GPU (no CPU fallback)")
@@ -321,18 +373,41 @@ def _fmt(r):
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="Score fused DTU point clouds (scan{N}.ply) on the GPU.")
-    ap.add_argument("--ply_dir", required=True)
+    ap = argparse.ArgumentParser(description="Score fused DTU point clouds or meshes (scan{N}.ply) "
+                                             "on the GPU.")
+    src = ap.add_mutually_exclusive_group(required=True)
+    src.add_argument("--ply_dir", help="fused point clouds scan{N}.ply")
+    src.add_argument("--mesh_dir", help="meshes scan{N}.ply (as eval_pipeline --mesh writes them): "
+                                        "the surface is sampled at --dst and scored like points")
     ap.add_argument("--gt_dir", required=True)
     ap.add_argument("--scans", nargs="+", type=int, default=list(USED_SETS))
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--dst", type=float, default=DST)
     ap.add_argument("--device", default="cuda:0")
     ap.add_argument("--out", default="")
+    ap.add_argument("--error_dir", default="",
+                    help="also write scan{N}_data2stl.ply and scan{N}_stl2data.ply here: the scored "
+                         "points coloured by their distance (BaseEval2Obj_web.m)")
     a = ap.parse_args(argv)
     results = []
     for s in a.scans:
-        r = evaluate_scan(os.path.join(a.ply_dir, f"scan{s}.ply"), s, a.gt_dir, a.dst, a.seed, a.device)
+        path = os.path.join(a.mesh_dir or a.ply_dir, f"scan{s}.ply")
+        arrays = bool(a.error_dir)
+        if a.mesh_dir:
+            r = evaluate_mesh(path, s, a.gt_dir, a.dst, a.seed, a.device, return_arrays=arrays)
+            data = r.pop("samples", None)
+        elif arrays:
+            dev = torch.device(a.device)
+            _require_device(dev)
+            data = torch.from_numpy(read_points(path)).to(dev)
+            r = evaluate_scan(data, s, a.gt_dir, a.dst, a.seed, return_arrays=True)
+        else:
+            r = evaluate_scan(path, s, a.gt_dir, a.dst, a.seed, a.device)
+        if arrays:
+            stl = read_points(stl_path(a.gt_dir, s))
+            write_error_clouds(a.error_dir, s, data.cpu().numpy(), stl, r)
+            for k in ("kept", "Ddata", "Dstl", "data_in_mask", "stl_above_plane"):
+                r.pop(k)
         print(_fmt(r), flush=True)
         results.append(r)
     summ = summarize(results)

@@ -45,6 +45,9 @@ reconstruction instead (poisson.py); --poisson_point_weight A > 0 screens it.
 (simplify.py).
 --mesh --mesh_texture also textures the mesh that is written from the scan's reference-view images
 at --img_wh and writes <out>/mesh/<scan>.obj, .mtl and _<k>.png beside the PLY (texture.py).
+--mesh --mesh_score with --dtu_gt or --tnt_gt also scores the mesh as it is written, through its
+surface samples (dtu_eval.evaluate_mesh / tnt_eval.evaluate_mesh), into <out>/mesh/<scan>_scores.json
+or <out>/mesh/<scan>_tnt.json.
 """
 from __future__ import annotations
 
@@ -445,6 +448,25 @@ def _simplify(name, verts, colours, faces, mesh_faces, log):
     return verts, colours, faces
 
 
+def _score_mesh(scan, mesh_path, verts, faces, dtu_gt, dtu_seed, tnt_gt, tnt_images, tnt_tau,
+                tnt_seed, run_dir):
+    """Scores of the written mesh against the Tanks and Temples (tnt_gt) or DTU (dtu_gt) ground
+    truth, written beside it as <mesh>_tnt.json or <mesh>_scores.json."""
+    stem = os.path.splitext(mesh_path)[0]
+    if tnt_gt is not None:
+        from . import tnt_eval
+        scores = tnt_eval.evaluate_mesh((verts, faces), run_dir, tnt_gt, scan.scan, tnt_tau, tnt_seed,
+                                        images=tnt_images)
+        tnt_eval.write_json(stem + "_tnt.json", scores)
+        return scores
+    from . import dtu_eval
+    scores = dtu_eval.evaluate_mesh((verts, faces), dtu_eval.scan_number(scan.scan), dtu_gt,
+                                    seed=dtu_seed)
+    with open(stem + "_scores.json", "w") as f:
+        json.dump(scores, f, indent=1)
+    return scores
+
+
 def _texture(name, mesh_path, verts, colours, faces, images, proj0, log):
     """Texture the written mesh from the reference views' images (cast to uint8) and proj0, and
     write <mesh_path without .ply>.obj / .mtl / _<k>.png."""
@@ -463,7 +485,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
              mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
-             mesh_texture=False):
+             mesh_texture=False, mesh_score=False):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -484,7 +506,13 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
-    is given, and (xyz, rgb, scores) is returned."""
+    is given, and (xyz, rgb, scores) is returned.
+    With `mesh_score` (it needs `mesh_path` and `tnt_gt` or `dtu_gt`), the mesh as written is also
+    scored through its surface samples by tnt_eval.evaluate_mesh or dtu_eval.evaluate_mesh, the
+    scores are written beside it as <mesh>_tnt.json or <mesh>_scores.json, and appended to the
+    returned tuple."""
+    if mesh_score and (mesh_path is None or (tnt_gt is None and dtu_gt is None)):
+        raise ValueError("mesh_score needs mesh_path and a ground truth (dtu_gt or tnt_gt)")
     depths, probas = {}, {}
     writer = io.DepthWriter(depth_dir) if depth_dir else None
     for ref, imgs, pm in scan.views(device):
@@ -524,6 +552,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
             _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log)
+        written = (verts, faces)
         log(f"{scan.scan}: poisson mesh at depth {st['depth']} (h {st['h']:.6g}): {st['points']} "
             f"points ({st['dropped']} dropped), {st['cycles']} cycles, {st['bricks']} bricks, "
             f"{st['vertices']} vertices, {st['triangles']} triangles")
@@ -540,16 +569,21 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
             _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log)
+        written = (verts, faces)
         log(f"{scan.scan}: mesh at voxel {st['voxel']:.6g}: {st['bricks']} bricks, {st['voxels']} "
             f"voxels, {st['vertices']} vertices, {st['triangles']} triangles, {st['dropped']} "
             "points dropped")
+    extra = ()
+    if mesh_score:
+        extra = (_score_mesh(scan, mesh_path, *written, dtu_gt, dtu_seed, tnt_gt, tnt_images, tnt_tau,
+                             tnt_seed, run_dir),)
     if tnt_gt is not None:
         from . import tnt_eval
         scores = tnt_eval.evaluate_scene(xyz, run_dir, tnt_gt, scan.scan, tnt_tau, tnt_seed,
                                          images=tnt_images)
         if ply_path:
             tnt_eval.write_json(os.path.splitext(ply_path)[0] + "_tnt.json", scores)
-        return xyz, rgb, scores
+        return (xyz, rgb, scores) + extra
     if dtu_gt is None:
         return xyz, rgb
     from . import dtu_eval
@@ -557,7 +591,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     if ply_path:
         with open(os.path.splitext(ply_path)[0] + "_scores.json", "w") as f:
             json.dump(scores, f, indent=1)
-    return xyz, rgb, scores
+    return (xyz, rgb, scores) + extra
 
 
 def open_scans(a):
@@ -652,7 +686,15 @@ def parse_args(argv=None):
     ap.add_argument("--mesh_texture", action="store_true",
                     help="with --mesh: also texture the mesh from the reference views and write "
                          "<out>/mesh/<scan>.obj with its .mtl and atlas PNGs")
+    ap.add_argument("--mesh_score", action="store_true",
+                    help="with --mesh and --dtu_gt or --tnt_gt: also score the mesh as written "
+                         "through its surface samples into <out>/mesh/<scan>_scores.json "
+                         "(DTU) or <scan>_tnt.json")
     a = ap.parse_args(argv)
+    if a.mesh_score and not a.mesh:
+        ap.error("--mesh_score needs --mesh")
+    if a.mesh_score and a.dtu_gt is None and a.tnt_gt is None:
+        ap.error("--mesh_score needs a ground truth: --dtu_gt or --tnt_gt")
     if a.mesh_texture and not a.mesh:
         ap.error("--mesh_texture needs --mesh")
     if a.mesh_faces is not None and not a.mesh:
@@ -718,7 +760,8 @@ def main(argv=None):
                        mesh_voxel=a.mesh_voxel, mesh_method=a.mesh_method,
                        poisson_depth=a.poisson_depth,
                        poisson_point_weight=a.poisson_point_weight or 0.0,
-                       mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture, **tnt)
+                       mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture,
+                       mesh_score=a.mesh_score, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt
@@ -726,6 +769,8 @@ def main(argv=None):
         if a.tnt_gt is not None:
             from .tnt_eval import _fmt
             print(_fmt(out[2]))
+        if a.mesh_score:
+            print(f"mesh {_fmt(out[3])}  ({out[3]['n_faces']} faces -> {out[3]['n_samples']} samples)")
 
 
 if __name__ == "__main__":

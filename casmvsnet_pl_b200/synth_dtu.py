@@ -37,6 +37,24 @@ def _surface(rng, n, L):
     return np.stack([x, y, _height(x, y, L)], axis=1)
 
 
+def height_mesh(stl, step, shift=0.0):
+    """The scene's height field triangulated over the x, y extent of its STL points `stl` (N,3)
+    on a grid of about `step` mm, lifted by `shift` mm in z -> (verts (V,3) float32, faces (F,3)
+    int32, L, the grid cells' diagonal)."""
+    L = float(np.sqrt(len(stl) / STL_DENSITY))
+    lo = np.asarray(stl, np.float64)[:, :2].min(0) - CENTER[:2]
+    hi = np.asarray(stl, np.float64)[:, :2].max(0) - CENTER[:2]
+    m = [int(np.ceil((hi[k] - lo[k]) / step)) for k in range(2)]
+    x, y = np.meshgrid(np.linspace(lo[0], hi[0], m[0] + 1), np.linspace(lo[1], hi[1], m[1] + 1),
+                       indexing="xy")
+    z = _height(x, y, L) + shift
+    verts = (np.stack([x.ravel(), y.ravel(), z.ravel()], 1) + CENTER).astype(np.float32)
+    i = (np.arange(m[0])[None, :] + (m[0] + 1) * np.arange(m[1])[:, None]).ravel()
+    faces = np.concatenate([np.stack([i, i + 1, i + m[0] + 2], 1),
+                            np.stack([i, i + m[0] + 2, i + m[0] + 1], 1)]).astype(np.int32)
+    return verts, faces, L, float(np.hypot(*[(hi[k] - lo[k]) / m[k] for k in range(2)]))
+
+
 def write_ground_truth(gt_dir, scan, stl, ground_z, empty_mask=False, res=1.0):
     """Writes the DTU ground-truth layout for the STL cloud `stl` (N,3): BB = bounds +- 10 mm,
     ObsMask = voxels of edge `res` within 3 voxels of an STL point (all false with empty_mask),

@@ -55,6 +55,33 @@ def sample_surfaces(rng, n):
     return p, which
 
 
+def surface_mesh(res=1.0):
+    """The plane, sphere and wall of sample_surfaces triangulated in the ground-truth frame ->
+    (verts (V,3) float64, faces (F,3) int32): grids of 100 res x 100 res squares on the plane,
+    256 res x 128 res longitude-latitude cells on the sphere and 30 x 15 squares on the wall."""
+    parts, faces, off = [], [], 0
+    for P in _surface_grids(res):
+        nv, nu = P.shape[0] - 1, P.shape[1] - 1
+        i = (np.arange(nu)[None, :] + (nu + 1) * np.arange(nv)[:, None]).ravel() + off
+        faces.append(np.concatenate([np.stack([i, i + 1, i + nu + 2], 1),
+                                     np.stack([i, i + nu + 2, i + nu + 1], 1)]))
+        parts.append(P.reshape(-1, 3))
+        off += len(parts[-1])
+    return np.concatenate(parts), np.concatenate(faces).astype(np.int32)
+
+
+def _surface_grids(res):
+    n = int(100 * res)
+    u, w = np.meshgrid(np.linspace(-2.5, 2.5, n + 1), np.linspace(-2.5, 2.5, n + 1), indexing="xy")
+    yield np.stack([u, w, np.zeros_like(u)], -1)
+    nt, nz = int(256 * res), int(128 * res)
+    th, ph = np.meshgrid(np.linspace(0, 2 * np.pi, nt + 1), np.linspace(0, np.pi, nz + 1), indexing="xy")
+    yield np.stack([0.8 * np.sin(ph) * np.cos(th), 0.8 * np.sin(ph) * np.sin(th),
+                    0.8 + 0.8 * np.cos(ph)], -1)
+    u, w = np.meshgrid(np.linspace(-1.5, 1.5, 31), np.linspace(0, 1.5, 16), indexing="xy")
+    yield np.stack([np.full_like(u, -1.5), u, w], -1)
+
+
 CROP_POLYGON = [[2.0, 0.0], [1.0, 1.9], [-1.9, 1.9], [-1.9, -1.9], [1.0, -1.9]]
 
 

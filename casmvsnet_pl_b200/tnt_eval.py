@@ -32,6 +32,10 @@ scores and transforms, bit for bit.
 
     python -m casmvsnet_pl_b200.tnt_eval --ply points/Barn.ply --run_dir results/colmap/Barn \\
         --gt_dir TNT_GT --scene Barn [--images Barn/images] [--out scores.json]
+    python -m casmvsnet_pl_b200.tnt_eval --mesh mesh/Barn.ply --run_dir results/colmap/Barn ...
+
+A mesh is scored through its surface samples at tau / 4 (mesh_sample.py); alignment uses only
+the cameras, so it is the same as for a cloud.
 """
 from __future__ import annotations
 
@@ -592,6 +596,29 @@ def evaluate_scene(points_or_ply, trajectory, gt_dir, scene, tau=None, seed=0, r
     return out
 
 
+def evaluate_mesh(mesh, trajectory, gt_dir, scene, tau=None, seed=0, images=None, device="cuda:0",
+                  return_arrays=False):
+    """Scores a mesh of one Tanks and Temples training scene: its surface is sampled at tau / 4
+    (mesh_sample.sample_surface), below the tau / 2 voxels scoring downsamples to, so every voxel
+    the surface crosses gets samples, and the samples are scored by evaluate_scene.  `mesh` is
+    (verts (V,3) float32, faces (F,3) int) CUDA tensors or a mesh PLY path.  Returns
+    evaluate_scene's dict plus n_faces, n_samples, spacing and time_s["sample_s"];
+    return_arrays adds the samples."""
+    from . import mesh_sample
+    tau = scene_tau(scene, tau)
+    prepare(trajectory, gt_dir, scene, tau, images)
+    verts, faces = mesh_sample.load_mesh(mesh, device)
+    t0 = _sync_time()
+    samples = mesh_sample.sample_surface(verts, faces, tau / 4)
+    t1 = _sync_time()
+    out = evaluate_scene(samples, trajectory, gt_dir, scene, tau, seed, return_arrays, images)
+    out.update(n_faces=int(len(faces)), n_samples=int(len(samples)), spacing=tau / 4)
+    out["time_s"]["sample_s"] = t1 - t0
+    if return_arrays:
+        out["samples"] = samples
+    return out
+
+
 def _fmt(r):
     t = r["time_s"]
     return (f"{r['scene']}: tau {r['tau']:g}  precision {r['precision']:.4f}  recall "
@@ -609,7 +636,10 @@ def write_json(path, result):
 def main(argv=None):
     ap = argparse.ArgumentParser(description="Score a reconstruction of a Tanks and Temples "
                                              "training scene on the GPU.")
-    ap.add_argument("--ply", required=True)
+    src = ap.add_mutually_exclusive_group(required=True)
+    src.add_argument("--ply", help="the reconstruction's point cloud")
+    src.add_argument("--mesh", help="a mesh PLY: its surface is sampled at tau / 4 and scored "
+                                    "like points")
     g = ap.add_mutually_exclusive_group(required=True)
     g.add_argument("--run_dir", help="a run's scan directory: cams/*_cam.txt and view_names.txt")
     g.add_argument("--log", help="the reconstruction's camera poses as a .log")
@@ -626,8 +656,12 @@ def main(argv=None):
         prepare(a.run_dir or a.log, a.gt_dir, a.scene, a.tau, a.images)
     except (ValueError, FileNotFoundError) as e:
         raise SystemExit(f"tnt_eval: {e}")
-    r = evaluate_scene(a.ply, a.run_dir or a.log, a.gt_dir, a.scene, a.tau, a.seed,
-                       images=a.images, device=a.device)
+    if a.mesh:
+        r = evaluate_mesh(a.mesh, a.run_dir or a.log, a.gt_dir, a.scene, a.tau, a.seed,
+                          images=a.images, device=a.device)
+    else:
+        r = evaluate_scene(a.ply, a.run_dir or a.log, a.gt_dir, a.scene, a.tau, a.seed,
+                           images=a.images, device=a.device)
     print(_fmt(r), flush=True)
     if a.out:
         write_json(a.out, r)

@@ -827,6 +827,24 @@ int casmvs_simplify_remap_faces(int* faces, int F, const int* map, unsigned char
                                 void* stream);
 int casmvs_simplify_mark_used(const int* faces, int F, int V, int* used, void* stream);
 
+/* ---- uniform surface sampling (csrc/mesh_sample.cu, casmvsnet_pl_b200/mesh_sample.py) --------
+ * Scores a mesh with the point-cloud scorers by sampling its surface.  A mesh is verts (V,3) f32
+ * and faces (F,3) int32, 3F < 2^31.  Every double operation is rounded to nearest in the order
+ * written, with no contraction, and no atomics are used, so results are bitwise reproducible.
+ * For face f = (a, b, c) in its stored corner order, vertices read as double, with spacing s:
+ *   L = the longest of |b - a|, |c - b|, |a - c|, |q - p| = sqrt((dx dx + dy dy) + dz dz),
+ *   n = max(1, (int)min(ceil(L / s), 2^16)), count = (n + 1)(n + 2) / 2 samples;
+ *   sample (i, j), i = 0..n, j = 0..n - i, has local index k = i (n + 1) - i (i - 1) / 2 + j and
+ *   position f32((a + (i/n)(b - a)) + (j/n)(c - a)) per coordinate.
+ * Output is face-major, then k; shared edges and vertices are sampled once per face.
+ * casmvs_mesh_sample_count: n (F) int32 and count (F) int64 per face; spacing finite and > 0.
+ * casmvs_mesh_sample_points: out (S,3) f32, S = sum of count < 2^31, given n and start (F) int64,
+ *   the exclusive prefix sum of count.  One thread per sample. */
+int casmvs_mesh_sample_count(const float* verts, const int* faces, int F, double spacing, int* n,
+                             long long* count, void* stream);
+int casmvs_mesh_sample_points(const float* verts, const int* faces, int F, const int* n,
+                              const long long* start, long long S, float* out, void* stream);
+
 /* ---- headless rendering of clouds and meshes (casmvsnet_pl_b200/render.py) -----------------
  * P is a HOST array of 16 floats, row-major, world -> pixel (rows 0..2 used): every float
  * operation below is rounded to nearest, no contraction, in the order written.
