@@ -217,7 +217,22 @@ SIGNATURES = {
     "casmvs_texture_fill": (c_int, [c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p]),
     "casmvs_texture_uvs": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4
                            + [c_int, c_void_p, c_void_p, c_void_p]),
-    "casmvs_visual_panels": (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "casmvs_texture_level_keys": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_texture_level_corners": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_texture_level_edges": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 6),
+    "casmvs_texture_level_samples": (c_int, [c_void_p] * 6 + [c_int] + [c_void_p] * 5),
+    "casmvs_texture_level_pairs": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_texture_level_system": (c_int, [c_void_p, c_void_p, c_longlong, c_int] + [c_void_p] * 7),
+    "casmvs_texture_level_cg_workspace_bytes": (c_size_t, [c_int]),
+    "casmvs_texture_level_cg": (c_int, [c_void_p] * 5 + [c_int, c_void_p, c_void_p, c_size_t, c_int,
+                                                         c_double, c_int, POINTER(c_int),
+                                                         POINTER(c_double), POINTER(c_int),
+                                                         c_void_p]),
+    "casmvs_texture_level_owners": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4
+                                    + [c_int, c_void_p, c_void_p]),
+    "casmvs_texture_level_apply": (c_int, [c_void_p, c_longlong] + [c_void_p] * 6
+                                   + [c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_visual_panels":(c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
 }

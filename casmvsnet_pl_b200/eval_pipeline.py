@@ -44,7 +44,8 @@ reconstruction instead (poisson.py); --poisson_point_weight A > 0 screens it.
 --mesh --mesh_faces N decimates either mesh to at most N faces on the GPU before it is written
 (simplify.py).
 --mesh --mesh_texture also textures the mesh that is written from the scan's reference-view images
-at --img_wh and writes <out>/mesh/<scan>.obj, .mtl and _<k>.png beside the PLY (texture.py).
+at --img_wh and writes <out>/mesh/<scan>.obj, .mtl and _<k>.png beside the PLY (texture.py);
+--mesh_texture_level also levels the colour seams between its charts, changing only the PNGs.
 --mesh --mesh_score with --dtu_gt or --tnt_gt also scores the mesh as it is written, through its
 surface samples (dtu_eval.evaluate_mesh / tnt_eval.evaluate_mesh), into <out>/mesh/<scan>_scores.json
 or <out>/mesh/<scan>_tnt.json.
@@ -467,16 +468,21 @@ def _score_mesh(scan, mesh_path, verts, faces, dtu_gt, dtu_seed, tnt_gt, tnt_ima
     return scores
 
 
-def _texture(name, mesh_path, verts, colours, faces, images, proj0, log):
+def _texture(name, mesh_path, verts, colours, faces, images, proj0, log, level=False):
     """Texture the written mesh from the reference views' images (cast to uint8) and proj0, and
-    write <mesh_path without .ply>.obj / .mtl / _<k>.png."""
+    write <mesh_path without .ply>.obj / .mtl / _<k>.png; with `level`, the seams are levelled."""
     from . import texture
     vids = sorted(images)
     ims = [images[v].to(torch.uint8).contiguous() for v in vids]
-    uv, page, atlas, st = texture.texture_mesh(verts, colours, faces, ims, [proj0[v] for v in vids])
+    uv, page, atlas, st = texture.texture_mesh(verts, colours, faces, ims, [proj0[v] for v in vids],
+                                               level=level, log=log)
     texture.write_textured_obj(os.path.splitext(mesh_path)[0] + ".obj", verts, faces, uv, page, atlas)
     log(f"{name}: textured {st['faces']} faces from {st['views']} views: {st['unseen_faces']} "
         f"unseen, {st['charts']} charts on {st['pages']} pages ({st['packed_share']:.1%} packed)")
+    if level:
+        lv = st["level"]
+        log(f"{name}: levelled {lv['seam_pairs']} seam pairs in {lv['cg_iterations']} CG iterations: "
+            f"seam RMS {lv['seam_rms_before']:.3f} -> {lv['seam_rms_after']:.3f}")
 
 
 @torch.no_grad()
@@ -485,7 +491,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
              mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
-             mesh_texture=False, mesh_score=False):
+             mesh_texture=False, mesh_score=False, mesh_texture_level=False):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -502,7 +508,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     `poisson_point_weight` when it is > 0.  With `mesh_faces`, either mesh is decimated to at most
     that many faces (simplify.py) before it is written.  With `mesh_texture`, the written mesh is
     also textured from the reference views' images and proj0 (texture.py) and written beside it
-    as an OBJ with its MTL and atlas PNGs.
+    as an OBJ with its MTL and atlas PNGs; `mesh_texture_level` also levels its colour seams.
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
@@ -551,7 +557,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
-            _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log)
+            _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log,
+                     mesh_texture_level)
         written = (verts, faces)
         log(f"{scan.scan}: poisson mesh at depth {st['depth']} (h {st['h']:.6g}): {st['points']} "
             f"points ({st['dropped']} dropped), {st['cycles']} cycles, {st['bricks']} bricks, "
@@ -568,7 +575,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
-            _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log)
+            _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log,
+                     mesh_texture_level)
         written = (verts, faces)
         log(f"{scan.scan}: mesh at voxel {st['voxel']:.6g}: {st['bricks']} bricks, {st['voxels']} "
             f"voxels, {st['vertices']} vertices, {st['triangles']} triangles, {st['dropped']} "
@@ -686,6 +694,9 @@ def parse_args(argv=None):
     ap.add_argument("--mesh_texture", action="store_true",
                     help="with --mesh: also texture the mesh from the reference views and write "
                          "<out>/mesh/<scan>.obj with its .mtl and atlas PNGs")
+    ap.add_argument("--mesh_texture_level", action="store_true",
+                    help="with --mesh_texture: level the colour seams between the atlas's charts "
+                         "(global colour adjustment); only the page PNGs change")
     ap.add_argument("--mesh_score", action="store_true",
                     help="with --mesh and --dtu_gt or --tnt_gt: also score the mesh as written "
                          "through its surface samples into <out>/mesh/<scan>_scores.json "
@@ -697,6 +708,8 @@ def parse_args(argv=None):
         ap.error("--mesh_score needs a ground truth: --dtu_gt or --tnt_gt")
     if a.mesh_texture and not a.mesh:
         ap.error("--mesh_texture needs --mesh")
+    if a.mesh_texture_level and not a.mesh_texture:
+        ap.error("--mesh_texture_level needs --mesh_texture")
     if a.mesh_faces is not None and not a.mesh:
         ap.error("--mesh_faces needs --mesh")
     if a.mesh_faces is not None and a.mesh_faces < 1:
@@ -761,7 +774,7 @@ def main(argv=None):
                        poisson_depth=a.poisson_depth,
                        poisson_point_weight=a.poisson_point_weight or 0.0,
                        mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture,
-                       mesh_score=a.mesh_score, **tnt)
+                       mesh_score=a.mesh_score, mesh_texture_level=a.mesh_texture_level, **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

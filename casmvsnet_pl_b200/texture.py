@@ -29,7 +29,38 @@ The rule (include/casmvs.h states every operation):
 7. a view chart's texels are a byte copy of its rectangle; a flat chart is the mean of its face's
    vertex colours (rounded half to even); unused texels are 0;
 8. a corner's UV is ((u - x0 + ox + 0.5) / S, 1 - (v - y0 + oy + 0.5) / S) in double, stored as
-   float32; a flat face's corners sit on texel centres inside its square."""
+   float32; a flat face's corners sit on texel centres inside its square.
+
+With level=True (`--level`), the seams between charts are then levelled by Waechter et al.'s
+global colour adjustment (csrc/texture_level.cu; numpy restatement in
+oracle/texture_level_oracle.py, bit for bit but for the solve).  UVs, pages, charts, the packing
+and flat charts do not change; only the texels of view charts do:
+1. seams: the edge of corner k of f is a seam when g = nbr[f][k] >= 0, both labels are >= 0 and
+   slot[f] != slot[g]; open and non-manifold edges never are, and flat charts take no part;
+2. unknowns: one RGB offset g per (chart, vertex) pair of a view-chart face's corner, numbered by
+   the sorted key (slot << 32) | vertex;
+3. seam colours: for each seam edge and each endpoint v, SEAM_SAMPLES points v + t (w - v),
+   t = k / SEAM_SAMPLES, in double, are projected into both charts' views and sampled bilinearly
+   (pixel centres at integer coordinates); f_(v,i) of the pair (v; i, j) is the (1 - t)-weighted
+   mean of the view(i) samples over v's seam edges between i and j, summed in record order;
+4. system: minimise sum_pairs (f_(v,i) + g_(v,i) - f_(v,j) - g_(v,j))^2 + SMOOTH_WEIGHT
+   sum over each chart's unique edges (g_a - g_b)^2 + EPS sum g^2, one CSR matrix for the three
+   channels.  SMOOTH_WEIGHT = 10 is Waechter's 1/lambda with lambda = 0.1.  EPS = 1e-4 only makes
+   the matrix definite: the right-hand side sums to zero over every group of charts joined by
+   seams, so the near-null modes it would otherwise leave carry no load.  Its damping of a chart's
+   mean offset is 1 / (1 + EPS N / (2 m)) for two charts of N unknowns each meeting at m seam
+   pairs: 5e-5 in the two-quad test, 0.25 % for N = 10^4 and m = 200;
+5. solve: Jacobi-preconditioned conjugate gradients in double, the three channels sharing each
+   SpMV, until every channel has ||r|| / ||b|| <= CG_TOL or after CG_MAX_ITERS iterations (an
+   unconverged solve is logged and recorded).  The host reads the convergence flag every
+   CG_CHECK_EVERY iterations; the device stops on the exact iteration either way;
+6. texel offsets: each texel of a view chart sits at view pixel (x0 + k, y0 + l); its owner is the
+   chart face whose projected triangle lies nearest that point, within REACH = 1.5 texels (>= sqrt 2,
+   so every bilinear tap of a point inside a face is reached and sliver faces that hold no texel
+   centre are still covered), ties to the lower face; its offset is the owner's corner offsets
+   interpolated at the barycentrics of the nearest point;
+7. apply: texel = clamp(rint(byte + offset), 0, 255) per channel; texels without an owner keep
+   their bytes."""
 from __future__ import annotations
 
 import argparse
@@ -55,6 +86,17 @@ FLAT = 4
 # keys, unique edges and sorts of the neighbour table (~120), labels, components, rectangles,
 # slots, UVs and pages (~72)
 BYTES_PER_FACE = 224
+SEAM_SAMPLES = 8
+SMOOTH_WEIGHT = 10.0
+LEVEL_EPS = 1e-4
+REACH = 1.5
+CG_TOL = 1e-9
+CG_MAX_ITERS = 10000
+CG_CHECK_EVERY = 16
+# device bytes per face of the levelling, at most 3 unknowns, 3 seam records and 15 matrix entries
+# per face: corner keys and unknowns (~60), edge keys and seam records with their sorts and
+# colours (~300), matrix keys, their sort and the CSR (~360), CG vectors (6 x 3 unknowns x 24 = 432)
+LEVEL_BYTES_PER_FACE = 1152
 
 
 def _ptr(t):
@@ -244,8 +286,163 @@ def pack(ids, w, h, S):
     return page, ox, oy, (p + 1 if len(ids) else 0)
 
 
+# ---------------------------------------------------------------------------- seam levelling
+def _i64(x):
+    return torch.as_tensor(x, dtype=torch.int64)
+
+
+def level_unknowns(faces, labels, slot):
+    """Levelling step 2 -> (unknowns (n,) int64 ascending, (slot << 32) | vertex of every corner
+    of a view-chart face; corner (F,3) int32, the unknown of each corner, -1 on flat faces)."""
+    lib, F = _lib.load(), len(faces)
+    keys = torch.empty(3 * F, dtype=torch.int64, device=faces.device)
+    _lib.check(lib.casmvs_texture_level_keys(_ptr(faces), F, _ptr(labels), _ptr(slot), _ptr(keys),
+                                             _stream()), "texture_level_keys")
+    unk = torch.unique(keys[keys >= 0], sorted=True)
+    corner = torch.empty(F, 3, dtype=torch.int32, device=faces.device)
+    _lib.check(lib.casmvs_texture_level_corners(_ptr(keys), F, _ptr(unk), len(unk), _ptr(corner),
+                                                _stream()), "texture_level_corners")
+    return unk, corner
+
+
+def level_edges(nbr, faces, labels, slot, corner):
+    """Levelling step 1 -> (rec_key, rec_sub) of the seam endpoint records, sorted by (pair key,
+    record), and the distinct smoothing-edge keys (min << 32) | max of unknowns, ascending."""
+    lib, F = _lib.load(), len(faces)
+    rec = torch.empty(6 * F, dtype=torch.int64, device=faces.device)
+    sm = torch.empty(3 * F, dtype=torch.int64, device=faces.device)
+    _lib.check(lib.casmvs_texture_level_edges(_ptr(nbr), _ptr(faces), F, _ptr(labels), _ptr(slot),
+                                              _ptr(corner), _ptr(rec), _ptr(sm), _stream()),
+               "texture_level_edges")
+    sub = torch.nonzero(rec >= 0).squeeze(1)
+    key, order = torch.sort(rec[sub], stable=True)
+    return key, sub[order].contiguous(), torch.unique(sm[sm >= 0], sorted=True)
+
+
+def level_seam_colours(verts, faces, labels, slot, nbr, rec_key, rec_sub, img_ptrs, img_wh, Pdev):
+    """Levelling step 3 -> (pair keys (P,) int64 ascending, (a << 32) | b; fpair (P,6) float64,
+    f_a and f_b: the seam colours of each pair in the lower and the upper chart's view)."""
+    lib, R = _lib.load(), len(rec_sub)
+    rec = torch.empty(R, 6, dtype=torch.float64, device=verts.device)
+    _lib.check(lib.casmvs_texture_level_samples(_ptr(verts), _ptr(faces), _ptr(labels), _ptr(slot),
+                                                _ptr(nbr), _ptr(rec_sub), R, _ptr(Pdev),
+                                                _ptr(img_ptrs), _ptr(img_wh), _ptr(rec), _stream()),
+               "texture_level_samples")
+    keys, cnt = torch.unique_consecutive(rec_key, return_counts=True)
+    seg = torch.zeros(len(keys) + 1, dtype=torch.int64, device=verts.device)
+    seg[1:] = torch.cumsum(cnt, 0)
+    fpair = torch.empty(len(keys), 6, dtype=torch.float64, device=verts.device)
+    _lib.check(lib.casmvs_texture_level_pairs(_ptr(rec), _ptr(seg), len(keys), _ptr(fpair),
+                                              _stream()), "texture_level_pairs")
+    return keys, fpair
+
+
+def level_system(pair_keys, smooth_keys, n, fpair):
+    """Levelling step 4 -> (rowptr (n+1) int32, col (nnz) int32, val (nnz), diag (n), rhs (n,3)
+    float64): A g = rhs, A in CSR with columns ascending in each row."""
+    dev = fpair.device
+    lo32 = 0xFFFFFFFF
+    lp, hp, ls, hs = pair_keys >> 32, pair_keys & lo32, smooth_keys >> 32, smooth_keys & lo32
+    a = torch.arange(n, dtype=torch.int64, device=dev)
+    P, E = len(pair_keys), len(smooth_keys)
+    ekey = torch.cat([(lp << 32) | hp, (hp << 32) | lp, (ls << 32) | hs, (hs << 32) | ls,
+                      (a << 32) | a])
+    pid = torch.arange(P, dtype=torch.int32, device=dev)
+    etype = torch.cat([pid, pid, torch.full((2 * E,), -2, dtype=torch.int32, device=dev),
+                       torch.full((n,), -1, dtype=torch.int32, device=dev)])
+    ekey, order = torch.sort(ekey)
+    etype = etype[order].contiguous()
+    del order
+    nnz = len(ekey)
+    rowptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    col = torch.empty(nnz, dtype=torch.int32, device=dev)
+    val = torch.empty(nnz, dtype=torch.float64, device=dev)
+    diag = torch.empty(n, dtype=torch.float64, device=dev)
+    rhs = torch.empty(n, 3, dtype=torch.float64, device=dev)
+    _lib.check(_lib.load().casmvs_texture_level_system(
+        _ptr(ekey), _ptr(etype), nnz, n, _ptr(fpair), _ptr(rowptr), _ptr(col), _ptr(val), _ptr(diag),
+        _ptr(rhs), _stream()), "texture_level_system")
+    return rowptr, col, val, diag, rhs
+
+
+def level_solve(rowptr, col, val, diag, rhs, tol=CG_TOL, max_iters=CG_MAX_ITERS,
+                check_every=CG_CHECK_EVERY):
+    """Levelling step 5 -> (g (n,3) float64, iterations, ratios (3 floats), converged)."""
+    lib, n = _lib.load(), len(diag)
+    g = torch.empty(n, 3, dtype=torch.float64, device=rhs.device)
+    ws = torch.empty(max(1, lib.casmvs_texture_level_cg_workspace_bytes(n)), dtype=torch.uint8,
+                     device=rhs.device)
+    iters, conv = ctypes.c_int(0), ctypes.c_int(0)
+    ratios = (ctypes.c_double * 3)()
+    _lib.check(lib.casmvs_texture_level_cg(
+        _ptr(rowptr), _ptr(col), _ptr(val), _ptr(diag), _ptr(rhs), n, _ptr(g), _ptr(ws), ws.numel(),
+        max_iters, tol, check_every, ctypes.byref(iters), ratios, ctypes.byref(conv), _stream()),
+        "texture_level_cg")
+    return g, iters.value, list(ratios), bool(conv.value)
+
+
+def level_owners(verts, faces, labels, slot, cdev, Pdev, S, n_pages):
+    """Levelling step 6 -> owner (pages,S,S) int64: (f32 distance bits << 32) | face of each
+    texel's owner, -1 (all bits set) where it has none."""
+    owner = torch.full((n_pages, S, S), -1, dtype=torch.int64, device=verts.device)
+    _lib.check(_lib.load().casmvs_texture_level_owners(
+        _ptr(verts), _ptr(faces), len(faces), _ptr(labels), _ptr(slot), _ptr(cdev), _ptr(Pdev), S,
+        _ptr(owner), _stream()), "texture_level_owners")
+    return owner
+
+
+def level_apply(owner, verts, faces, labels, slot, cdev, Pdev, corner, g, atlas):
+    """Levelling step 7, in place on atlas (pages,S,S,3) uint8."""
+    _lib.check(_lib.load().casmvs_texture_level_apply(
+        _ptr(owner), owner.numel(), _ptr(verts), _ptr(faces), _ptr(labels), _ptr(slot), _ptr(cdev),
+        _ptr(Pdev), atlas.shape[1], _ptr(corner), _ptr(g), _ptr(atlas), _stream()),
+        "texture_level_apply")
+
+
+def seam_rms(fpair, g=None, pair_keys=None):
+    """RMS over seam pairs and channels of f_a - f_b, or with g of f_a + g_a - f_b - g_b."""
+    if not len(fpair):
+        return 0.0
+    d = fpair[:, :3] - fpair[:, 3:]
+    if g is not None:
+        d = d + g[pair_keys >> 32] - g[pair_keys & 0xFFFFFFFF]
+    return float(torch.sqrt((d * d).mean()))
+
+
+def level_seams(verts, faces, labels, slot, cdev, Pdev, img_ptrs, img_wh, nbr, atlas, mark=None,
+                log=print):
+    """Steps 1-7 of the seam levelling on texture_mesh's state, atlas changed in place -> the
+    stats of texture_mesh's stats["level"].  `mark(phase)` after seams, assembly, solve, apply."""
+    mark = mark or (lambda phase: None)
+    unk, corner = level_unknowns(faces, labels, slot)
+    rec_key, rec_sub, smooth_keys = level_edges(nbr, faces, labels, slot, corner)
+    pair_keys, fpair = level_seam_colours(verts, faces, labels, slot, nbr, rec_key, rec_sub,
+                                          img_ptrs, img_wh, Pdev)
+    n_records = len(rec_sub)
+    del rec_key, rec_sub
+    mark("seams")
+    rowptr, col, val, diag, rhs = level_system(pair_keys, smooth_keys, len(unk), fpair)
+    mark("assembly")
+    g, iters, ratios, converged = level_solve(rowptr, col, val, diag, rhs)
+    nnz = len(col)
+    del rowptr, col, val, diag, rhs
+    mark("solve")
+    if not converged:
+        log(f"texture level: conjugate gradients stopped after {iters} iterations with relative "
+            f"residuals {', '.join(f'{r:.3g}' for r in ratios)} above {CG_TOL:g}")
+    pages, S = atlas.shape[0], atlas.shape[1]
+    owner = level_owners(verts, faces, labels, slot, cdev, Pdev, S, pages)
+    level_apply(owner, verts, faces, labels, slot, cdev, Pdev, corner, g, atlas)
+    adjusted = int((owner != -1).sum())
+    mark("apply")
+    return dict(unknowns=len(unk), seam_pairs=len(pair_keys), seam_records=n_records,
+                smoothing_edges=len(smooth_keys), nnz=nnz, texels_adjusted=adjusted,
+                cg_iterations=iters, cg_ratios=ratios, converged=converged,
+                seam_rms_before=seam_rms(fpair), seam_rms_after=seam_rms(fpair, g, pair_keys))
+
+
 def texture_mesh(verts, colours, faces, images, Ps, rounds=SMOOTH_ROUNDS, max_bytes=None,
-                 mark=None):
+                 mark=None, level=False, log=print):
     """Texture a mesh (verts (N,3) float32, colours (N,3) uint8, faces (M,3) int32 or int64, CUDA
     tensors) from views (images: (H,W,3) uint8 CUDA tensors; Ps: 4x4 world -> pixel matrices of
     those images) -> (uv (M,3,2) float32 per corner, page (M,) int32, atlas (pages,S,S,3) uint8,
@@ -254,7 +451,10 @@ def texture_mesh(verts, colours, faces, images, Ps, rounds=SMOOTH_ROUNDS, max_by
     views every face is flat.  Bad input raises ValueError before the GPU is used; work that
     would not fit in mesh.device_budget raises CasMVSError naming the bytes.  `mark(phase)`, when
     given, is called after each phase: keys and scores (once per batch of views), smooth, charts,
-    pack, fill."""
+    pack, fill, and with `level` seams, assembly, solve, apply.  `level` levels the seams after
+    the fill (the module docstring's second rule) and adds stats["level"]: unknowns, seam_pairs,
+    seam_records, smoothing_edges, nnz, texels_adjusted, cg_iterations, cg_ratios, converged,
+    seam_rms_before, seam_rms_after; an unconverged solve is reported through `log`."""
     images, Ps = _check_inputs(verts, colours, faces, images, Ps)
     if not (isinstance(rounds, int) and rounds >= 0):
         raise ValueError(f"rounds must be an integer >= 0, got {rounds!r}")
@@ -264,7 +464,7 @@ def texture_mesh(verts, colours, faces, images, Ps, rounds=SMOOTH_ROUNDS, max_by
     lib = _lib.load()
     with torch.cuda.device(dev):
         budget = mesh.device_budget(dev, max_bytes)
-        need = _bytes_needed(F, wh)
+        need = _bytes_needed(F, wh) + (F * LEVEL_BYTES_PER_FACE if level else 0)
         if need > budget:
             raise _lib.CasMVSError(
                 f"texturing {F} faces from {len(images)} views needs {need} bytes of device memory "
@@ -286,7 +486,7 @@ def texture_mesh(verts, colours, faces, images, Ps, rounds=SMOOTH_ROUNDS, max_by
         S = page_side(w, h)
         charts[:, 6], charts[:, 7], charts[:, 8], n_pages = pack(charts[:, 0], w, h, S)
         mark("pack")
-        page_bytes = n_pages * S * S * 3
+        page_bytes = n_pages * S * S * (3 + (8 if level else 0))
         budget = mesh.device_budget(dev, max_bytes if max_bytes is None else max_bytes - need)
         if page_bytes > budget:
             raise _lib.CasMVSError(
@@ -306,6 +506,9 @@ def texture_mesh(verts, colours, faces, images, Ps, rounds=SMOOTH_ROUNDS, max_by
                                           _ptr(cdev), _ptr(Pdev), S, _ptr(uv), _ptr(page), _stream()),
                    "texture_uvs")
         mark("fill")
+        if level:
+            level_stats = level_seams(verts, faces, labels, slot, cdev, Pdev, img_ptrs, img_wh, nbr,
+                                      atlas, mark, log)
         n_cand = (view >= 0).sum(1)
         stats = dict(views=len(images), faces=F,
                      candidates_per_face=float(n_cand.float().mean()) if F else 0.0,
@@ -316,6 +519,8 @@ def texture_mesh(verts, colours, faces, images, Ps, rounds=SMOOTH_ROUNDS, max_by
                      packed_share=float((w.astype(np.int64) * h).sum() / (n_pages * S * S))
                      if n_pages else 0.0,
                      hook_rounds=hook_rounds)
+        if level:
+            stats["level"] = level_stats
     return uv, page, atlas, stats
 
 
@@ -470,6 +675,8 @@ def parse_args(argv=None):
     ap.add_argument("--view_names", default=None,
                     help="view_names.txt pairing view ids with image names (default: sorted order)")
     ap.add_argument("--out", required=True, help="the OBJ to write (its .mtl and _<k>.png beside it)")
+    ap.add_argument("--level", action="store_true",
+                    help="level the colour seams between charts (global colour adjustment)")
     a = ap.parse_args(argv)
     if not a.out.endswith(".obj"):
         ap.error("--out must end in .obj")
@@ -489,11 +696,17 @@ def main(argv=None):
         images.append(torch.from_numpy(np.asarray(Image.open(p).convert("RGB")).copy()).to(dev))
     uv, page, atlas, st = texture_mesh(torch.from_numpy(np.ascontiguousarray(v)).to(dev),
                                        torch.from_numpy(np.ascontiguousarray(c)).to(dev),
-                                       torch.from_numpy(np.ascontiguousarray(f)).to(dev), images, Ps)
+                                       torch.from_numpy(np.ascontiguousarray(f)).to(dev), images, Ps,
+                                       level=a.level)
     write_textured_obj(a.out, v, f, uv, page, atlas)
     print(f"{a.ply}: {st['faces']} faces from {st['views']} views, {st['unseen_faces']} unseen, "
           f"{st['charts']} charts on {st['pages']} pages of {st['page_side']} "
           f"({st['packed_share']:.1%} packed); wrote {a.out}")
+    if a.level:
+        lv = st["level"]
+        print(f"levelled {lv['seam_pairs']} seam pairs over {lv['unknowns']} unknowns in "
+              f"{lv['cg_iterations']} CG iterations: seam RMS {lv['seam_rms_before']:.3f} -> "
+              f"{lv['seam_rms_after']:.3f}")
 
 
 if __name__ == "__main__":

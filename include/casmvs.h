@@ -955,6 +955,95 @@ int casmvs_texture_uvs(const float* verts, const int* faces, int F, const int* l
                        const int* slot, const int* charts, const float* Ps, int S, float* uv,
                        int* page, void* stream);
 
+/* ---- seam levelling of a textured mesh (csrc/texture_level.cu, casmvsnet_pl_b200/texture.py) --
+ * Waechter et al. 2014's global colour adjustment, run on texture_mesh's labels, slot, charts,
+ * nbr and atlas.  Constants: SEAM_SAMPLES = 8, SMOOTH_WEIGHT = 10, EPS = 1e-4, REACH = 1.5 texels.
+ * Every double operation below is rounded as written (no contraction), left to right.
+ * casmvs_texture_level_keys: keys (3F) int64 = (slot[f] << 32) | faces[f][k] for a face of label
+ *   >= 0, else -1.  The unknowns are the distinct keys >= 0 in ascending order (one RGB offset g
+ *   per (chart, vertex) pair), n of them, sorted by the caller.
+ * casmvs_texture_level_corners: corner (3F) int32 = the index of keys[i] among the n unknowns
+ *   (-1 for a flat face).
+ * casmvs_texture_level_edges: per corner c = 3f + k, the edge faces[f][k] -- faces[f][(k+1)%3]:
+ *   smooth_key[c] = (min << 32) | max of its two corners' unknowns when label[f] >= 0 and they
+ *   differ, else -1 (the caller keeps the distinct keys: the smoothing edges);
+ *   rec_key[2c + e] (e = 0 for the corner-k endpoint, 1 for the other) = (a << 32) | b, a < b the
+ *   endpoint's unknowns in the two charts, when the edge is a seam seen from its lower face:
+ *   g = nbr[f][k] >= 0, f < g, label[f] >= 0, label[g] >= 0, slot[f] != slot[g]; else -1.  A seam
+ *   pair is a distinct such key; the caller keeps the records rec_sub = 2c + e with a key,
+ *   stably sorted by key.
+ * casmvs_texture_level_samples: rec (R,6) f64 per record: for s = 0..7, t = s / 8, the point
+ *   X = x0 + t (x1 - x0) per coordinate in double (x0 the record's endpoint, x1 the edge's other
+ *   end, f32 vertices), projected by Ps[view] as u = (((P0 X + P1 Y) + P2 Z) + P3) / w (w and v
+ *   likewise, P widened to double), clamped to [0, W-1] x [0, H-1]; a = u - floor(u), the taps
+ *   (floor, floor + 1 clamped to W-1) of images[view] (pixel centres at integer coordinates)
+ *   c = (1 - ay) ((1 - ax) c00 + ax c10) + ay ((1 - ax) c01 + ax c11); acc += (1 - t) c.
+ *   Columns 0..2 in the view of the lower chart (the chart of unknown a), 3..5 in the upper's.
+ * casmvs_texture_level_pairs: fpair (P,6) f64: per pair, num = sum of its records' rec and
+ *   den = sum of W = sum_s (1 - s / 8), both from 0 in record order; f = num / den, f_a in
+ *   columns 0..2, f_b in 3..5.
+ * casmvs_texture_level_system: ekey (nnz) int64 ascending = (row << 32) | col of every entry:
+ *   both orders of each seam pair and smoothing edge, and (a, a) per unknown; etype (nnz) int32
+ *   = the seam pair's index, -2 for a smoothing edge, -1 for the diagonal.  Writes rowptr (n+1),
+ *   col (nnz) int32 and val (nnz), diag (n), rhs (n,3) f64, one thread per row in column order:
+ *   off-diagonal -1 (seam) or -10 (smoothing), s = their sum from 0, diagonal -s + EPS;
+ *   rhs[a] += f_b - f_a over the row's seam pairs with a the row's unknown (f_a - f_b when it is
+ *   b), from 0.  This is A g = rhs for the minimum of sum_pairs (f_a + g_a - f_b - g_b)^2
+ *   + SMOOTH_WEIGHT sum_edges (g_a - g_b)^2 + EPS sum g^2.
+ * casmvs_texture_level_cg: Jacobi-preconditioned CG from x = 0 on the three columns of rhs at
+ *   once (x (n,3) f64), until every column has ||r|| / ||b|| <= tol (0 when b = 0) or after
+ *   max_iters iterations.  Dot products are per-thread sums in grid-stride order, a fixed
+ *   256-wide tree per block and one block over the block partials, over min(1024, ceil(n/256))
+ *   blocks.  alpha = rz / pq (0 unless pq > 0), beta = rz' / rz (0 unless rz > 0).  The host
+ *   reads the done flag every check_every iterations; iterations after convergence are no-ops,
+ *   so *iters does not depend on check_every.  HOST outputs: *iters, ratios[3], *converged.
+ *   workspace: casmvs_texture_level_cg_workspace_bytes(n).
+ * casmvs_texture_level_owners: owner (pages,S,S) u64, all ~0 from the caller.  One warp per face
+ *   of label L >= 0: its corners projected by Ps[L] (the UVs' f32 projection) widened to double;
+ *   for every integer view pixel p = (x, y) of its chart's rectangle within REACH of the
+ *   triangle's bounding box, the nearest point of the triangle: inside (area = (u1-u0)(v2-v0) -
+ *   (v1-v0)(u2-u0) != 0 and l_k = ((u_{k+1}-x)(v_{k+2}-y) - (v_{k+1}-y)(u_{k+2}-x)) / area >= 0
+ *   for all k) -> distance 0, barycentrics l; else the edge k -> k+1 of least squared distance
+ *   (ties to the lower k), t = clamp(((x-u_k) du + (y-v_k) dv) / (du du + dv dv), 0, 1) (0 for a
+ *   zero-length edge), e = p - (P_k + t d), d2 = ex ex + ey ey, distance sqrt(d2), barycentrics
+ *   1 - t at k and t at k+1.  When distance <= REACH, atomicMin(owner[page][oy + y - y0][ox + x -
+ *   x0], (f32(distance) bits << 32) | f).
+ * casmvs_texture_level_apply: per atlas texel (64-bit index over n_texels = pages S S) with an
+ *   owner f: the nearest point's barycentrics l of its view pixel as above, offset
+ *   o = ((l0 g[c0] + l1 g[c1]) + l2 g[c2]) per channel (c_k = corner[3f + k], g (n,3) f64), and
+ *   the byte becomes min(max(rint(byte + o), 0), 255) (rint: half to even).  Texels without an
+ *   owner, flat charts and unused texels are untouched. */
+int casmvs_texture_level_keys(const int* faces, int F, const int* label, const int* slot,
+                              long long* keys, void* stream);
+int casmvs_texture_level_corners(const long long* keys, int F, const long long* unknowns, int n,
+                                 int* corner, void* stream);
+int casmvs_texture_level_edges(const int* nbr, const int* faces, int F, const int* label,
+                               const int* slot, const int* corner, long long* rec_key,
+                               long long* smooth_key, void* stream);
+int casmvs_texture_level_samples(const float* verts, const int* faces, const int* label,
+                                 const int* slot, const int* nbr, const long long* rec_sub, int R,
+                                 const float* Ps, const unsigned long long* images, const int* wh,
+                                 double* rec, void* stream);
+int casmvs_texture_level_pairs(const double* rec, const long long* seg, int P, double* fpair,
+                               void* stream);
+int casmvs_texture_level_system(const long long* ekey, const int* etype, long long nnz, int n,
+                                const double* fpair, int* rowptr, int* col, double* val,
+                                double* diag, double* rhs, void* stream);
+size_t casmvs_texture_level_cg_workspace_bytes(int n);
+int casmvs_texture_level_cg(const int* rowptr, const int* col, const double* val,
+                            const double* diag, const double* rhs, int n, double* x,
+                            void* workspace, size_t workspace_bytes, int max_iters, double tol,
+                            int check_every, int* iters, double* ratios, int* converged,
+                            void* stream);
+int casmvs_texture_level_owners(const float* verts, const int* faces, int F, const int* label,
+                                const int* slot, const int* charts, const float* Ps, int S,
+                                unsigned long long* owner, void* stream);
+int casmvs_texture_level_apply(const unsigned long long* owner, long long n_texels,
+                               const float* verts, const int* faces, const int* label,
+                               const int* slot, const int* charts, const float* Ps, int S,
+                               const int* corner, const double* g, unsigned char* atlas,
+                               void* stream);
+
 /* ---- training panels (csrc/visual.cu; utils/visualization.py, train.py:107-114) ---------
  * The original's TensorBoard image strip as uint8 (H, n*W, 3), n = the number of non-NULL panel
  * inputs, panels left to right in the order img, depth_gt, depth_pred, conf:
