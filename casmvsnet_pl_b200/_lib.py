@@ -195,7 +195,15 @@ SIGNATURES = {
                                          c_void_p]),
     "casmvs_mesh_sample_points": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_longlong,
                                           c_void_p, c_void_p]),
-    "casmvs_render_points_fwd": (c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
+    "casmvs_mesh_clean_face_area": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_mesh_clean_sums": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "casmvs_mesh_clean_boundary": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int]
+                                   + [c_void_p] * 5),
+    "casmvs_mesh_clean_loop_sizes": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                             c_void_p]),
+    "casmvs_mesh_clean_fill": (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_int]
+                               + [c_void_p] * 5),
+    "casmvs_render_points_fwd":(c_int, [c_void_p, c_void_p, c_longlong, POINTER(c_float), c_int,
                                          c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "casmvs_render_mesh_workspace_bytes": (c_size_t, [c_int]),
     "casmvs_render_mesh_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, POINTER(c_float),

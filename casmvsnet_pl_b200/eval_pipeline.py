@@ -41,6 +41,9 @@ proba_XXXX.pfm are written as well).
 marching-cubes mesh to <out>/mesh/<scan>.ply (mesh.py); nothing else it writes changes.
 --mesh --mesh_method poisson [--poisson_depth 9] meshes the scan's fused points by Poisson surface
 reconstruction instead (poisson.py); --poisson_point_weight A > 0 screens it.
+--mesh --mesh_clean drops either mesh's small disconnected pieces (--mesh_clean_ratio R of the
+largest piece's faces, default 0.01) and fills its holes of at most --mesh_max_hole E edges
+(default 0: none) on the GPU before anything else sees it (mesh_clean.py).
 --mesh --mesh_faces N decimates either mesh to at most N faces on the GPU before it is written
 (simplify.py).
 --mesh --mesh_texture also textures the mesh that is written from the scan's reference-view images
@@ -449,6 +452,16 @@ def _simplify(name, verts, colours, faces, mesh_faces, log):
     return verts, colours, faces
 
 
+def _clean(name, verts, colours, faces, mesh_clean, log):
+    """The mesh cleaned by mesh_clean.clean_mesh(**mesh_clean) (unchanged when it is None)."""
+    if mesh_clean is None:
+        return verts, colours, faces
+    from . import mesh_clean as mc
+    verts, colours, faces, st = mc.clean_mesh(verts, colours, faces, **mesh_clean)
+    log(f"{name}: cleaned the mesh: {mc.summary(st)}")
+    return verts, colours, faces
+
+
 def _score_mesh(scan, mesh_path, verts, faces, dtu_gt, dtu_seed, tnt_gt, tnt_images, tnt_tau,
                 tnt_seed, run_dir):
     """Scores of the written mesh against the Tanks and Temples (tnt_gt) or DTU (dtu_gt) ground
@@ -491,7 +504,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
              mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
-             mesh_texture=False, mesh_score=False, mesh_texture_level=False):
+             mesh_texture=False, mesh_score=False, mesh_texture_level=False, mesh_clean=None):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -505,7 +518,9 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     mesh is instead the Poisson surface (poisson.py, grid depth `poisson_depth`, default 9) of
     every fused point (not thinned by `skip`), coloured by the refined image at its pixel, its
     normals oriented toward the reference cameras, screened with point weight
-    `poisson_point_weight` when it is > 0.  With `mesh_faces`, either mesh is decimated to at most
+    `poisson_point_weight` when it is > 0.  With `mesh_clean` (a dict of mesh_clean.clean_mesh's
+    options, possibly empty), either mesh is first cleaned (mesh_clean.py), so that everything
+    below sees the cleaned mesh.  With `mesh_faces`, either mesh is decimated to at most
     that many faces (simplify.py) before it is written.  With `mesh_texture`, the written mesh is
     also textured from the reference views' images and proj0 (texture.py) and written beside it
     as an OBJ with its MTL and atlas PNGs; `mesh_texture_level` also levels its colour seams.
@@ -554,6 +569,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
             depth=poisson.DEFAULT_DEPTH if poisson_depth is None else poisson_depth, log=log,
             point_weight=poisson_point_weight)
         del pts, cols
+        verts, colours, faces = _clean(scan.scan, verts, colours, faces, mesh_clean, log)
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
@@ -572,6 +588,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
                                                     [f["image"] for f in fused],
                                                     [f["P"] for f in fused], mesh_voxel)
         del fused
+        verts, colours, faces = _clean(scan.scan, verts, colours, faces, mesh_clean, log)
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
@@ -688,6 +705,16 @@ def parse_args(argv=None):
     ap.add_argument("--poisson_point_weight", type=float, default=None,
                     help="with --mesh_method poisson: the screening weight alpha >= 0 that pulls "
                          "the surface through the points (default 0, unscreened)")
+    ap.add_argument("--mesh_clean", action="store_true",
+                    help="with --mesh: drop the mesh's small disconnected pieces (and, with "
+                         "--mesh_max_hole, fill its small holes) on the GPU before it is "
+                         "simplified, textured, scored or written")
+    ap.add_argument("--mesh_clean_ratio", type=float, default=None,
+                    help="with --mesh_clean: drop pieces of fewer faces than this fraction of the "
+                         "largest piece's, in [0, 1] (default 0.01)")
+    ap.add_argument("--mesh_max_hole", type=int, default=None,
+                    help="with --mesh_clean: fill holes of at most this many boundary edges, 0 "
+                         "(none, the default) or 3..128")
     ap.add_argument("--mesh_faces", type=int, default=None,
                     help="with --mesh: simplify the mesh to at most this many faces (>= 1) by "
                          "quadric edge-collapse decimation before it is written")
@@ -710,6 +737,17 @@ def parse_args(argv=None):
         ap.error("--mesh_texture needs --mesh")
     if a.mesh_texture_level and not a.mesh_texture:
         ap.error("--mesh_texture_level needs --mesh_texture")
+    if a.mesh_clean and not a.mesh:
+        ap.error("--mesh_clean needs --mesh")
+    if a.mesh_clean_ratio is not None and not a.mesh_clean:
+        ap.error("--mesh_clean_ratio needs --mesh_clean")
+    if a.mesh_max_hole is not None and not a.mesh_clean:
+        ap.error("--mesh_max_hole needs --mesh_clean")
+    if a.mesh_clean_ratio is not None and not (math.isfinite(a.mesh_clean_ratio)
+                                               and 0 <= a.mesh_clean_ratio <= 1):
+        ap.error("--mesh_clean_ratio must be in [0, 1]")
+    if a.mesh_max_hole is not None and not (a.mesh_max_hole == 0 or 3 <= a.mesh_max_hole <= 128):
+        ap.error("--mesh_max_hole must be 0 or in 3..128")
     if a.mesh_faces is not None and not a.mesh:
         ap.error("--mesh_faces needs --mesh")
     if a.mesh_faces is not None and a.mesh_faces < 1:
@@ -734,6 +772,15 @@ def parse_args(argv=None):
         a.depth_interval = DEFAULT_DEPTH_INTERVAL[a.dataset_name]
     a.out_dir = a.out or os.path.join("results", a.dataset_name)
     return a
+
+
+def _clean_options(a):
+    """clean_mesh's options from --mesh_clean_ratio / --mesh_max_hole, or None without
+    --mesh_clean."""
+    if not a.mesh_clean:
+        return None
+    opts = dict(min_ratio=a.mesh_clean_ratio, max_hole=a.mesh_max_hole)
+    return {k: v for k, v in opts.items() if v is not None}
 
 
 def main(argv=None):
@@ -774,7 +821,8 @@ def main(argv=None):
                        poisson_depth=a.poisson_depth,
                        poisson_point_weight=a.poisson_point_weight or 0.0,
                        mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture,
-                       mesh_score=a.mesh_score, mesh_texture_level=a.mesh_texture_level, **tnt)
+                       mesh_score=a.mesh_score, mesh_texture_level=a.mesh_texture_level,
+                       mesh_clean=_clean_options(a), **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

@@ -845,6 +845,47 @@ int casmvs_mesh_sample_count(const float* verts, const int* faces, int F, double
 int casmvs_mesh_sample_points(const float* verts, const int* faces, int F, const int* n,
                               const long long* start, long long S, float* out, void* stream);
 
+/* ---- mesh cleaning (csrc/mesh_clean.cu, casmvsnet_pl_b200/mesh_clean.py) ----------------------
+ * Drops small pieces and fills small holes.  A mesh, its edges and corners are as for
+ * casmvs_simplify_* above; the faces here have passed casmvs_simplify_clean.  Every double
+ * operation is rounded to nearest in the order written, with no contraction; the only atomics are
+ * integer ones, so results are bitwise reproducible.
+ * casmvs_mesh_clean_face_area: area (F) f64 = 0.5 sqrt(n.n), n = (p1 - p0) x (p2 - p0),
+ *   n.n = (nx nx + ny ny) + nz nz.
+ * casmvs_mesh_clean_sums: out[p] = 0 + value[order[start[p]]] + ... + value[order[start[p+1]-1]]
+ *   summed left to right (order int64, or NULL for the identity).  A piece's area is the sum of
+ *   its chunk sums, a chunk being up to 1024 of its faces in face order.
+ * casmvs_mesh_clean_boundary: a boundary half-edge is corner c's directed edge a -> b with
+ *   edge_count = 1.  out_deg / in_deg (V) int32 count them at a and b; next (V) int32 = b and
+ *   next_face (V) int32 = c / 3 where a has out_deg = in_deg = 1, else -1 (all set here).
+ * casmvs_mesh_clean_loop_sizes: with comp (V) the least vertex of each component of the graph
+ *   v -- next[v] over the vertices with next >= 0 (casmvs_texture_charts): size (V) int32 counts
+ *   the vertices with next >= 0 per root, open (V) u8 = 1 at a root whose component holds a v with
+ *   next[next[v]] < 0 (a path, not a loop); both zeroed here.
+ * casmvs_mesh_clean_fill: one loop per owner[L] (its least vertex) of size[L] = n in 3..max_size
+ *   <= 128 edges; position i is next^i(owner).  cost(i, i+1) = 0; for j - i >= 2,
+ *   cost(i, j) = min over i < k < j of (cost(i, k) + cost(k, j)) + 0.5 sqrt(m.m),
+ *   m = (p_k - p_i) x (p_j - p_i), least k on ties, skipping k with m = 0, and +inf when (i, j) is
+ *   not 0 -- n-1 and the edge vid_i -- vid_j is in edge_keys (E sorted int64, binary search) or
+ *   when no k is admissible.  area[L] f64 = cost(0, n-1); status[L] u8 = 2 when it is +inf, else
+ *   1 when area <= 0.1 x piece_area[next_face[owner]] (piece_area per face), else 3.
+ *   tris (sum (n - 2), 3) int32 from row tri_off[L] (int64): pre-order from (0, n-1), (i, j)
+ *   emitting (vid_j, vid_k, vid_i) with its split k, then (i, k), then (k, j); -1 when status 2. */
+int casmvs_mesh_clean_face_area(const float* verts, const int* faces, int F, double* area,
+                                void* stream);
+int casmvs_mesh_clean_sums(const double* value, const long long* order, const long long* start,
+                           int n, double* out, void* stream);
+int casmvs_mesh_clean_boundary(const int* faces, int F, const int* corner_edge,
+                               const int* edge_count, int V, int* out_deg, int* in_deg, int* next,
+                               int* next_face, void* stream);
+int casmvs_mesh_clean_loop_sizes(const int* next, const int* comp, int V, int* size,
+                                 unsigned char* open, void* stream);
+int casmvs_mesh_clean_fill(const float* verts, const int* next, const int* next_face,
+                           const int* owner, const int* size, int n_loops, int max_size,
+                           const long long* tri_off, const long long* edge_keys, int E,
+                           const double* piece_area, unsigned char* status, double* area, int* tris,
+                           void* stream);
+
 /* ---- headless rendering of clouds and meshes (casmvsnet_pl_b200/render.py) -----------------
  * P is a HOST array of 16 floats, row-major, world -> pixel (rows 0..2 used): every float
  * operation below is rounded to nearest, no contraction, in the order written.
