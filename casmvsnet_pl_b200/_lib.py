@@ -103,6 +103,10 @@ SIGNATURES = {
                                     POINTER(c_float), POINTER(c_float), c_void_p, c_int, c_int,
                                     c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_geo_fuse_dynamic_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            POINTER(c_float), POINTER(c_float), c_void_p, c_int,
+                                            c_int, c_int, c_float, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "casmvs_pcd_cell_keys": (c_int, [c_void_p, c_int, c_double, c_double, c_double, c_double,
                                      c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "casmvs_pcd_thin_workspace_bytes": (c_size_t, [c_int, c_int]),

@@ -6,14 +6,39 @@
 //   mask / average / back-projection of one ref view    eval.py:262-318
 // One thread per reference pixel walks the source views: project with the reference depth,
 // sample the source depth map and image bilinearly (cv2.remap semantics, see remap_tap), lift
-// back, test the reprojection (|dp| < 1 px, |dd|/d < 1 %), accumulate.  HBM-bound: per ref
-// pixel it reads 4 B + S x (4 taps x 16 B) and writes 4 + 12 + 4 (+ 12 + 1) bytes; the depth
+// back, measure e_pix = dx^2 + dy^2 and e_dep = |(rz - d) / d|, accumulate.  Two rules decide
+// from those errors, one template instantiation each (FuseRule):
+//   reference  a source is consistent when e_pix < 1 and e_dep < 0.01f; the pixel passes when
+//              at least min_consistent sources are (eval.py:143-147,300).
+//   dynamic    dynamic consistency checking (D2HC-RMVSNet, Yan et al., ECCV 2020, in its
+//              count-based form).  Source s is consistent at level k (k = 2..10) when
+//              e_pix < (k/4)^2 and e_dep < T_k = float32(k / 1300) (rounded once from double);
+//              k_s is its least such level, 0 when there is none (NaN compares false).  With
+//              n_k = #{s : 0 < k_s <= k}, the pixel passes when n_k >= k for some
+//              2 <= k <= min(10, S); with S < 2 it never does.  The average and geo_count use
+//              the sources with k_s > 0 (consistent at level 10).
+// Both then AND the confidence test.  HBM-bound, the same bytes for both rules: per ref pixel
+// it reads 4 B + S x (4 taps x 16 B) and writes 4 + 12 + 4 (+ 12 + 1) bytes; the depth
 // maps of a scan stay resident, so the PFM round trip of eval.py:228-229,269-272 disappears.
 #include "common.cuh"
 
 namespace casmvs {
 
 constexpr int kMaxFuseSrc = 16;
+
+// The dynamic rule's constants (fusion.py states them again; a test keeps the two in step):
+// levels k = kDynLevelMin..kDynLevelMax, pixel threshold k / kDynPixDiv px, relative depth
+// threshold k / kDynDepDiv.
+constexpr int kDynLevelMin = 2;
+constexpr int kDynLevelMax = 10;
+constexpr int kDynPixDiv = 4;
+constexpr int kDynDepDiv = 1300;
+// geo_fuse_kernel<kDynamic> counts the sources per level in 5-bit fields of one 64-bit word
+constexpr int kDynCountBits = 5;
+static_assert(kMaxFuseSrc < (1 << kDynCountBits), "a level count must fit its field");
+static_assert((kDynLevelMax - kDynLevelMin + 1) * kDynCountBits <= 64, "level counts overflow");
+
+enum class FuseRule { kReference, kDynamic };
 
 struct FuseParams {
   float rs[kMaxFuseSrc][12];   // (P_world2src @ inv(P_world2ref))[:3]   eval.py:120
@@ -74,6 +99,21 @@ __device__ __forceinline__ float upsample4_linear(const float* __restrict__ p, i
   return __fadd_rn(__fmul_rn(r0, 1.f - fy), __fmul_rn(r1, fy));
 }
 
+// Least level k at which a source with errors (e_pix, e_dep) is consistent, 0 for none.
+// (k / kDynPixDiv)^2 = k^2 / 16 is exact in fp32, so the squared pixel error is compared.
+__device__ __forceinline__ int dynamic_level(float e_pix, float e_dep) {
+#pragma unroll
+  for (int k = kDynLevelMin; k <= kDynLevelMax; ++k) {
+    const float pix_th = (float)(k * k) / (float)(kDynPixDiv * kDynPixDiv);
+    const float dep_th = (float)((double)k / (double)kDynDepDiv);
+    if (e_pix < pix_th && e_dep < dep_th) return k;
+  }
+  return 0;
+}
+
+// R = kReference: flag_dbg holds the per-source mask (0 / 1) and min_consistent applies.
+// R = kDynamic:   flag_dbg holds k_s and min_consistent is unused.
+template <FuseRule R>
 __global__ void __launch_bounds__(256)
 geo_fuse_kernel(const __grid_constant__ FuseParams P, int S, const float* __restrict__ depth_ref,
                 const float* __restrict__ image_ref, const float* __restrict__ proba_ref,
@@ -81,7 +121,7 @@ geo_fuse_kernel(const __grid_constant__ FuseParams P, int S, const float* __rest
                 float* __restrict__ depth_refined, float* __restrict__ image_refined,
                 int* __restrict__ geo_count, unsigned char* __restrict__ mask_final,
                 float* __restrict__ points, float* __restrict__ reproj_dbg,
-                unsigned char* __restrict__ mask_dbg, int H, int W) {
+                unsigned char* __restrict__ flag_dbg, int H, int W) {
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
   if (pix >= H * W) return;
   const int y = pix / W, x = pix - y * W;
@@ -94,6 +134,7 @@ geo_fuse_kernel(const __grid_constant__ FuseParams P, int S, const float* __rest
     for (int c = 0; c < 3; ++c) csum[c] = __ldg(image_ref + (size_t)pix * 3 + c);
   }
   int cnt = 0;
+  unsigned long long level_count = 0;   // kDynamic: sources per level, kDynCountBits each
   for (int s = 0; s < S; ++s) {
     const float* A = P.rs[s];
     // xyz_ref = (x, y, 1) * depth_ref; homogeneous 1      eval.py:117-118
@@ -116,16 +157,26 @@ geo_fuse_kernel(const __grid_constant__ FuseParams P, int S, const float* __rest
     const float ry = Bm[4] * U + Bm[5] * Vv + Bm[6] * ds + Bm[7];
     const float rz = Bm[8] * U + Bm[9] * Vv + Bm[10] * ds + Bm[11];
     const float dx = rx / rz - xf, dy = ry / rz - yf;
-    const bool m_pix = dx * dx + dy * dy < 1.f;                         // eval.py:143-144
-    const bool m_dep = fabsf((rz - d) / d) < 0.01f;                     // eval.py:147
-    const bool m = m_pix && m_dep;                                       // NaN compares false
+    bool m;                                            // the source joins the average
+    unsigned char flag;
+    if constexpr (R == FuseRule::kReference) {
+      const bool m_pix = dx * dx + dy * dy < 1.f;                       // eval.py:143-144
+      const bool m_dep = fabsf((rz - d) / d) < 0.01f;                   // eval.py:147
+      m = m_pix && m_dep;                                               // NaN compares false
+      flag = m ? 1 : 0;
+    } else {
+      const int level = dynamic_level(dx * dx + dy * dy, fabsf((rz - d) / d));
+      m = level > 0;
+      if (m) level_count += 1ull << (kDynCountBits * (level - kDynLevelMin));
+      flag = (unsigned char)level;
+    }
     if (m) {
       dsum += rz;                                      // depth_ref_reproj[~mask_geo] = 0
       csum[0] += col[0]; csum[1] += col[1]; csum[2] += col[2];
       ++cnt;
     }
     if (reproj_dbg) reproj_dbg[(size_t)s * H * W + pix] = m ? rz : 0.f;
-    if (mask_dbg) mask_dbg[(size_t)s * H * W + pix] = m ? 1 : 0;
+    if (flag_dbg) flag_dbg[(size_t)s * H * W + pix] = flag;
   }
   const float inv = 1.f / (float)(cnt + 1);
   const float dref = dsum / (float)(cnt + 1);                            // eval.py:301-302
@@ -135,7 +186,18 @@ geo_fuse_kernel(const __grid_constant__ FuseParams P, int S, const float* __rest
     for (int c = 0; c < 3; ++c) image_refined[(size_t)pix * 3 + c] = csum[c] * inv;
   }
   geo_count[pix] = cnt;
-  bool keep = cnt >= min_consistent;                                     // eval.py:300
+  bool keep;
+  if constexpr (R == FuseRule::kReference) {
+    keep = cnt >= min_consistent;                                        // eval.py:300
+  } else {
+    keep = false;
+    int n = 0;                                         // n_k = #{s : 0 < k_s <= k}
+#pragma unroll
+    for (int k = kDynLevelMin; k <= kDynLevelMax; ++k) {
+      n += (int)((level_count >> (kDynCountBits * (k - kDynLevelMin))) & ((1u << kDynCountBits) - 1));
+      keep = keep || (k <= S && n >= k);
+    }
+  }
   if (proba_ref) keep = keep && upsample4_linear(proba_ref, H / 4, W / 4, x, y) > conf_thresh;
   if (mask_final) mask_final[pix] = keep ? 1 : 0;
   if (points) {
@@ -153,14 +215,15 @@ geo_fuse_kernel(const __grid_constant__ FuseParams P, int S, const float* __rest
 
 using namespace casmvs;
 
-extern "C" int casmvs_geo_fuse_fwd(const float* depth_ref, const float* image_ref,
-                                   const float* proba_ref, const float* const* depth_src,
-                                   const float* const* image_src, const float* proj_ref2src,
-                                   const float* proj_src2ref, const float* ref2world, int S, int H,
-                                   int W, float conf_thresh, int min_consistent,
-                                   float* depth_refined, float* image_refined, int* geo_count,
-                                   unsigned char* mask_final, float* points, float* reproj_dbg,
-                                   unsigned char* mask_dbg, void* stream) {
+// Argument checks and launch shared by both entries.
+template <FuseRule R>
+static int geo_fuse_launch(const float* depth_ref, const float* image_ref, const float* proba_ref,
+                           const float* const* depth_src, const float* const* image_src,
+                           const float* proj_ref2src, const float* proj_src2ref,
+                           const float* ref2world, int S, int H, int W, float conf_thresh,
+                           int min_consistent, float* depth_refined, float* image_refined,
+                           int* geo_count, unsigned char* mask_final, float* points,
+                           float* reproj_dbg, unsigned char* flag_dbg, void* stream) {
   CASMVS_REQUIRE(depth_ref && depth_refined && geo_count, "geo_fuse: null pointer");
   CASMVS_REQUIRE(S >= 0 && S <= kMaxFuseSrc, "geo_fuse: at most %d source views", kMaxFuseSrc);
   CASMVS_REQUIRE(H > 0 && W > 0 && (size_t)H * W < (1u << 30), "geo_fuse: bad dims");
@@ -180,8 +243,38 @@ extern "C" int casmvs_geo_fuse_fwd(const float* depth_ref, const float* image_re
     CASMVS_REQUIRE(!image_ref || !image_src || image_src[s], "geo_fuse: null source image %d", s);
   }
   const int n = H * W;
-  geo_fuse_kernel<<<(n + 255) / 256, 256, 0, as_stream(stream)>>>(
+  geo_fuse_kernel<R><<<(n + 255) / 256, 256, 0, as_stream(stream)>>>(
       P, S, depth_ref, image_ref, proba_ref, conf_thresh, min_consistent, ref2world, depth_refined,
-      image_refined, geo_count, mask_final, points, reproj_dbg, mask_dbg, H, W);
+      image_refined, geo_count, mask_final, points, reproj_dbg, flag_dbg, H, W);
   return after_launch("geo_fuse");
+}
+
+extern "C" int casmvs_geo_fuse_fwd(const float* depth_ref, const float* image_ref,
+                                   const float* proba_ref, const float* const* depth_src,
+                                   const float* const* image_src, const float* proj_ref2src,
+                                   const float* proj_src2ref, const float* ref2world, int S, int H,
+                                   int W, float conf_thresh, int min_consistent,
+                                   float* depth_refined, float* image_refined, int* geo_count,
+                                   unsigned char* mask_final, float* points, float* reproj_dbg,
+                                   unsigned char* mask_dbg, void* stream) {
+  return geo_fuse_launch<FuseRule::kReference>(
+      depth_ref, image_ref, proba_ref, depth_src, image_src, proj_ref2src, proj_src2ref,
+      ref2world, S, H, W, conf_thresh, min_consistent, depth_refined, image_refined, geo_count,
+      mask_final, points, reproj_dbg, mask_dbg, stream);
+}
+
+extern "C" int casmvs_geo_fuse_dynamic_fwd(const float* depth_ref, const float* image_ref,
+                                           const float* proba_ref, const float* const* depth_src,
+                                           const float* const* image_src,
+                                           const float* proj_ref2src, const float* proj_src2ref,
+                                           const float* ref2world, int S, int H, int W,
+                                           float conf_thresh, float* depth_refined,
+                                           float* image_refined, int* geo_count,
+                                           unsigned char* mask_final, float* points,
+                                           float* reproj_dbg, unsigned char* level_dbg,
+                                           void* stream) {
+  return geo_fuse_launch<FuseRule::kDynamic>(
+      depth_ref, image_ref, proba_ref, depth_src, image_src, proj_ref2src, proj_src2ref,
+      ref2world, S, H, W, conf_thresh, 0, depth_refined, image_refined, geo_count, mask_final,
+      points, reproj_dbg, level_dbg, stream);
 }

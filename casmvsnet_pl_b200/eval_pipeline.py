@@ -504,7 +504,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              dtu_gt=None, dtu_seed=0, save_visual=False, mesh_path=None, mesh_voxel=None, log=print,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
              mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
-             mesh_texture=False, mesh_score=False, mesh_texture_level=False, mesh_clean=None):
+             mesh_texture=False, mesh_score=False, mesh_texture_level=False, mesh_clean=None,
+             fusion_rule="reference"):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -528,6 +529,9 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
     is given, and (xyz, rgb, scores) is returned.
+    `fusion_rule` is fusion.fuse_scan's `rule`: "dynamic" fuses with the dynamic consistency
+    check (min_geo_consistent is then ignored) and logs the count of kept points; everything
+    downstream takes its cloud unchanged.
     With `mesh_score` (it needs `mesh_path` and `tnt_gt` or `dtu_gt`), the mesh as written is also
     scored through its surface samples by tnt_eval.evaluate_mesh or dtu_eval.evaluate_mesh, the
     scores are written beside it as <mesh>_tnt.json or <mesh>_scores.json, and appended to the
@@ -550,7 +554,9 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     proj0 = {v: scan.proj_mats[v][0].numpy() for v in scan.proj_mats}     # finest level (eval.py:108)
     fused = [] if mesh_path else None
     xyz, rgb = fusion.fuse_scan(scan.metas, depths, probas, images, proj0, conf, min_geo_consistent,
-                                skip, max_ref_views, collect=fused)
+                                skip, max_ref_views, collect=fused, rule=fusion_rule)
+    if fusion_rule != "reference":
+        log(f"{scan.scan}: {fusion_rule} fusion kept {len(xyz)} points")
     if ply_path:
         fusion.write_ply(ply_path, xyz, rgb)
     if mesh_path and mesh_method == "poisson":
@@ -677,6 +683,11 @@ def parse_args(argv=None):
                          "(default 192)")
     ap.add_argument("--conf", type=float, default=0.999)
     ap.add_argument("--min_geo_consistent", type=int, default=5)
+    ap.add_argument("--fusion", choices=list(fusion.RULES), default=argparse.SUPPRESS,
+                    help="the geometric consistency rule: reference (default; at least "
+                         "--min_geo_consistent sources within 1 px and 1 %% depth) or dynamic "
+                         "(for some k in 2..10, at least k sources within k/4 px and k/1300 "
+                         "relative depth)")
     ap.add_argument("--max_ref_views", type=int, default=400)
     ap.add_argument("--skip", type=int, default=1)
     ap.add_argument("--precision", default="tf32", choices=["fp32", "tf32"])
@@ -729,6 +740,11 @@ def parse_args(argv=None):
                          "through its surface samples into <out>/mesh/<scan>_scores.json "
                          "(DTU) or <scan>_tnt.json")
     a = ap.parse_args(argv)
+    if getattr(a, "fusion", "reference") == "dynamic":
+        ap.set_defaults(min_geo_consistent=None)                  # given explicitly?
+        if ap.parse_args(argv).min_geo_consistent is not None:
+            ap.error("--min_geo_consistent applies to --fusion reference only; the dynamic "
+                     "rule sets its own view counts")
     if a.mesh_score and not a.mesh:
         ap.error("--mesh_score needs --mesh")
     if a.mesh_score and a.dtu_gt is None and a.tnt_gt is None:
@@ -822,7 +838,8 @@ def main(argv=None):
                        poisson_point_weight=a.poisson_point_weight or 0.0,
                        mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture,
                        mesh_score=a.mesh_score, mesh_texture_level=a.mesh_texture_level,
-                       mesh_clean=_clean_options(a), **tnt)
+                       mesh_clean=_clean_options(a),
+                       fusion_rule=getattr(a, "fusion", "reference"), **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

@@ -460,6 +460,27 @@ int casmvs_geo_fuse_fwd(const float* depth_ref, const float* image_ref, const fl
                         int* geo_count, unsigned char* mask_final, float* points,
                         float* reproj_dbg, unsigned char* mask_dbg, void* stream);
 
+/* ---- dynamic consistency fusion ---------------------------------------------------------
+ * casmvs_geo_fuse_fwd with the count-based dynamic consistency check of D2HC-RMVSNet (Yan et
+ * al., ECCV 2020) in place of the fixed one: the same arguments without min_consistent, the
+ * same projection, sampling and back-projection, and per source the same fp32 errors
+ * e_pix = dx*dx + dy*dy and e_dep = |(rz - d) / d|.  Source s is consistent at level k
+ * (k = 2..10) when e_pix < (k/4)^2 and e_dep < T_k = float32(k / 1300), computed in double and
+ * rounded once; k_s is its least such level, 0 when there is none (NaN compares false).  With
+ * n_k = #{s : 0 < k_s <= k}, the geometric mask holds when n_k >= k for some 2 <= k <= min(10, S)
+ * (never when S < 2); mask_final is that AND the confidence test.  depth_refined, image_refined
+ * and geo_count average and count the sources with k_s > 0, in source order.  reproj_dbg holds rz
+ * for those sources, else 0; level_dbg (S,H,W) uint8 or NULL holds k_s.  Same checks as above:
+ * S <= 16, dims, null pointers, proba needs H, W % 4 == 0. */
+int casmvs_geo_fuse_dynamic_fwd(const float* depth_ref, const float* image_ref,
+                                const float* proba_ref, const float* const* depth_src,
+                                const float* const* image_src, const float* proj_ref2src,
+                                const float* proj_src2ref, const float* ref2world, int S, int H,
+                                int W, float conf_thresh, float* depth_refined,
+                                float* image_refined, int* geo_count, unsigned char* mask_final,
+                                float* points, float* reproj_dbg, unsigned char* level_dbg,
+                                void* stream);
+
 /* ---- DTU point-cloud scoring (reference evaluations/dtu, MATLAB)--------------------------
  * The two heavy steps of the DTU scorer on the device; the masks, statistics and the sort /
  * run-length scan that turn cell keys into cells are torch ops (casmvsnet_pl_b200/dtu_eval.py).
