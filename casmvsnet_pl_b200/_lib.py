@@ -121,6 +121,12 @@ SIGNATURES = {
                                            c_void_p, POINTER(c_double), c_double, POINTER(c_int),
                                            POINTER(c_double), POINTER(c_double), c_double,
                                            c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_pcd_knn_mean": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                    POINTER(c_double), c_double, POINTER(c_int), c_double,
+                                    c_void_p, c_void_p, c_void_p]),
+    "casmvs_pcd_sor_workspace_bytes": (c_size_t, [c_int]),
+    "casmvs_pcd_sor_keep": (c_int, [c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_size_t, c_void_p]),
     "casmvs_tnt_crop_blocks": (c_int, [c_int]),
     "casmvs_tnt_transform_crop": (c_int, [c_void_p, c_int, POINTER(c_double), c_int, c_double,
                                           c_double, c_void_p, c_int, c_void_p, c_void_p, c_void_p,

@@ -159,19 +159,45 @@ struct NNGrid {
   double cap, cap2;
 };
 
-// squared distance from q to the box [b, b + e]^3, boxes widened by 1e-6 mm so that a point
-// binned into a cell by a rounded floor() is never pruned with it
+// squared distance from q to the box [b, b + e]^3, boxes widened by `pad` (1e-6 mm for the DTU
+// searches) so that a point binned into a cell by a rounded floor() is never pruned with it
 __device__ __forceinline__ double box_d2(const double q[3], double bx, double by, double bz,
-                                         double e) {
-  const double b[3] = {bx - 1e-6, by - 1e-6, bz - 1e-6};
+                                         double e, double pad = 1e-6) {
+  const double b[3] = {bx - pad, by - pad, bz - pad};
   double d2 = 0.0;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    const double lo = b[a], hi = b[a] + e + 2e-6;
+    const double lo = b[a], hi = b[a] + e + 2 * pad;
     const double d = q[a] < lo ? lo - q[a] : (q[a] > hi ? q[a] - hi : 0.0);
     d2 += d * d;
   }
   return d2;
+}
+
+// Visits the super cells of the Chebyshev rings R = 0, 1, ... around super cell c (clipped to
+// the S grid) in a fixed order, calling visit(x, y, z) for each, until stop(R) holds before ring
+// R or the rings have covered the grid.
+template <class Stop, class Visit>
+__device__ __forceinline__ void ring_walk(const int c[3], const int S[3], Stop stop, Visit visit) {
+  const int rmax = max(S[0], max(S[1], S[2]));
+  for (int R = 0; R <= rmax; ++R) {
+    if (stop(R)) break;
+    const int x0 = max(c[0] - R, 0), x1 = min(c[0] + R, S[0] - 1);
+    const int y0 = max(c[1] - R, 0), y1 = min(c[1] + R, S[1] - 1);
+    for (int x = x0; x <= x1; ++x) {
+      const bool xface = x == c[0] - R || x == c[0] + R;
+      for (int y = y0; y <= y1; ++y) {
+        const bool face = xface || y == c[1] - R || y == c[1] + R;
+        if (face) {
+          const int z0 = max(c[2] - R, 0), z1 = min(c[2] + R, S[2] - 1);
+          for (int z = z0; z <= z1; ++z) visit(x, y, z);
+        } else {
+          if (c[2] - R >= 0) visit(x, y, c[2] - R);
+          if (R > 0 && c[2] + R < S[2]) visit(x, y, c[2] + R);
+        }
+      }
+    }
+  }
 }
 
 // kIndex == false is the DTU search (casmvs_pcd_capped_nn).  kIndex == true also returns the
@@ -246,35 +272,153 @@ pcd_capped_nn_kernel(const __grid_constant__ NNGrid G, const float* __restrict__
     c[a] = min(max((int)floor((q[a] - G.org[a]) / G.hs), 0), G.S[a] - 1);
   double best2 = G.cap2;
   int64_t best_i = INT64_MAX;
-  const int rmax = max(G.S[0], max(G.S[1], G.S[2]));
-  for (int R = 0; R <= rmax; ++R) {
-    // every cell of ring R is at least (R - 1) super edges away along one axis
-    const double lb = (R - 1) * G.hs - 1e-6;
-    if (R >= 2 && (kIndex ? lb * lb > best2 : lb * lb >= best2)) break;
-    const int x0 = max(c[0] - R, 0), x1 = min(c[0] + R, G.S[0] - 1);
-    const int y0 = max(c[1] - R, 0), y1 = min(c[1] + R, G.S[1] - 1);
-    for (int x = x0; x <= x1; ++x) {
-      const bool xface = x == c[0] - R || x == c[0] + R;
-      for (int y = y0; y <= y1; ++y) {
-        const bool face = xface || y == c[1] - R || y == c[1] + R;
-        if (face) {
-          const int z0 = max(c[2] - R, 0), z1 = min(c[2] + R, G.S[2] - 1);
-          for (int z = z0; z <= z1; ++z)
-            scan_super<kIndex>(G, q, x, y, z, super_begin, cell_keys, cell_start, tgt, tgt_index,
-                               best2, best_i);
-        } else {
-          if (c[2] - R >= 0)
-            scan_super<kIndex>(G, q, x, y, c[2] - R, super_begin, cell_keys, cell_start, tgt,
-                               tgt_index, best2, best_i);
-          if (R > 0 && c[2] + R < G.S[2])
-            scan_super<kIndex>(G, q, x, y, c[2] + R, super_begin, cell_keys, cell_start, tgt,
-                               tgt_index, best2, best_i);
+  ring_walk(
+      c, G.S,
+      [&](int R) {
+        // every cell of ring R is at least (R - 1) super edges away along one axis
+        const double lb = (R - 1) * G.hs - 1e-6;
+        return R >= 2 && (kIndex ? lb * lb > best2 : lb * lb >= best2);
+      },
+      [&](int x, int y, int z) {
+        scan_super<kIndex>(G, q, x, y, z, super_begin, cell_keys, cell_start, tgt, tgt_index,
+                           best2, best_i);
+      });
+  dist[i] = best2 < G.cap2 ? sqrt(best2) : G.cap;
+  if (kIndex) index[i] = best2 < G.cap2 ? best_i : -1;
+}
+
+// ---------------------------------------------------------------------------------- k nearest
+// Statistical outlier removal (casmvsnet_pl_b200/cloud_filter.py).  One thread per point of the
+// key-sorted cloud keeps its k smallest squared distances to the other points in registers,
+// sorted descending in a[0..k) with a[0] the current k-th; the slots k..KMAX-1 hold -inf so that
+// a fully unrolled bubble pass never moves a distance into them.  The ring walk and the pruning
+// are capped_nn's with a box widening `pad` scaled to the cloud, and a box or ring is skipped when
+// its nearest possible distance is >= the k-th: the multiset of the k smallest distances, and so
+// the mean, does not depend on which of several tied points is kept.
+struct KnnGrid {
+  double org[3];
+  double h, hs;       // fine and super cell edges
+  int S[3];
+  double pad;
+};
+
+template <int KMAX>
+__device__ __forceinline__ void knn_scan_super(const KnnGrid& G, const double q[3], int self,
+                                               int k, int sx, int sy, int sz,
+                                               const int* __restrict__ super_begin,
+                                               const int64_t* __restrict__ cell_keys,
+                                               const int* __restrict__ cell_start,
+                                               const float* __restrict__ pts, double (&a)[KMAX]) {
+  const int s = (sx * G.S[1] + sy) * G.S[2] + sz;
+  const int c0 = __ldg(super_begin + s), c1 = __ldg(super_begin + s + 1);
+  if (c0 == c1) return;
+  const double bx = G.org[0] + sx * G.hs, by = G.org[1] + sy * G.hs, bz = G.org[2] + sz * G.hs;
+  if (box_d2(q, bx, by, bz, G.hs, G.pad) >= a[0]) return;
+  for (int c = c0; c < c1; ++c) {
+    const int l = (int)(__ldg(cell_keys + c) & 511);
+    if (box_d2(q, bx + (l >> 6) * G.h, by + ((l >> 3) & 7) * G.h, bz + (l & 7) * G.h, G.h,
+               G.pad) >= a[0])
+      continue;
+    for (int t = __ldg(cell_start + c), e = __ldg(cell_start + c + 1); t < e; ++t) {
+      if (t == self) continue;
+      const double dx = __dsub_rn((double)__ldg(pts + 3 * (size_t)t), q[0]);
+      const double dy = __dsub_rn((double)__ldg(pts + 3 * (size_t)t + 1), q[1]);
+      const double dz = __dsub_rn((double)__ldg(pts + 3 * (size_t)t + 2), q[2]);
+      const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+      if (d2 < a[0]) {
+        a[0] = d2;
+#pragma unroll
+        for (int j = 0; j + 1 < KMAX; ++j) {
+          if (j + 1 >= k) break;
+          const double x = a[j], y = a[j + 1];
+          a[j] = fmax(x, y);
+          a[j + 1] = fmin(x, y);
         }
       }
     }
   }
-  dist[i] = best2 < G.cap2 ? sqrt(best2) : G.cap;
-  if (kIndex) index[i] = best2 < G.cap2 ? best_i : -1;
+}
+
+template <int KMAX>
+__global__ void __launch_bounds__(128)
+pcd_knn_mean_kernel(const __grid_constant__ KnnGrid G, const float* __restrict__ pts, int n, int k,
+                    const int64_t* __restrict__ cell_keys, const int* __restrict__ cell_start,
+                    const int* __restrict__ super_begin, const int64_t* __restrict__ point_index,
+                    double* __restrict__ mean) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double q[3] = {(double)__ldg(pts + 3 * (size_t)i), (double)__ldg(pts + 3 * (size_t)i + 1),
+                       (double)__ldg(pts + 3 * (size_t)i + 2)};
+  double a[KMAX];
+#pragma unroll
+  for (int j = 0; j < KMAX; ++j) a[j] = j < k ? INFINITY : -INFINITY;
+  int c[3];
+#pragma unroll
+  for (int ax = 0; ax < 3; ++ax)
+    c[ax] = min(max((int)floor((q[ax] - G.org[ax]) / G.hs), 0), G.S[ax] - 1);
+  ring_walk(
+      c, G.S,
+      [&](int R) {
+        const double lb = (R - 1) * G.hs - G.pad;
+        return R >= 2 && lb * lb >= a[0];
+      },
+      [&](int x, int y, int z) {
+        knn_scan_super<KMAX>(G, q, i, k, x, y, z, super_begin, cell_keys, cell_start, pts, a);
+      });
+  double s = 0.0;                        // ascending: a[k-1] first
+#pragma unroll
+  for (int j = KMAX - 1; j >= 0; --j)
+    if (j < k) s = __dadd_rn(s, __dsqrt_rn(a[j]));
+  mean[__ldg(point_index + i)] = __ddiv_rn(s, (double)k);
+}
+
+// ---------------------------------------------------------------------------------- statistics
+constexpr int kSorChunk = 1024;
+constexpr int kSorThreads = 256;     // = tnt_eval.cu's compaction block, whose offsets it feeds
+
+// chunk[c] = sum of v (mu == nullptr) or of (v - *mu)^2 over chunk c, left to right
+__global__ void __launch_bounds__(256)
+pcd_sor_chunk_kernel(const double* __restrict__ v, int n, const double* __restrict__ mu,
+                     double* __restrict__ chunk) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  const int lo = c * kSorChunk;
+  if (lo >= n) return;
+  const int hi = min(n, lo + kSorChunk);
+  double s = 0.0;
+  if (mu) {
+    const double m = *mu;
+    for (int i = lo; i < hi; ++i) {
+      const double d = __dsub_rn(__ldg(v + i), m);
+      s = __dadd_rn(s, __dmul_rn(d, d));
+    }
+  } else {
+    for (int i = lo; i < hi; ++i) s = __dadd_rn(s, __ldg(v + i));
+  }
+  chunk[c] = s;
+}
+
+// one thread: the chunk sums left to right; pass 0 writes mu, pass 1 sigma and the threshold
+__global__ void pcd_sor_total_kernel(const double* __restrict__ chunk, int nchunks, int n,
+                                     double ratio, int pass, double* __restrict__ stats) {
+  double s = 0.0;
+  for (int c = 0; c < nchunks; ++c) s = __dadd_rn(s, chunk[c]);
+  if (pass == 0) {
+    stats[0] = __ddiv_rn(s, (double)n);
+  } else {
+    const double sigma = __dsqrt_rn(__ddiv_rn(s, (double)(n - 1)));
+    stats[1] = sigma;
+    stats[2] = __dadd_rn(stats[0], __dmul_rn(ratio, sigma));
+  }
+}
+
+__global__ void __launch_bounds__(kSorThreads)
+pcd_sor_keep_kernel(const double* __restrict__ v, int n, const double* __restrict__ stats,
+                    unsigned char* __restrict__ mask, int* __restrict__ block_counts) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool keep = i < n && __ldg(v + i) <= __ldg(stats + 2);
+  if (i < n) mask[i] = keep;
+  const int c = __syncthreads_count(keep);
+  if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
 }
 
 }  // namespace casmvs
@@ -412,4 +556,74 @@ extern "C" int casmvs_pcd_capped_nn_index(const float* queries, int nq, const fl
   return capped_nn_launch("pcd_capped_nn_index", queries, nq, targets, cell_keys, cell_start,
                           ncells, super_begin, origin3, h, super_dims3, box_lo3, box_hi3, cap,
                           target_index, dist, index, stream);
+}
+
+extern "C" int casmvs_pcd_knn_mean(const float* points, int n, int k, const int64_t* cell_keys,
+                                   const int* cell_start, int ncells, const int* super_begin,
+                                   const double* origin3, double h, const int* super_dims3,
+                                   double pad, const int64_t* point_index, double* mean,
+                                   void* stream) {
+  CASMVS_REQUIRE(k >= 1 && k <= 64, "pcd_knn_mean: k = %d must lie in 1..64", k);
+  CASMVS_REQUIRE(n > k, "pcd_knn_mean: n = %d points must exceed k = %d", n, k);
+  CASMVS_REQUIRE(ncells >= 1 && ncells <= n, "pcd_knn_mean: bad cell count %d", ncells);
+  CASMVS_REQUIRE(origin3 && super_dims3, "pcd_knn_mean: null host array");
+  CASMVS_REQUIRE(h > 0.0 && pad >= 0.0, "pcd_knn_mean: h must be > 0 and pad >= 0");
+  CASMVS_REQUIRE(points && cell_keys && cell_start && super_begin && point_index && mean,
+                 "pcd_knn_mean: null pointer");
+  KnnGrid G;
+  size_t nsuper = 1;
+  for (int a = 0; a < 3; ++a) {
+    CASMVS_REQUIRE(super_dims3[a] > 0 && super_dims3[a] < (1 << 17), "pcd_knn_mean: bad super dims");
+    nsuper *= (size_t)super_dims3[a];
+    G.org[a] = origin3[a];
+    G.S[a] = super_dims3[a];
+  }
+  CASMVS_REQUIRE(nsuper < (1u << 31), "pcd_knn_mean: too many super cells");
+  G.h = h;
+  G.hs = 8.0 * h;
+  G.pad = pad;
+  const dim3 grid((n + 127) / 128);
+  cudaStream_t st = as_stream(stream);
+#define KNN_LAUNCH(KM)                                                                          \
+  pcd_knn_mean_kernel<KM><<<grid, 128, 0, st>>>(G, points, n, k, cell_keys, cell_start,         \
+                                                super_begin, point_index, mean)
+  if (k <= 8) KNN_LAUNCH(8);
+  else if (k <= 16) KNN_LAUNCH(16);
+  else if (k <= 32) KNN_LAUNCH(32);
+  else KNN_LAUNCH(64);
+#undef KNN_LAUNCH
+  return after_launch("pcd_knn_mean");
+}
+
+extern "C" size_t casmvs_pcd_sor_workspace_bytes(int n) {
+  if (n <= 0) return 0;
+  return 2 * (size_t)((n + kSorChunk - 1) / kSorChunk) * sizeof(double);
+}
+
+extern "C" int casmvs_pcd_sor_keep(const double* mean, int n, double std_ratio, double* stats,
+                                   unsigned char* mask, int* block_counts, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+  CASMVS_REQUIRE(n >= 2, "pcd_sor_keep: n = %d must be >= 2", n);
+  CASMVS_REQUIRE(std_ratio > 0.0 && std_ratio <= 1.7976931348623157e308,
+                 "pcd_sor_keep: std_ratio must be finite and > 0");
+  CASMVS_REQUIRE(workspace_bytes >= casmvs_pcd_sor_workspace_bytes(n),
+                 "pcd_sor_keep: workspace too small (%zu < %zu bytes)", workspace_bytes,
+                 casmvs_pcd_sor_workspace_bytes(n));
+  CASMVS_REQUIRE(mean && stats && mask && block_counts && workspace, "pcd_sor_keep: null pointer");
+  const int nchunks = (n + kSorChunk - 1) / kSorChunk;
+  double* sums = static_cast<double*>(workspace);
+  double* sq = sums + nchunks;
+  cudaStream_t st = as_stream(stream);
+  const int cb = (nchunks + 255) / 256;
+  pcd_sor_chunk_kernel<<<cb, 256, 0, st>>>(mean, n, nullptr, sums);
+  if (int rc = after_launch("pcd_sor_chunk")) return rc;
+  pcd_sor_total_kernel<<<1, 1, 0, st>>>(sums, nchunks, n, std_ratio, 0, stats);
+  if (int rc = after_launch("pcd_sor_total")) return rc;
+  pcd_sor_chunk_kernel<<<cb, 256, 0, st>>>(mean, n, stats, sq);
+  if (int rc = after_launch("pcd_sor_chunk")) return rc;
+  pcd_sor_total_kernel<<<1, 1, 0, st>>>(sq, nchunks, n, std_ratio, 1, stats);
+  if (int rc = after_launch("pcd_sor_total")) return rc;
+  pcd_sor_keep_kernel<<<casmvs_tnt_crop_blocks(n), kSorThreads, 0, st>>>(mean, n, stats, mask,
+                                                                        block_counts);
+  return after_launch("pcd_sor_keep");
 }

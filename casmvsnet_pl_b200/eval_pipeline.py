@@ -52,6 +52,8 @@ at --img_wh and writes <out>/mesh/<scan>.obj, .mtl and _<k>.png beside the PLY (
 --mesh --mesh_score with --dtu_gt or --tnt_gt also scores the mesh as it is written, through its
 surface samples (dtu_eval.evaluate_mesh / tnt_eval.evaluate_mesh), into <out>/mesh/<scan>_scores.json
 or <out>/mesh/<scan>_tnt.json.
+--remove_outliers [--outlier_neighbours K] [--outlier_std R] removes the fused cloud's statistical
+outliers on the GPU (cloud_filter.py) before it is written, scored or Poisson-meshed.
 """
 from __future__ import annotations
 
@@ -452,6 +454,21 @@ def _simplify(name, verts, colours, faces, mesh_faces, log):
     return verts, colours, faces
 
 
+def _remove_outliers(name, xyz, outlier_filter, log):
+    """-> (the points cloud_filter.filter_points keeps, their indices), or (xyz, None) for a
+    cloud of k points or fewer, which is kept whole."""
+    from . import cloud_filter
+    k = outlier_filter.get("k", cloud_filter.DEFAULT_K)
+    std_ratio = outlier_filter.get("std_ratio", cloud_filter.DEFAULT_STD_RATIO)
+    if len(xyz) <= k:
+        log(f"{name}: outliers not removed: {len(xyz)} points, and the filter needs more than "
+            f"k = {k}")
+        return xyz, None
+    kept, index, st = cloud_filter.filter_points(xyz, k, std_ratio)
+    log(f"{name}: removed outliers: {cloud_filter.summary(st)}")
+    return kept, index
+
+
 def _clean(name, verts, colours, faces, mesh_clean, log):
     """The mesh cleaned by mesh_clean.clean_mesh(**mesh_clean) (unchanged when it is None)."""
     if mesh_clean is None:
@@ -505,7 +522,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
              mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
              mesh_texture=False, mesh_score=False, mesh_texture_level=False, mesh_clean=None,
-             fusion_rule="reference"):
+             fusion_rule="reference", outlier_filter=None):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -532,6 +549,11 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     `fusion_rule` is fusion.fuse_scan's `rule`: "dynamic" fuses with the dynamic consistency
     check (min_geo_consistent is then ignored) and logs the count of kept points; everything
     downstream takes its cloud unchanged.
+    With `outlier_filter` (dict(k=..., std_ratio=...), either may be left out for its default),
+    the fused cloud (after `skip`) loses its statistical outliers (cloud_filter.py) before it is
+    written, scored or returned, and Poisson meshing's unthinned points lose theirs by the same
+    rule on that cloud; TSDF meshing is unchanged.  A cloud of k points or fewer is kept whole,
+    and the log says so.
     With `mesh_score` (it needs `mesh_path` and `tnt_gt` or `dtu_gt`), the mesh as written is also
     scored through its surface samples by tnt_eval.evaluate_mesh or dtu_eval.evaluate_mesh, the
     scores are written beside it as <mesh>_tnt.json or <mesh>_scores.json, and appended to the
@@ -557,6 +579,11 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
                                 skip, max_ref_views, collect=fused, rule=fusion_rule)
     if fusion_rule != "reference":
         log(f"{scan.scan}: {fusion_rule} fusion kept {len(xyz)} points")
+    kept_index = None
+    if outlier_filter is not None:
+        xyz, kept_index = _remove_outliers(scan.scan, xyz, outlier_filter, log)
+        if kept_index is not None:
+            rgb = rgb[kept_index]
     if ply_path:
         fusion.write_ply(ply_path, xyz, rgb)
     if mesh_path and mesh_method == "poisson":
@@ -567,6 +594,12 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         cols = torch.cat([f["image"][f["depth"] != 0] for f in fused]).to(torch.uint8)
         if len(cols) != len(pts):
             raise ValueError(f"{scan.scan}: the fused depth maps and points disagree")
+        if outlier_filter is not None:
+            if skip != 1:                       # Poisson's points are not the written cloud
+                _, kept_index = _remove_outliers(f"{scan.scan} (poisson points)", pts,
+                                                 outlier_filter, log)
+            if kept_index is not None:
+                pts, cols = pts[kept_index].contiguous(), cols[kept_index].contiguous()
         cams = np.stack([-np.linalg.inv(np.asarray(f["P"], np.float64)[:3, :3]) @
                          np.asarray(f["P"], np.float64)[:3, 3] for f in fused])
         del fused
@@ -739,12 +772,29 @@ def parse_args(argv=None):
                     help="with --mesh and --dtu_gt or --tnt_gt: also score the mesh as written "
                          "through its surface samples into <out>/mesh/<scan>_scores.json "
                          "(DTU) or <scan>_tnt.json")
+    ap.add_argument("--remove_outliers", action="store_true",
+                    help="remove statistical outliers from the fused cloud (and from Poisson's "
+                         "points) on the GPU before it is written, scored or meshed: points whose "
+                         "mean distance to their neighbours exceeds the cloud's mean by more than "
+                         "--outlier_std standard deviations")
+    ap.add_argument("--outlier_neighbours", type=int, default=None,
+                    help="with --remove_outliers: neighbours per point, 1..64 (default 20)")
+    ap.add_argument("--outlier_std", type=float, default=None,
+                    help="with --remove_outliers: the standard-deviation ratio, > 0 (default 2.0)")
     a = ap.parse_args(argv)
     if getattr(a, "fusion", "reference") == "dynamic":
         ap.set_defaults(min_geo_consistent=None)                  # given explicitly?
         if ap.parse_args(argv).min_geo_consistent is not None:
             ap.error("--min_geo_consistent applies to --fusion reference only; the dynamic "
                      "rule sets its own view counts")
+    if a.outlier_neighbours is not None and not a.remove_outliers:
+        ap.error("--outlier_neighbours needs --remove_outliers")
+    if a.outlier_std is not None and not a.remove_outliers:
+        ap.error("--outlier_std needs --remove_outliers")
+    if a.outlier_neighbours is not None and not 1 <= a.outlier_neighbours <= 64:
+        ap.error("--outlier_neighbours must be in 1..64")
+    if a.outlier_std is not None and not (math.isfinite(a.outlier_std) and a.outlier_std > 0):
+        ap.error("--outlier_std must be a finite number > 0")
     if a.mesh_score and not a.mesh:
         ap.error("--mesh_score needs --mesh")
     if a.mesh_score and a.dtu_gt is None and a.tnt_gt is None:
@@ -799,6 +849,15 @@ def _clean_options(a):
     return {k: v for k, v in opts.items() if v is not None}
 
 
+def _outlier_options(a):
+    """filter options from --outlier_neighbours / --outlier_std, or None without
+    --remove_outliers."""
+    if not a.remove_outliers:
+        return None
+    opts = dict(k=a.outlier_neighbours, std_ratio=a.outlier_std)
+    return {k: v for k, v in opts.items() if v is not None}
+
+
 def main(argv=None):
     a = parse_args(argv)
     if a.dtu_gt is not None and a.dataset_name != "dtu":
@@ -839,7 +898,8 @@ def main(argv=None):
                        mesh_faces=a.mesh_faces, mesh_texture=a.mesh_texture,
                        mesh_score=a.mesh_score, mesh_texture_level=a.mesh_texture_level,
                        mesh_clean=_clean_options(a),
-                       fusion_rule=getattr(a, "fusion", "reference"), **tnt)
+                       fusion_rule=getattr(a, "fusion", "reference"),
+                       outlier_filter=_outlier_options(a), **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

@@ -703,6 +703,49 @@ def pcd_capped_nn_index(queries, targets, cell_keys, cell_start, super_begin, or
     return dist, index
 
 
+@_on_tensor_device
+def pcd_knn_mean(points, k, cell_keys, cell_start, super_begin, origin, h, super_dims, pad,
+                 point_index):
+    """Mean distance (float64, input order) of every point of a key-sorted (N,3) float32 cloud
+    to its k nearest other points (casmvs_pcd_knn_mean); point_index (N,) int64 maps the sorted
+    points back to the input order."""
+    pts = _points("points", points)
+    _require_cuda_typed(points=(pts, torch.float32), cell_keys=(cell_keys, torch.int64),
+                        cell_start=(cell_start, torch.int32), super_begin=(super_begin, torch.int32),
+                        point_index=(point_index, torch.int64))
+    ncells = cell_keys.shape[0]
+    if cell_start.shape[0] != ncells + 1 or super_begin.shape[0] != math.prod(int(v) for v in super_dims) + 1:
+        raise _lib.CasMVSError("cell_start / super_begin sizes do not match the grid")
+    if point_index.shape != (pts.shape[0],):
+        raise _lib.CasMVSError("point_index must hold one index per point")
+    mean = torch.empty(pts.shape[0], device=pts.device, dtype=torch.float64)
+    check(_lib.load().casmvs_pcd_knn_mean(
+        _ptr(pts), pts.shape[0], int(k), _ptr(cell_keys.contiguous()), _ptr(cell_start.contiguous()),
+        ncells, _ptr(super_begin.contiguous()), (ctypes.c_double * 3)(*map(float, origin)), float(h),
+        (ctypes.c_int * 3)(*map(int, super_dims)), float(pad), _ptr(point_index.contiguous()),
+        _ptr(mean), _stream()), "pcd_knn_mean")
+    return mean
+
+
+@_on_tensor_device
+def pcd_sor_keep(mean, std_ratio):
+    """Statistics and keep mask of (N,) float64 mean distances (casmvs_pcd_sor_keep) ->
+    (stats (3,) float64 device tensor mu, sigma, threshold; mask (N,) uint8; block counts (int32,
+    as tnt_compact takes them); chunk sums (2, ceil(N / 1024)) float64)."""
+    _require_cuda_typed(mean=(mean, torch.float64))
+    m = mean.contiguous()
+    n = m.shape[0]
+    lib = _lib.load()
+    nbytes = lib.casmvs_pcd_sor_workspace_bytes(n)
+    ws = torch.empty(max(nbytes // 8, 2), device=m.device, dtype=torch.float64)
+    stats = torch.empty(3, device=m.device, dtype=torch.float64)
+    mask = torch.empty(n, device=m.device, dtype=torch.uint8)
+    counts = torch.empty(max(lib.casmvs_tnt_crop_blocks(n), 1), device=m.device, dtype=torch.int32)
+    check(lib.casmvs_pcd_sor_keep(_ptr(m), n, float(std_ratio), _ptr(stats), _ptr(mask),
+                                  _ptr(counts), _ptr(ws), nbytes, _stream()), "pcd_sor_keep")
+    return stats, mask, counts, ws.view(2, -1)
+
+
 # ------------------------------------------------------------------ Tanks and Temples scoring
 @_on_tensor_device
 def tnt_transform_crop(points, T=None, crop=None):
@@ -734,13 +777,28 @@ def tnt_transform_crop(points, T=None, crop=None):
     check(lib.casmvs_tnt_transform_crop(_ptr(pts), n, Tp, int(axis), float(amin), float(amax),
                                         _ptr(poly), poly.shape[0], _ptr(out), _ptr(mask),
                                         _ptr(counts), _stream()), "tnt_transform_crop")
+    return tnt_compact(out, mask, counts)
+
+
+@_on_tensor_device
+def tnt_compact(points, mask, block_counts):
+    """The points with mask != 0 in input order and their input indices (int64), given the kept
+    count of each block of casmvs_tnt_crop_blocks(N) (casmvs_tnt_compact)."""
+    pts = _points("points", points)
+    _require_cuda_typed(points=(pts, torch.float32), mask=(mask, torch.uint8),
+                        block_counts=(block_counts, torch.int32))
+    n = pts.shape[0]
+    lib = _lib.load()
+    nb = lib.casmvs_tnt_crop_blocks(n)
+    if mask.shape != (n,) or block_counts.numel() < nb:
+        raise _lib.CasMVSError("mask must hold one entry per point and block_counts one per block")
     offsets = torch.zeros(max(nb, 1) + 1, device=pts.device, dtype=torch.int64)
-    torch.cumsum(counts[:nb], 0, out=offsets[1:nb + 1])
+    torch.cumsum(block_counts[:nb], 0, out=offsets[1:nb + 1])
     kept = int(offsets[nb].item()) if nb else 0
     res = torch.empty((kept, 3), device=pts.device, dtype=torch.float32)
     idx = torch.empty(kept, device=pts.device, dtype=torch.int64)
-    check(lib.casmvs_tnt_compact(_ptr(out), _ptr(mask), n, _ptr(offsets), _ptr(res), _ptr(idx),
-                                 _stream()), "tnt_compact")
+    check(lib.casmvs_tnt_compact(_ptr(pts), _ptr(mask.contiguous()), n, _ptr(offsets), _ptr(res),
+                                 _ptr(idx), _stream()), "tnt_compact")
     return res, idx
 
 

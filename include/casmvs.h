@@ -530,6 +530,33 @@ int casmvs_pcd_capped_nn_index(const float* queries, int nq, const float* target
                                const double* box_hi3, double cap, const int64_t* target_index,
                                double* dist, int64_t* index, void* stream);
 
+/* ---- Statistical outlier removal (casmvsnet_pl_b200/cloud_filter.py) -------------------------
+ * Every double operation below is rounded to nearest, no contraction, in the order written.
+ * casmvs_pcd_knn_mean: mean[point_index[i]] = m_i, the mean distance from point i to its k
+ *   (1..64) nearest other points of the same cloud, for n > k points.  points are in key order of
+ *   a sub == 8 grid of edge h at origin3 that holds every point (cell lists and super_begin as for
+ *   casmvs_pcd_capped_nn); point_index (n int64) maps them back to the input order.  d(i, j) =
+ *   sqrt((dx*dx + dy*dy) + dz*dz), dx = double(x_j) - double(x_i); the point itself is not its
+ *   own neighbour but exact duplicates are, at 0.  m_i = (the k smallest d(i, j) summed left to
+ *   right in ascending order) / k.  Boxes are widened by `pad` (>= 0; it must cover the rounding
+ *   of the cell keys and of the box bounds at the cloud's coordinates) before they are pruned.
+ *   The result is exact for every h.  origin3 and super_dims3 are HOST arrays of 3.
+ * casmvs_pcd_sor_keep: the statistics and keep mask of n >= 2 mean distances.  With chunks of
+ *   1024 values in order, workspace (casmvs_pcd_sor_workspace_bytes(n)) gets the chunk sums of
+ *   the m_i, then those of (m_i - mu)^2; stats (3 doubles, device) = mu = (chunk sums summed left
+ *   to right) / n, sigma = sqrt((the same for the squares) / (n - 1)) and the threshold
+ *   t = mu + std_ratio * sigma (std_ratio finite, > 0).  mask[i] = m_i <= t, and block_counts
+ *   (casmvs_tnt_crop_blocks(n) ints) the kept count of each block, as casmvs_tnt_compact takes
+ *   them.  No float atomics: two runs give the same bits. */
+int casmvs_pcd_knn_mean(const float* points, int n, int k, const int64_t* cell_keys,
+                        const int* cell_start, int ncells, const int* super_begin,
+                        const double* origin3, double h, const int* super_dims3, double pad,
+                        const int64_t* point_index, double* mean, void* stream);
+size_t casmvs_pcd_sor_workspace_bytes(int n);
+int casmvs_pcd_sor_keep(const double* mean, int n, double std_ratio, double* stats,
+                        unsigned char* mask, int* block_counts, void* workspace,
+                        size_t workspace_bytes, void* stream);
+
 /* ---- Tanks and Temples scoring (casmvsnet_pl_b200/tnt_eval.py) ------------------------------
  * Every double operation below is rounded to nearest, no contraction, in the order written.
  * casmvs_tnt_transform_crop: out[i] = p_i, or with T (a HOST array of 12 doubles, rows 0..2 of a
