@@ -172,8 +172,7 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
           mbar_expect_tx(full, 4 * kU9Data);
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            const Coords5 k =
-                brick_coords(true, 1, 4, q, t.w0 / 2 - 1, t.h0 / 2 - 1, t.s0 + st, t.b);
+            const Coords5 k = brick_coords(true, q, t.w0 / 2 - 1, t.h0 / 2 - 1, t.s0 + st, t.b);
             tma_load_5d(dst + q * kU9Bytes, &u9map, full, k.c[0], k.c[1], k.c[2], k.c[3], k.c[4]);
           }
           if (st > 0) {                             // the first step's u11 slices are not used
@@ -185,7 +184,7 @@ conv3d_tail_kernel(const __grid_constant__ CUtensorMap u9map,
             for (int k2 = 0; k2 < 2; ++k2) {
 #pragma unroll
               for (int q = 0; q < 2; ++q) {
-                const Coords5 k = brick_coords(true, 1, 2, q, t.w0 - 1, t.h0 - 1,
+                const Coords5 k = brick_coords(true, q, t.w0 - 1, t.h0 - 1,
                                                2 * (t.s0 + st) - 1 + k2, t.b);
                 tma_load_5d(dc0 + k2 * kSliceBytes + q * kBrickBytes, &c0map, fc0, k.c[0], k.c[1],
                             k.c[2], k.c[3], k.c[4]);

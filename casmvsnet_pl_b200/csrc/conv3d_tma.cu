@@ -162,7 +162,7 @@ conv3d_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
           mbar_expect_tx(full, S::CQ * S::kBrickData);
 #pragma unroll
           for (int q = 0; q < S::CQ; ++q) {
-            const Coords5 k = brick_coords(!PLANAR && p.x_blocked, 1, S::CQ, q, w0 - 1, h0 - 1,
+            const Coords5 k = brick_coords(!PLANAR && p.x_blocked, q, w0 - 1, h0 - 1,
                                            d0 - halo + it, b);
             tma_load_5d(dst + q * S::kBrickBytes, &xmap, full, k.c[0], k.c[1], k.c[2], k.c[3],
                         k.c[4]);
@@ -279,15 +279,17 @@ int encode_map(const MapDesc& d, CUtensorMap* out) {
 
 int input_map(CUtensorMap* out, const float* x, int B, int D, int H, int W, int C, int box_w,
               int box_h, int stride_w, bool blocked) {
+  if (blocked && stride_w != 1) {
+    set_error("tma: a blocked input map walks W with stride 1 (got %d)", stride_w);
+    return -2;
+  }
   const uint64_t c = C, w = W, h = H, dp = D, b = B, vox = dp * h * w;
   const uint32_t bw = box_w, bh = box_h, sw = stride_w;
   const MapDesc d =
-      !blocked        ? MapDesc{x, 5, 0, {c, w, h, dp, b}, {4 * c, 4 * c * w, 4 * c * w * h, 4 * c * vox},
-                                {4, bw, bh, 1, 1}, {1, sw, 1, 1, 1}}
-      : stride_w == 1 ? MapDesc{x, 5, 0, {4 * w, h, dp, c / 4, b}, {16 * w, 16 * w * h, 16 * vox, 4 * c * vox},
-                                {4 * bw, bh, 1, 1, 1}, {1, 1, 1, 1, 1}}
-                      : MapDesc{x, 5, 0, {4, w, h, dp, c / 4 * b}, {16, 16 * w, 16 * w * h, 16 * vox},
-                                {4, bw, bh, 1, 1}, {1, sw, 1, 1, 1}};
+      !blocked ? MapDesc{x, 5, 0, {c, w, h, dp, b}, {4 * c, 4 * c * w, 4 * c * w * h, 4 * c * vox},
+                         {4, bw, bh, 1, 1}, {1, sw, 1, 1, 1}}
+               : MapDesc{x, 5, 0, {4 * w, h, dp, c / 4, b}, {16 * w, 16 * w * h, 16 * vox, 4 * c * vox},
+                         {4 * bw, bh, 1, 1, 1}, {1, 1, 1, 1, 1}};
   return encode_map(d, out);
 }
 

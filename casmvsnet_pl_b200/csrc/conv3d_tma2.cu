@@ -25,6 +25,10 @@
 //     of it (start address + rows*columns + column);
 //   * MODE_S2 / MODE_P5: the even and odd input columns are two planes, each loaded by a TMA
 //     whose box walks W with element stride 2 (tensor map elementStrides = {1,2,1,1,1});
+//   * MODE_S2 with blocked input: one TMA load per channel quad brings the 33 rows of 18
+//     input columns (2*w0-1 .. 2*w0+16) as one [33][18][4] run, 288 contiguous bytes per row,
+//     into the space of the quad's two planes; the consumer warpgroups then rewrite it in place
+//     into the even / odd planes (split_parities), so the GEMM reads the same planes as above;
 //   * persistent CTAs, 9 warps (two consumer warpgroups of 64 GEMM rows each, one TMA
 //     producer); the consumer keeps the accumulators of the output slices an input slice
 //     reaches in registers and runs the epilogue of a slice as soon as it is complete.
@@ -70,6 +74,9 @@ struct Cfg {
   static constexpr int kPlaneData = BR * BW * 16;
   static constexpr int kPlaneBytes = (kPlaneData + 127) / 128 * 128;
   static constexpr int kSlotBytes = NPL * kPlaneBytes;
+  // MODE_S2, blocked input: the run of one channel quad, [BR][2 BW][4], at the quad's planes
+  static constexpr int kRunData = BR * 2 * BW * 16;
+  static_assert(MODE != MODE_S2 || kRunData == PAR * kPlaneData, "a run fills the quad's planes");
   // accumulator group (columns per output group) and B image rows per tap
   static constexpr int GW = MODE == MODE_T ? 8 * COUT : (COUT <= 16 ? 16 : 32);
   static constexpr int BROWS = MODE == MODE_S2 ? 3 * GW : MODE == MODE_T ? 12 * COUT : GW;
@@ -134,18 +141,28 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
           const uint32_t g = gs + it;
           const uint32_t dst = s_ring + ring.acquire(g) * C::kSlotBytes, full = ring.full_bar(g);
           mbar_expect_tx(full, C::NPL * C::kPlaneData);
+          if (MODE == MODE_S2 && p.x_blocked) {
+            // one contiguous run per channel quad, split into its planes by the consumers
 #pragma unroll
-          for (int pl = 0; pl < C::NPL; ++pl) {
-            // plane pl = PAR * (channel quad) + column parity
-            const int q = pl / C::PAR, par = pl % C::PAR;
-            const int wc = MODE == MODE_S2 ? 2 * w0 - 1 + par
-                           : MODE == MODE_T ? w0 : 2 * w0 - 2 + par;
-            const int hc = MODE == MODE_S2 ? 2 * h0 - 1 : MODE == MODE_T ? h0 : 2 * h0 - 2;
-            const tma::Coords5 k = tma::brick_coords(MODE != MODE_P5 && p.x_blocked,
-                                                     MODE == MODE_T ? 1 : 2, C::CQ,
-                                                     q, wc, hc, s_first + it, b);
-            tma_load_5d(dst + pl * C::kPlaneBytes, &xmap, full, k.c[0], k.c[1], k.c[2], k.c[3],
-                        k.c[4]);
+            for (int q = 0; q < C::CQ; ++q) {
+              const tma::Coords5 k =
+                  tma::brick_coords(true, q, 2 * w0 - 1, 2 * h0 - 1, s_first + it, b);
+              tma_load_5d(dst + q * C::PAR * C::kPlaneBytes, &xmap, full, k.c[0], k.c[1], k.c[2],
+                          k.c[3], k.c[4]);
+            }
+          } else {
+#pragma unroll
+            for (int pl = 0; pl < C::NPL; ++pl) {
+              // plane pl = PAR * (channel quad) + column parity
+              const int q = pl / C::PAR, par = pl % C::PAR;
+              const int wc = MODE == MODE_S2 ? 2 * w0 - 1 + par
+                             : MODE == MODE_T ? w0 : 2 * w0 - 2 + par;
+              const int hc = MODE == MODE_S2 ? 2 * h0 - 1 : MODE == MODE_T ? h0 : 2 * h0 - 2;
+              const tma::Coords5 k = tma::brick_coords(MODE == MODE_T && p.x_blocked, q, wc, hc,
+                                                       s_first + it, b);
+              tma_load_5d(dst + pl * C::kPlaneBytes, &xmap, full, k.c[0], k.c[1], k.c[2], k.c[3],
+                          k.c[4]);
+            }
           }
         }
       }
@@ -197,6 +214,51 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
         }
         wgmma_commit();
         wgmma_wait_all();
+      };
+
+      // MODE_S2, blocked input: the slot holds each channel quad as one [BR][2 BW][4] run
+      // (input columns 2*w0-1 .. 2*w0+16 side by side) where its two planes go.  Column c of
+      // the run belongs to plane c & 1, column c >> 1.  The planes of a quad overlap its run
+      // and nothing else, so the quads are split in batches of up to four: every consumer thread
+      // loads its voxels of the batch into registers, and stores them once all 256 have loaded.
+      // A thread handles the same run voxels i = t + 256 k in every quad.  The stores are
+      // generic-proxy writes that the wgmma (async proxy) read: each thread fences them before
+      // the last barrier.
+      constexpr int kRun = C::BR * 2 * BW;                           // voxels of one run
+      constexpr int kPer = (kRun + kConsumerThreads - 1) / kConsumerThreads;
+      constexpr int kBatch = C::CQ < 4 ? C::CQ : 4;                  // quads per batch
+      static_assert(C::CQ % kBatch == 0, "whole batches");
+      uint32_t run_off[kPer], plane_off[kPer];
+#pragma unroll
+      for (int k = 0; k < kPer; ++k) {
+        const int i = threadIdx.x + k * kConsumerThreads;
+        const int r = i / (2 * BW), c = i - r * (2 * BW);
+        run_off[k] = i < kRun ? i * 16 : ~0u;                        // ~0u: no voxel
+        plane_off[k] = (c & 1) * C::kPlaneBytes + (r * BW + (c >> 1)) * 16;
+      }
+      auto split_parities = [&](int slot) {
+        unsigned char* s = smem + C::kRingOff + slot * C::kSlotBytes;
+#pragma unroll
+        for (int q0 = 0; q0 < C::CQ; q0 += kBatch) {
+          float4 v[kBatch][kPer];
+#pragma unroll
+          for (int j = 0; j < kBatch; ++j)
+#pragma unroll
+            for (int k = 0; k < kPer; ++k)
+              if (run_off[k] != ~0u)
+                v[j][k] = *reinterpret_cast<const float4*>(
+                    s + (q0 + j) * C::PAR * C::kPlaneBytes + run_off[k]);
+          asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+#pragma unroll
+          for (int j = 0; j < kBatch; ++j)
+#pragma unroll
+            for (int k = 0; k < kPer; ++k)
+              if (run_off[k] != ~0u)
+                *reinterpret_cast<float4*>(s + (q0 + j) * C::PAR * C::kPlaneBytes +
+                                           plane_off[k]) = v[j][k];
+        }
+        fence_proxy_async();
+        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
       };
 
       // stores two adjacent channels (c, c+1) of output voxel (od, oh, ow)
@@ -303,6 +365,7 @@ conv3d_tma2_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
         if (!w_ready) { mbar_wait(bar_w, 0); w_ready = true; }
         const uint64_t a_s = a_desc0 + ((slot * C::kSlotBytes) >> 4);
         if constexpr (MODE == MODE_S2) {
+          if (p.x_blocked) split_parities(slot);
           // B rows [W(kd=1) | W(kd=2) | W(kd=0)]
           if ((it & 1) == 0) issue(std::integral_constant<int, 2 * GW>{}, a_s, GW);  // kd=2 -> a-1, kd=0 -> a
           else issue(std::integral_constant<int, GW>{}, a_s, 0);                    // kd=1 -> a
@@ -445,12 +508,15 @@ static int launch2(const ConvArgs& a, cudaStream_t st) {
   p.round_out = a.round_out;
   p.x_blocked = (a.layout & kLayoutXBlocked) ? 1 : 0;
   p.y_blocked = (a.layout & kLayoutYBlocked) ? 1 : 0;
-  // S2: box {4, 17 traversed -> 9 loaded, 33, 1, 1} walking W with stride 2; T: {4, 9, 17}
+  // S2: box {4, 17 traversed -> 9 loaded, 33, 1, 1} walking W with stride 2, or, blocked, one
+  // run of 18 voxels x 33 rows {72, 33, 1, 1, 1}; T: {4, 9, 17}
   // P5: box {4, 19 traversed -> 10 loaded, 35, 1, 1} walking W with stride 2
   CUtensorMap map;
   const int rc =
-      MODE == MODE_S2   ? tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 17, C::BR, 2,
-                                         p.x_blocked)
+      MODE == MODE_S2   ? (p.x_blocked ? tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN,
+                                                        2 * C::BW, C::BR, 1, true)
+                                       : tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 17,
+                                                        C::BR, 2))
       : MODE == MODE_P5 ? tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, 19, C::BR, 2)
                         : tma::input_map(&map, a.x, p.B, p.Di, p.Hi, p.Wi, CIN, C::BW, C::BR, 1,
                                          p.x_blocked);

@@ -84,28 +84,26 @@ struct MapDesc {
 int encode_map(const MapDesc& d, CUtensorMap* out);
 
 // The map of a conv kernel's input x (B,D,H,W,C): a box of one channel quad, box_w x box_h
-// voxels of one slice (16 bytes per voxel, no swizzle).  Three forms:
+// voxels of one slice (16 bytes per voxel, no swizzle).  Two forms:
 //   * channels-last: {C, W, H, D, B}, box {4, box_w, box_h, 1, 1};
-//   * blocked by channel quads, (B, C/4, D, H, W, 4) fp32, stride 1: {4W, H, D, C/4, B}, box
+//   * blocked by channel quads, (B, C/4, D, H, W, 4) fp32: {4W, H, D, C/4, B}, box
 //     {4 box_w, box_h, 1, 1, 1} -- the quad folded into the inner dimension, so one brick row
-//     is 16 box_w contiguous bytes;
-//   * blocked, stride_w = 2: {4, W, H, D, C/4 B}, box {4, box_w, box_h, 1, 1}.
-// stride_w = 2: the box walks every second voxel along W (box_w counts traversed positions, so
-// ceil(box_w / 2) voxels are loaded): the even / odd column planes of the stride-2 convolutions.
-// Every form writes the same [box_h][box_w][4] brick to shared memory; only the load
-// coordinates differ (brick_coords).  0, or -2 with the casmvs error set.  (conv3d_tma.cu)
+//     is 16 box_w contiguous bytes.
+// stride_w = 2 (channels-last only): the box walks every second voxel along W (box_w counts
+// traversed positions, so ceil(box_w / 2) voxels are loaded): the even / odd column planes of
+// the stride-2 convolutions.  Both forms write the same [box_h][box_w][4] brick to shared
+// memory; only the load coordinates differ (brick_coords).  0, or -2 with the casmvs error set.
+// (conv3d_tma.cu)
 int input_map(CUtensorMap* out, const float* x, int B, int D, int H, int W, int C, int box_w,
               int box_h, int stride_w = 1, bool blocked = false);
 
 // Load coordinates of the brick of channel quad q whose first voxel is (w, h, d) of batch item
-// b, for the map input_map built (cq = C/4).  Blocked, stride 1: {4w, h, d, q, b}; blocked,
-// stride 2: {0, w, h, d, b cq + q}; channels-last: {4q, w, h, d, b}.
+// b, for the map input_map built.  Blocked: {4w, h, d, q, b}; channels-last: {4q, w, h, d, b}.
 struct Coords5 { int c[5]; };
-__host__ __device__ __forceinline__ Coords5 brick_coords(bool blocked, int stride_w, int cq, int q,
-                                                         int w, int h, int d, int b) {
+__host__ __device__ __forceinline__ Coords5 brick_coords(bool blocked, int q, int w, int h, int d,
+                                                         int b) {
   if (!blocked) return {{4 * q, w, h, d, b}};
-  if (stride_w == 1) return {{4 * w, h, d, q, b}};
-  return {{0, w, h, d, b * cq + q}};
+  return {{4 * w, h, d, q, b}};
 }
 
 // Element offset of channel c of voxel (b, d, h, w) in a (B, D, H, W, C) volume stored
