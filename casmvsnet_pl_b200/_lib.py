@@ -99,6 +99,13 @@ SIGNATURES = {
                             + [c_void_p] * 4 + [c_size_t, c_void_p]),
     "casmvs_sl1_loss_bwd": (c_int, [POINTER(c_void_p)] * 3 + [POINTER(c_int), c_int, c_int]
                             + [c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
+    "casmvs_photo_loss_workspace_bytes": (c_size_t, [c_int] * 4),
+    "casmvs_photo_loss_fwd": (c_int, [c_void_p] * 3 + [POINTER(c_void_p), POINTER(c_float)]
+                              + [c_int] * 6 + [c_float, POINTER(c_void_p)] + [c_void_p] * 3
+                              + [POINTER(c_void_p)] * 3 + [c_void_p, c_size_t, c_void_p]),
+    "casmvs_photo_loss_bwd": (c_int, [c_void_p] * 3 + [POINTER(c_void_p), POINTER(c_float)]
+                              + [c_int] * 6 + [c_float, POINTER(c_void_p)]
+                              + [c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
     "casmvs_geo_fuse_fwd":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     POINTER(c_float), POINTER(c_float), c_void_p, c_int, c_int,
                                     c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -116,3 +116,103 @@ def depth_metrics(pred, gt, mask):
     errors e = pred - gt (metrics.py: abs_error and acc_threshold at 1, 2, 4, summed)."""
     with torch.no_grad():
         return _forward([pred], [gt], [mask])[1]
+
+
+# ------------------------------------------------------------------ photometric (csrc/photo_loss.cu)
+def _photo_inputs(depths, imgs, proj_mats, depth_interval, interval_ratios, levels):
+    _require_cuda(imgs, proj_mats, *depths)
+    if imgs.dim() != 5 or imgs.shape[2] != 3:
+        raise _lib.CasMVSError(f"photo loss expects imgs (B,V,3,H,W), got {tuple(imgs.shape)}")
+    B, V, _, H, W = imgs.shape
+    if tuple(proj_mats.shape) != (B, V - 1, levels, 3, 4):
+        raise _lib.CasMVSError(f"photo loss expects proj_mats {(B, V - 1, levels, 3, 4)}, "
+                               f"got {tuple(proj_mats.shape)}")
+    for l, d in enumerate(depths):
+        if tuple(d.shape) != (B, H >> l, W >> l) or d.device != imgs.device or d.dtype != torch.float32:
+            raise _lib.CasMVSError(f"depth_{l} must be float32 {(B, H >> l, W >> l)} on the images' device, "
+                                   f"got {tuple(d.shape)}")
+    if len(interval_ratios) < levels:
+        raise _lib.CasMVSError(f"{levels} levels need {levels} interval ratios")
+    dint = torch.as_tensor(depth_interval, dtype=torch.float32, device=imgs.device).reshape(-1)
+    if dint.numel() == 1 and B > 1:
+        dint = dint.expand(B)
+    if dint.numel() != B:
+        raise _lib.CasMVSError(f"depth_interval must have one value per sample, got {dint.numel()}")
+    ratios = (ctypes.c_float * levels)(*[float(r) for r in interval_ratios[:levels]])
+    return (imgs.detach().float().contiguous(), proj_mats.detach().float().contiguous(),
+            dint.contiguous(), [d.detach().contiguous() for d in depths], ratios, (B, V, H, W))
+
+
+class _PhotoLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, levels, topk, smooth_weight, interval_ratios, debug_maps, imgs, proj_mats,
+                depth_interval, *depths):
+        im, pm, dint, ds, ratios, (B, V, H, W) = _photo_inputs(depths, imgs, proj_mats, depth_interval,
+                                                               interval_ratios, levels)
+        dev = im.device
+        lib = _lib.load()
+        loss = torch.empty((), device=dev, dtype=torch.float32)
+        stats = torch.empty(levels, 3, device=dev, dtype=torch.float32)
+        counts = torch.empty(levels, device=dev, dtype=torch.int64)
+        sel = [torch.empty(d.shape, device=dev, dtype=torch.int16) for d in ds]
+        ws_bytes = lib.casmvs_photo_loss_workspace_bytes(B, H, W, levels)
+        ws = torch.empty(max(ws_bytes, 1), device=dev, dtype=torch.uint8)
+        dbg_e = dbg_valid = dbg_lossq = None
+        if debug_maps is not None:
+            dbg_e = [torch.empty(B, V - 1, *d.shape[1:], device=dev) for d in ds]
+            dbg_valid = [torch.empty(d.shape, device=dev, dtype=torch.int16) for d in ds]
+            dbg_lossq = [torch.empty(d.shape, device=dev) for d in ds]
+        opt = lambda ts: None if ts is None else _ptr_array(ts)   # noqa: E731
+        with torch.cuda.device(dev):
+            check(lib.casmvs_photo_loss_fwd(_ptr(im), _ptr(pm), _ptr(dint), _ptr_array(ds), ratios, B, V,
+                                            H, W, levels, topk, smooth_weight, _ptr_array(sel),
+                                            _ptr(loss), _ptr(stats), _ptr(counts), opt(dbg_e),
+                                            opt(dbg_valid), opt(dbg_lossq), _ptr(ws), ws_bytes,
+                                            _stream()), "photo_loss_fwd")
+        ctx.save_for_backward(im, pm, dint, counts, *ds, *sel)
+        ctx.args = (levels, topk, smooth_weight, ratios, (B, V, H, W))
+        ctx.mark_non_differentiable(stats)
+        if debug_maps is not None:
+            debug_maps += [{"e": e, "valid": _bits(v, V - 1), "selected": _bits(s, V - 1), "loss_q": q}
+                           for e, v, s, q in zip(dbg_e, dbg_valid, sel, dbg_lossq)]
+        return loss, stats
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_stats):
+        levels, topk, smooth_weight, ratios, (B, V, H, W) = ctx.args
+        im, pm, dint, counts, *rest = ctx.saved_tensors
+        ds, sel = rest[:levels], rest[levels:]
+        grads = [torch.empty_like(d) for d in ds]
+        go = grad_loss.detach().to(torch.float32).contiguous()
+        with torch.cuda.device(im.device):
+            check(_lib.load().casmvs_photo_loss_bwd(_ptr(im), _ptr(pm), _ptr(dint), _ptr_array(ds), ratios,
+                                                    B, V, H, W, levels, topk, smooth_weight,
+                                                    _ptr_array(sel), _ptr(counts), _ptr(go),
+                                                    _ptr_array(grads), _stream()), "photo_loss_bwd")
+        return (None,) * 8 + tuple(grads)
+
+
+def _bits(mask16, S):
+    """(B,h,w) int16 bit masks -> (B,S,h,w) bool, bit s -> [:, s]."""
+    m = mask16.to(torch.int32) & 0xFFFF
+    return torch.stack([(m >> s) & 1 for s in range(S)], 1).bool()
+
+
+def photo_loss(results, imgs, proj_mats, depth_interval, interval_ratios, levels=3, topk=1,
+               smooth_weight=0.01, debug=False):
+    """Self-supervised photometric loss of depth maps `results['depth_l']` (csrc/photo_loss.cu
+    states the rule): each source image is warped into the reference view with the predicted
+    depth, the 3x3 SSIM + L1 errors of the `topk` best sources per pixel are averaged, and an
+    edge-aware smoothness of depth in hypothesis spacings is added with weight smooth_weight.
+
+    imgs (B,V,3,H,W) normalised network input, proj_mats (B,V-1,levels,3,4) as the model takes,
+    depth_interval (B,1) or (B,), interval_ratios one per level.  Returns (loss (), stats
+    (levels,3) = [P_l, S_l, N_l]), device tensors, with no host synchronisation; only the depth
+    maps get a gradient.  debug=True adds a third value, per level {e (B,S,h,w) NaN where
+    invalid, valid (B,S,h,w) bool, selected (B,S,h,w) bool, loss_q (B,h,w) NaN where no source
+    is valid}."""
+    depths = [results[f"depth_{l}"] for l in range(levels)]
+    maps = [] if debug else None
+    loss, stats = _PhotoLossFn.apply(levels, topk, float(smooth_weight), list(interval_ratios), maps,
+                                     imgs, proj_mats, depth_interval, *depths)
+    return (loss, stats, maps) if debug else (loss, stats)

@@ -287,30 +287,96 @@ def sparse_tracks(n_img=300, n_pts=500_000, track_len=(3, 11), seed=0):
     return centres, xyz, ptr, img
 
 
+def height_field_depth(K, E, wh, depth=3.0):
+    """Per-pixel depth (h,w) float64 of colmap_model's surface z = depth + 0.05 depth
+    sin(3x / depth) cos(2y / depth) seen by a pinhole camera K (3,3), world->camera E (4,4) of
+    size wh = (w, h): the camera z of the ray-surface intersection through each pixel centre,
+    found by Newton's method in float64 (the surface's slope is at most 0.15, so from the
+    plane z = depth it converges in a few steps).  Also returns the world points (h,w,3)."""
+    w, h = wh
+    K, E = np.asarray(K, np.float64), np.asarray(E, np.float64)
+    R, t = E[:3, :3], E[:3, 3]
+    C = -R.T @ t
+    ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    r = np.einsum("ij,hwj->hwi", R.T @ np.linalg.inv(K), np.stack([xs, ys, np.ones_like(xs)], -1))
+    a, b = 3.0 / depth, 2.0 / depth
+    s = (depth - C[2]) / r[..., 2]
+    for _ in range(50):
+        X = C + s[..., None] * r
+        hz = depth + 0.05 * depth * np.sin(a * X[..., 0]) * np.cos(b * X[..., 1])
+        dhx = 0.05 * depth * a * np.cos(a * X[..., 0]) * np.cos(b * X[..., 1])
+        dhy = -0.05 * depth * b * np.sin(a * X[..., 0]) * np.sin(b * X[..., 1])
+        g = X[..., 2] - hz
+        step = g / (r[..., 2] - dhx * r[..., 0] - dhy * r[..., 1])
+        s = s - step
+        if np.abs(step).max() < 1e-13 * depth:
+            break
+    X = C + s[..., None] * r
+    return s, X
+
+
+def surface_texture(X, seed, px_per_unit):
+    """A seeded band-limited RGB texture (h,w,3) uint8 at world points X (h,w,3): 16 plane waves
+    in world (x, y) per channel, their periods between 16 and 64 pixels at `px_per_unit` image
+    pixels per world unit, so even the strided quarter-resolution level sees them unaliased."""
+    rng = np.random.default_rng(seed)
+    out = np.empty(X.shape[:2] + (3,))
+    for c in range(3):
+        acc = np.zeros(X.shape[:2])
+        for _ in range(16):
+            f = px_per_unit / rng.uniform(16, 64)
+            th = rng.uniform(0, 2 * np.pi)
+            acc += np.sin(2 * np.pi * f * (np.cos(th) * X[..., 0] + np.sin(th) * X[..., 1])
+                          + rng.uniform(0, 2 * np.pi))
+        out[..., c] = 0.5 + 0.4 * acc / 16 * 2.5
+    return np.clip(np.rint(out * 255), 0, 255).astype(np.uint8)
+
+
 def make_colmap(root, n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=0,
-                fmt="bin", layout="undistorted", image_ext="jpg", image_dir=None, **kw):
+                fmt="bin", layout="undistorted", image_ext="jpg", image_dir=None, textured=False, **kw):
     """An undistorted COLMAP workspace: <root>/images/view_XXX.jpg at each view's camera size and
     the model of colmap_model under <root>/sparse, in binary ("bin"), text ("txt") or both
     formats ("both"; the reader prefers the binary one).  layout="mapper" puts the model under
     <root>/sparse/0 as `colmap mapper` does; image_ext="png" writes lossless images (the same
     bytes from every decoder); image_dir replaces <root>/images; `distortion` (colmap_model)
-    makes the cameras distorted.  Returns the model."""
+    makes the cameras distorted.  Returns the model.
+
+    textured=True instead renders every view of the model's surface with one seeded texture in
+    world coordinates (surface_texture), always as lossless PNGs, so the views agree
+    photometrically under the true depth; it returns (model, depths) with depths[v] the (h,w)
+    float64 ground-truth depth of view v (height_field_depth) at its camera's size."""
     from PIL import Image
 
     from . import colmap
     if layout not in ("undistorted", "mapper") or image_ext not in ("jpg", "png"):
         raise ValueError(f"unknown layout {layout!r} or image extension {image_ext!r}")
+    if textured:
+        if kw.get("distortion") is not None:
+            raise ValueError("textured views are rendered with pinhole cameras; no distortion")
+        image_ext = "png"
     model = colmap_model(n_views, image_wh, depth, n_points, seed, ext=image_ext, **kw)
     rng = np.random.default_rng(seed + 1)
     image_dir = image_dir or os.path.join(root, "images")
     os.makedirs(image_dir, exist_ok=True)
+    depths = {}
     for q, t, cid, name in model.images.values():
-        _, w, h, _ = model.cameras[cid]
+        cam_name, w, h, prm = model.cameras[cid]
         opts = {"quality": 92} if image_ext == "jpg" else {}
-        Image.fromarray(_image(rng, w, h)).save(os.path.join(image_dir, name), **opts)
+        if textured:
+            E = np.eye(4)
+            E[:3, :3], E[:3, 3] = colmap.qvec_to_rotmat(q), t
+            K = colmap.intrinsics(cam_name, prm)
+            v = int(name[len("view_"):-len(".png")])
+            depths[v], X = height_field_depth(K, E, (w, h), depth)
+            img = surface_texture(X, seed + 1, K[0, 0] / depth)
+        else:
+            img = _image(rng, w, h)
+        Image.fromarray(img).save(os.path.join(image_dir, name), **opts)
     sparse = os.path.join(root, "sparse", "0") if layout == "mapper" else os.path.join(root, "sparse")
     for f in (("bin", "txt") if fmt == "both" else (fmt,)):
         colmap.write_model(sparse, model, f)
+    if textured:
+        return model, [depths[v] for v in range(n_views)]
     return model
 
 

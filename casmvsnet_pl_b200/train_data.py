@@ -1,5 +1,6 @@
 """Training readers: datasets/dtu.py of the reference with img_wh=None (DTUTrainDataset) and
-datasets/blendedmvs.py in training mode (BlendedMVSTrainDataset), splits train / val.
+datasets/blendedmvs.py in training mode (BlendedMVSTrainDataset), splits train / val, and a
+COLMAP capture without ground truth for the photometric loss (ColmapTrainSet).
 
 DTU:
 
@@ -185,6 +186,67 @@ class BlendedMVSTrainDataset(torch.utils.data.Dataset):
         if jitter:
             sample["jitter"] = torch.tensor(jitter, dtype=torch.float32)
         return sample
+
+
+class ColmapTrainSet:
+    """A COLMAP capture as a training set for the self-supervised photometric loss (test-time
+    adaptation to the scene that will be reconstructed).  eval_pipeline.ColmapScan selects the
+    views, depth ranges and projections and logs the views that are not reference views; its
+    SceneImages decodes every image once, undistorts distorted cameras and keeps them on the
+    device.  A sample is a reference view with its first n_views - 1 sources; there are no
+    depths or masks.  Batches are built on the device in to_device's layout (imgs, proj_mats,
+    init_depth_min, depth_interval, scan_vid) by `loader`."""
+
+    def __init__(self, root_dir, n_views=3, levels=3, n_depths_arg=192.0, img_wh=(640, 512),
+                 image_dir=None, device="cuda:0", log=print):
+        from .eval_pipeline import ColmapScan
+        self.scan = ColmapScan(root_dir, None, tuple(img_wh), n_views, n_depths_arg, levels,
+                               device=device, log=log, image_dir=image_dir)
+        if not self.scan.metas:
+            raise ValueError(f"{root_dir}: no view has {n_views - 1} sources to train on")
+        self.images = self.scan._image_cache(device)
+        self.ids = [[ref] + srcs[: n_views - 1] for ref, srcs in self.scan.metas]
+        self.proj_mats = torch.stack([io.relative_proj_mats(self.scan.proj_mats, ids)
+                                      for ids in self.ids]).to(device)
+        self.ranges = torch.tensor([self.scan.depth_range(ids[0], None) for ids in self.ids],
+                                   dtype=torch.float32, device=device)
+        self.device = device
+
+    def __len__(self):
+        return len(self.ids)
+
+    def batch(self, idx):
+        """The device sample of the reference views at positions `idx` (a list)."""
+        sel = torch.tensor(idx, device=self.device)
+        return {"imgs": torch.stack([self.images.network(self.ids[i]) for i in idx]),
+                "proj_mats": self.proj_mats.index_select(0, sel),
+                "init_depth_min": self.ranges.index_select(0, sel)[:, :1],
+                "depth_interval": self.ranges.index_select(0, sel)[:, 1:],
+                "scan_vid": (self.scan.scan, [self.ids[i][0] for i in idx])}
+
+    def loader(self, batch_size, shuffle, seed=None):
+        """An iterable of batches, re-iterable per epoch; with shuffle, each pass draws a new
+        order from one generator seeded with `seed` (a random seed when None)."""
+        g = torch.Generator()
+        if seed is None:
+            g.seed()
+        else:
+            g.manual_seed(seed)
+        return _Batches(self, batch_size, shuffle, g)
+
+
+class _Batches:
+    def __init__(self, dataset, batch_size, shuffle, generator):
+        self.dataset, self.batch_size, self.shuffle, self.g = dataset, batch_size, shuffle, generator
+
+    def __len__(self):
+        return (len(self.dataset) + self.batch_size - 1) // self.batch_size
+
+    def __iter__(self):
+        n = len(self.dataset)
+        order = torch.randperm(n, generator=self.g).tolist() if self.shuffle else list(range(n))
+        for i in range(0, n, self.batch_size):
+            yield self.dataset.batch(order[i:i + self.batch_size])
 
 
 def loader(dataset, batch_size, shuffle, num_workers=4, seed=None):

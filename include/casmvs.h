@@ -388,6 +388,36 @@ int casmvs_sl1_loss_bwd(const float* const* pred, const float* const* gt,
                         const long long* counts, const float* grad_loss, float* const* grad_pred,
                         void* stream);
 
+/* ---- self-supervised photometric loss (csrc/photo_loss.cu has the full rule) ---------------
+ * imgs (B,V,3,H,W) float32 normalised network input (view 0 = reference), proj_mats
+ * (B,V-1,levels,3,4), depth_interval (B) float32, all device; depth / selection / grad_depth /
+ * dbg_* are HOST arrays of `levels` device pointers to (B,H/2^l,W/2^l) maps (dbg_e: (B,V-1,h,w));
+ * interval_ratios is a HOST float[levels].
+ *   L = sum_l 2^(1-l) (P_l + smooth_weight S_l), P_l = mean over pixels with a valid source of
+ *   the mean of the topk smallest 0.85 (1 - SSIM3x3) / 2 + 0.15 |L1| errors over the warped
+ *   sources, S_l the edge-aware smoothness of depth / (depth_interval * interval_ratios[l]).
+ * casmvs_photo_loss_fwd: loss (device float[1]), stats (device float[levels][3] = P_l, S_l,
+ *   N_l), counts (device int64[levels] = N_l) and selection (uint16 per pixel, bit s = source
+ *   s selected) for the backward.  dbg_e (NaN where (q, s) is not valid), dbg_valid (uint16
+ *   bits) and dbg_lossq (NaN where no source is valid) may be NULL.  fp64 sums in a fixed order,
+ *   no atomics: bit-identical run to run.  workspace: casmvs_photo_loss_workspace_bytes bytes.
+ * casmvs_photo_loss_bwd: grad_depth[l] (every pixel written) = dL/d depth_l * (*grad_loss,
+ *   device float), a gather that needs no host synchronisation.
+ * Refused (status -1): V - 1 outside 1..16, topk outside 1..V-1, levels outside 1..4, a level
+ * smaller than 3x3 or H, W not divisible by 2^(levels-1), smooth_weight not finite or < 0. */
+size_t casmvs_photo_loss_workspace_bytes(int B, int H, int W, int levels);
+int casmvs_photo_loss_fwd(const float* imgs, const float* proj_mats, const float* depth_interval,
+                          const float* const* depth, const float* interval_ratios, int B, int V,
+                          int H, int W, int levels, int topk, float smooth_weight,
+                          uint16_t* const* selection, float* loss, float* stats, long long* counts,
+                          float* const* dbg_e, uint16_t* const* dbg_valid, float* const* dbg_lossq,
+                          void* workspace, size_t workspace_bytes, void* stream);
+int casmvs_photo_loss_bwd(const float* imgs, const float* proj_mats, const float* depth_interval,
+                          const float* const* depth, const float* interval_ratios, int B, int V,
+                          int H, int W, int levels, int topk, float smooth_weight,
+                          const uint16_t* const* selection, const long long* counts,
+                          const float* grad_loss, float* const* grad_depth, void* stream);
+
 /* ---- input pipeline (SURVEY.md 8 f-4) -------------------------------------
  * T.ToTensor() + T.Normalize(mean, std) of the reference's data sets (datasets/dtu.py:130-137)
  * for images uploaded as bytes: images (N,H,W,3) uint8 RGB -> out (N,3,H,W) float32,
