@@ -15,6 +15,7 @@ ROUND_TF32 = 256
 KEEP_FP32_OUT = 256      # OR-ed into conv3d precision
 BLOCKED = 512            # OR-ed into costreg precision / warp_cost_ladder round_tf32
 FUSED_TAIL = 1024        # OR-ed into costreg precision: conv11 + prob in one kernel, u11 not kept
+INVERSE_DEPTH = 2048     # OR-ed into regress input_is_prob / regress_bwd dv_is_vector / warp_cost_ladder round_tf32
 FP32, TF32 = 0, 1
 CONV, CONV_TRANSPOSE, CONV_PLANAR = 0, 1, 2
 PRECISIONS = {"fp32": FP32, "tf32": TF32}
@@ -69,6 +70,11 @@ SIGNATURES = {
                                             c_float, c_void_p] + [c_int] * 8 + [c_void_p]),
     "casmvs_regress_ladder_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_float,
                                           c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
+    "casmvs_inverse_hypotheses_fwd": (c_int, [c_void_p, c_float, c_void_p, c_float, c_void_p, c_float,
+                                              c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
+    "casmvs_regress_ladder_inverse_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p,
+                                                  c_float, c_void_p, c_void_p, c_void_p] + [c_int] * 4
+                                          + [c_void_p]),
     "casmvs_fpn_level_fwd": (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_void_p]),
     "casmvs_fpn_merge_fwd": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p]),
     "casmvs_conv2d_rgb8_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p] + [c_int] * 4 + [c_void_p]),

@@ -168,26 +168,47 @@ def _wgrad(x, gy, B, ca, cb, xdims, ydims, stride):
     return dw
 
 
+def _regress_fwd(ctx, logits, depth_values, inverse):
+    lg = logits.detach().contiguous()
+    dv = depth_values.contiguous()
+    depth, conf, _, _ = ops.regress(lg, dv, inverse=inverse)
+    ctx.save_for_backward(lg, dv)
+    ctx.mark_non_differentiable(conf)
+    return depth, conf
+
+
+def _regress_bwd(ctx, gdepth, inverse):
+    lg, dv = ctx.saved_tensors
+    B, D, h, w = lg.shape
+    out = torch.empty_like(lg)
+    with torch.cuda.device(lg.device):
+        flags = int(dv.dim() == 1) | (ops.INVERSE_DEPTH if inverse else 0)
+        check(_lib.load().casmvs_regress_bwd(_ptr(lg), _ptr(dv), flags,
+                                             _ptr(gdepth.contiguous()), _ptr(out), B, D, h, w,
+                                             _stream()), "regress_bwd")
+    return out, None
+
+
 class RegressFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, depth_values):
-        lg = logits.detach().contiguous()
-        dv = depth_values.contiguous()
-        depth, conf, _, _ = ops.regress(lg, dv)
-        ctx.save_for_backward(lg, dv)
-        ctx.mark_non_differentiable(conf)
-        return depth, conf
+        return _regress_fwd(ctx, logits, depth_values, False)
 
     @staticmethod
     def backward(ctx, gdepth, _gconf):
-        lg, dv = ctx.saved_tensors
-        B, D, h, w = lg.shape
-        out = torch.empty_like(lg)
-        with torch.cuda.device(lg.device):
-            check(_lib.load().casmvs_regress_bwd(_ptr(lg), _ptr(dv), int(dv.dim() == 1),
-                                                 _ptr(gdepth.contiguous()), _ptr(out), B, D, h, w,
-                                                 _stream()), "regress_bwd")
-        return out, None
+        return _regress_bwd(ctx, gdepth, False)
+
+
+class RegressInverseFn(torch.autograd.Function):
+    """RegressFn in 1/depth: depth = 1/sum_d p_d/dv_d, d depth/d l_d = -depth^2 p_d (1/dv_d - 1/depth)."""
+
+    @staticmethod
+    def forward(ctx, logits, depth_values):
+        return _regress_fwd(ctx, logits, depth_values, True)
+
+    @staticmethod
+    def backward(ctx, gdepth, _gconf):
+        return _regress_bwd(ctx, gdepth, True)
 
 
 class Upsample2xFn(torch.autograd.Function):
@@ -229,5 +250,6 @@ def warp_cost(feats, proj_mats, depth_values, num_groups=1):
     return WarpCostFn.apply(feats, proj_mats, depth_values, num_groups)
 
 
-def regress(logits, depth_values):
-    return RegressFn.apply(logits, depth_values)
+def regress(logits, depth_values, inverse=False):
+    """inverse=True: the inverse-depth regression, depth = 1/sum_d p_d/depth_values_d."""
+    return (RegressInverseFn if inverse else RegressFn).apply(logits, depth_values)

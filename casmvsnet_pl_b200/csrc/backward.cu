@@ -473,6 +473,35 @@ __global__ void upsample2x_bilinear_bwd_kernel(const float* __restrict__ gy, flo
   gx[i] = acc;
 }
 
+// inverse depth (regress.cu, rule 5): ubar = sum_d p_d RN(1/dv_d), depth = RN(1/ubar)
+//   =>  d depth / d l_d = -depth^2 p_d (RN(1/dv_d) - ubar)
+__global__ void __launch_bounds__(128)
+regress_inv_bwd_kernel(const float* __restrict__ logits, const float* __restrict__ dv,
+                       int dv_is_vector, const float* __restrict__ gdepth,
+                       float* __restrict__ glogits, int D, int hw) {
+  const int b = blockIdx.y;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= hw) return;
+  const float* lp = logits + (size_t)b * D * hw + pix;
+  const float* dp = dv_is_vector ? dv : dv + (size_t)b * D * hw + pix;
+  const size_t ds = dv_is_vector ? 1 : (size_t)hw;
+  float m = -INFINITY;
+  for (int d = 0; d < D; ++d) m = fmaxf(m, __ldg(lp + (size_t)d * hw));
+  float den = 0.f, num = 0.f;
+  for (int d = 0; d < D; ++d) {
+    const float e = expf(__ldg(lp + (size_t)d * hw) - m);
+    den += e;
+    num = fmaf(e, __frcp_rn(__ldg(dp + d * ds)), num);
+  }
+  const float ubar = num / den, depth = __frcp_rn(ubar);
+  const float g = -(depth * depth) * (__ldg(gdepth + (size_t)b * hw + pix) / den);
+  float* op = glogits + (size_t)b * D * hw + pix;
+  for (int d = 0; d < D; ++d) {
+    const float e = expf(__ldg(lp + (size_t)d * hw) - m);
+    op[(size_t)d * hw] = e * (__frcp_rn(__ldg(dp + d * ds)) - ubar) * g;
+  }
+}
+
 // depth = sum_d softmax(l)_d * dv_d  =>  d depth / d l_d = p_d (dv_d - depth)
 __global__ void __launch_bounds__(128)
 regress_bwd_kernel(const float* __restrict__ logits, const float* __restrict__ dv,
@@ -708,8 +737,14 @@ extern "C" int casmvs_regress_bwd(const float* logits, const float* depth_values
                                   int w, void* stream) {
   CASMVS_REQUIRE(logits && depth_values && grad_depth && grad_logits, "regress_bwd: null pointer");
   CASMVS_REQUIRE(B >= 0 && B <= 65535 && D > 0 && h > 0 && w > 0, "regress_bwd: bad dims");
+  CASMVS_REQUIRE((dv_is_vector & ~(1 | CASMVS_INVERSE_DEPTH)) == 0, "regress_bwd: bad dv_is_vector flags");
   if (B == 0) return 0;
   const int hw = h * w;
+  if (dv_is_vector & CASMVS_INVERSE_DEPTH) {
+    regress_inv_bwd_kernel<<<dim3((hw + 127) / 128, B), 128, 0, as_stream(stream)>>>(
+        logits, depth_values, dv_is_vector & 1, grad_depth, grad_logits, D, hw);
+    return after_launch("regress_bwd");
+  }
   regress_bwd_kernel<<<dim3((hw + 127) / 128, B), 128, 0, as_stream(stream)>>>(
       logits, depth_values, dv_is_vector, grad_depth, grad_logits, D, hw);
   return after_launch("regress_bwd");

@@ -145,10 +145,18 @@ __device__ __forceinline__ void variance(const u64 (&S)[4], const u64 (&Q)[4], u
 }
 
 
+// Plane d of an inverse-depth ladder (README "Wide depth ranges", regress.cu): u_d = first -
+// step*d in 1/depth, multiply and subtract each rounded, depth = RN(1/u_d).
+__device__ __forceinline__ float inverse_plane(float first, float step, int d) {
+  return __frcp_rn(__fsub_rn(first, __fmul_rn(step, (float)d)));
+}
+
 // Where a pixel's depth hypotheses come from: the (B,D,h,w) tensor of the public API, or -- in
 // the cascade -- the ladder first + step*d that get_depth_values / the initial planes define
 // (models/modules.py:44-48, models/mvsnet.py:215-229), generated in the kernel with the SAME two
 // roundings (multiply, then add) so that the (B,D,h,w) tensor never has to exist in HBM.
+// INV: the ladder is in inverse depth, first and step in 1/depth units (inverse_plane).  A
+// template parameter, so that the uniform consumers compile exactly as they did without it.
 struct Hyp {
   const float* dv;         // (B,D,h,w) or null => ladder
   const float* first_map;  // (B,h,w) first hypothesis per pixel, or null
@@ -156,25 +164,31 @@ struct Hyp {
   const float* step_b;     // (B) plane spacing per batch item, or null
   float first, step;       // scalars used when the pointers above are null
 };
-struct HypPix {
+template <bool INV = false>
+struct HypPixT {
   const float* p;
   size_t hw;
   float first, step;
-  __device__ __forceinline__ HypPix(const Hyp& h, int b, int D, size_t hw_, int pix) : hw(hw_) {
+  __device__ __forceinline__ HypPixT(const Hyp& h, int b, int D, size_t hw_, int pix) : hw(hw_) {
     p = h.dv ? h.dv + (size_t)b * D * hw_ + pix : nullptr;
     first = h.first_map ? __ldg(h.first_map + (size_t)b * hw_ + pix) : h.first_b ? __ldg(h.first_b + b) : h.first;
     step = h.step_b ? __ldg(h.step_b + b) : h.step;
   }
   __device__ __forceinline__ float at(int d) const {
-    return p ? __ldg(p + (size_t)d * hw) : __fadd_rn(first, __fmul_rn(step, (float)d));
+    if constexpr (INV)
+      return p ? __ldg(p + (size_t)d * hw) : inverse_plane(first, step, d);
+    else
+      return p ? __ldg(p + (size_t)d * hw) : __fadd_rn(first, __fmul_rn(step, (float)d));
   }
 };
+using HypPix = HypPixT<false>;
 
 // The TMA-staged cost-volume kernels (warp_cost_smem.cu): channels-last features, channels-last
 // or (blocked != 0) blocked output.  warp_cost_staged returns the launcher of a shape from their
 // coverage table, or null (the shape runs on the gather kernel, or not at all from a ladder).
+// inverse != 0: a ladder dv is in inverse depth (HypPixT<true>).
 using StagedK1 = int (*)(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
-                         int D, int h, int w, int rnd, int blocked, cudaStream_t st);
+                         int D, int h, int w, int rnd, int blocked, int inverse, cudaStream_t st);
 StagedK1 warp_cost_staged(int V, int C, int num_groups);
 
 }  // namespace casmvs

@@ -389,7 +389,7 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   const unsigned xblocks = (unsigned)((threads + kK1Threads - 1) / kK1Threads);
   if (StagedK1 run = nhwc ? warp_cost_staged(V, C, num_groups) : nullptr) {
     const Hyp hyp{depth_values, nullptr, nullptr, nullptr, 0.f, 0.f};
-    return run(f, proj, hyp, cost, B, D, h, w, rnd, 0, st);
+    return run(f, proj, hyp, cost, B, D, h, w, rnd, 0, 0, st);
   }
   // depth chunks: enough CTAs to fill every SM several times over, but chunks long
   // enough (>= 8 planes) for the texel-window cache to pay off
@@ -449,7 +449,8 @@ extern "C" int casmvs_warp_cost_ladder_supported(int V, int C, int num_groups) {
 }
 
 // Cascade-internal variant of casmvs_warp_cost_fwd: the hypotheses are the ladder
-// first + step*d (see Hyp in k1_common.cuh) instead of a (B,D,h,w) tensor.  The staged kernels
+// first + step*d (see Hyp in k1_common.cuh) instead of a (B,D,h,w) tensor, or with
+// CASMVS_INVERSE_DEPTH the inverse-depth ladder 1/(first - step*d).  The staged kernels
 // read the features and write the cost volume (either layout) in 16-byte vectors.
 extern "C" int casmvs_warp_cost_ladder_fwd(const float* feats, const float* proj,
                                            const float* first_map, const float* first_b,
@@ -468,7 +469,8 @@ extern "C" int casmvs_warp_cost_ladder_fwd(const float* feats, const float* proj
                  "(casmvs_warp_cost_ladder_supported): materialise the hypotheses and call "
                  "casmvs_warp_cost_fwd (got V=%d C=%d G=%d)", V, C, num_groups);
   const int blocked = (round_tf32 & CASMVS_BLOCKED) ? 1 : 0;
-  const int rnd = (round_tf32 & ~CASMVS_BLOCKED) ? 1 : 0;
+  const int inverse = (round_tf32 & CASMVS_INVERSE_DEPTH) ? 1 : 0;
+  const int rnd = (round_tf32 & ~(CASMVS_BLOCKED | CASMVS_INVERSE_DEPTH)) ? 1 : 0;
   const Hyp hyp{nullptr, first_map, first_b, step_b, first, step};
-  return run(feats, proj, hyp, cost, B, D, h, w, rnd, blocked, as_stream(stream));
+  return run(feats, proj, hyp, cost, B, D, h, w, rnd, blocked, inverse, as_stream(stream));
 }

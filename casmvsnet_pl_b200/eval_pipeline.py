@@ -721,6 +721,9 @@ def parse_args(argv=None):
                          "--min_geo_consistent sources within 1 px and 1 %% depth) or dynamic "
                          "(for some k in 2..10, at least k sources within k/4 px and k/1300 "
                          "relative depth)")
+    ap.add_argument("--depth_sampling", choices=["uniform", "inverse"], default=argparse.SUPPRESS,
+                    help="plane spacing of the sweep: uniform (default; evenly in depth) or inverse "
+                         "(evenly in 1/depth and regressed in 1/depth, for wide depth ranges)")
     ap.add_argument("--max_ref_views", type=int, default=400)
     ap.add_argument("--skip", type=int, default=1)
     ap.add_argument("--precision", default="tf32", choices=["fp32", "tf32"])
@@ -875,7 +878,8 @@ def main(argv=None):
     from . import ABN
     from .models.mvsnet import CascadeMVSNet
     model = CascadeMVSNet(n_depths=a.n_depths, interval_ratios=a.interval_ratios,
-                          num_groups=a.num_groups, norm_act=ABN, precision=a.precision)
+                          num_groups=a.num_groups, norm_act=ABN, precision=a.precision,
+                          depth_sampling=getattr(a, "depth_sampling", "uniform"))
     if a.ckpt:
         load_checkpoint(model, a.ckpt)
     model = model.eval().cuda()

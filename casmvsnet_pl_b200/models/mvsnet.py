@@ -392,7 +392,7 @@ class CostRegNet(nn.Module):
 
 class CascadeMVSNet(nn.Module):
     def __init__(self, n_depths=[8, 32, 48], interval_ratios=[1, 2, 4], num_groups=1,
-                 norm_act=InPlaceABN, precision="fp32"):
+                 norm_act=InPlaceABN, precision="fp32", depth_sampling="uniform"):
         super().__init__()
         self.levels = 3
         self.n_depths = n_depths
@@ -414,6 +414,25 @@ class CascadeMVSNet(nn.Module):
             cin = self.G if self.G > 1 else 8 * 2 ** l
             setattr(self, f"cost_reg_{l}", CostRegNet(cin, norm_act))
         self.set_precision(precision)
+        self.set_depth_sampling(depth_sampling)
+
+    DEPTH_SAMPLINGS = ("uniform", "inverse")
+
+    def set_depth_sampling(self, depth_sampling):
+        """'uniform' (the reference: planes evenly spaced in depth) or 'inverse' (evenly spaced in
+        1/depth, regressed in 1/depth; README "Wide depth ranges").  Not part of the state dict:
+        the same weights run either way."""
+        if depth_sampling not in self.DEPTH_SAMPLINGS:
+            raise ValueError(f"depth_sampling must be one of {list(self.DEPTH_SAMPLINGS)}")
+        self.depth_sampling = depth_sampling
+        return self
+
+    def inverse_steps(self, init_depth_min, depth_interval, B, device):
+        """ops.inverse_steps for this model's stages (inverse mode), else None."""
+        if self.depth_sampling != "inverse":
+            return None
+        return ops.inverse_steps(init_depth_min, depth_interval, self.n_depths,
+                                 self.interval_ratios, B, device)
 
     def set_precision(self, precision):
         """'fp32' (CUDA-core FMA, bit-faithful products) or 'tf32' (wgmma) for the convs."""
@@ -427,22 +446,22 @@ class CascadeMVSNet(nn.Module):
         self.feature.allow_tf32 = precision == "tf32"
         return self
 
-    def predict_depth(self, feats, proj_mats, depth_values, cost_reg):
+    def predict_depth(self, feats, proj_mats, depth_values, cost_reg, inverse=False):
         """feats (B,V,C,h,w), proj_mats (B,V-1,3,4), depth_values (B,D,h,w),
         cost_reg: module (B,C,D,h,w)->(B,1,D,h,w).  Returns depth, confidence (B,h,w)
-        (reference models/mvsnet.py:125-195)."""
+        (reference models/mvsnet.py:125-195).  inverse: regress in 1/depth."""
         if torch.is_grad_enabled() and (feats.requires_grad or
                                         any(p.requires_grad for p in cost_reg.parameters())):
             from .. import autograd as AG
             cost = AG.warp_cost(feats, proj_mats, depth_values, self.G)
             logits = cost_reg(cost).squeeze(1)
-            return AG.regress(logits, depth_values)
+            return AG.regress(logits, depth_values, inverse=inverse)
         cost = ops.warp_cost(feats, proj_mats, depth_values, self.G, ops.NHWC,
                              round_tf32=(getattr(cost_reg, "precision", "fp32") == "tf32"))
         logits = cost_reg(cost).squeeze(1)
         del cost
         depth, confidence, index, _ = ops.regress(logits, depth_values,
-                                                  want_index=self.return_index)
+                                                  want_index=self.return_index, inverse=inverse)
         self._last_index = index
         return depth, confidence
 
@@ -456,6 +475,8 @@ class CascadeMVSNet(nn.Module):
         # around this forward: the flag has to be set process-wide.  The reference is fp32
         # (opt.py:69-70), so fp32 precision means fp32 here too.
         torch.backends.cudnn.allow_tf32 = self.precision == "tf32"
+        # before the feature net: the range check's synchronise then waits for a few tiny ops only
+        inv = self.inverse_steps(init_depth_min, depth_interval, B, imgs.device)
         feats = self.feature(imgs.reshape(B * V, 3, H, W))
         proj_by_level = proj_mats.permute(2, 0, 1, 3, 4).contiguous()
         results = {}
@@ -467,14 +488,19 @@ class CascadeMVSNet(nn.Module):
             D = self.n_depths[l]
             h, w = feats_l.shape[-2:]
             with torch.no_grad():
-                if l == self.levels - 1:
+                if inv is not None:
+                    depth_values = ops.inverse_hypotheses(
+                        inv, l, D, h, w, imgs.device,
+                        current_depth=None if l == self.levels - 1 else depth_l.detach())
+                elif l == self.levels - 1:
                     depth_values = ops.uniform_hypotheses(init_depth_min, depth_interval_l, D, B,
                                                           h, w, imgs.device)
                 else:
                     depth_values = ops.depth_hypotheses(depth_l.detach(), D, depth_interval_l,
                                                         upsample=True)
             depth_l, confidence_l = self.predict_depth(feats_l, proj_by_level[l], depth_values,
-                                                       getattr(self, f"cost_reg_{l}"))
+                                                       getattr(self, f"cost_reg_{l}"),
+                                                       inverse=inv is not None)
             results[f"depth_{l}"] = depth_l
             results[f"confidence_{l}"] = confidence_l
         return results
@@ -491,18 +517,28 @@ class CascadeMVSNet(nn.Module):
         bufs += list(getattr(f, "_pack_cache", {}).values()) + list(getattr(f, "_smooth_pack", ()))
         return [b for b in bufs if torch.is_tensor(b) and b.is_cuda]
 
-    def run_stage(self, l, feats_l, proj_mats_l, depth_prev, init_depth_min, depth_interval):
+    def run_stage(self, l, feats_l, proj_mats_l, depth_prev, init_depth_min, depth_interval,
+                  inv=None):
         """One cascade stage of the inference path (no grad): hypotheses -> K1 -> K2 -> K3.
         feats_l (B,V,C,h,w) channels-last, proj_mats_l (B,V-1,3,4), depth_prev (B,h/2,w/2) or None
-        for the coarsest stage.  Returns depth, confidence (B,h,w)."""
+        for the coarsest stage.  Returns depth, confidence (B,h,w).  In the inverse depth sampling
+        inv is the forward's ops.InverseSteps (computed here when None)."""
         B, V, C, h, w = feats_l.shape
         D = self.n_depths[l]
         depth_interval_l = depth_interval * self.interval_ratios[l]
         cost_reg = getattr(self, f"cost_reg_{l}")
+        inverse = self.depth_sampling == "inverse"
+        if inverse and inv is None:
+            inv = self.inverse_steps(init_depth_min, depth_interval, B, feats_l.device)
         if self.fuse_hypotheses and ops.ladder_supported(V, C, self.G) and \
                 ops.is_channels_last_feats(feats_l):
-            first = init_depth_min if depth_prev is None else ops.depth_first(depth_prev, D, depth_interval_l)
-            lad = ops.Ladder(first, depth_interval_l, D, B, h, w, feats_l.device)
+            if inverse:
+                first = inv.u_near if depth_prev is None else ops.inverse_hypotheses(
+                    inv, l, D, h, w, feats_l.device, current_depth=depth_prev, first_only=True)
+                lad = ops.Ladder(first, inv.step[l], D, B, h, w, feats_l.device, inverse=True)
+            else:
+                first = init_depth_min if depth_prev is None else ops.depth_first(depth_prev, D, depth_interval_l)
+                lad = ops.Ladder(first, depth_interval_l, D, B, h, w, feats_l.device)
             # the cost volume goes to CostRegNet blocked by channel quads where its tensor-core
             # path takes that layout (DESIGN.md §2)
             blocked = cost_reg.blocked_supported()
@@ -513,12 +549,15 @@ class CascadeMVSNet(nn.Module):
             depth, confidence, self._last_index = ops.regress_ladder(logits, lad,
                                                                      want_index=self.return_index)
             return depth, confidence
-        if depth_prev is None:
+        if inverse:
+            depth_values = ops.inverse_hypotheses(inv, l, D, h, w, feats_l.device,
+                                                  current_depth=depth_prev)
+        elif depth_prev is None:
             depth_values = ops.uniform_hypotheses(init_depth_min, depth_interval_l, D, B, h, w,
                                                   feats_l.device)
         else:
             depth_values = ops.depth_hypotheses(depth_prev, D, depth_interval_l, upsample=True)
-        return self.predict_depth(feats_l, proj_mats_l, depth_values, cost_reg)
+        return self.predict_depth(feats_l, proj_mats_l, depth_values, cost_reg, inverse=inverse)
 
     def forward(self, imgs, proj_mats, init_depth_min, depth_interval):
         """imgs (B,V,3,H,W); proj_mats (B,V-1,levels,3,4) fine->coarse;
@@ -540,6 +579,8 @@ class CascadeMVSNet(nn.Module):
             return self._forward_autograd(imgs, proj_mats, init_depth_min, depth_interval)
         results = {}
         with torch.no_grad():
+            # before the feature net: the range check's synchronise then waits for a few tiny ops
+            inv = self.inverse_steps(init_depth_min, depth_interval, B, imgs.device)
             feats = self.feature(imgs.reshape(B * V, 3, H, W), overlap=self.overlap_pyramid)
             ready = feats.get("_ready", {})
             # one re-layout for all levels instead of a strided slice copy per stage
@@ -552,7 +593,7 @@ class CascadeMVSNet(nn.Module):
                 feats_l = feats_l.view(B, V, *feats_l.shape[1:])
                 proj_mats_l = proj_by_level[l]
                 depth_l, confidence_l = self.run_stage(l, feats_l, proj_mats_l, depth_l,
-                                                       init_depth_min, depth_interval)
+                                                       init_depth_min, depth_interval, inv)
                 results[f"depth_{l}"] = depth_l
                 results[f"confidence_{l}"] = confidence_l
                 if self.return_index:

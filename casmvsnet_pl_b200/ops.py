@@ -13,8 +13,8 @@ import math
 import torch
 
 from . import _lib
-from ._lib import (BLOCKED, CONV, CONV_PLANAR, CONV_TRANSPOSE, FP32, FUSED_TAIL, KEEP_FP32_OUT, NCHW, NHWC, PRECISIONS, TF32,  # noqa: F401
-                   check)
+from ._lib import (BLOCKED, CONV, CONV_PLANAR, CONV_TRANSPOSE, FP32, FUSED_TAIL, INVERSE_DEPTH, KEEP_FP32_OUT, NCHW,  # noqa: F401
+                   NHWC, PRECISIONS, TF32, check)
 
 _checked_devices = set()
 
@@ -273,9 +273,11 @@ def costreg(x, params, cin, precision=FP32, blocked=False, fused_tail=True):
 
 # --------------------------------------------------------------------------- K3
 @_on_tensor_device
-def regress(logits, depth_values, input_is_prob=False, want_index=False, want_prob=False):
+def regress(logits, depth_values, input_is_prob=False, want_index=False, want_prob=False,
+            inverse=False):
     """softmax + soft-argmax depth + confidence (+ index, prob).
-    logits (B,D,h,w); depth_values (B,D,h,w) or (D,)."""
+    logits (B,D,h,w); depth_values (B,D,h,w) or (D,).  inverse=True regresses in 1/depth:
+    depth = 1/sum_d p_d/depth_values_d (README "Wide depth ranges")."""
     _require_cuda(logits, depth_values)
     _no_grad_only(logits)
     lg = logits.contiguous()
@@ -286,7 +288,8 @@ def regress(logits, depth_values, input_is_prob=False, want_index=False, want_pr
     conf = torch.empty_like(depth)
     index = torch.empty(B, h, w, device=lg.device, dtype=torch.int64) if want_index else None
     prob = torch.empty_like(lg) if want_prob else None
-    check(_lib.load().casmvs_regress_fwd(_ptr(lg), _ptr(dv), int(dv_vec), int(input_is_prob),
+    flags = int(bool(input_is_prob)) | (INVERSE_DEPTH if inverse else 0)
+    check(_lib.load().casmvs_regress_fwd(_ptr(lg), _ptr(dv), int(dv_vec), flags,
                                          _ptr(depth), _ptr(conf), _ptr(index), _ptr(prob),
                                          B, D, h, w, _stream()), "regress")
     return depth, conf, index, prob
@@ -343,14 +346,113 @@ def _uniform_hypotheses(init_depth_min, depth_interval, n_depths, B, h, w, devic
     return out
 
 
+# --------------------------------------------------------------------------- inverse depth
+class InverseSteps:
+    """Rules 1-2 of the inverse-depth plane sweep (csrc/regress.cu, README "Wide depth ranges")
+    for one forward: u_near = 1/near, u_far = 1/far and the per-stage plane spacing step[l] in
+    1/depth, each a float (float depth parameters) or a (B,) float32 device tensor."""
+
+    def __init__(self, u_near, u_far, step, B):
+        self.u_near, self.u_far, self.step, self.B = u_near, u_far, step, B
+
+
+def _depth_param(x, B):
+    t = x.reshape(-1).to(torch.float32)
+    return t.expand(B).contiguous() if t.numel() == 1 and B > 1 else t
+
+
+def inverse_steps(init_depth_min, depth_interval, n_depths, interval_ratios, B, device=None):
+    """u_near, u_far and s_l of the inverse-depth sweep (stage l = 0 finest .. len-1 coarsest).
+    near = init_depth_min, far = the uniform mode's last coarse plane
+    init_depth_min + (D-1)*depth_interval*ratio, formed in float32 as the hypothesis kernel forms
+    it; then in float64, each rounded once to float32: u_near = 1/near, u_far = 1/far,
+    s_top = (u_near - u_far)/(D_top - 1), s_l = s_top*ratio_l/ratio_top.
+    Raises CasMVSError unless 0 < near < far, both finite.  Floats and CPU tensors are checked
+    on the host; device tensors with one synchronise (skipped while a CUDA graph is captured:
+    the capturing caller has run the same tensors eagerly first)."""
+    top = len(n_depths) - 1
+    D, r_top = n_depths[top], interval_ratios[top]
+    if D < 2:
+        raise _lib.CasMVSError("inverse depth sampling needs at least 2 planes in the coarsest stage")
+    tensors = [t for t in (init_depth_min, depth_interval) if torch.is_tensor(t)]
+    dev = tensors[0].device if tensors else torch.device("cpu")
+    # the coarse stage's interval and far plane exactly as the uniform mode forms them
+    m = _depth_param(init_depth_min, B) if torch.is_tensor(init_depth_min) else \
+        torch.full((B,), float(init_depth_min), dtype=torch.float32, device=dev)
+    if torch.is_tensor(depth_interval):
+        step_top = _depth_param(depth_interval, B).to(m.device) * r_top
+    else:
+        step_top = torch.full((B,), float(depth_interval * r_top), dtype=torch.float32, device=m.device)
+    m = m.to(step_top.device)
+    far = m + step_top * float(D - 1)
+    bad = ~(torch.isfinite(m) & torch.isfinite(far) & (m > 0) & (far > m))
+    if m.device.type != "cuda" or not torch.cuda.is_current_stream_capturing():
+        if bool(bad.any()):
+            i = int(bad.nonzero()[0, 0])
+            raise _lib.CasMVSError(
+                "inverse depth sampling needs 0 < near < far, both finite: batch item "
+                f"{i} has near {float(m[i])}, far {float(far[i])} (init_depth_min, "
+                "init_depth_min + (n_depths-1)*depth_interval*ratio of the coarsest stage)")
+    u_near = 1.0 / m.double()
+    u_far = 1.0 / far.double()
+    s_top = (u_near - u_far) / (D - 1)
+    steps = [(s_top * interval_ratios[l] / r_top).float() for l in range(top + 1)]
+    u_near, u_far = u_near.float(), u_far.float()
+    if not tensors:
+        return InverseSteps(float(u_near[0]), float(u_far[0]), [float(s[0]) for s in steps], B)
+    dev = torch.device(device) if device is not None else m.device
+    return InverseSteps(u_near.to(dev), u_far.to(dev), [s.to(dev) for s in steps], B)
+
+
+def _scalar_or_tensor(x, device):
+    """float -> (value, None); tensor -> (0.0, a float32 copy on `device` when it lives elsewhere)."""
+    if not torch.is_tensor(x):
+        return float(x), None
+    return 0.0, x.reshape(-1).to(device=device, dtype=torch.float32).contiguous()
+
+
+def inverse_hypotheses(steps, level, n_depths, h, w, device, current_depth=None, first_only=False):
+    """Planes evenly spaced in inverse depth (README "Wide depth ranges").  current_depth None:
+    the coarsest stage, d_k = 1/(u_near - s*k); else current_depth (B,h/2,w/2) is upsampled x2
+    and u_0 = max(1/c + (D/2)*s, u_far + (D-1)*s), d_k = 1/(u_0 - s*k).  Returns the depths
+    (B,D,h,w), or with first_only=True (finer stages) u_0 (B,h,w), the first rung of an inverse
+    Ladder."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise _lib.CasMVSError(f"inverse_hypotheses runs on a CUDA device (no CPU fallback); got {device}")
+    with torch.cuda.device(device):
+        B, D = steps.B, n_depths
+        cur = None
+        if current_depth is not None:
+            _require_cuda(current_depth)
+            cur = current_depth.contiguous()
+            assert cur.shape == (B, h // 2, w // 2) and cur.device == device
+        elif first_only:
+            raise _lib.CasMVSError("inverse_hypotheses: first_only needs current_depth (the "
+                                   "coarsest stage's first rung is steps.u_near)")
+        # steps of CPU tensors (inverse_steps without a device) or of another GPU are copied here
+        uf, uf_dev = _scalar_or_tensor(steps.u_near, device)
+        ur, ur_dev = _scalar_or_tensor(steps.u_far, device)
+        s, s_dev = _scalar_or_tensor(steps.step[level], device)
+        planes = 1 if first_only else D
+        out = torch.empty((B, h, w) if first_only else (B, D, h, w), device=device, dtype=torch.float32)
+        check(_lib.load().casmvs_inverse_hypotheses_fwd(_ptr(cur), uf, _ptr(uf_dev), ur, _ptr(ur_dev), s,
+                                                        _ptr(s_dev), _ptr(out), planes, B, D, h, w,
+                                                        _stream()), "inverse_hypotheses")
+        return out
+
+
 # --------------------------------------------------------------------------- ladder forms
 class Ladder:
     """Hypotheses first + step*d of one cascade stage, never materialised as (B,D,h,w):
     `first` is a (B,h,w) tensor [per-pixel], a (B,) tensor [per batch item] or a float; `step` a
-    (B,) tensor or a float; D planes.  `materialize()` gives the tensor the public API takes."""
+    (B,) tensor or a float; D planes.  `materialize()` gives the tensor the public API takes.
+    inverse=True: the ladder is in inverse depth, the hypotheses are 1/(first - step*d) with
+    first and step in 1/depth units (inverse_hypotheses)."""
 
-    def __init__(self, first, step, D, B, h, w, device):
+    def __init__(self, first, step, D, B, h, w, device, inverse=False):
         self.first, self.step, self.D, self.B, self.h, self.w, self.device = first, step, D, B, h, w, device
+        self.inverse = inverse
 
     def _args(self):
         fm = fb = sb = None
@@ -373,6 +475,9 @@ class Ladder:
         first = self.first if torch.is_tensor(self.first) else torch.tensor(float(self.first), device=self.device)
         step = self.step if torch.is_tensor(self.step) else torch.tensor(float(self.step), device=self.device)
         first = first.view(self.B, 1, self.h, self.w) if first.dim() == 3 else first.reshape(-1, 1, 1, 1)
+        if self.inverse:
+            u = first - step.reshape(-1, 1, 1, 1) * d
+            return torch.reciprocal(u).expand(self.B, self.D, self.h, self.w).contiguous()
         return (first + step.reshape(-1, 1, 1, 1) * d).expand(self.B, self.D, self.h, self.w).contiguous()
 
 
@@ -397,7 +502,8 @@ def warp_cost_ladder(feats, proj_mats, ladder, num_groups=1, round_tf32=False, b
     fm, fb, f, sb, s = ladder._args()
     check(_lib.load().casmvs_warp_cost_ladder_fwd(_ptr(feats), _ptr(proj_mats.contiguous()), _ptr(fm),
                                                   _ptr(fb), f, _ptr(sb), s, _ptr(out),
-                                                  (1 if round_tf32 else 0) | (BLOCKED if blocked else 0),
+                                                  (1 if round_tf32 else 0) | (BLOCKED if blocked else 0)
+                                                  | (INVERSE_DEPTH if ladder.inverse else 0),
                                                   B, V, C, ladder.D, h, w, num_groups, _stream()),
           "warp_cost_ladder")
     return out if blocked else as_volume_view(out)
@@ -413,9 +519,10 @@ def regress_ladder(logits, ladder, want_index=False):
     conf = torch.empty_like(depth)
     index = torch.empty(B, h, w, device=lg.device, dtype=torch.int64) if want_index else None
     fm, fb, f, sb, s = ladder._args()
-    check(_lib.load().casmvs_regress_ladder_fwd(_ptr(lg), _ptr(fm), _ptr(fb), f, _ptr(sb), s,
-                                                _ptr(depth), _ptr(conf), _ptr(index), B, D, h, w,
-                                                _stream()), "regress_ladder")
+    lib = _lib.load()
+    fn = lib.casmvs_regress_ladder_inverse_fwd if ladder.inverse else lib.casmvs_regress_ladder_fwd
+    check(fn(_ptr(lg), _ptr(fm), _ptr(fb), f, _ptr(sb), s, _ptr(depth), _ptr(conf), _ptr(index),
+             B, D, h, w, _stream()), "regress_ladder")
     return depth, conf, index
 
 

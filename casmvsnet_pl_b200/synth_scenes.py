@@ -206,7 +206,7 @@ def _distorted(cam, model, coeffs):
 
 
 def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=0, n_single=20,
-                 n_dup=20, distortion=None, ext="jpg"):
+                 n_dup=20, distortion=None, ext="jpg", tilt=0.0):
     """The arc cameras of the other layouts as a COLMAP model (colmap.ColmapModel) looking at a
     known surface, z = depth + 0.05 depth sin(3x / depth) cos(2y / depth) in world coordinates,
     which every optical axis meets at depth `depth` (the cameras sit on a circle of that radius
@@ -216,7 +216,11 @@ def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=
     n_single tracks of length > 1 are cut to one view and n_dup others list their first view
     twice.  `distortion`, (model, coefficients) or {camera id: (model, coefficients)}, turns
     both cameras (or the ones named) into that COLMAP model with the same fx, fy, cx and cy
-    (tracks as without it); `ext` is the image names' extension."""
+    (tracks as without it); `ext` is the image names' extension.
+    tilt != 0 adds tilt*y to the surface's z: a slope that recedes towards the bottom of every
+    image (tilt > 0), so one view sees a wide range of depths (tilt 2.25 at the default focal
+    length: about 0.55 to 5.5 times `depth` from the top row to the bottom one); the points then
+    cover y in [-0.3, 2.2] * depth.  tilt = 0 gives the model it always gave."""
     from . import colmap
     rng = np.random.default_rng(seed)
     W, H = image_wh
@@ -238,8 +242,9 @@ def colmap_model(n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, seed=
         Ks.append(colmap.intrinsics(name, prm))
         whs.append((w, h))
     x = rng.uniform(-0.5, 0.5, n_points) * depth
-    y = rng.uniform(-0.3, 0.3, n_points) * depth
-    xyz = np.stack([x, y, depth + 0.05 * depth * np.sin(3 * x / depth) * np.cos(2 * y / depth)], 1)
+    y = rng.uniform(-0.3, 0.3, n_points) * depth if tilt == 0 else \
+        rng.uniform(-0.3, 2.2, n_points) * depth
+    xyz = np.stack([x, y, depth + tilt * y + 0.05 * depth * np.sin(3 * x / depth) * np.cos(2 * y / depth)], 1)
     tracks = []
     for p in xyz:
         tr = []
@@ -287,12 +292,13 @@ def sparse_tracks(n_img=300, n_pts=500_000, track_len=(3, 11), seed=0):
     return centres, xyz, ptr, img
 
 
-def height_field_depth(K, E, wh, depth=3.0):
+def height_field_depth(K, E, wh, depth=3.0, tilt=0.0):
     """Per-pixel depth (h,w) float64 of colmap_model's surface z = depth + 0.05 depth
     sin(3x / depth) cos(2y / depth) seen by a pinhole camera K (3,3), world->camera E (4,4) of
     size wh = (w, h): the camera z of the ray-surface intersection through each pixel centre,
     found by Newton's method in float64 (the surface's slope is at most 0.15, so from the
-    plane z = depth it converges in a few steps).  Also returns the world points (h,w,3)."""
+    plane z = depth it converges in a few steps).  tilt: colmap_model's tilt, the surface then
+    starts from the plane z = depth + tilt*y.  Also returns the world points (h,w,3)."""
     w, h = wh
     K, E = np.asarray(K, np.float64), np.asarray(E, np.float64)
     R, t = E[:3, :3], E[:3, 3]
@@ -300,12 +306,12 @@ def height_field_depth(K, E, wh, depth=3.0):
     ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
     r = np.einsum("ij,hwj->hwi", R.T @ np.linalg.inv(K), np.stack([xs, ys, np.ones_like(xs)], -1))
     a, b = 3.0 / depth, 2.0 / depth
-    s = (depth - C[2]) / r[..., 2]
+    s = (depth - C[2] + tilt * C[1]) / (r[..., 2] - tilt * r[..., 1])
     for _ in range(50):
         X = C + s[..., None] * r
-        hz = depth + 0.05 * depth * np.sin(a * X[..., 0]) * np.cos(b * X[..., 1])
+        hz = depth + tilt * X[..., 1] + 0.05 * depth * np.sin(a * X[..., 0]) * np.cos(b * X[..., 1])
         dhx = 0.05 * depth * a * np.cos(a * X[..., 0]) * np.cos(b * X[..., 1])
-        dhy = -0.05 * depth * b * np.sin(a * X[..., 0]) * np.sin(b * X[..., 1])
+        dhy = tilt - 0.05 * depth * b * np.sin(a * X[..., 0]) * np.sin(b * X[..., 1])
         g = X[..., 2] - hz
         step = g / (r[..., 2] - dhx * r[..., 0] - dhy * r[..., 1])
         s = s - step
@@ -354,6 +360,7 @@ def make_colmap(root, n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, 
         if kw.get("distortion") is not None:
             raise ValueError("textured views are rendered with pinhole cameras; no distortion")
         image_ext = "png"
+    tilt = kw.get("tilt", 0.0)
     model = colmap_model(n_views, image_wh, depth, n_points, seed, ext=image_ext, **kw)
     rng = np.random.default_rng(seed + 1)
     image_dir = image_dir or os.path.join(root, "images")
@@ -367,7 +374,7 @@ def make_colmap(root, n_views=8, image_wh=(160, 120), depth=3.0, n_points=2000, 
             E[:3, :3], E[:3, 3] = colmap.qvec_to_rotmat(q), t
             K = colmap.intrinsics(cam_name, prm)
             v = int(name[len("view_"):-len(".png")])
-            depths[v], X = height_field_depth(K, E, (w, h), depth)
+            depths[v], X = height_field_depth(K, E, (w, h), depth, tilt)
             img = surface_texture(X, seed + 1, K[0, 0] / depth)
         else:
             img = _image(rng, w, h)

@@ -137,6 +137,9 @@ def build_parser(depth_interval=2.65):
                     help="colmap: network input size, multiples of 32 (default 640 512)")
     ap.add_argument("--image_dir", type=str, default=argparse.SUPPRESS,
                     help="colmap: the images (default <root_dir>/images)")
+    ap.add_argument("--depth_sampling", choices=["uniform", "inverse"], default=argparse.SUPPRESS,
+                    help="plane spacing of the sweep: uniform (default) or inverse (evenly in "
+                         "1/depth, regressed in 1/depth); not stored in the checkpoint")
     return ap
 
 
@@ -319,7 +322,8 @@ def build_model(a, device):
     from . import InPlaceABN
     from .models.mvsnet import CascadeMVSNet
     model = CascadeMVSNet(n_depths=a.n_depths, interval_ratios=a.interval_ratios,
-                          num_groups=a.num_groups, norm_act=InPlaceABN, precision=a.precision)
+                          num_groups=a.num_groups, norm_act=InPlaceABN, precision=a.precision,
+                          depth_sampling=getattr(a, "depth_sampling", "uniform"))
     if a.ckpt_path:
         load_ckpt(model, a.ckpt_path, a.prefixes_to_ignore)
     return model.to(device).train()

@@ -70,6 +70,13 @@ enum casmvs_precision {
  * stored.  Without it every activation c0 .. u11 is left in the workspace. */
 #define CASMVS_FUSED_TAIL 1024
 
+/* Inverse-depth plane sweep (README "Wide depth ranges"; the rule is stated in regress.cu).
+ * OR-ed into casmvs_regress_fwd's input_is_prob: regress in 1/depth (depth = 1/sum p_d/dv_d).
+ * OR-ed into casmvs_regress_bwd's dv_is_vector: the gradient of that regression.
+ * OR-ed into casmvs_warp_cost_ladder_fwd's round_tf32: the ladder is in inverse depth, the
+ * hypotheses are 1/(first - step*d) (first and step in 1/depth units). */
+#define CASMVS_INVERSE_DEPTH 2048
+
 enum casmvs_conv_kind {
   CASMVS_CONV = 0,           /* Conv3d(k=3, pad=1, stride 1|2)   modules.py:26      */
   CASMVS_CONV_TRANSPOSE = 1, /* ConvTranspose3d(k=3,s=2,p=1,op=1) mvsnet.py:75,80,85 */
@@ -263,6 +270,24 @@ int casmvs_regress_ladder_fwd(const float* logits, const float* first_map, const
                               float first, const float* step_b, float step, float* depth,
                               float* confidence, int64_t* index, int B, int D, int h, int w,
                               void* stream);
+
+/* ---- inverse-depth forms (CASMVS_INVERSE_DEPTH) -----------------------------------------
+ * casmvs_inverse_hypotheses_fwd: planes evenly spaced in 1/depth, d_k = 1/(u_0 - step*k).
+ * cur == NULL: the coarsest stage, u_0 = u_first; planes must be D.
+ * cur (B,h/2,w/2): a finer stage; cur is upsampled x2 as in casmvs_depth_hypotheses_fwd and
+ * u_0 = max(1/c + (D/2)*step, u_far + (D-1)*step).  planes == D writes the depths (B,D,h,w);
+ * planes == 1 writes u_0 (B,h,w), the first rung of an inverse ladder.
+ * u_first_dev, u_far_dev, step_dev: (B) device values that override the scalars when non-NULL.
+ * casmvs_regress_ladder_inverse_fwd: casmvs_regress_ladder_fwd over the inverse ladder
+ * 1/(first - step*d), with the inverse regression. */
+int casmvs_inverse_hypotheses_fwd(const float* cur, float u_first, const float* u_first_dev,
+                                  float u_far, const float* u_far_dev, float step,
+                                  const float* step_dev, float* out, int planes, int B, int D,
+                                  int h, int w, void* stream);
+int casmvs_regress_ladder_inverse_fwd(const float* logits, const float* first_map,
+                                      const float* first_b, float first, const float* step_b,
+                                      float step, float* depth, float* confidence, int64_t* index,
+                                      int B, int D, int h, int w, void* stream);
 
 /* ---- FeatureNet top-down path, fused (adjacent to the hot path; SURVEY.md §8f-2) ----
  * One pyramid level of models/mvsnet.py:36-52:
