@@ -4,6 +4,8 @@
     rounded once to float32;
   * hypotheses_f32 / first_rung_f32: rules 3-4 with one float32 rounding per operation, in the
     kernels' order (numpy).  The kernels must equal these bit for bit;
+  * ladder_f32: the depths of an inverse ladder (first, step), the same way: the hypotheses the
+    K1 and K3 checks give their float64 references for a ladder call;
   * regress_f64 / regress_bwd_f64: rule 5 and its backward in float64;
   * cascade_forward_inverse: the cascade oracle (casmvs_oracle) with inverse hypotheses and the
     inverse regression.  The uniform cascade_forward stays the default.
@@ -90,6 +92,24 @@ def hypotheses_f32(steps, level, D, h, w, cur=None):
     k = np.arange(D, dtype=f32).reshape(1, -1, 1, 1)
     u = (u0[:, None] - (s * k).astype(f32)).astype(f32)
     return _rcp(u)
+
+
+def _np32(x):
+    if torch.is_tensor(x):
+        return x.detach().cpu().numpy().astype(f32)
+    return np.asarray(x, dtype=f32)
+
+
+def ladder_f32(first, step, D, B, h, w):
+    """The depths of an inverse ops.Ladder -> (B,D,h,w) float32, d_k = RN(1/RN(first - RN(step*k)))
+    (inverse_plane, k1_common.cuh).  first: a float, a (B,) or a (B,h,w) array or tensor in
+    1/depth; step: a float or a (B,) array or tensor."""
+    fa, sa = _np32(first), _np32(step)
+    u0 = fa.reshape(B, 1, h, w) if fa.ndim == 3 else np.broadcast_to(fa.reshape(-1, 1, 1, 1), (B, 1, 1, 1))
+    s = np.broadcast_to(sa.reshape(-1, 1, 1, 1), (B, 1, 1, 1))
+    k = np.arange(D, dtype=f32).reshape(1, -1, 1, 1)
+    u = (u0 - (s * k).astype(f32)).astype(f32)
+    return np.ascontiguousarray(np.broadcast_to(_rcp(u), (B, D, h, w)))
 
 
 def regress_f64(logits, dv):

@@ -31,6 +31,16 @@ terms); eps is the measured relative error of the kernels' fp32 reductions:
   ddepth = sum p delta |dv| + (sum p delta + u) |depth64|,
       bound0 = |g| p64 (ddepth + |dv - depth64| (delta_d + sum p delta + 4u)) SAFE,
       A = |g| p64 (sum p |dv| + |depth64| + |dv - depth64|).
+* Inverse mode (README "Wide depth ranges", regress.cu rule 5).  The kernels average
+  v_d = RN(1/dv_d), one IEEE float32 division the oracle takes exactly, so ubar = sum p_d v_d
+  carries the depth bound above with dv replaced by v.  depth = RN(1/ubar): with Dl = that bound
+  (eps included), |1/ubar~ - 1/ubar| <= Dl / (ubar (ubar - Dl)) = depth64^2 Dl ubar / (ubar - Dl),
+  plus half an ulp of the depth.  Index and confidence are the uniform mode's.
+  Backward: d depth / d l_d = -depth^2 p_d (v_d - ubar): the uniform bound of p_d (v_d - ubar) g
+  (regress_inv_bwd_kernel forms ubar = num / den as the uniform kernel forms its depth), scaled
+  by depth64^2, plus that term times the relative error of the kernel's depth^2: twice ubar's
+  (ddepth / ubar above, and 2 eps for its two sums) plus 4u (the reciprocal, the square and the
+  two products with it).
 * K4.  first = max(up(cur) - half, 1e-7f), out = first + step d.  up is the upsample of
   oracle/feature_fp64.py (position and blend bound); half = D/2 step is rounded once (the
   scalar path also rounds step itself: 2u |half|); the subtraction, the product and the sum add
@@ -56,6 +66,11 @@ def _dv(hyp, like):
     return dv.view(1, -1, 1, 1) if dv.dim() == 1 else dv
 
 
+def inverse_values(hyp):
+    """v = RN(1/hyp) in float32: what the inverse-mode kernels average (plane_value<true>)."""
+    return torch.div(1.0, hyp.detach().cpu().float()).to(hyp.device)
+
+
 def softmax_ref(logits, input_is_prob=False):
     """-> p64, its bound without eps dp0, the per-plane relative error delta of exp, and
     theta = sum p64 delta (all (B, D, h, w) but theta (B, 1, h, w))."""
@@ -76,9 +91,12 @@ def softmax_ref(logits, input_is_prob=False):
     return p, dp0, delta, theta
 
 
-def regress_ref(logits, hyp, input_is_prob=False):
+def regress_ref(logits, hyp, input_is_prob=False, inverse=False):
     """Float64 K3 without the index decision: dict of p, dp0, pA (the eps magnitude of p),
-    depth / fidx with their bound0 and A."""
+    depth / fidx with their bound0 and A.  inverse: 'depth' is ubar = sum p RN(1/hyp), the
+    average before the final reciprocal."""
+    if inverse:
+        hyp = inverse_values(hyp)
     p, dp0, _, _ = softmax_ref(logits, input_is_prob)
     pA = torch.zeros_like(p) if input_is_prob else p
     dv = _dv(hyp, p)
@@ -122,9 +140,11 @@ def confidence_ref(ref, index):
     return c[:, 0], b0[:, 0], A[:, 0]
 
 
-def regress_bwd_ref(logits, hyp, gdepth):
+def regress_bwd_ref(logits, hyp, gdepth, inverse=False):
     """Float64 gradient of sum(depth * gdepth) with respect to the logits: (B, D, h, w) g64,
-    bound0, A."""
+    bound0, A.  inverse: the inverse regression's, -depth^2 p (RN(1/hyp) - ubar) gdepth."""
+    if inverse:
+        hyp = inverse_values(hyp)
     p, _, delta, theta = softmax_ref(logits)
     dv = _dv(hyp, p)
     depth = (p * dv).sum(1, keepdim=True)
@@ -135,7 +155,14 @@ def regress_bwd_ref(logits, hyp, gdepth):
     b0 = g.abs() * p * (ddepth + diff.abs() * (delta + theta + 4 * ULP)) * SAFE
     b0 = b0 + g.abs() * ABS_E * (p.shape[1] + 2) * (dv.abs() + depth.abs())
     A = g.abs() * p * (sabs + depth.abs() + diff.abs())
-    return g * p * diff, b0, A
+    gu = g * p * diff
+    if not inverse:
+        return gu, b0, A
+    dep2 = depth ** -2                                     # depth = ubar here
+    rel = 2 * ddepth / depth.abs() + 4 * ULP
+    # SAFE once more: the product of depth^2's relative error with the error b0 already bounds
+    # is second order
+    return -dep2 * gu, dep2 * (b0 + gu.abs() * rel) * SAFE, dep2 * (A + 4 * gu.abs())
 
 
 # ------------------------------------------------------------------------------- K4
@@ -191,11 +218,20 @@ def check(y, y64, bound0, A, eps, names, scale=None):
 
 @torch.no_grad()
 def check_regress(logits, hyp, depth, conf, index=None, prob=None, input_is_prob=False,
-                  eps=2.0 ** -17):
+                  eps=2.0 ** -17, inverse=False):
     """Every output of one K3 call against float64 -> dict of Reports ('prob', 'depth',
     'conf') plus 'index': (number of wrong pixels, number of ambiguous pixels, first wrong
-    (b, y, x) or None)."""
-    ref = regress_ref(logits, hyp, input_is_prob)
+    (b, y, x) or None).  inverse: the call regressed in 1/depth (regress(..., inverse=True))."""
+    ref = regress_ref(logits, hyp, input_is_prob, inverse)
+    if inverse:
+        u, ub0, uA = ref["depth"], ref["depth_b0"], ref["depth_A"]
+        dl = ub0 + eps * uA
+        # a bound as large as ubar itself cannot be carried through 1/ubar: infinite there
+        grow = torch.where(dl < u, u / (u - dl), torch.full_like(u, float("inf")))
+        d64 = 1.0 / u
+        ref["depth"] = d64
+        ref["depth_b0"] = d64 ** 2 * ub0 * grow + ULP * d64
+        ref["depth_A"] = d64 ** 2 * uA * grow
     D = logits.shape[1]
     out = {}
     names3 = ("b", "y", "x")

@@ -169,7 +169,7 @@ CASCADES = {
 }
 RECORDED = ("conv2d_rgb8", "conv2d_planar", "conv2d_5x5s2", "conv2d_5x5s2_fp32", "fpn_merge",
             "fpn_level", "uniform_hypotheses", "depth_hypotheses", "depth_first", "warp_cost",
-            "warp_cost_ladder", "costreg", "regress", "regress_ladder")
+            "warp_cost_ladder", "costreg", "regress", "regress_ladder", "inverse_hypotheses")
 _CHUNK = 1 << 26
 
 
@@ -189,11 +189,13 @@ def _digest(t):
 
 def _leaves(obj):
     """The values of a call's arguments or result that carry data: tensors and floats (a Ladder
-    by its first rung and step).  Ints and flags are shapes and modes, equal by construction."""
+    by its first rung and step, InverseSteps by u_near, u_far and the steps).  Ints and flags are shapes and modes, equal by construction."""
     if torch.is_tensor(obj) or isinstance(obj, float):
         return [obj]
     if isinstance(obj, ops.Ladder):
         return _leaves(obj.first) + _leaves(obj.step)
+    if isinstance(obj, ops.InverseSteps):
+        return _leaves(obj.u_near) + _leaves(obj.u_far) + _leaves(list(obj.step))
     if isinstance(obj, (tuple, list)):
         return [x for o in obj for x in _leaves(o)]
     if isinstance(obj, dict):

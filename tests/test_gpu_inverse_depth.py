@@ -4,8 +4,8 @@
     oracle/inverse_depth_fp64.py bit for bit: coarse and fine stages, the far clamp, float and
     per-batch device depth parameters, D in {8, 32, 48}, ratios (1, 2, 4) and (1, 2.5, 5.5);
   * rule 1's refusal for device tensors;
-  * the fused ladder path and the materialised path give the same depth and confidence bits;
-  * K3's inverse forward and backward against float64;
+  * the fused ladder path and the materialised path give the same depth and confidence bits
+    (K3's inverse forward and backward against float64: test_gpu_regress_fp64.py);
   * the cascade in inverse mode against the inverse cascade oracle at 640x512 (V = 3) and
     1152x864 (V = 5), fp32 and tf32, with the full-size parity test's bounds;
   * steps held in CPU tensors are copied to the device;
@@ -22,7 +22,6 @@ from oracle import inverse_depth_fp64 as INV
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-EPS = 2.0 ** -23
 
 
 def _params(kind, B):
@@ -94,54 +93,6 @@ def test_ladder_equals_materialised(size, precision, G):
         assert torch.equal(out[True][k], out[False][k]), k
     d = out[True]["depth_0"]
     assert bool(torch.isfinite(d).all())
-
-
-def test_regress_inverse_vs_fp64():
-    """depth = 1/sum p_k/d_k.  Each of the D products and sums rounds once (Cascade16), the two
-    reciprocals once each: |depth - depth64| <= (D + 3) eps depth."""
-    g = torch.Generator(device=DEV).manual_seed(5)
-    st = ops.inverse_steps(1.5, 0.38, (8, 32, 48), (1, 2, 4), 2)
-    for D, level, h, w in ((48, 2, 128, 160), (32, 1, 256, 320), (8, 0, 512, 640)):
-        cur = None if level == 2 else 1.5 + 70 * torch.rand(2, h // 2, w // 2, generator=g, device=DEV)
-        dv = ops.inverse_hypotheses(st, level, D, h, w, DEV, current_depth=cur)
-        for scale in (1.0, 4.0):
-            logits = torch.randn(2, D, h, w, generator=g, device=DEV) * scale
-            depth, conf, index, _ = ops.regress(logits, dv, want_index=True, inverse=True)
-            d64, c64, i64, _, _ = INV.regress_f64(logits, dv)
-            err = (depth.double().cpu() - d64).abs() / d64
-            assert float(err.max()) <= (D + 3) * EPS, (D, float(err.max()))
-            same = index.cpu() == i64
-            assert float((~same).double().mean()) < 2 ** -10
-            # four probabilities of magnitude <= 1, each within a few ulp, summed in order
-            assert float((conf.double().cpu() - c64).abs()[same].max()) <= 16 * EPS
-            if cur is None:
-                continue
-            first = ops.inverse_hypotheses(st, level, D, h, w, DEV, current_depth=cur, first_only=True)
-            lad = ops.Ladder(first, st.step[level], D, 2, h, w, DEV, inverse=True)
-            dl, cl, il = ops.regress_ladder(logits, lad, want_index=True)
-            assert torch.equal(dl, depth) and torch.equal(cl, conf) and torch.equal(il, index)
-
-
-def test_regress_inverse_backward_vs_fp64():
-    from casmvsnet_pl_b200 import autograd as AG
-    g = torch.Generator(device=DEV).manual_seed(6)
-    st = ops.inverse_steps(1.5, 0.38, (8, 32, 48), (1, 2, 4), 2)
-    for D, level, h, w in ((48, 2, 128, 160), (8, 0, 512, 640)):
-        cur = None if level == 2 else 1.5 + 70 * torch.rand(2, h // 2, w // 2, generator=g, device=DEV)
-        dv = ops.inverse_hypotheses(st, level, D, h, w, DEV, current_depth=cur)
-        logits = (torch.randn(2, D, h, w, generator=g, device=DEV) * 4).requires_grad_()
-        gd = torch.randn(2, h, w, generator=g, device=DEV)
-        with torch.enable_grad():
-            depth, _ = AG.regress(logits, dv, inverse=True)
-            depth.backward(gd)
-        g64 = INV.regress_bwd_f64(logits.detach(), dv, gd)
-        # every term is depth^2 p_k |1/d_k - ubar| |grad| times a few roundings; the sums over D
-        # add D roundings of the largest term
-        d64 = INV.regress_f64(logits.detach(), dv)[0]
-        scale = (d64 ** 2).unsqueeze(1) * (1.0 / dv.double().cpu()).amax(1, keepdim=True) * \
-            gd.double().cpu().abs().unsqueeze(1)
-        err = (logits.grad.double().cpu() - g64).abs()
-        assert bool((err <= (2 * D + 16) * EPS * scale + 1e-30).all()), (D, float((err / scale).max()))
 
 
 FULL = {   # the benchmarked sizes: test_gpu_cascade.py's FULL_CONFIGS cfg2 and cfg4_view

@@ -1,9 +1,12 @@
 """Training in the inverse-depth mode (README "Wide depth ranges"):
 
-  * one train.Trainer step with --depth_sampling inverse, every autograd call recorded as
-    test_gpu_train_step_fp64.py records them: the convolutions and K1 checked with that file's
-    float64 checks, K3 (RegressInverseFn) forward and backward against the inverse regression in
-    float64 (oracle/inverse_depth_fp64.py).  The recorded hypotheses are the inverse planes;
+  * train.Trainer steps with --depth_sampling inverse (640x512 in fp32 and tf32, the shape
+    sweep's training cases, and 768x576 at B = 2 with per-item depth ranges), every autograd
+    call recorded as test_gpu_train_step_fp64.py records them: the convolutions and K1 checked with that file's
+    float64 checks, K3 (RegressInverseFn) forward and backward with test_gpu_regress_fp64.py's
+    per-element checks of the inverse regression.  Every stage's recorded hypotheses equal rules
+    3-4 restated in float32 (oracle/inverse_depth_fp64.py) bit for bit, a finer stage's on the
+    previous stage's recorded depth;
   * two `train --depth_sampling inverse --deterministic --seed 0` processes, with the sl1 loss on
     a DTU-layout set and with the photometric loss on a COLMAP capture, write the same log and
     checkpoint bits, and the checkpoints differ from a uniform run's."""
@@ -14,16 +17,18 @@ import sys
 import pytest
 import torch
 
+import test_gpu_regress_fp64 as R
+import test_gpu_shape_sweep_fp64 as SW
 import test_gpu_train_step_fp64 as T
 from casmvsnet_pl_b200 import _lib, ops, synth_scenes, train
 from casmvsnet_pl_b200 import autograd as AG
 from oracle import inverse_depth_fp64 as INV
+from oracle import regress_fp64 as RG
 from oracle import warp_cost_fp64 as W
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EPS = 2.0 ** -23
 
 
 @pytest.fixture(autouse=True)
@@ -76,9 +81,11 @@ def _check_k1_k3_inverse(case, rec, steps, n_depths):
     for i, c in enumerate(rec.warp):
         tag = f"{case} L{T.LEVELS[i]}"
         B, V, h, w, C = c["f"].shape
-        if i == 0:          # the coarsest stage's planes are known in advance: rule 3, bit for bit
-            want = INV.hypotheses_f32(steps, T.LEVELS[i], n_depths[T.LEVELS[i]], h, w)
-            assert torch.equal(c["dv"].cpu(), torch.from_numpy(want.copy())), tag
+        # rules 3-4 bit for bit: the coarsest stage's planes are known in advance, a finer
+        # stage's follow from the previous stage's recorded depth
+        cur = None if i == 0 else rec.reg[i - 1]["depth"].cpu().numpy()
+        want = INV.hypotheses_f32(steps, T.LEVELS[i], n_depths[T.LEVELS[i]], h, w, cur)
+        assert torch.equal(c["dv"].cpu(), torch.from_numpy(want.copy())), tag
         fam = "staged" if ops.ladder_supported(V, C, c["G"]) else "gather"
         rep = W.check_cost(c["cost"], c["f"], c["P"], c["dv"], c["G"], T.EPS_K1[fam])
         print(f"[inverse train-fp64] {tag} warp_cost [{fam}]: {rep.describe()}")
@@ -90,47 +97,55 @@ def _check_k1_k3_inverse(case, rec, steps, n_depths):
         assert rep.ok, f"{tag} warp_cost_bwd: {rep.describe()}"
     for i, c in enumerate(rec.reg):
         tag = f"{case} L{T.LEVELS[i]}"
-        D = c["logits"].shape[1]
         depth, conf, index, _ = ops.regress(c["logits"], c["dv"], want_index=True, inverse=True)
         assert torch.equal(depth, c["depth"]) and torch.equal(conf, c["conf"]), tag
-        d64, c64, i64, _, _ = INV.regress_f64(c["logits"], c["dv"])
-        err = float(((c["depth"].double().cpu() - d64).abs() / d64).max())
-        print(f"[inverse train-fp64] {tag} regress depth: max rel err {err:.3e}")
-        # D products and sums rounded once each (Cascade16), two reciprocals
-        assert err <= (D + 3) * EPS, tag
-        same = index.cpu() == i64
-        assert float((~same).double().mean()) < 2 ** -10, tag
-        assert float((conf.double().cpu() - c64).abs()[same].max()) <= 16 * EPS, tag
+        # test_gpu_regress_fp64.py's per-element checks of the inverse regression
+        R._check_k3(f"[inverse train] {tag}", c["logits"], c["dv"], depth, conf, index,
+                    inverse=True)
         b = rb[i]
-        g64 = INV.regress_bwd_f64(c["logits"], c["dv"], b["gdepth"])
-        scale = (d64 ** 2).unsqueeze(1) * (1.0 / c["dv"].double().cpu()).amax(1, keepdim=True) * \
-            b["gdepth"].double().cpu().abs().unsqueeze(1)
-        e = (b["glogits"].double().cpu() - g64).abs()
-        worst = float((e / (scale + 1e-300)).max())
-        print(f"[inverse train-fp64] {tag} regress_bwd: worst err / scale {worst:.3e}")
-        assert bool((e <= (2 * D + 16) * EPS * scale + 1e-30).all()), tag
+        g64, b0, A = RG.regress_bwd_ref(c["logits"], c["dv"], b["gdepth"], inverse=True)
+        R._report(f"[inverse train] {tag} bwd", "k3_inv_bwd",
+                  RG.check(b["glogits"], g64, b0, A, R.EPS["k3_inv_bwd"], ("b", "d", "y", "x")))
 
 
-@pytest.mark.parametrize("precision", ["fp32", "tf32"])
-def test_inverse_training_step_vs_fp64(precision, rec_inv):
-    case = f"dtu_{precision}_inverse"
+def _inverse_step(case, rec_inv, precision, W_, H, V=3, G=1, n_depths=(8, 32, 48), B=1):
     a = train.build_parser().parse_args(["--precision", precision, "--optimizer", "sgd",
-                                         "--depth_sampling", "inverse"])
+                                         "--depth_sampling", "inverse", "--num_groups", str(G),
+                                         "--n_views", str(V), "--n_depths", *map(str, n_depths)])
     torch.manual_seed(0)
     model = train.build_model(a, DEV)
     assert model.depth_sampling == "inverse"
     tr = train.Trainer(a, model, DEV)
-    s = T._sample(1, 640, 512, seed=1)
+    s = T._sample(B, W_, H, seed=1, V=V)
+    if B > 1:           # per-item depth ranges: per-item steps in every stage
+        s["init_depth_min"] = torch.tensor([[425.0 + 26.5 * b] for b in range(B)], device=DEV)
+        s["depth_interval"] = torch.tensor([[2.65 + 0.4 * b] for b in range(B)], device=DEV)
     f0 = _lib.fallback_count()
     loss, _ = tr.train_step(s)
     torch.cuda.synchronize()
     assert torch.isfinite(loss).item()
-    steps = INV.steps_f32(s["init_depth_min"], s["depth_interval"], a.n_depths, a.interval_ratios, 1)
+    steps = INV.steps_f32(s["init_depth_min"], s["depth_interval"], a.n_depths, a.interval_ratios, B)
     with torch.no_grad():
         fallbacks = T._check_conv_calls(case, rec_inv, precision == "tf32")
-        want = T._expected_fallbacks(precision == "tf32", 1)
-        assert fallbacks == want and _lib.fallback_count() - f0 == len(want)
+        want = T._expected_fallbacks(precision == "tf32", G)
+        assert fallbacks == want and _lib.fallback_count() - f0 == len(want), (fallbacks, want)
         _check_k1_k3_inverse(case, rec_inv, steps, a.n_depths)
+
+
+@pytest.mark.parametrize("precision", ["fp32", "tf32"])
+def test_inverse_training_step_vs_fp64(precision, rec_inv):
+    _inverse_step(f"dtu_{precision}_inverse", rec_inv, precision, 640, 512)
+
+
+# test_gpu_shape_sweep_fp64.py's training cases (G = 2, G = 4; V = 4 with odd D/8 on the gather
+# K1 path), and a 768x576 step at B = 2 with per-item depth ranges
+TRAIN_CASES = {**SW.TRAIN_CASES, "blendedmvs_b2": (768, 576, 3, 1, (8, 32, 48), 2)}
+
+
+@pytest.mark.parametrize("case", list(TRAIN_CASES))
+def test_inverse_training_cases_vs_fp64(case, rec_inv):
+    W_, H, V, G, Ds, *B = TRAIN_CASES[case]
+    _inverse_step(f"{case}_inverse", rec_inv, "tf32", W_, H, V, G, Ds, B[0] if B else 1)
 
 
 # ------------------------------------------------------------------------------- the CLI

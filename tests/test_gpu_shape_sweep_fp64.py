@@ -20,6 +20,12 @@ library call recorded.  Then:
     asserts it is the only layer on the CUDA-core kernel and checks it at the `direct` eps;
   * four cases again in the fp32 precision; the B = 3 cases equal three B = 1 forwards bit for
     bit (test_gpu_cfg5_batch_fp64's call digests name the first library call that differs);
+  * the *_inv cases with the inverse-depth sweep (README "Wide depth ranges"), together over
+    G in {1, 2, 4, 8}, V in {2, 3, 4, 9}, odd D/8, D = 192, 32x32 and 2048x96, B = 3 with
+    distinct (B, 1) depth ranges, interval ratios (1, 2.5, 5.5) and a far / near ratio >= 10
+    (wide_range).  K1 takes its hypotheses from INV.ladder_f32, K3 and K4 the inverse checks of
+    test_gpu_regress_fp64; FeatureNet's calls must equal the uniform run's bit for bit, and
+    CostRegNet's fused tail the two-layer re-run bit for bit, per element on costreg_fp64 cases;
   * odd-D stage shapes under CASMVS_TMA_DCHUNK = 1, 2, 3 in child processes: every layer within
     eps and the fused tail bit-identical to the two-layer path under every chunking;
   * a training step at num_groups 2, num_groups 4 and D = 8 / 24 / 56 with 4 views, through
@@ -79,7 +85,22 @@ CASES = {
                             edges=("large",)),
     "960x544_g4_v9_d56": dict(W=960, H=544, V=9, G=4, Ds=(8, 56, 24), B=1, fp32=False,
                               edges=("d8_odd", "generic_k1")),
+    # the inverse-depth sweep; depth=(init_depth_min, depth_interval) where not synth's DTU range
+    "32x32_g8_b3_inv": dict(W=32, H=32, V=3, G=8, Ds=(8, 16, 24), B=3, fp32=False,
+                            sampling="inverse", costreg_fp64=True,
+                            edges=("d8_odd", "conv5_1x1", "batch3")),
+    "2048x96_g2_wide_inv": dict(W=2048, H=96, V=2, G=2, Ds=(8, 24, 56), B=1, fp32=False,
+                                sampling="inverse", depth=(100.0, 1400.0 / (55 * 4)),
+                                edges=("aspect", "d8_odd", "wide_range")),
+    "800x608_g4_v4_ratios_inv": dict(W=800, H=608, V=4, G=4, Ds=(8, 32, 56), B=1, fp32=False,
+                                     sampling="inverse", ratios=(1, 2.5, 5.5),
+                                     edges=("d8_odd", "conv5_25x19")),
+    "1152x864_d192_inv": dict(W=1152, H=864, V=3, G=1, Ds=(8, 32, 192), B=1, fp32=False,
+                              sampling="inverse", edges=("many_chunks",)),
+    "960x544_g4_v9_inv": dict(W=960, H=544, V=9, G=4, Ds=(8, 56, 24), B=1, fp32=False,
+                              sampling="inverse", edges=("d8_odd", "generic_k1")),
 }
+INV_CASES = [n for n, c in CASES.items() if c.get("sampling") == "inverse"]
 TAIL_CHUNK = 16            # the fused tail's largest depth chunk, in u9 slices (conv3d_tail.cu)
 
 
@@ -87,6 +108,12 @@ def stages(c):
     """level -> (Cin as CostRegNet takes it, D, h, w); level 2 is the coarse stage."""
     return {l: (c["G"] if c["G"] > 1 else 8 << l, c["Ds"][l], c["H"] >> l, c["W"] >> l)
             for l in range(3)}
+
+
+def depth_range(c):
+    """(near, far) of the coarse stage: init_depth_min and its last uniform plane."""
+    dmin, dint = c.get("depth", (synth.DEPTH_MIN, synth.DEPTH_INTERVAL))
+    return dmin, dmin + (c["Ds"][2] - 1) * dint * c.get("ratios", (1, 2, 4))[2]
 
 
 def conv5_dims(c):
@@ -110,6 +137,8 @@ EDGES = {
     "batch3": lambda c: c["B"] == 3,
     # 8 source views: no gather instantiation (1, 2, 4, 6 sources), the run-time-V kernel
     "generic_k1": lambda c: c["V"] - 1 not in (1, 2, 4, 6),
+    # the range the inverse sweep exists for
+    "wide_range": lambda c: depth_range(c)[1] >= 10 * depth_range(c)[0],
 }
 RUNS = [(n, "tf32") for n in CASES] + [(n, "fp32") for n, c in CASES.items() if c["fp32"]]
 BATCH_CASES = [n for n, c in CASES.items() if c["B"] > 1]
@@ -140,8 +169,9 @@ def sweep_rec(monkeypatch):
 def _model(c, precision):
     from casmvsnet_pl_b200.models.mvsnet import CascadeMVSNet
     torch.manual_seed(0)
-    m = CascadeMVSNet(n_depths=list(c["Ds"]), num_groups=c["G"], norm_act=ABN,
-                      precision=precision)
+    m = CascadeMVSNet(n_depths=list(c["Ds"]), interval_ratios=list(c.get("ratios", (1, 2, 4))),
+                      num_groups=c["G"], norm_act=ABN, precision=precision,
+                      depth_sampling=c.get("sampling", "uniform"))
     synth.randomize_model_(m, 0)
     m = m.eval().to(DEV)
     m.return_index = True
@@ -159,7 +189,7 @@ def check_k1_call(tag, rec_, name, a, k, out, worst):
     B, V, C, h, w = feats.shape
     if name == "warp_cost_ladder":
         y = R.from_blocked(out) if k.get("blocked", False) else ops.volume_storage(out)
-        dv, fam = hyp.materialize(), "staged"
+        dv, fam = REG_T.ladder_hyp(hyp), "staged"
         unrounded = lambda: rec_.orig[name](feats, P, hyp, G, round_tf32=False)   # noqa: E731
     else:
         y, dv = ops.volume_storage(out), hyp
@@ -221,7 +251,24 @@ def _assert_bits(tag, got, want):
                             f"(b,d,h,w)={tuple(int(i) for i in diff.nonzero()[0])}")
 
 
-def check_costreg_call(tag, a, k, out, fb, G, worst):
+def _clone(out):
+    if torch.is_tensor(out):
+        return out.clone()
+    if isinstance(out, (tuple, list)):
+        return type(out)(_clone(t) for t in out)
+    return out
+
+
+def _same_bits(x, y):
+    if torch.is_tensor(x):
+        return torch.is_tensor(y) and x.shape == y.shape and torch.equal(
+            x.contiguous().view(torch.int32), y.contiguous().view(torch.int32))
+    if isinstance(x, (tuple, list)):
+        return len(x) == len(y) and all(_same_bits(a, b) for a, b in zip(x, y))
+    return x == y
+
+
+def check_costreg_call(tag, a, k, out, fb, G, worst, elements=True):
     x, params, cin = a[:3]
     prec = a[3] if len(a) > 3 else k.get("precision", ops.FP32)
     blocked_in = k.get("blocked", False)
@@ -248,6 +295,8 @@ def check_costreg_call(tag, a, k, out, fb, G, worst):
     assert fb2 == fb, f"{tag}: re-run made {fb2} fallback launches, the cascade {fb}"
     tail = bool(_lib.load().casmvs_costreg_tail_supported(cin, prec))
     _assert_bits(f"{tag} {'fused tail' if tail else 'logits'} vs two-layer re-run", out, logits)
+    if not elements:
+        return tail
     # the driver stores its activations blocked wherever every layer has a tensor-core kernel,
     # whatever the input's layout
     xb = R.to_blocked(xs) if ws_blocked and not blocked_in else xs
@@ -271,6 +320,11 @@ def test_cascade_calls_vs_fp64(case, precision, sweep_rec, monkeypatch):
     t0 = time.time()
     model = _model(c, precision)
     imgs, pm, dmin, dint = synth.make_inputs(B=c["B"], V=c["V"], W=c["W"], H=c["H"], seed=c["B"])
+    inverse = c.get("sampling") == "inverse"
+    dmin, dint = c.get("depth", (dmin, dint))
+    if inverse and c["B"] > 1:           # per-item ranges: the ladders' first_b / step_b
+        dmin = torch.tensor([[dmin + 2.5 * i] for i in range(c["B"])], device=DEV)
+        dint = torch.tensor([[dint * (1.0 + 0.05 * i)] for i in range(c["B"])], device=DEV)
     f0 = _lib.fallback_count()
     model(imgs.to(DEV), pm.to(DEV), dmin, dint)
     torch.cuda.synchronize()
@@ -288,16 +342,29 @@ def test_cascade_calls_vs_fp64(case, precision, sweep_rec, monkeypatch):
     tag = f"{case} {precision}"
     worst = {}
     tails = 0
+    if inverse:
+        # the same images through FeatureNet: the uniform run's calls, bit for bit
+        feat = [(n, _clone(out)) for n, _, _, out, _ in calls if n in FEAT_T.RECORDED]
+        model.set_depth_sampling("uniform")
+        model(imgs.to(DEV), pm.to(DEV), dmin, dint)
+        torch.cuda.synchronize()
+        uni = [(n, out) for n, _, _, out, _ in sweep_rec.calls if n in FEAT_T.RECORDED]
+        sweep_rec.calls.clear()
+        assert [n for n, _ in feat] == [n for n, _ in uni], tag
+        for i, ((n, x), (_, y)) in enumerate(zip(feat, uni)):
+            assert _same_bits(x, y), f"{tag}: FeatureNet call {i} ({n}) differs from the uniform run"
     for name, a, k, out, fb in calls:
         if name in FEAT_T.RECORDED:
-            FEAT_T.check_call(sweep_rec, name, a, k, out, tag)
-            torch.cuda.empty_cache()
+            if not inverse:
+                FEAT_T.check_call(sweep_rec, name, a, k, out, tag)
+                torch.cuda.empty_cache()
         elif name in REG_T.RECORDED:
             REG_T.check_call(name, a, k, out, tag)
         elif name == "costreg":
             D = out.shape[1]
             tails += check_costreg_call(f"{tag} costreg D={D} {tuple(out.shape[2:])} B={c['B']}",
-                                        a, k, out, fb, c["G"], worst)
+                                        a, k, out, fb, c["G"], worst,
+                                        elements=c.get("costreg_fp64", not inverse))
             torch.cuda.empty_cache()
         else:
             check_k1_call(f"{tag} {name} D={a[2].D if name == 'warp_cost_ladder' else a[2].shape[1]}"
@@ -321,6 +388,7 @@ def test_batch_equals_single_forwards(case, monkeypatch):
     c = CASES[case]
     B = c["B"]
     model = _model(c, "tf32")
+    # each view with its own (1, 1) depth range tensors
     views = [CFG5._view(c, i) for i in range(B)]
     rec_ = CFG5._CallDigests(monkeypatch)
     singles, records = [], []
@@ -501,6 +569,14 @@ def test_case_table_edges():
     for name, (cin, B, D, h, w) in DCHUNK_SHAPES.items():
         assert D // 8 % 2 == 1 and D > 8 and h % 8 == 0 and w % 8 == 0, name
     assert TRAIN_CASES["blendedmvs_v4_d8_24_56"][4][1] // 8 % 2 == 1
+    inv = [CASES[n] for n in INV_CASES]
+    assert {c["G"] for c in inv} == {1, 2, 4, 8} and {c["V"] for c in inv} >= {2, 3, 4, 9}
+    assert any(D // 8 % 2 and D > 8 for c in inv for D in c["Ds"])
+    assert any(c["Ds"][2] == 192 for c in inv) and any(c["B"] == 3 for c in inv)
+    assert {(c["W"], c["H"]) for c in inv} >= {(32, 32), (2048, 96)}
+    assert any(c.get("ratios") == (1, 2.5, 5.5) for c in inv)
+    assert any("wide_range" in c["edges"] for c in inv)
+    assert any(c.get("costreg_fp64") for c in inv)
 
 
 _ODD = (8, 1, 24, 16, 16)        # Cin, B, D, h, w: D/8 = 3

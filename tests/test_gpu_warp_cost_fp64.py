@@ -5,7 +5,14 @@
     V=3, G=1 / 8) at all three levels through warp_cost_ladder in its three hypothesis forms,
     TF32-rounded and blocked as well as channels-last fp32; cfg4 (1152x864, V=5) and cfg5
     (1920x1056, V=7) through ops.warp_cost with the materialised hypotheses;
-  * every instantiation: the 24 TMA-staged kernels, the 68 gather kernels (1, 2, 4, 6 source
+  * the inverse-depth sweep (README "Wide depth ranges") through the same entry point: the cfg2 /
+    cfg3 stages with a float u_near, per-item (B,) first and step and a (B, h, w) first map, and
+    the staging geometries at 1 and 2 source views, C in {8, 16, 32}, G in {1, 8}, among them
+    two asserted by construction on the CPU (INV_EDGES): inverse-wide (far / near >= 10, a pair
+    of near planes already spans more than the staged box, so stage_boxes halves its runs) and
+    inverse-behind (part of the near sweep has q_z <= 1e-7).  The oracle's hypotheses come from
+    INV.ladder_f32, which Ladder.materialize() must equal bit for bit;
+  * every instantiation: the 48 TMA-staged kernels (24 uniform, 24 inverse), the 68 gather kernels (1, 2, 4, 6 source
     views x C in {8, 16, 32, other} x variance / group-wise x NCHW / NHWC output, plus the
     generic run-time-V kernel), both homo_warp kernels and the NCHW-feature transpose, at
     ragged shapes, h or w = 2, D = 1, odd D and D not a multiple of the depth chunk, under
@@ -31,6 +38,7 @@ import pytest
 import torch
 
 from casmvsnet_pl_b200 import _lib, ops, synth
+from oracle import inverse_depth_fp64 as INV
 from oracle import warp_cost_fp64 as W
 
 pytestmark = pytest.mark.gpu
@@ -108,8 +116,49 @@ def _first_map(g, B, h, w, D, step, kind):
     return first.contiguous()
 
 
-def _hyp(g, kind, B, D, h, w, step):
+# near / far depth of the inverse ladders: the DTU range of synth.make_inputs; wide: a ratio of
+# 12 whose near plane still lands in the source image while one plane step of a short sweep
+# moves a sample by more than a staged box; behind: a ratio of 12 across the depth (about 600)
+# where the behind_view camera's q_z changes sign (INV_EDGES)
+_INV_RANGE = {"dtu": (synth.DEPTH_MIN, synth.DEPTH_MIN + 47 * 4 * synth.DEPTH_INTERVAL),
+              "wide": (90.0, 1080.0), "behind": (300.0, 3600.0)}
+assert _INV_RANGE["wide"][1] >= 10 * _INV_RANGE["wide"][0]
+
+
+def _inv_ladder(g, kind, B, D, h, w, level):
+    """An inverse ops.Ladder (first and step in 1/depth): the coarse stage's u_near and step as
+    floats (inv_float) or per item over distinct ranges (inv_batch, inv_wide), or a per-pixel
+    first rung (inv_map, inv_behind) from a smooth depth field spanning the range geometrically,
+    rule 4's far clamp applied.  Ladders over the DTU range with 8, 32 or 48 planes take
+    ops.inverse_steps's steps for (8, 32, 48) planes; the others sweep their range in D planes."""
+    near, far = _INV_RANGE[{"inv_wide": "wide", "inv_behind": "behind"}.get(kind, "dtu")]
+    nb = [near * (1 + 0.06 * b) for b in range(B)]
+    fb = [far * (1 + 0.1 * b) for b in range(B)]
+    dtu = kind in ("inv_float", "inv_batch") or (kind == "inv_map" and D in (8, 32, 48))
+    Ds, ratios = ((8, 32, 48), (1, 2, 4)) if dtu else ((D, D, D), (1, 1, 1))
+    per = kind != "inv_float"
+    dmin = torch.tensor(nb[:B] if per else nb[:1]).view(-1, 1)
+    dint = torch.tensor([(f - n) / ((Ds[2] - 1) * ratios[2]) for n, f in zip(nb, fb)][:B if per else 1]).view(-1, 1)
+    st = ops.inverse_steps(dmin if per else float(dmin), dint if per else float(dint), Ds, ratios,
+                           B, DEV)
+    if kind in ("inv_float", "inv_batch", "inv_wide"):      # floats or (B,) tensors
+        return ops.Ladder(st.u_near, st.step[level], D, B, h, w, DEV, inverse=True)
+    ys = torch.arange(h, device=DEV, dtype=torch.float32).view(1, h, 1)
+    xs = torch.arange(w, device=DEV, dtype=torch.float32).view(1, 1, w)
+    bb = torch.arange(B, device=DEV, dtype=torch.float32).view(B, 1, 1)
+    t = 0.5 + 0.5 * torch.sin(xs / 23.0 + bb) * torch.cos(ys / 17.0)
+    t = (t + 0.05 * torch.rand(B, h, w, generator=g, device=DEV)).clamp(0, 1)
+    nt, ft = torch.tensor(nb, device=DEV).view(B, 1, 1), torch.tensor(fb, device=DEV).view(B, 1, 1)
+    depth = nt * (ft / nt) ** t
+    s = st.step[level].view(B, 1, 1)
+    first = torch.maximum(1 / depth + D / 2 * s, st.u_far.view(B, 1, 1) + (D - 1) * s)
+    return ops.Ladder(first.contiguous(), st.step[level], D, B, h, w, DEV, inverse=True)
+
+
+def _hyp(g, kind, B, D, h, w, step, level=0):
     """-> ops.Ladder, or a (B, D, h, w) tensor for the public warp_cost."""
+    if kind.startswith("inv_"):
+        return _inv_ladder(g, kind, B, D, h, w, level)
     if kind == "float":
         return ops.Ladder(425.0, step, D, B, h, w, DEV)
     if kind == "batch":
@@ -133,7 +182,14 @@ def _hyp(g, kind, B, D, h, w, step):
 
 
 def _hyp_tensor(hyp):
-    return hyp.materialize() if isinstance(hyp, ops.Ladder) else hyp
+    if not isinstance(hyp, ops.Ladder):
+        return hyp
+    m = hyp.materialize()
+    if not hyp.inverse:
+        return m
+    want = torch.from_numpy(INV.ladder_f32(hyp.first, hyp.step, hyp.D, hyp.B, hyp.h, hyp.w)).to(DEV)
+    assert torch.equal(m, want), "inverse Ladder.materialize() != INV.ladder_f32"
+    return want
 
 
 # ------------------------------------------------------------------------------- case table
@@ -156,6 +212,11 @@ for _G, _cfg in ((1, "cfg2"), (8, "cfg3")):
     _add(f"{_cfg}_L2_batch", "ladder", 2, 3, 32, _G, 128, 160, 48, "default", "batch", "staged")
     _add(f"{_cfg}_L1_stress", "ladder", 2, 3, 16, _G, 256, 320, 32, "stress", "map", "staged")
     _add(f"{_cfg}_L0_clamped", "ladder", 2, 3, 8, _G, 512, 640, 8, "default", "clamped", "staged")
+    for _l, (_C, _D) in _LEVELS.items():
+        _add(f"{_cfg}_L{_l}_inv", "ladder", 2, 3, _C, _G, 512 >> _l, 640 >> _l, _D, "default",
+             "inv_float" if _l == 2 else "inv_map", "staged")
+    _add(f"{_cfg}_L2_inv_batch", "ladder", 2, 3, 32, _G, 128, 160, 48, "default", "inv_batch",
+         "staged")
 for _cfg, (_W, _H, _V, _Ds) in {"cfg4": (1152, 864, 5, (8, 32, 48)),
                                 "cfg5": (1920, 1056, 7, (8, 32, 64))}.items():
     for _l in (2, 1, 0):
@@ -175,6 +236,20 @@ for _V in (2, 3):
                      _pose, _hk, "staged")
         _add(f"staged_v{_V}_c{_C}_nonmono", "warp_nhwc", 2, _V, _C, 1, 21, 47, 9, "default",
              "nonmono", "staged")
+# the same kernels in the inverse mode: every (V, C, G) at inverse-wide, inverse-behind and one of
+# the other inverse forms
+_INV_GEOS = [("default", "inv_map", 13, 37, 7), ("default", "inv_float", 17, 33, 5),
+             ("stress", "inv_batch", 9, 40, 9)]
+for _V in (2, 3):
+    for _C in (8, 16, 32):
+        for _G in (1, 8):
+            _add(f"staged_v{_V}_c{_C}_g{_G}_inv_wide", "ladder", 2, _V, _C, _G, 24, 160, 3,
+                 "default", "inv_wide", "staged")
+            _add(f"staged_v{_V}_c{_C}_g{_G}_inv_behind", "ladder", 2, _V, _C, _G, 16, 96, 9,
+                 "stress", "inv_behind", "staged")
+            _pose, _hk, _h, _w, _D = _INV_GEOS[(_V + _C // 8 + _G) % 3]
+            _add(f"staged_v{_V}_c{_C}_g{_G}_{_pose}_{_hk}", "ladder", 2, _V, _C, _G, _h, _w, _D,
+                 _pose, _hk, "staged")
 # gather kernels: 1, 2, 4, 6 source views x C x variance / group-wise x output layout;
 # group sizes C/G in {1, 2, 4, 8, 16, 32} over the table
 _GW = {("nchw", 8): 8, ("nhwc", 8): 2, ("nchw", 16): 8, ("nhwc", 16): 2, ("nchw", 32): 8,
@@ -215,10 +290,65 @@ def _inputs(name, spec):
     W_, H = w << level, h << level
     feats = _feats(g, B, V, C, h, w, nchw=entry.endswith("_nchwf"))
     P = _proj(pose, V, W_, H, level, B)
-    hyp = _hyp(g, hk, B, D, h, w, _STEP[level])
+    hyp = _hyp(g, hk, B, D, h, w, _STEP[level], level)
     if entry != "ladder" and isinstance(hyp, ops.Ladder):
         hyp = hyp.materialize()
     return feats, P, hyp
+
+
+# The staged kernels' pixel tile (TW, TH) per C and their box: BW = TW + 16 columns, rounded up to
+# a 1024-byte row for the plane-group kernel (2 source views, variance), BH = TH + 4 rows
+# (warp_cost_smem.cu: kShapes and launch()).
+_TILE = {8: (32, 4), 16: (32, 2), 32: (16, 2)}
+
+
+def _box(V, C, G):
+    tw, th = _TILE[C]
+    wq = 1024 // (C * 4) if (V == 3 and G == 1) else 1
+    return tw, th, -(-(tw + 16) // wq) * wq, th + 4
+
+
+def _samples(P, dv):
+    """Float64 source coordinates of every (b, view, plane, y, x) as the kernels form them:
+    q = R (x, y, 1) + t / d, u = q_x / q_z -> (u, v, q_z)."""
+    P, dv = P.double().cpu(), dv.double().cpu()
+    B, D, h, w = dv.shape
+    ys, xs = torch.meshgrid(torch.arange(h, dtype=torch.float64), torch.arange(w, dtype=torch.float64),
+                            indexing="ij")
+    pix = torch.stack([xs, ys, torch.ones_like(xs)], 0).view(3, -1)                 # (3, hw)
+    a = (P[..., :3] @ pix).view(B, -1, 3, 1, h, w)                                    # (B,S,3,1,h,w)
+    q = a + P[..., 3].view(B, -1, 3, 1, 1, 1) / dv.view(B, 1, 1, D, h, w)
+    return q[:, :, 0] / q[:, :, 2], q[:, :, 1] / q[:, :, 2], q[:, :, 2]
+
+
+def _wide(spec, P, dv):
+    """Planes 0 and 1 alone already need more than the staged box in some tile and view: the
+    kernel's first run, whatever its length, is halved down to single planes."""
+    _, B, V, C, G, h, w = spec[:7]
+    tw, th, bw, bh = _box(V, C, G)
+    u, v, qz = (t[:, :, :2] for t in _samples(P, dv))
+    ok = (qz > 1e-7) & (u > -2) & (u < w + 1) & (v > -2) & (v < h + 1)
+    hp, wp = -(-h // th) * th, -(-w // tw) * tw
+    spans = []
+    for t in (u.floor(), v.floor()):
+        big = torch.where(ok, t, torch.full_like(t, float("nan")))
+        big = torch.nn.functional.pad(big, (0, wp - w, 0, hp - h), value=float("nan"))
+        tiles = big.reshape(*big.shape[:3], hp // th, th, wp // tw, tw).transpose(4, 5)
+        tiles = tiles.reshape(*tiles.shape[:5], -1).flatten(2, 2)
+        tiles = tiles.permute(0, 1, 3, 4, 2, 5).flatten(4)                  # (B,S,ty,tx,2*th*tw)
+        mx = torch.where(tiles.isnan(), -torch.inf, tiles).amax(-1)
+        mn = torch.where(tiles.isnan(), torch.inf, tiles).amin(-1)
+        spans.append(mx + 2 - mn)
+    return bool(((spans[0] > bw) | (spans[1] > bh)).any())
+
+
+def _behind(spec, P, dv):
+    """Part of the sweep lies behind a source camera (q_z <= 1e-7), part in front of it."""
+    qz = _samples(P, dv)[2]
+    return bool((qz <= 1e-7).any()) and bool((qz > 1e-7).any())
+
+
+INV_EDGES = {"inv_wide": _wide, "inv_behind": _behind}
 
 
 def _cl5(feats):
@@ -290,6 +420,10 @@ def _assert(name, spec, reps):
 def test_k1_vs_fp64(name):
     spec = CASES[name]
     feats, P, hyp = _inputs(name, spec)
+    hk = spec[9]
+    if hk in INV_EDGES:
+        dv = _hyp_tensor(hyp).cpu()
+        assert INV_EDGES[hk](spec, P, dv), f"{name}: {hk} does not hold"
     out = _launch(spec, feats, P, hyp)
     _assert(name, spec, _check_outputs(name, spec, feats, P, hyp, out))
 
@@ -333,10 +467,11 @@ def _expected_kernels():
     exp = set()
     for c in (8, 16, 32):
         for blk in (False, True):
-            exp.add(("smem", 1, c, False, blk))
-            exp.add(("smem", 1, c, True, blk))
-            exp.add(("smem", 2, c, True, blk))
-            exp.add(("smem_pg", 2, c, False, blk))
+            for inv in (False, True):
+                exp.add(("smem", 1, c, False, blk, inv))
+                exp.add(("smem", 1, c, True, blk, inv))
+                exp.add(("smem", 2, c, True, blk, inv))
+                exp.add(("smem_pg", 2, c, False, blk, inv))
     for ns in (1, 2, 4, 6):
         for ct in (8, 16, 32, 0):
             for gwc in (False, True):
@@ -353,12 +488,13 @@ def _parse_kernels(names):
     b = lambda s: s == "true"                                           # noqa: E731
     got = set()
     for n in names:
-        m = re.search(r"warp_var_smem_kernel<(\d+), (\d+), \d+, \d+, \d+, (true|false), (true|false)>", n)
+        m = re.search(r"warp_var_smem(_inv)?_kernel<(\d+), (\d+), \d+, \d+, \d+, (true|false), "
+                      r"(true|false)>", n)
         if m:
-            got.add(("smem", int(m[1]), int(m[2]), b(m[3]), b(m[4])))
-        m = re.search(r"warp_var_smem_pg_kernel<(\d+), \d+, \d+, \d+, \d+, (true|false)>", n)
+            got.add(("smem", int(m[2]), int(m[3]), b(m[4]), b(m[5]), bool(m[1])))
+        m = re.search(r"warp_var_smem_pg(_inv)?_kernel<(\d+), \d+, \d+, \d+, \d+, (true|false)>", n)
         if m:
-            got.add(("smem_pg", 2, int(m[1]), False, b(m[2])))
+            got.add(("smem_pg", 2, int(m[2]), False, b(m[3]), bool(m[1])))
         m = re.search(r"warp_cost_kernel<(\d+), (\d+), (true|false), (true|false)>", n)
         if m:
             got.add(("gather", int(m[1]), int(m[2]), b(m[3]), b(m[4])))
@@ -384,8 +520,10 @@ def test_every_k1_instantiation_launched(child):
     names = {e.name for e in prof.events()} | set(child["kernels"])
     got = _parse_kernels(names)
     missing = sorted(_expected_kernels() - got, key=str)
+    staged = {k for k in _expected_kernels() if k[0].startswith("smem")}
     print(f"[k1-fp64] {len(got & _expected_kernels())} of {len(_expected_kernels())} K1 "
-          f"instantiations launched")
+          f"instantiations launched, {len(got & staged)} of {len(staged)} staged (uniform and "
+          f"inverse)")
     assert not missing, f"never launched: {missing}"
 
 
