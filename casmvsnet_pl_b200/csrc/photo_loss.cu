@@ -22,6 +22,10 @@
 //     S_l = sum |d^(x+1,y) - d^(x,y)| exp(-g_x) / (B h_l (w_l - 1)) + the same in y over
 //     (B (h_l - 1) w_l), g_x = mean_c |I_ref,c(x+1, y) - I_ref,c(x, y)|.
 //   L = sum_l 2^(1-l) (P_l + lambda S_l); d|t|/dt at 0 is 0; only depth_l gets a gradient.
+//   Non-finite depths follow IEEE arithmetic and torch autograd of the expression above: a
+//   depth that is not finite and > 0 makes its pairs invalid, so P_l and N_l stay finite; a NaN
+//   depth makes S_l and L NaN, a +inf one makes them +inf (NaN if two +inf are neighbours), and
+//   the gradient stays finite, since d|t|/dt = sign(t) with sign(NaN) = 0, as torch.sign gives.
 //
 // Forward: one block per 16x16 tile of one (b, level).  The reference tile and, per source, the
 // warped tile are staged in shared memory with a 1-pixel halo; each thread keeps its pixel's

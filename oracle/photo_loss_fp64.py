@@ -30,24 +30,24 @@ EPS32 = 2.0 ** -24
 E_FLOOR = 64 * EPS32
 
 
-def level_images(imgs, l):
+def level_images(imgs, l, dtype=torch.float64):
     """imgs (B,V,3,H,W) normalised -> float64 un-normalised level-l images (strided subsample)."""
-    x = imgs.double()[..., :: 1 << l, :: 1 << l]
-    mean = torch.tensor(MEAN, dtype=torch.float64, device=x.device).view(3, 1, 1)
-    std = torch.tensor(STD, dtype=torch.float64, device=x.device).view(3, 1, 1)
+    x = imgs.to(dtype)[..., :: 1 << l, :: 1 << l]
+    mean = torch.tensor(MEAN, dtype=dtype, device=x.device).view(3, 1, 1)
+    std = torch.tensor(STD, dtype=dtype, device=x.device).view(3, 1, 1)
     return x * std + mean
 
 
-def warp(depth, P, w, h):
+def warp(depth, P, w, h, dtype=torch.float64):
     """depth (B,h,w), P (B,S,3,4) -> u, v, valid, du, dv (B,S,h,w), float64, differentiable in depth."""
     B = depth.shape[0]
     dev = depth.device
-    ys, xs = torch.meshgrid(torch.arange(h, device=dev, dtype=torch.float64),
-                            torch.arange(w, device=dev, dtype=torch.float64), indexing="ij")
-    d = depth.double()[:, None]
+    ys, xs = torch.meshgrid(torch.arange(h, device=dev, dtype=dtype),
+                            torch.arange(w, device=dev, dtype=dtype), indexing="ij")
+    d = depth.to(dtype)[:, None]
     ok_d = torch.isfinite(d) & (d > 0)
     inv = 1.0 / torch.where(ok_d, d, torch.ones_like(d))
-    P = P.double()
+    P = P.to(dtype)
 
     def row(r):
         m = P[:, :, r, :, None, None]
@@ -107,14 +107,14 @@ class LevelResult:
     N: torch.Tensor
 
 
-def level_loss(depth, imgs, P, dint, ratio, l, topk, selected=None):
+def level_loss(depth, imgs, P, dint, ratio, l, topk, selected=None, dtype=torch.float64):
     """One level.  depth (B,h,w) (may require grad), imgs (B,V,3,H,W), P (B,S,3,4) of level l,
     dint (B,).  `selected` (B,S,h,w) bool replaces the float64 top-K selection."""
-    I = level_images(imgs, l)
+    I = level_images(imgs, l, dtype)
     B, V, _, h, w = I.shape
     S = V - 1
     ref, src = I[:, 0], I[:, 1:]
-    u, v, ok, du, dv = warp(depth, P, w, h)
+    u, v, ok, du, dv = warp(depth, P, w, h, dtype)
     y = sample(src, u, v, ok)                                    # (B,S,3,h,w)
     x = ref[:, None].expand_as(y)
     okw = _win(ok).all(0)                                        # (B,S,h-2,w-2)
@@ -167,7 +167,7 @@ def level_loss(depth, imgs, P, dint, ratio, l, topk, selected=None):
     Pl = torch.where(has, torch.nan_to_num(loss_q, nan=0.0), torch.zeros_like(loss_q)).sum()
     Pl = Pl / N if N > 0 else Pl * 0
     # smoothness
-    dhat = depth.double() / (dint.double().view(-1, 1, 1) * ratio)
+    dhat = depth.to(dtype) / (dint.to(dtype).view(-1, 1, 1) * ratio)
     with torch.no_grad():
         kink = _kinks(u, v, ok, du, dv, x, y, dhat.detach())
     gx = (ref[..., :, 1:] - ref[..., :, :-1]).abs().mean(1)
@@ -197,7 +197,8 @@ def _kinks(u, v, ok, du, dv, x, y, dhat):
     return k
 
 
-def photo_loss(depths, imgs, proj_mats, dint, ratios, topk=1, smooth_weight=0.1, selected=None):
+def photo_loss(depths, imgs, proj_mats, dint, ratios, topk=1, smooth_weight=0.1, selected=None,
+               dtype=torch.float64):
     """depths [(B,h_l,w_l)], imgs (B,V,3,H,W), proj_mats (B,S,levels,3,4), dint (B,) ->
     (L, [LevelResult]).  L = sum_l 2^(1-l) (P_l + smooth_weight S_l), differentiable in depths;
     `selected` is None or one (B,S,h,w) bool per level."""
@@ -205,16 +206,20 @@ def photo_loss(depths, imgs, proj_mats, dint, ratios, topk=1, smooth_weight=0.1,
     total, out = 0.0, []
     for l, d in enumerate(depths):
         r = level_loss(d, imgs, proj_mats[:, :, l], dint, float(ratios[l]), l, topk,
-                       None if selected is None else selected[l])
+                       None if selected is None else selected[l], dtype)
         total = total + 2.0 ** (1 - l) * (r.P + smooth_weight * r.S)
         out.append(r)
     return total, out
 
 
-def gradient(depths, imgs, proj_mats, dint, ratios, topk=1, smooth_weight=0.1, selected=None):
-    """(L, [LevelResult], [dL/d depth_l]) in float64 (autograd of photo_loss)."""
-    ds = [d.detach().double().requires_grad_(True) for d in depths]
-    L, res = photo_loss(ds, imgs, proj_mats, dint, ratios, topk, smooth_weight, selected)
+def gradient(depths, imgs, proj_mats, dint, ratios, topk=1, smooth_weight=0.1, selected=None,
+             dtype=torch.float64):
+    """(L, [LevelResult], [dL/d depth_l]) in float64 (autograd of photo_loss).  dtype=float32
+    evaluates the same expression in float32 (the bounds and margins are then meaningless): the
+    difference of its gradient from the float64 one measures how far float32 rounding alone can
+    move each element, which no a-priori bound here captures where SSIM's centred sums cancel."""
+    ds = [d.detach().to(dtype).requires_grad_(True) for d in depths]
+    L, res = photo_loss(ds, imgs, proj_mats, dint, ratios, topk, smooth_weight, selected, dtype)
     grads = torch.autograd.grad(L, ds, allow_unused=True)
     grads = [torch.zeros_like(d) if g is None else g for d, g in zip(ds, grads)]
     return L.detach(), res, grads

@@ -3,7 +3,8 @@
   * per element against float64 (oracle/photo_loss_fp64.py, run in float64 on the device) at
     the level shapes of 640x512 (V = 3, K = 1) and 1152x864 (V = 5, K = 1..4), B = 2: validity,
     e within the oracle's bound, the selection wherever the oracle's margin exceeds twice its
-    bound, loss_q, P_l, S_l, N_l and the loss, and the gradient given the kernel's selection;
+    bound, loss_q, P_l, S_l, N_l and the loss, and the gradient given the kernel's selection
+    (check_against_fp64, which test_gpu_loss_sweep_fp64 runs at every shape the loss accepts);
   * two calls give the same bits; the call makes no host synchronisation;
   * the gradient is useful: Adam on the depth maps alone, from the ground truth of the textured
     capture plus a smooth perturbation of several depth intervals, halves the depth error;
@@ -42,10 +43,15 @@ VALID_MISMATCH_MAX = 2.0 ** -14
 # 2^-14 of the level's largest gradient.  Every pixel meets it except the oracle's kinks
 # (LevelResult.kink: p's own warp within the warp bound of a tap-cell edge, where the bilinear
 # slope differs between the precisions, or a sign of |x - y| or of a depth difference within
-# rounding of 0) and the 3x3 neighbourhood of a window whose validity differs.  The kinks come
-# from a worst-case warp bound, so they are a wide net (up to a fifth of the pixels at
-# 1152x864 with 4 sources); the pixels actually out of tolerance, all of which must be kinks,
-# were at most 2.0e-4 of a level, and may be at most 2^-12.
+# rounding of 0), the 3x3 neighbourhood of a window whose validity differs, and the
+# ill-conditioned elements: those where the oracle's own expression evaluated in float32
+# misses float64 by more than a quarter of the tolerance (SSIM's coefficients are differences
+# of terms up to 1 / (C1 C2) that cancel in low-contrast windows, so a few elements are far off
+# in any float32 evaluation: at 1600x1184 and on a training step's depths, the kernel's
+# out-of-tolerance non-kink pixels were off by 0.7 to 1.4 times what the float32 oracle was).
+# The kinks come from a worst-case warp bound, so they are a wide net (up to a fifth of the
+# pixels at 1152x864 with 4 sources); the pixels actually out of tolerance, all of which must be
+# exempt, were at most 2.0e-4 of a level, and may be at most 2^-12.
 GRAD_REL, GRAD_ABS, OVER_SHARE_MAX = 2.0 ** -10, 2.0 ** -14, 2.0 ** -12
 
 
@@ -55,44 +61,55 @@ def _grad_mode():
         yield
 
 
-def make_case(B, V, W, H, seed=0):
+def make_case(B, V, W, H, seed=0, levels=3):
     """Blurred-noise views (un-normalised in [0, 1]), the synthetic DTU projections, smooth
-    depth maps around the views' convergence depth, different per level and sample."""
+    depth maps around the views' convergence depth, different per level and sample, and a
+    depth interval per sample (distinct for up to 4 samples)."""
     rng = np.random.default_rng(seed)
     u8 = np.stack([cv2.GaussianBlur(rng.integers(0, 256, (H, W, 3), dtype=np.uint8), (0, 0), 2.0)
                    for _ in range(B * V)])
     imgs = io.normalize_images(torch.from_numpy(u8).to(DEV)).view(B, V, 3, H, W)
-    pm = synth.projection_matrices(V, W, H, 3).unsqueeze(0).expand(B, -1, -1, -1, -1).contiguous().to(DEV)
+    pm = synth.projection_matrices(V, W, H, levels).unsqueeze(0).expand(B, -1, -1, -1, -1).contiguous().to(DEV)
     depths = []
-    for l in range(3):
+    for l in range(levels):
         ys, xs = np.mgrid[0:H >> l, 0:W >> l].astype(np.float64) * (1 << l)
         d = np.stack([synth.CONVERGE_MM + 40 * np.sin(xs / 37 + b) * np.cos(ys / 53) + 3 * l
                       + rng.normal(0, 0.5, xs.shape) for b in range(B)])
         depths.append(torch.from_numpy(d).float().to(DEV))
-    dint = torch.tensor([[2.65], [3.1]][:B], device=DEV)
+    dint = torch.tensor([[2.65], [3.1], [1.9], [2.2]][:B], device=DEV)
     return imgs, pm, depths, dint
 
 
-def run(imgs, pm, depths, dint, K, debug=False):
+def run(imgs, pm, depths, dint, K, debug=False, ratios=RATIOS, lam=LAM):
     ds = [d.clone().requires_grad_(True) for d in depths]
-    out = losses.photo_loss({f"depth_{l}": d for l, d in enumerate(ds)}, imgs, pm, dint, RATIOS, 3, K,
-                            LAM, debug=debug)
+    out = losses.photo_loss({f"depth_{l}": d for l, d in enumerate(ds)}, imgs, pm, dint, ratios, len(ds), K,
+                            lam, debug=debug)
     out[0].backward()
     return out, [d.grad for d in ds]
 
 
-CASES = [(640, 512, 3, 1), (1152, 864, 5, 1), (1152, 864, 5, 2), (1152, 864, 5, 3), (1152, 864, 5, 4)]
+def _same_nonfinite(a, b):
+    """a and b (tensors or floats) are NaN at the same places and equal where infinite."""
+    a, b = torch.as_tensor(a, dtype=torch.float64), torch.as_tensor(b, dtype=torch.float64)
+    return (torch.equal(torch.isnan(a), torch.isnan(b)) and torch.equal(torch.isinf(a), torch.isinf(b))
+            and torch.equal(a[torch.isinf(a)], b[torch.isinf(b)]))
 
 
-@pytest.mark.parametrize("W,H,V,K", CASES)
-def test_matches_float64(W, H, V, K):
-    imgs, pm, depths, dint = make_case(2, V, W, H)
-    (loss, stats, dbg), grads = run(imgs, pm, depths, dint, K, debug=True)
+def check_against_fp64(imgs, pm, depths, dint, ratios, K, lam, loss, stats, dbg, grads, tag=""):
+    """The kernel's outputs of one call (loss, stats, debug maps and the depth gradients for an
+    incoming gradient of 1) against oracle/photo_loss_fp64 on the same inputs, at any level
+    count: validity, e within the oracle's bound, the selection wherever the oracle's margin
+    exceeds twice its bound, loss_q, P_l, S_l, N_l, the loss, and the gradient given the
+    kernel's selection.  Non-finite S_l, loss and gradients must be non-finite at the same
+    places as in float64.  Returns per level the largest e error / bound (0 without a valid
+    pair) and the largest gradient error over the level's largest gradient."""
+    levels = len(depths)
     with torch.no_grad():
-        _, own = O.photo_loss(depths, imgs, pm, dint, RATIOS, K, LAM)
+        _, own = O.photo_loss(depths, imgs, pm, dint, ratios, K, lam)
     sel = [k["selected"] & r.valid for k, r in zip(dbg, own)]
-    L64, res, g64 = O.gradient(depths, imgs, pm, dint, RATIOS, K, LAM, selected=sel)
-    tol_loss = 0.0
+    L64, res, g64 = O.gradient(depths, imgs, pm, dint, ratios, K, lam, selected=sel)
+    g32 = O.gradient(depths, imgs, pm, dint, ratios, K, lam, selected=sel, dtype=torch.float32)[2]
+    tol_loss, worst = 0.0, []
     for l, (k, r, rk) in enumerate(zip(dbg, own, res)):
         mism = (k["valid"] != r.valid).sum().item()
         assert mism <= VALID_MISMATCH_MAX * r.valid.numel(), (l, mism)
@@ -100,7 +117,7 @@ def test_matches_float64(W, H, V, K):
         assert torch.isnan(k["e"][~k["valid"]]).all()
         err = (k["e"].double() - r.e).abs()[both]
         bound = r.e_bound[both]
-        ratio = (err / bound).max().item()
+        ratio = (err / bound).max().item() if err.numel() else 0.0
         assert ratio <= 1.0, (l, ratio)
         qbound = torch.where(r.valid, r.e_bound, torch.zeros_like(r.e_bound)).amax(1)
         clear = (r.margin > 2 * qbound) & (k["valid"] == r.valid).all(1)
@@ -115,25 +132,50 @@ def test_matches_float64(W, H, V, K):
         assert N == rk.N.item() or mism, (l, N, rk.N.item())
         tolP = qbound.max().item() + 4 * EPS32
         assert abs(P - rk.P.item()) <= tolP, (l, P, rk.P.item())
-        assert abs(S - rk.S.item()) <= 1e-5 * abs(rk.S.item()) + 1e-12, (l, S, rk.S.item())
-        tol_loss += 2.0 ** (1 - l) * (tolP + LAM * 1e-5 * abs(rk.S.item()))
+        S64 = rk.S.item()
+        assert _same_nonfinite(S, S64), (l, S, S64)
+        if np.isfinite(S64):
+            assert abs(S - S64) <= 1e-5 * abs(S64) + 1e-12, (l, S, S64)
+            tol_loss += 2.0 ** (1 - l) * (tolP + lam * 1e-5 * abs(S64))
         g, gr = grads[l].double(), g64[l]
+        assert _same_nonfinite(g, gr), (l, "non-finite gradients differ")
+        fin = torch.isfinite(gr)
+        g, gr = torch.where(fin, g, 0.0), torch.where(fin, gr, 0.0)
         scale = gr.abs().max().item()
         gerr = (g - gr).abs()
-        over = gerr > GRAD_REL * gr.abs() + GRAD_ABS * scale
+        tol = GRAD_REL * gr.abs() + GRAD_ABS * scale
+        over = gerr > tol
         moved = (k["valid"] != r.valid).any(1).double()[:, None]
-        exempt = rk.kink | (torch.nn.functional.max_pool2d(moved, 3, 1, 1)[:, 0] > 0)
+        ill = (torch.where(fin, g32[l].double(), 0.0) - gr).abs() > tol / 4
+        exempt = rk.kink | (torch.nn.functional.max_pool2d(moved, 3, 1, 1)[:, 0] > 0) | ill
         bad = over & ~exempt
         assert not bad.any(), (l, bad.sum().item(), gerr[bad].max().item() / scale)
         share = over.double().mean().item()
         exempt_share = exempt.double().mean().item()
         assert share <= OVER_SHARE_MAX, (l, share)
-        print(f"[photo {W}x{H} V={V} K={K} l={l}] e err/bound max {ratio:.3e}, e err max "
-              f"{err.max().item():.3e}, loss_q err max {lq_err.max().item():.3e}, ambiguous "
-              f"selection {ambiguous:.2e}, grad err max / level max {gerr.max().item() / scale:.3e}, "
-              f"over tolerance {share:.2e} (all exempt; exempt share {exempt_share:.2e}), "
-              f"validity mismatches {mism}")
-    assert abs(loss.item() - L64.item()) <= tol_loss + 4 * EPS32 * abs(L64.item())
+        grel = gerr.max().item() / scale if scale > 0 else gerr.max().item()
+        worst.append((ratio, grel))
+        print(f"[photo {tag} l={l}] e err/bound max {ratio:.3e}, e err max "
+              f"{err.max().item() if err.numel() else 0.0:.3e}, loss_q err max "
+              f"{lq_err.max().item() if lq_err.numel() else 0.0:.3e}, ambiguous selection {ambiguous:.2e}, "
+              f"grad err max / level max {grel:.3e}, over tolerance {share:.2e} (all exempt; exempt "
+              f"share {exempt_share:.2e}, ill-conditioned {ill.double().mean().item():.2e}), validity mismatches {mism}, valid pairs {both.sum().item()}")
+    assert len(worst) == levels
+    lk, l64 = loss.item(), L64.item()
+    assert _same_nonfinite(lk, l64), (lk, l64)
+    if np.isfinite(l64):
+        assert abs(lk - l64) <= tol_loss + 4 * EPS32 * abs(l64), (lk, l64)
+    return worst
+
+
+CASES = [(640, 512, 3, 1), (1152, 864, 5, 1), (1152, 864, 5, 2), (1152, 864, 5, 3), (1152, 864, 5, 4)]
+
+
+@pytest.mark.parametrize("W,H,V,K", CASES)
+def test_matches_float64(W, H, V, K):
+    imgs, pm, depths, dint = make_case(2, V, W, H)
+    (loss, stats, dbg), grads = run(imgs, pm, depths, dint, K, debug=True)
+    check_against_fp64(imgs, pm, depths, dint, RATIOS, K, LAM, loss, stats, dbg, grads, f"{W}x{H} V={V} K={K}")
 
 
 def test_level_without_valid_pixels():
