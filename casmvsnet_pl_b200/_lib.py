@@ -263,6 +263,17 @@ SIGNATURES = {
                                     + [c_int, c_void_p, c_void_p]),
     "casmvs_texture_level_apply": (c_int, [c_void_p, c_longlong] + [c_void_p] * 6
                                    + [c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "casmvs_refine_grey": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p]),
+    "casmvs_refine_normals": (c_int, [c_void_p, c_int] + [c_void_p] * 5),
+    "casmvs_refine_visibility": (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(c_float),
+                                         POINTER(c_double), POINTER(c_int), POINTER(c_int),
+                                         POINTER(c_void_p), c_void_p, c_int, c_void_p]),
+    "casmvs_refine_select": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int]
+                             + [c_void_p] * 6),
+    "casmvs_refine_sweep": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 6
+                            + [c_int] + [c_void_p] * 7),
+    "casmvs_refine_smooth": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 5),
+    "casmvs_refine_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "casmvs_visual_panels":(c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "casmvs_nchw_to_nhwc":(c_int,[c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),
     "casmvs_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_size_t, c_void_p]),

@@ -479,6 +479,21 @@ def _clean(name, verts, colours, faces, mesh_clean, log):
     return verts, colours, faces
 
 
+def _refine(name, verts, colours, faces, images, proj0, metas, iterations, log):
+    """The mesh refined against the reference views' images (cast to uint8), proj0 and the scan's
+    pair sources by refine.refine_mesh (unchanged when iterations is None)."""
+    if iterations is None:
+        return verts, colours, faces
+    from . import refine
+    vids = sorted(images)
+    ims = [images[v].to(torch.uint8).contiguous() for v in vids]
+    sources = refine.pair_sources(metas, vids)
+    verts, colours, faces, st = refine.refine_mesh(verts, colours, faces, ims, [proj0[v] for v in vids],
+                                                   sources, iterations=iterations, log=log)
+    log(f"{name}: refined the mesh against {st['views']} views: {refine.summary(st)}")
+    return verts, colours, faces
+
+
 def _score_mesh(scan, mesh_path, verts, faces, dtu_gt, dtu_seed, tnt_gt, tnt_images, tnt_tau,
                 tnt_seed, run_dir):
     """Scores of the written mesh against the Tanks and Temples (tnt_gt) or DTU (dtu_gt) ground
@@ -522,7 +537,7 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
              tnt_gt=None, tnt_images=None, tnt_tau=None, tnt_seed=0, run_dir=None,
              mesh_method="tsdf", poisson_depth=None, poisson_point_weight=0.0, mesh_faces=None,
              mesh_texture=False, mesh_score=False, mesh_texture_level=False, mesh_clean=None,
-             fusion_rule="reference", outlier_filter=None):
+             fusion_rule="reference", outlier_filter=None, mesh_refine=None):
     """-> (xyz (N,3) float32, rgb (N,3) uint8) CUDA tensors; optional PFM / PLY outputs.
     `scan` is a DTUTestScan, TanksTestScan, BlendedMVSTestScan or ColmapScan; each gives the depth range of
     its reference views (scan.depth_range).  With `save_visual` and `depth_dir`, the JET depth
@@ -542,6 +557,9 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
     that many faces (simplify.py) before it is written.  With `mesh_texture`, the written mesh is
     also textured from the reference views' images and proj0 (texture.py) and written beside it
     as an OBJ with its MTL and atlas PNGs; `mesh_texture_level` also levels its colour seams.
+    With `mesh_refine` (a number of iterations >= 1), either mesh is refined against the reference
+    views' images, proj0 and the scan's pair sources (refine.py) after it is cleaned and
+    simplified, before it is written, textured or scored; only its vertices move.
     With `tnt_gt` (a Tanks and Temples ground-truth directory holding the scan's scene) the fused
     cloud is scored by tnt_eval.evaluate_scene from the device tensors against the cameras the run
     recorded in `run_dir`, the scores are written next to the PLY as <ply>_tnt.json when ply_path
@@ -610,6 +628,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         del pts, cols
         verts, colours, faces = _clean(scan.scan, verts, colours, faces, mesh_clean, log)
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
+        verts, colours, faces = _refine(scan.scan, verts, colours, faces, images, proj0, scan.metas,
+                                        mesh_refine, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
             _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log,
@@ -629,6 +649,8 @@ def run_scan(model, scan, depth_interval=2.65, conf=0.999, min_geo_consistent=5,
         del fused
         verts, colours, faces = _clean(scan.scan, verts, colours, faces, mesh_clean, log)
         verts, colours, faces = _simplify(scan.scan, verts, colours, faces, mesh_faces, log)
+        verts, colours, faces = _refine(scan.scan, verts, colours, faces, images, proj0, scan.metas,
+                                        mesh_refine, log)
         mesh.write_mesh_ply(mesh_path, verts, colours, faces)
         if mesh_texture:
             _texture(scan.scan, mesh_path, verts, colours, faces, images, proj0, log,
@@ -771,6 +793,12 @@ def parse_args(argv=None):
     ap.add_argument("--mesh_texture_level", action="store_true",
                     help="with --mesh_texture: level the colour seams between the atlas's charts "
                          "(global colour adjustment); only the page PNGs change")
+    ap.add_argument("--mesh_refine", action="store_true",
+                    help="with --mesh: move each vertex of the mesh along its normal to where the "
+                         "reference views agree photometrically (after cleaning and simplifying, "
+                         "before it is written, textured or scored)")
+    ap.add_argument("--mesh_refine_iterations", type=int, default=None,
+                    help="with --mesh_refine: refinement iterations, >= 1 (default 3)")
     ap.add_argument("--mesh_score", action="store_true",
                     help="with --mesh and --dtu_gt or --tnt_gt: also score the mesh as written "
                          "through its surface samples into <out>/mesh/<scan>_scores.json "
@@ -817,6 +845,12 @@ def parse_args(argv=None):
         ap.error("--mesh_clean_ratio must be in [0, 1]")
     if a.mesh_max_hole is not None and not (a.mesh_max_hole == 0 or 3 <= a.mesh_max_hole <= 128):
         ap.error("--mesh_max_hole must be 0 or in 3..128")
+    if a.mesh_refine and not a.mesh:
+        ap.error("--mesh_refine needs --mesh")
+    if a.mesh_refine_iterations is not None and not a.mesh_refine:
+        ap.error("--mesh_refine_iterations needs --mesh_refine")
+    if a.mesh_refine_iterations is not None and a.mesh_refine_iterations < 1:
+        ap.error("--mesh_refine_iterations must be >= 1")
     if a.mesh_faces is not None and not a.mesh:
         ap.error("--mesh_faces needs --mesh")
     if a.mesh_faces is not None and a.mesh_faces < 1:
@@ -850,6 +884,15 @@ def _clean_options(a):
         return None
     opts = dict(min_ratio=a.mesh_clean_ratio, max_hole=a.mesh_max_hole)
     return {k: v for k, v in opts.items() if v is not None}
+
+
+def _refine_iterations(a):
+    """refine_mesh's iterations from --mesh_refine_iterations (default refine.ITERATIONS), or
+    None without --mesh_refine."""
+    if not a.mesh_refine:
+        return None
+    from . import refine
+    return refine.ITERATIONS if a.mesh_refine_iterations is None else a.mesh_refine_iterations
 
 
 def _outlier_options(a):
@@ -903,7 +946,7 @@ def main(argv=None):
                        mesh_score=a.mesh_score, mesh_texture_level=a.mesh_texture_level,
                        mesh_clean=_clean_options(a),
                        fusion_rule=getattr(a, "fusion", "reference"),
-                       outlier_filter=_outlier_options(a), **tnt)
+                       outlier_filter=_outlier_options(a), mesh_refine=_refine_iterations(a), **tnt)
         print(f"{scan.scan} contains {len(out[0]) / 1e6:.2f} M points")
         if a.dtu_gt is not None:
             from .dtu_eval import _fmt

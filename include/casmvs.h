@@ -1188,6 +1188,57 @@ int casmvs_texture_level_apply(const unsigned long long* owner, long long n_texe
                                const int* corner, const double* g, unsigned char* atlas,
                                void* stream);
 
+/* ---- mesh refinement against the views (csrc/refine.cu, casmvsnet_pl_b200/refine.py) ----------
+ * Moves vertex positions only.  Constants: R = 2 (a 5 x 5 patch), K = 4, STEP = 1, SPACING = 4,
+ * S_MAX = 4, VAR_MIN = 1e-4, MIN_GAIN = 5e-4, MIN_SCORE = 0.3, lambda = 1; PAD = 2, MIN_COS = 0.1 and DEPTH_TOL = 0.01 as in
+ * texturing; at most 8 views per visibility call.  The caller runs, per iteration it = 0 .. T-1:
+ * normals, the key buffers of the current mesh (casmvs_render_mesh_keys) and visibility one batch
+ * at a time, selection, the sweep, J = 4 smoothing rounds from d = d0, and apply.  Each vertex is
+ * one thread; sums run in the order stated; there are no atomics.
+ * casmvs_refine_grey: grey (n) f64 = ((0.299 R + 0.587 G) + 0.114 B) / 255 of rgb (n,3) u8,
+ *   each operation rounded.
+ * casmvs_refine_normals: normal (V,3) f64 = s / |s|, s the sum from 0 over vf_face[vf_ptr[v] ..
+ *   vf_ptr[v+1]) (the faces of v, ascending) of (x1 - x0) x (x2 - x0) in double, each operation
+ *   rounded as written ((a1 b2 - a2 b1) etc., |s| = sqrt((s0 s0 + s1 s1) + s2 s2)); 0 when |s| = 0.
+ * casmvs_refine_visibility: for the views of one batch (HOST arrays as casmvs_texture_scores':
+ *   P n*16 f32, eye n*3 f64, wh n*2, view_index n, zbufs n DEVICE key buffers), sets bit
+ *   view_index[j] of vertex v in vis (V, words) u32 (zeroed by the caller before the first batch)
+ *   when v projects (render_mesh_fwd's projection) with PAD <= u <= W-1-PAD, PAD <= v <= H-1-PAD,
+ *   the key at (rint(u), rint(v)) is not empty and w <= f32(depth * 1.01f), and
+ *   |n.d| >= 0.1 sqrt(d.d), d = eye - v, dots ((a0 b0 + a1 b1) + a2 b2).
+ * casmvs_refine_select: ref (V) int32 = the visible view of largest |n.d| / sqrt(d.d) (ties to the
+ *   lower index; eyes (n_views,3) f64 DEVICE); src (V,4) int32 = the reference's sources
+ *   src_ids[src_ptr[ref] .. src_ptr[ref+1]) (DEVICE CSR over the views) in which v is visible, in
+ *   that order, at most 4, -1 after the last.  ref = -1 without a reference or a source.
+ * casmvs_refine_sweep: per vertex with ref >= 0: rho, the tangent frame, the candidates at
+ *   delta_k = k rho 2^-iteration and the ZNCC scores S_k of csrc/refine.cu's rule, step 4, in
+ *   double; Ps (n,16) f32 and Pinv (n,16) f64 (inv of P in double) DEVICE; grey DEVICE array of
+ *   (H,W) f64 device pointers (casmvs_refine_grey), wh (n,2) int32 DEVICE.  Outputs (V): rho,
+ *   best = S_k* (NaN without a valid k), kstar (-1000 without one), d (step 5's d, 0 unless
+ *   confident), conf (c); sk (V,9) f64 (NaN where k is invalid) only when not NULL.
+ * casmvs_refine_smooth: one Jacobi round d_out = (conf d0 + sum d_in[nb]) / (conf + |nb|), the sum
+ *   from 0 over nb_ids[nb_ptr[v] .. nb_ptr[v+1]) (the one-ring, ascending); 0 when the divisor is 0.
+ * casmvs_refine_apply: verts_out = f32(verts_in + d normal) per coordinate, in double. */
+int casmvs_refine_grey(const unsigned char* rgb, long long n_pixels, double* grey, void* stream);
+int casmvs_refine_normals(const float* verts, int V, const int* faces, const int* vf_ptr,
+                          const int* vf_face, double* normal, void* stream);
+int casmvs_refine_visibility(const float* verts, const double* normal, int V, int n_views,
+                             const float* P, const double* eye, const int* wh,
+                             const int* view_index, unsigned long long* const* zbufs,
+                             unsigned* vis, int words, void* stream);
+int casmvs_refine_select(const float* verts, const double* normal, int V, const unsigned* vis,
+                         int words, int n_views, const double* eyes, const int* src_ptr,
+                         const int* src_ids, int* ref, int* src, void* stream);
+int casmvs_refine_sweep(const float* verts, const double* normal, int V, const int* ref,
+                        const int* src, const float* Ps, const double* Pinv,
+                        const unsigned long long* grey, const int* wh, int iteration, double* rho,
+                        double* best, int* kstar, double* d, double* conf, double* sk,
+                        void* stream);
+int casmvs_refine_smooth(const int* nb_ptr, const int* nb_ids, int V, const double* d0,
+                         const double* conf, const double* d_in, double* d_out, void* stream);
+int casmvs_refine_apply(const float* verts_in, const double* normal, const double* d, int V,
+                        float* verts_out, void* stream);
+
 /* ---- training panels (csrc/visual.cu; utils/visualization.py, train.py:107-114) ---------
  * The original's TensorBoard image strip as uint8 (H, n*W, 3), n = the number of non-NULL panel
  * inputs, panels left to right in the order img, depth_gt, depth_pred, conf:
