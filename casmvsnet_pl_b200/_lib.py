@@ -75,7 +75,14 @@ SIGNATURES = {
     "casmvs_regress_ladder_inverse_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p,
                                                   c_float, c_void_p, c_void_p, c_void_p] + [c_int] * 4
                                           + [c_void_p]),
-    "casmvs_fpn_level_fwd": (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_void_p]),
+    "casmvs_adaptive_hypotheses_fwd": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p]
+                                       + [c_int] * 5 + [c_void_p]),
+    "casmvs_regress_spread_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int] + [c_void_p] * 5
+                                  + [c_int] * 4 + [c_void_p]),
+    "casmvs_regress_ladder_spread_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_float]
+                                         + [c_void_p] * 5 + [c_int] * 4 + [c_void_p]),
+    "casmvs_warp_cost_ladder_step_fwd": (c_int, [c_void_p] * 5 + [c_int] * 8 + [c_void_p]),
+    "casmvs_fpn_level_fwd":(c_int, [c_void_p] * 8 + [c_int] * 5 + [c_void_p]),
     "casmvs_fpn_merge_fwd": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p]),
     "casmvs_conv2d_rgb8_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p] + [c_int] * 4 + [c_void_p]),
     "casmvs_conv2d_5x5s2_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p] + [c_int] * 6 + [c_void_p]),

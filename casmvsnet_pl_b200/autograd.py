@@ -211,6 +211,24 @@ class RegressInverseFn(torch.autograd.Function):
         return _regress_bwd(ctx, gdepth, True)
 
 
+class RegressSpreadFn(torch.autograd.Function):
+    """RegressFn that also returns the adaptive mode's spread (README "Adaptive depth ranges"),
+    non-differentiable like the confidence; depth's gradient is RegressFn's."""
+
+    @staticmethod
+    def forward(ctx, logits, depth_values):
+        lg = logits.detach().contiguous()
+        dv = depth_values.contiguous()
+        depth, conf, _, _, spread = ops.regress(lg, dv, want_spread=True)
+        ctx.save_for_backward(lg, dv)
+        ctx.mark_non_differentiable(conf, spread)
+        return depth, conf, spread
+
+    @staticmethod
+    def backward(ctx, gdepth, _gconf, _gspread):
+        return _regress_bwd(ctx, gdepth, False)
+
+
 class Upsample2xFn(torch.autograd.Function):
     """F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=True) of a CUDA fp32
     (N,C,h,w) tensor, NCHW or channels-last: ATen's forward, the gather backward."""
@@ -250,6 +268,11 @@ def warp_cost(feats, proj_mats, depth_values, num_groups=1):
     return WarpCostFn.apply(feats, proj_mats, depth_values, num_groups)
 
 
-def regress(logits, depth_values, inverse=False):
-    """inverse=True: the inverse-depth regression, depth = 1/sum_d p_d/depth_values_d."""
+def regress(logits, depth_values, inverse=False, want_spread=False):
+    """inverse=True: the inverse-depth regression, depth = 1/sum_d p_d/depth_values_d.
+    want_spread=True: (depth, confidence, spread), the spread without a gradient."""
+    if want_spread:
+        if inverse:
+            raise _lib.CasMVSError("regress: want_spread is the adaptive mode's, not the inverse mode's")
+        return RegressSpreadFn.apply(logits, depth_values)
     return (RegressInverseFn if inverse else RegressFn).apply(logits, depth_values)

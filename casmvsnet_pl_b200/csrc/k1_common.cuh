@@ -157,14 +157,17 @@ __device__ __forceinline__ float inverse_plane(float first, float step, int d) {
 // roundings (multiply, then add) so that the (B,D,h,w) tensor never has to exist in HBM.
 // INV: the ladder is in inverse depth, first and step in 1/depth units (inverse_plane).  A
 // template parameter, so that the uniform consumers compile exactly as they did without it.
+// PIX: the per-pixel-step ladder of the adaptive mode (README "Adaptive depth ranges",
+// regress.cu): step_b is then a (B,h,w) map of plane spacings, read at the pixel like first_map.
+// The struct keeps its layout, so the kernels that take it keep their parameter offsets.
 struct Hyp {
   const float* dv;         // (B,D,h,w) or null => ladder
   const float* first_map;  // (B,h,w) first hypothesis per pixel, or null
   const float* first_b;    // (B) first hypothesis per batch item, or null
-  const float* step_b;     // (B) plane spacing per batch item, or null
+  const float* step_b;     // (B) plane spacing per batch item [PIX: (B,h,w) per pixel], or null
   float first, step;       // scalars used when the pointers above are null
 };
-template <bool INV = false>
+template <bool INV = false, bool PIX = false>
 struct HypPixT {
   const float* p;
   size_t hw;
@@ -172,7 +175,10 @@ struct HypPixT {
   __device__ __forceinline__ HypPixT(const Hyp& h, int b, int D, size_t hw_, int pix) : hw(hw_) {
     p = h.dv ? h.dv + (size_t)b * D * hw_ + pix : nullptr;
     first = h.first_map ? __ldg(h.first_map + (size_t)b * hw_ + pix) : h.first_b ? __ldg(h.first_b + b) : h.first;
-    step = h.step_b ? __ldg(h.step_b + b) : h.step;
+    if constexpr (PIX)
+      step = __ldg(h.step_b + (size_t)b * hw_ + pix);
+    else
+      step = h.step_b ? __ldg(h.step_b + b) : h.step;
   }
   __device__ __forceinline__ float at(int d) const {
     if constexpr (INV)
@@ -186,9 +192,11 @@ using HypPix = HypPixT<false>;
 // The TMA-staged cost-volume kernels (warp_cost_smem.cu): channels-last features, channels-last
 // or (blocked != 0) blocked output.  warp_cost_staged returns the launcher of a shape from their
 // coverage table, or null (the shape runs on the gather kernel, or not at all from a ladder).
-// inverse != 0: a ladder dv is in inverse depth (HypPixT<true>).
+// form: how a ladder dv is read -- kLadderUniform, kLadderInverse (in inverse depth,
+// HypPixT<true>) or kLadderPixelStep (a (B,h,w) step map, HypPixT<false, true>).
+enum LadderForm { kLadderUniform = 0, kLadderInverse = 1, kLadderPixelStep = 2 };
 using StagedK1 = int (*)(const float* feats, const float* proj, const Hyp& dv, float* cost, int B,
-                         int D, int h, int w, int rnd, int blocked, int inverse, cudaStream_t st);
+                         int D, int h, int w, int rnd, int blocked, int form, cudaStream_t st);
 StagedK1 warp_cost_staged(int V, int C, int num_groups);
 
 }  // namespace casmvs

@@ -17,6 +17,22 @@
 // Every product, sum and difference above is one float32 operation rounded to nearest; depth is
 // increasing in k as in the uniform mode.
 //
+// Adaptive depth ranges (opt-in; README "Adaptive depth ranges"; after UCS-Net, Cheng et al.,
+// CVPR 2020).  Stage l has D_l planes; g_l = depth_interval*r_l is the uniform mode's step.
+//   1. Coarsest stage: the uniform planes, init_depth_min + k*g_2.
+//   2. Spread: after stage l+1 (l+1 in {2,1}) regresses dhat = sum_k p_k*d_k, K3 also writes
+//      sigma = sqrt_rn(sum_k RN(p_k * RN(RN(d_k - dhat)^2))), a second pass over the planes with
+//      the same float32 p_k, summed in the plane order and Cascade16 structure of the depth sum
+//      (never E[d^2] - dhat^2, which cancels at DTU depths).  Depth, confidence and index are
+//      unchanged.  The finest stage writes no spread.
+//   3. Finer stage l in {1,0}: c = upsample2x_at(dhat_{l+1}), s = upsample2x_at(sigma_{l+1}),
+//      r = fmaxf(RN(lambda*s), g_l) with lambda = kAdaptiveLambda = 1.5, lo = fmaxf(RN(c - r),
+//      1e-7f), hi = RN(c + r), step = RN(RN(hi - lo) / (D_l - 1)) (IEEE division), and plane k
+//      is RN(lo + RN(step*k)), the uniform ladder's expression with a per-pixel first and step.
+//      The floor keeps a confident pixel searching at least +-g_l; fmaxf ignores NaN, so a NaN
+//      spread gives r = g_l, while a NaN c propagates as in the uniform mode.  D_l >= 2.
+//   4. Regression, confidence and the backward are the uniform mode's; sigma carries no gradient.
+//
 // Replaces (reference, relative to /root/reference):
 //   F.softmax + depth_regression    models/mvsnet.py:174-177, models/modules.py:95-104
 //   confidence block                models/mvsnet.py:179-193
@@ -28,6 +44,8 @@
 namespace casmvs {
 
 constexpr int kK3Threads = 128;
+// lambda of the adaptive mode (rule 3 above), ops.ADAPTIVE_LAMBDA on the Python side
+constexpr float kAdaptiveLambda = 1.5f;
 
 // What K3 averages for plane depth x: x itself, or RN(1/x) in the inverse mode.
 template <bool INV>
@@ -57,13 +75,16 @@ struct Cascade16 {
 // dependent passes over global memory) and exp(l - m) is evaluated once per hypothesis.  The
 // arithmetic -- every operation and its order -- is the generic path's, so results are
 // bit-identical (tests/test_gpu_kernels.py::test_regress_register_path_bit_identical).
-// INV: inverse-depth regression (rule 5 above).  The body of regress_kernel (uniform) and
-// regress_inv_kernel; the uniform kernel keeps its name and its code.
-template <bool IS_PROB, int DT, bool INV>
+// INV: inverse-depth regression (rule 5 above).  SPREAD: the adaptive mode's spread (rule 2 of
+// "Adaptive depth ranges"), written where `spread` is not null; PIX: the per-pixel-step ladder.
+// The body of regress_kernel (uniform), regress_inv_kernel and regress_spread_kernel; the uniform
+// kernel keeps its name and its code.
+template <bool IS_PROB, int DT, bool INV, bool SPREAD = false, bool PIX = false>
 __device__ __forceinline__ void
 regress_body(const float* __restrict__ logits, const float* __restrict__ dv, int dv_is_vector,
              const Hyp hyp, float* __restrict__ depth, float* __restrict__ conf,
-             long long* __restrict__ index, float* __restrict__ prob, int D, int hw) {
+             long long* __restrict__ index, float* __restrict__ prob, int D, int hw,
+             float* __restrict__ spread = nullptr) {
   const int b = blockIdx.y;
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
   if (pix >= hw) return;
@@ -71,7 +92,7 @@ regress_body(const float* __restrict__ logits, const float* __restrict__ dv, int
   // hypotheses: (D,) vector, (B,D,h,w) tensor, or (dv == null) the ladder first + step*d
   const float* dp = !dv ? nullptr : dv_is_vector ? dv : dv + (size_t)b * D * hw + pix;
   const size_t dstride = dv_is_vector ? 1 : (size_t)hw;
-  const HypPixT<INV> hp(hyp, b, D, (size_t)hw, pix);
+  const HypPixT<INV, PIX> hp(hyp, b, D, (size_t)hw, pix);
 
   float m = 0.f, denom = 1.f;
   Cascade16 acc_depth, acc_idx;
@@ -135,6 +156,18 @@ regress_body(const float* __restrict__ logits, const float* __restrict__ dv, int
   depth[(size_t)b * hw + pix] = dep;
   conf[(size_t)b * hw + pix] = c;
   if (index) index[(size_t)b * hw + pix] = (long long)idx;
+  if constexpr (SPREAD) {
+    // second pass with the same p_k and d_k, now that dep is known
+    if (!spread) return;
+    Cascade16 acc_var;
+    for (int d = 0; d < D; ++d) {
+      float p = __ldg(lp + (size_t)d * hw);
+      if (!IS_PROB) p = __fdiv_rn(expf(p - m), denom);
+      const float t = __fsub_rn(dp ? __ldg(dp + d * dstride) : hp.at(d), dep);
+      acc_var.add(__fmul_rn(p, __fmul_rn(t, t)));
+    }
+    spread[(size_t)b * hw + pix] = __fsqrt_rn(acc_var.result());
+  }
 }
 
 template <bool IS_PROB, int DT>
@@ -150,6 +183,16 @@ regress_inv_kernel(const float* __restrict__ logits, const float* __restrict__ d
                    const Hyp hyp, float* __restrict__ depth, float* __restrict__ conf,
                    long long* __restrict__ index, float* __restrict__ prob, int D, int hw) {
   regress_body<IS_PROB, DT, true>(logits, dv, dv_is_vector, hyp, depth, conf, index, prob, D, hw);
+}
+// regress_kernel with the adaptive mode's spread (null: none) and, PIX, a per-pixel-step ladder
+template <bool IS_PROB, int DT, bool PIX>
+__global__ void __launch_bounds__(kK3Threads)
+regress_spread_kernel(const float* __restrict__ logits, const float* __restrict__ dv,
+                      int dv_is_vector, const Hyp hyp, float* __restrict__ depth,
+                      float* __restrict__ conf, long long* __restrict__ index,
+                      float* __restrict__ prob, float* __restrict__ spread, int D, int hw) {
+  regress_body<IS_PROB, DT, false, true, PIX>(logits, dv, dv_is_vector, hyp, depth, conf, index,
+                                              prob, D, hw, spread);
 }
 
 // Plane-parallel variant (the default): the generic kernel above runs ~80 instructions per
@@ -236,12 +279,14 @@ regress_par_kernel(const float* __restrict__ logits, const float* __restrict__ d
 
 // The inverse-depth variant of regress_par_kernel (rule 5 above), the same walk with RN(1/d)
 // averaged.  regress_par_kernel keeps its own copy: moved into a shared device function, its
-// code (not its results) changed with ptxas's register assignment.
-template <bool IS_PROB, bool INV>
+// code (not its results) changed with ptxas's register assignment.  SPREAD / PIX: as in
+// regress_body; the spread's terms are formed plane-parallel like T1 and walked by warp 0.
+template <bool IS_PROB, bool INV, bool SPREAD = false, bool PIX = false>
 __device__ __forceinline__ void
 regress_par_body(const float* __restrict__ logits, const float* __restrict__ dv, int dv_is_vector,
                  const Hyp hyp, float* __restrict__ depth, float* __restrict__ conf,
-                 long long* __restrict__ index, float* __restrict__ prob, int D, int hw) {
+                 long long* __restrict__ index, float* __restrict__ prob, int D, int hw,
+                 float* __restrict__ spread = nullptr) {
   extern __shared__ float sh[];
   float* P = sh;                       // [D][32]  exp, then probability
   float* T1 = sh + (size_t)D * 32;     // [D][32]  p * depth_value
@@ -256,7 +301,7 @@ regress_par_body(const float* __restrict__ logits, const float* __restrict__ dv,
   // hypotheses: (D,) vector, (B,D,h,w) tensor, or (dv == null) the ladder first + step*d
   const float* dp = !dv ? nullptr : dv_is_vector ? dv : dv + (size_t)b * D * hw + pix;
   const size_t dstride = dv_is_vector ? 1 : (size_t)hw;
-  const HypPixT<INV> hp(hyp, b, D, (size_t)hw, pix);
+  const HypPixT<INV, PIX> hp(hyp, b, D, (size_t)hw, pix);
   float m = 0.f;
   if (!IS_PROB) {
     float lmax = -INFINITY;
@@ -288,6 +333,48 @@ regress_par_body(const float* __restrict__ logits, const float* __restrict__ dv,
     if (prob && valid) prob[(size_t)b * D * hw + (size_t)d * hw + pix] = pr;
   }
   __syncthreads();
+  if constexpr (SPREAD) {
+    // warp 0 finishes depth, index and confidence (every pixel, valid or not, so that the
+    // block meets at the barriers below) and leaves the depth in red[]
+    if (s == 0) {
+      Cascade16 acc_depth, acc_idx;
+      for (int d = 0; d < D; ++d) {
+        acc_depth.add(T1[d * 32 + p]);
+        acc_idx.add(T2[d * 32 + p]);
+      }
+      const float fidx = acc_idx.result();
+      int idx;
+      if (!(fidx > 0.f)) idx = 0;
+      else if (fidx >= (float)(D - 1)) idx = D - 1;
+      else idx = (int)fidx;
+      float c = 0.f;
+#pragma unroll
+      for (int k = -1; k <= 2; ++k) {
+        const int d = idx + k;
+        c = __fadd_rn(c, (d >= 0 && d < D) ? P[d * 32 + p] : 0.f);
+      }
+      const float dep = acc_depth.result();
+      red[p] = dep;
+      if (valid) {
+        depth[(size_t)b * hw + pix] = dep;
+        conf[(size_t)b * hw + pix] = c;
+        if (index) index[(size_t)b * hw + pix] = (long long)idx;
+      }
+    }
+    if (!spread) return;                 // the same for the whole block
+    __syncthreads();
+    const float dep = red[p];
+    for (int d = s; d < D; d += kK3Lanes) {
+      const float t = __fsub_rn(dp ? __ldg(dp + d * dstride) : hp.at(d), dep);
+      T1[d * 32 + p] = __fmul_rn(P[d * 32 + p], __fmul_rn(t, t));
+    }
+    __syncthreads();
+    if (s != 0 || !valid) return;
+    Cascade16 acc_var;
+    for (int d = 0; d < D; ++d) acc_var.add(T1[d * 32 + p]);
+    spread[(size_t)b * hw + pix] = __fsqrt_rn(acc_var.result());
+    return;
+  }
   if (s != 0 || !valid) return;
   Cascade16 acc_depth, acc_idx;
   for (int d = 0; d < D; ++d) {
@@ -317,6 +404,15 @@ regress_par_inv_kernel(const float* __restrict__ logits, const float* __restrict
                        float* __restrict__ conf, long long* __restrict__ index,
                        float* __restrict__ prob, int D, int hw) {
   regress_par_body<IS_PROB, true>(logits, dv, dv_is_vector, hyp, depth, conf, index, prob, D, hw);
+}
+template <bool IS_PROB, bool PIX>
+__global__ void __launch_bounds__(32 * kK3Lanes)
+regress_par_spread_kernel(const float* __restrict__ logits, const float* __restrict__ dv,
+                          int dv_is_vector, const Hyp hyp, float* __restrict__ depth,
+                          float* __restrict__ conf, long long* __restrict__ index,
+                          float* __restrict__ prob, float* __restrict__ spread, int D, int hw) {
+  regress_par_body<IS_PROB, false, true, PIX>(logits, dv, dv_is_vector, hyp, depth, conf, index,
+                                              prob, D, hw, spread);
 }
 
 // Pixel pix of (h,w) from the (B,h/2,w/2) map cur upsampled x2, bilinear with
@@ -411,6 +507,33 @@ inverse_hypotheses_kernel(const float* __restrict__ cur, float u_first,
   for (int d = 0; d < D; ++d) op[(size_t)d * hw] = inverse_plane(u0, step, d);
 }
 
+// Adaptive planes (rule 3 of "Adaptive depth ranges" above) from the previous stage's depth cur
+// and spread, both (B,h/2,w/2) and upsampled x2.  step / step_dev: g_l, a scalar or (B) device
+// values.  planes == D writes the planes (B,D,h,w) to out; planes == 1 writes the ladder's first
+// rung lo to out and its step to step_out, both (B,h,w).
+__global__ void __launch_bounds__(256)
+adaptive_hypotheses_kernel(const float* __restrict__ cur, const float* __restrict__ spread,
+                           float step, const float* __restrict__ step_dev, float* __restrict__ out,
+                           float* __restrict__ step_out, int D, int h, int w, int planes) {
+  const int b = blockIdx.y;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw = h * w;
+  if (pix >= hw) return;
+  if (step_dev) step = __ldg(step_dev + b);
+  const float c = upsample2x_at(cur, b, h, w, pix);
+  const float r = fmaxf(__fmul_rn(kAdaptiveLambda, upsample2x_at(spread, b, h, w, pix)), step);
+  const float lo = fmaxf(__fsub_rn(c, r), 1e-7f);
+  const float hi = __fadd_rn(c, r);
+  const float st = __fdiv_rn(__fsub_rn(hi, lo), (float)(D - 1));
+  if (planes == 1) {
+    out[(size_t)b * hw + pix] = lo;
+    step_out[(size_t)b * hw + pix] = st;
+    return;
+  }
+  float* op = out + (size_t)b * D * hw + pix;
+  for (int d = 0; d < D; ++d) op[(size_t)d * hw] = __fadd_rn(lo, __fmul_rn(st, (float)d));
+}
+
 }  // namespace casmvs
 
 using namespace casmvs;
@@ -463,6 +586,49 @@ static int regress_impl(const float* logits, const float* depth_values, int dv_i
   return after_launch("regress");
 }
 
+// The K3 forms of the adaptive mode: the uniform regression plus the spread (null: none) and,
+// PIX, the per-pixel-step ladder.  The same path choice as regress_impl.
+template <bool PIX>
+static int regress_spread_impl(const float* logits, const float* depth_values, int dv_is_vector,
+                               const Hyp& hyp, int input_is_prob, float* depth, float* confidence,
+                               int64_t* index, float* prob, float* spread, int B, int D, int h,
+                               int w, void* stream) {
+  CASMVS_REQUIRE(logits && depth && confidence, "regress: null pointer");
+  CASMVS_REQUIRE(B >= 0 && B <= 65535 && D > 0 && h > 0 && w > 0, "regress: bad dims");
+  if (B == 0) return 0;
+  const int hw = h * w;
+  cudaStream_t st = as_stream(stream);
+  const bool par_path = switches().k3_reg;
+  const size_t smem = ((size_t)3 * D * 32 + kK3Lanes * 32) * sizeof(float);
+  // a ladder is never a probability input: the per-pixel-step kernels exist for logits only
+  auto pick = [input_is_prob](auto kp, auto kl) { return input_is_prob ? kp : kl; };
+  if (D == 8 && par_path) {
+    const auto k = PIX ? regress_spread_kernel<false, 8, true>
+                       : pick(regress_spread_kernel<true, 8, false>, regress_spread_kernel<false, 8, false>);
+    dim3 grd8((hw + kK3Threads - 1) / kK3Threads, B);
+    k<<<grd8, kK3Threads, 0, st>>>(logits, depth_values, dv_is_vector, hyp, depth, confidence,
+                                   (long long*)index, prob, spread, D, hw);
+    return after_launch("regress");
+  }
+  if (par_path && smem <= 96 * 1024) {
+    const auto k = PIX ? regress_par_spread_kernel<false, true>
+                       : pick(regress_par_spread_kernel<true, false>, regress_par_spread_kernel<false, false>);
+    static std::atomic<bool> a[3][kMaxDevices];
+    if (int rc = opt_in_smem(k, 96 * 1024, a[PIX ? 2 : input_is_prob ? 1 : 0], "regress")) return rc;
+    dim3 grd((hw + 31) / 32, B);
+    k<<<grd, 32 * kK3Lanes, smem, st>>>(logits, depth_values, dv_is_vector, hyp, depth, confidence,
+                                        (long long*)index, prob, spread, D, hw);
+    return after_launch("regress");
+  }
+  const auto k = PIX ? regress_spread_kernel<false, 0, true>
+                     : pick(regress_spread_kernel<true, 0, false>, regress_spread_kernel<false, 0, false>);
+  const int threads = (long)hw * B < (long)num_sms() * 4 * kK3Threads ? 32 : kK3Threads;
+  dim3 grd((hw + threads - 1) / threads, B);
+  k<<<grd, threads, 0, st>>>(logits, depth_values, dv_is_vector, hyp, depth, confidence,
+                             (long long*)index, prob, spread, D, hw);
+  return after_launch("regress");
+}
+
 extern "C" int casmvs_regress_fwd(const float* logits, const float* depth_values,
                                   int dv_is_vector, int input_is_prob, float* depth,
                                   float* confidence, int64_t* index, float* prob, int B, int D,
@@ -497,6 +663,38 @@ extern "C" int casmvs_regress_ladder_inverse_fwd(const float* logits, const floa
   const Hyp hyp{nullptr, first_map, first_b, step_b, first, step};
   return regress_impl<true>(logits, nullptr, 0, hyp, 0, depth, confidence, index, nullptr, B, D, h,
                             w, stream);
+}
+
+// casmvs_regress_fwd (uniform regression only) that also writes the spread (B,h,w).
+extern "C" int casmvs_regress_spread_fwd(const float* logits, const float* depth_values,
+                                         int dv_is_vector, int input_is_prob, float* depth,
+                                         float* confidence, int64_t* index, float* prob,
+                                         float* spread, int B, int D, int h, int w, void* stream) {
+  CASMVS_REQUIRE(depth_values && spread, "regress_spread: null pointer");
+  CASMVS_REQUIRE((input_is_prob & ~1) == 0, "regress_spread: bad input_is_prob flags");
+  const Hyp hyp{depth_values, nullptr, nullptr, nullptr, 0.f, 0.f};
+  return regress_spread_impl<false>(logits, depth_values, dv_is_vector, hyp, input_is_prob, depth,
+                                    confidence, index, prob, spread, B, D, h, w, stream);
+}
+
+// casmvs_regress_ladder_fwd with the spread (may be null only with step_map) and the per-pixel
+// step: step_map (B,h,w) non-null takes the ladder first_map + step_map*d (first_map required).
+extern "C" int casmvs_regress_ladder_spread_fwd(const float* logits, const float* first_map,
+                                                const float* first_b, float first,
+                                                const float* step_b, float step,
+                                                const float* step_map, float* depth,
+                                                float* confidence, int64_t* index, float* spread,
+                                                int B, int D, int h, int w, void* stream) {
+  if (step_map) {
+    CASMVS_REQUIRE(first_map, "regress_ladder_spread: a step map needs a first map");
+    const Hyp hyp{nullptr, first_map, nullptr, step_map, 0.f, 0.f};
+    return regress_spread_impl<true>(logits, nullptr, 0, hyp, 0, depth, confidence, index, nullptr,
+                                     spread, B, D, h, w, stream);
+  }
+  CASMVS_REQUIRE(spread, "regress_ladder_spread: null spread without a step map");
+  const Hyp hyp{nullptr, first_map, first_b, step_b, first, step};
+  return regress_spread_impl<false>(logits, nullptr, 0, hyp, 0, depth, confidence, index, nullptr,
+                                    spread, B, D, h, w, stream);
 }
 
 extern "C" int casmvs_depth_hypotheses_fwd(const float* cur, int upsample, float half_range,
@@ -554,4 +752,21 @@ extern "C" int casmvs_inverse_hypotheses_fwd(const float* cur, float u_first, co
   inverse_hypotheses_kernel<<<grd, 256, 0, as_stream(stream)>>>(
       cur, u_first, u_first_dev, u_far, u_far_dev, step, step_dev, out, D, h, w, planes);
   return after_launch("inverse_hypotheses");
+}
+
+extern "C" int casmvs_adaptive_hypotheses_fwd(const float* cur, const float* spread, float step,
+                                              const float* step_dev, float* out, float* step_out,
+                                              int planes, int B, int D, int h, int w,
+                                              void* stream) {
+  CASMVS_REQUIRE(cur && spread && out, "adaptive_hypotheses: null pointer");
+  CASMVS_REQUIRE(B >= 0 && B <= 65535 && D >= 2 && h > 0 && w > 0,
+                 "adaptive_hypotheses: bad dims (D >= 2)");
+  CASMVS_REQUIRE(planes == D || (planes == 1 && step_out),
+                 "adaptive_hypotheses: planes must be D, or 1 with step_out");
+  CASMVS_REQUIRE(h % 2 == 0 && w % 2 == 0, "adaptive_hypotheses: upsample needs even h,w");
+  if (B == 0) return 0;
+  dim3 grd((h * w + 255) / 256, B);
+  adaptive_hypotheses_kernel<<<grd, 256, 0, as_stream(stream)>>>(cur, spread, step, step_dev, out,
+                                                                 step_out, D, h, w, planes);
+  return after_launch("adaptive_hypotheses");
 }

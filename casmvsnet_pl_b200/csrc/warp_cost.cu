@@ -389,7 +389,7 @@ extern "C" int casmvs_warp_cost_fwd(const float* feats, int feat_layout, const f
   const unsigned xblocks = (unsigned)((threads + kK1Threads - 1) / kK1Threads);
   if (StagedK1 run = nhwc ? warp_cost_staged(V, C, num_groups) : nullptr) {
     const Hyp hyp{depth_values, nullptr, nullptr, nullptr, 0.f, 0.f};
-    return run(f, proj, hyp, cost, B, D, h, w, rnd, 0, 0, st);
+    return run(f, proj, hyp, cost, B, D, h, w, rnd, 0, kLadderUniform, st);
   }
   // depth chunks: enough CTAs to fill every SM several times over, but chunks long
   // enough (>= 8 planes) for the texel-window cache to pay off
@@ -469,8 +469,34 @@ extern "C" int casmvs_warp_cost_ladder_fwd(const float* feats, const float* proj
                  "(casmvs_warp_cost_ladder_supported): materialise the hypotheses and call "
                  "casmvs_warp_cost_fwd (got V=%d C=%d G=%d)", V, C, num_groups);
   const int blocked = (round_tf32 & CASMVS_BLOCKED) ? 1 : 0;
-  const int inverse = (round_tf32 & CASMVS_INVERSE_DEPTH) ? 1 : 0;
+  const int form = (round_tf32 & CASMVS_INVERSE_DEPTH) ? kLadderInverse : kLadderUniform;
   const int rnd = (round_tf32 & ~(CASMVS_BLOCKED | CASMVS_INVERSE_DEPTH)) ? 1 : 0;
   const Hyp hyp{nullptr, first_map, first_b, step_b, first, step};
-  return run(feats, proj, hyp, cost, B, D, h, w, rnd, blocked, inverse, as_stream(stream));
+  return run(feats, proj, hyp, cost, B, D, h, w, rnd, blocked, form, as_stream(stream));
+}
+
+// The per-pixel-step ladder of the adaptive mode (README "Adaptive depth ranges", regress.cu):
+// plane d of pixel p is first_map[p] + step_map[p]*d, multiply and add each rounded.  Same
+// coverage, layouts and flags (1, CASMVS_BLOCKED) as casmvs_warp_cost_ladder_fwd.
+extern "C" int casmvs_warp_cost_ladder_step_fwd(const float* feats, const float* proj,
+                                                const float* first_map, const float* step_map,
+                                                float* cost, int round_tf32, int B, int V, int C,
+                                                int D, int h, int w, int num_groups, void* stream) {
+  CASMVS_REQUIRE_ALIGNED("warp_cost_ladder_step", feats, 16);
+  CASMVS_REQUIRE_ALIGNED("warp_cost_ladder_step", cost, 16);
+  CASMVS_REQUIRE(feats && proj && cost && first_map && step_map,
+                 "warp_cost_ladder_step: null pointer");
+  CASMVS_REQUIRE(B >= 0 && B <= 65535 && V >= 2 && C > 0 && D > 0 && h >= 2 && w >= 2,
+                 "warp_cost_ladder_step: bad dims (h,w >= 2)");
+  CASMVS_REQUIRE((size_t)h * w * C < (1u << 31), "warp_cost_ladder_step: view too large");
+  CASMVS_REQUIRE((round_tf32 & ~(1 | CASMVS_BLOCKED)) == 0, "warp_cost_ladder_step: bad flags");
+  if (B == 0) return 0;
+  const StagedK1 run = warp_cost_staged(V, C, num_groups);
+  CASMVS_REQUIRE(run, "warp_cost_ladder_step: shape not covered by the staged kernel "
+                 "(casmvs_warp_cost_ladder_supported): materialise the hypotheses and call "
+                 "casmvs_warp_cost_fwd (got V=%d C=%d G=%d)", V, C, num_groups);
+  const int blocked = (round_tf32 & CASMVS_BLOCKED) ? 1 : 0;
+  const Hyp hyp{nullptr, first_map, nullptr, step_map, 0.f, 0.f};
+  return run(feats, proj, hyp, cost, B, D, h, w, round_tf32 & 1, blocked, kLadderPixelStep,
+             as_stream(stream));
 }

@@ -187,9 +187,11 @@ __device__ __forceinline__ int stage_boxes(const Tile<NSRC>& t, const CUtensorMa
 // plane-group kernel below re-uses them); variance or 8-group correlation epilogue.
 // BLOCKED: the cost volume is stored blocked by channel quads (B, COUT/4, D, h, w, 4) instead of
 // channels-last.  A template parameter: as a run-time value it cost the channels-last kernels
-// about 5 % of their rate.  INV: a ladder is in inverse depth (HypPixT).  The body of
-// warp_var_smem_kernel (uniform) and warp_var_smem_inv_kernel below.
-template <int NSRC, int C, int TW, int TH, int MINB, bool GWC, bool BLOCKED, bool INV>
+// about 5 % of their rate.  INV: a ladder is in inverse depth (HypPixT).  PIX: a ladder has a
+// per-pixel step map (the adaptive mode).  The body of warp_var_smem_kernel (uniform),
+// warp_var_smem_inv_kernel and warp_var_smem_pix_kernel below.
+template <int NSRC, int C, int TW, int TH, int MINB, bool GWC, bool BLOCKED, bool INV,
+          bool PIX = false>
 __device__ __forceinline__ void
 warp_var_smem(const CUtensorMap& fmap, const float* __restrict__ feats,
               const float* __restrict__ proj, const Hyp hyp,
@@ -213,7 +215,7 @@ warp_var_smem(const CUtensorMap& fmap, const float* __restrict__ feats,
 
   const int d_begin = blockIdx.z * dchunk;
   const int d_end = min(D, d_begin + dchunk);
-  const HypPixT<INV> hp(hyp, b, D, (size_t)hw, pix);
+  const HypPixT<INV, PIX> hp(hyp, b, D, (size_t)hw, pix);
   // output: channels-last, or blocked by channel quads (B, COUT/4, D, h, w, 4)
   const int co = GWC ? t.sub * NG : c0;
   const size_t pstr = BLOCKED ? (size_t)hw * 4 : (size_t)hw * COUT;      // next plane
@@ -331,6 +333,15 @@ warp_var_smem_inv_kernel(const __grid_constant__ CUtensorMap fmap, const float* 
   warp_var_smem<NSRC, C, TW, TH, MINB, GWC, BLOCKED, true>(
       fmap, feats, proj, hyp, cost, D, h, w, dchunk, BW, BH, box_stride, tiles_x, round_tf32);
 }
+template <int NSRC, int C, int TW, int TH, int MINB, bool GWC, bool BLOCKED>
+__global__ void __launch_bounds__(TW* TH*(C / kCPT), MINB)
+warp_var_smem_pix_kernel(const __grid_constant__ CUtensorMap fmap, const float* __restrict__ feats,
+                         const float* __restrict__ proj, const Hyp hyp, float* __restrict__ cost,
+                         int D, int h, int w, int dchunk, int BW, int BH, int box_stride,
+                         int tiles_x, int round_tf32) {
+  warp_var_smem<NSRC, C, TW, TH, MINB, GWC, BLOCKED, false, true>(
+      fmap, feats, proj, hyp, cost, D, h, w, dchunk, BW, BH, box_stride, tiles_x, round_tf32);
+}
 
 // ---- plane-group variant: window reuse WITHOUT persistent registers -----------------------------
 // Both K1 generations are bound by the LSU data pipe (32 B of tap traffic per output float),
@@ -342,7 +353,7 @@ warp_var_smem_inv_kernel(const __grid_constant__ CUtensorMap fmap, const float* 
 // persists between the views is one blended value per (plane, channel) -- 8 registers per plane.
 // 2 source views, variance cost.  out = (ref^2 + r1^2 + r2^2)/3 - ((ref + r1 + r2)/3)^2, summed
 // in the order of the kernel above (bit-identical).
-template <int C, int TW, int TH, int PG, int MINB, bool BLOCKED, bool INV>
+template <int C, int TW, int TH, int PG, int MINB, bool BLOCKED, bool INV, bool PIX = false>
 __device__ __forceinline__ void
 warp_var_smem_pg(const CUtensorMap& fmap, const float* __restrict__ feats,
                  const float* __restrict__ proj, const Hyp hyp, float* __restrict__ cost,
@@ -361,7 +372,7 @@ warp_var_smem_pg(const CUtensorMap& fmap, const float* __restrict__ feats,
   const u64 inv_v2 = pk2(inv_v, inv_v), ninv_v2 = pk2(-inv_v, -inv_v);
   const int d_begin = blockIdx.z * dchunk;
   const int d_end = min(D, d_begin + dchunk);
-  const HypPixT<INV> hp(hyp, b, D, (size_t)hw, pix);
+  const HypPixT<INV, PIX> hp(hyp, b, D, (size_t)hw, pix);
   // output: channels-last, or blocked by channel quads (B, C/4, D, h, w, 4)
   const size_t pstr = BLOCKED ? (size_t)hw * 4 : (size_t)hw * C;        // next plane
   const size_t qstr = BLOCKED ? (size_t)D * hw * 4 : 4;                 // next channel quad
@@ -470,6 +481,16 @@ warp_var_smem_pg_inv_kernel(const __grid_constant__ CUtensorMap fmap,
   warp_var_smem_pg<C, TW, TH, PG, MINB, BLOCKED, true>(
       fmap, feats, proj, hyp, cost, D, h, w, dchunk, BW, BH, box_stride, tiles_x, round_tf32);
 }
+template <int C, int TW, int TH, int PG, int MINB, bool BLOCKED>
+__global__ void __launch_bounds__(TW* TH*(C / kCPT), MINB)
+warp_var_smem_pg_pix_kernel(const __grid_constant__ CUtensorMap fmap,
+                            const float* __restrict__ feats, const float* __restrict__ proj,
+                            const Hyp hyp, float* __restrict__ cost, int D, int h, int w,
+                            int dchunk, int BW, int BH, int box_stride, int tiles_x,
+                            int round_tf32) {
+  warp_var_smem_pg<C, TW, TH, PG, MINB, BLOCKED, false, true>(
+      fmap, feats, proj, hyp, cost, D, h, w, dchunk, BW, BH, box_stride, tiles_x, round_tf32);
+}
 
 // ---- host side -------------------------------------------------------------------------------
 // The features (BV, h, w, C) as {C, w, h, BV}, box {C, BW, BH, 1}, swizzle C*4 bytes.
@@ -483,10 +504,11 @@ static int feature_map(CUtensorMap* out, const float* feats, int BV, int h, int 
 }
 
 // One launcher for both kernels: NSRC source views, TW x TH pixel tiles.  PG > 0 launches the
-// plane-group kernel, whose box row is rounded up to a multiple of 1024 B (see rowal).
+// plane-group kernel, whose box row is rounded up to a multiple of 1024 B (see rowal).  form: the
+// ladder form (LadderForm), which picks the uniform, _inv or _pix instantiation.
 template <int NSRC, int C, int TW, int TH, int MINB, bool GWC, int PG>
 static int launch(const float* feats, const float* proj, const Hyp& dv, float* cost, int B, int D,
-                  int h, int w, int rnd, int blocked, int inverse, cudaStream_t st) {
+                  int h, int w, int rnd, int blocked, int form, cudaStream_t st) {
   constexpr int NT = TW * TH * (C / kCPT);
   // box = tile + margins: sweep of the depth run + scale/rotation of the view + the 2x2 window
   constexpr int wq = PG > 0 ? 1024 / (C * 4) : 1;
@@ -494,23 +516,29 @@ static int launch(const float* feats, const float* proj, const Hyp& dv, float* c
   constexpr int box_stride = (BW * BH * C * 4 + 1023) & ~1023;
   constexpr size_t smem = (size_t)NSRC * box_stride + sizeof(Small) + 1024;
   static_assert(smem <= 200 * 1024, "shared memory budget");
-  auto kfn = [blocked, inverse] {
+  auto kfn = [blocked, form] {
     if constexpr (PG > 0) {
-      if (inverse)
+      if (form == kLadderPixelStep)
+        return blocked ? warp_var_smem_pg_pix_kernel<C, TW, TH, PG, MINB, true>
+                       : warp_var_smem_pg_pix_kernel<C, TW, TH, PG, MINB, false>;
+      if (form == kLadderInverse)
         return blocked ? warp_var_smem_pg_inv_kernel<C, TW, TH, PG, MINB, true>
                        : warp_var_smem_pg_inv_kernel<C, TW, TH, PG, MINB, false>;
       return blocked ? warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, true>
                      : warp_var_smem_pg_kernel<C, TW, TH, PG, MINB, false>;
     } else {
-      if (inverse)
+      if (form == kLadderPixelStep)
+        return blocked ? warp_var_smem_pix_kernel<NSRC, C, TW, TH, MINB, GWC, true>
+                       : warp_var_smem_pix_kernel<NSRC, C, TW, TH, MINB, GWC, false>;
+      if (form == kLadderInverse)
         return blocked ? warp_var_smem_inv_kernel<NSRC, C, TW, TH, MINB, GWC, true>
                        : warp_var_smem_inv_kernel<NSRC, C, TW, TH, MINB, GWC, false>;
       return blocked ? warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, true>
                      : warp_var_smem_kernel<NSRC, C, TW, TH, MINB, GWC, false>;
     }
   }();
-  static std::atomic<bool> attr_set[2][2][kMaxDevices];
-  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[inverse ? 1 : 0][blocked ? 1 : 0], "warp_cost"))
+  static std::atomic<bool> attr_set[3][2][kMaxDevices];
+  if (int rc = opt_in_smem(kfn, 200 * 1024, attr_set[form][blocked ? 1 : 0], "warp_cost"))
     return rc;
   CUtensorMap map;
   if (int rc = feature_map(&map, feats, B * (NSRC + 1), h, w, C, BW, BH)) return rc;

@@ -743,9 +743,12 @@ def parse_args(argv=None):
                          "--min_geo_consistent sources within 1 px and 1 %% depth) or dynamic "
                          "(for some k in 2..10, at least k sources within k/4 px and k/1300 "
                          "relative depth)")
-    ap.add_argument("--depth_sampling", choices=["uniform", "inverse"], default=argparse.SUPPRESS,
-                    help="plane spacing of the sweep: uniform (default; evenly in depth) or inverse "
-                         "(evenly in 1/depth and regressed in 1/depth, for wide depth ranges)")
+    ap.add_argument("--depth_sampling", choices=["uniform", "inverse", "adaptive"],
+                    default=argparse.SUPPRESS,
+                    help="plane spacing of the sweep: uniform (default; evenly in depth), inverse "
+                         "(evenly in 1/depth and regressed in 1/depth, for wide depth ranges) or "
+                         "adaptive (each finer stage searches +-1.5 spreads of the previous stage's "
+                         "probability volume, at least +-its uniform step)")
     ap.add_argument("--max_ref_views", type=int, default=400)
     ap.add_argument("--skip", type=int, default=1)
     ap.add_argument("--precision", default="tf32", choices=["fp32", "tf32"])

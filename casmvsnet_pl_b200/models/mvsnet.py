@@ -406,6 +406,8 @@ class CascadeMVSNet(nn.Module):
         # confidence gather uses; the reference keeps them internal
         self.return_index = False
         self._last_index = None
+        # adaptive depth sampling: the spread (B,h,w) of the stage run last, None when it wrote none
+        self._last_spread = None
         # cascade-internal fusion: K4 writes only the first rung of each stage's hypothesis ladder
         # and K1 / K3 generate first + step*d themselves (bit-identical results; the (B,D,h,w)
         # hypothesis tensor is neither written nor read)
@@ -416,16 +418,26 @@ class CascadeMVSNet(nn.Module):
         self.set_precision(precision)
         self.set_depth_sampling(depth_sampling)
 
-    DEPTH_SAMPLINGS = ("uniform", "inverse")
+    DEPTH_SAMPLINGS = ("uniform", "inverse", "adaptive")
 
     def set_depth_sampling(self, depth_sampling):
-        """'uniform' (the reference: planes evenly spaced in depth) or 'inverse' (evenly spaced in
-        1/depth, regressed in 1/depth; README "Wide depth ranges").  Not part of the state dict:
-        the same weights run either way."""
+        """'uniform' (the reference: planes evenly spaced in depth), 'inverse' (evenly spaced in
+        1/depth, regressed in 1/depth; README "Wide depth ranges") or 'adaptive' (each finer
+        stage's window sized from the previous stage's probability spread; README "Adaptive depth
+        ranges").  Not part of the state dict: the same weights run either way."""
         if depth_sampling not in self.DEPTH_SAMPLINGS:
             raise ValueError(f"depth_sampling must be one of {list(self.DEPTH_SAMPLINGS)}")
+        if depth_sampling == "adaptive":
+            ops.check_adaptive_depths(self.n_depths)
         self.depth_sampling = depth_sampling
         return self
+
+    def _adaptive(self):
+        """True in the adaptive mode; checks the depth counts again (n_depths may have changed)."""
+        if self.depth_sampling != "adaptive":
+            return False
+        ops.check_adaptive_depths(self.n_depths)
+        return True
 
     def inverse_steps(self, init_depth_min, depth_interval, B, device):
         """ops.inverse_steps for this model's stages (inverse mode), else None."""
@@ -446,22 +458,32 @@ class CascadeMVSNet(nn.Module):
         self.feature.allow_tf32 = precision == "tf32"
         return self
 
-    def predict_depth(self, feats, proj_mats, depth_values, cost_reg, inverse=False):
+    def predict_depth(self, feats, proj_mats, depth_values, cost_reg, inverse=False,
+                      want_spread=False):
         """feats (B,V,C,h,w), proj_mats (B,V-1,3,4), depth_values (B,D,h,w),
         cost_reg: module (B,C,D,h,w)->(B,1,D,h,w).  Returns depth, confidence (B,h,w)
-        (reference models/mvsnet.py:125-195).  inverse: regress in 1/depth."""
+        (reference models/mvsnet.py:125-195).  inverse: regress in 1/depth.  want_spread: the
+        adaptive mode's spread goes to self._last_spread (else None)."""
+        self._last_spread = None
         if torch.is_grad_enabled() and (feats.requires_grad or
                                         any(p.requires_grad for p in cost_reg.parameters())):
             from .. import autograd as AG
             cost = AG.warp_cost(feats, proj_mats, depth_values, self.G)
             logits = cost_reg(cost).squeeze(1)
+            if want_spread:
+                depth, confidence, self._last_spread = AG.regress(logits, depth_values, want_spread=True)
+                return depth, confidence
             return AG.regress(logits, depth_values, inverse=inverse)
         cost = ops.warp_cost(feats, proj_mats, depth_values, self.G, ops.NHWC,
                              round_tf32=(getattr(cost_reg, "precision", "fp32") == "tf32"))
         logits = cost_reg(cost).squeeze(1)
         del cost
-        depth, confidence, index, _ = ops.regress(logits, depth_values,
-                                                  want_index=self.return_index, inverse=inverse)
+        if want_spread:
+            depth, confidence, index, _, self._last_spread = ops.regress(
+                logits, depth_values, want_index=self.return_index, want_spread=True)
+        else:
+            depth, confidence, index, _ = ops.regress(logits, depth_values,
+                                                      want_index=self.return_index, inverse=inverse)
         self._last_index = index
         return depth, confidence
 
@@ -477,10 +499,11 @@ class CascadeMVSNet(nn.Module):
         torch.backends.cudnn.allow_tf32 = self.precision == "tf32"
         # before the feature net: the range check's synchronise then waits for a few tiny ops only
         inv = self.inverse_steps(init_depth_min, depth_interval, B, imgs.device)
+        adaptive = self._adaptive()
         feats = self.feature(imgs.reshape(B * V, 3, H, W))
         proj_by_level = proj_mats.permute(2, 0, 1, 3, 4).contiguous()
         results = {}
-        depth_l = None
+        depth_l = spread_l = None
         for l in reversed(range(self.levels)):
             feats_l = feats[f"level_{l}"]
             feats_l = feats_l.view(B, V, *feats_l.shape[1:])
@@ -492,6 +515,9 @@ class CascadeMVSNet(nn.Module):
                     depth_values = ops.inverse_hypotheses(
                         inv, l, D, h, w, imgs.device,
                         current_depth=None if l == self.levels - 1 else depth_l.detach())
+                elif adaptive and l != self.levels - 1:
+                    depth_values = ops.adaptive_hypotheses(depth_l.detach(), spread_l, D,
+                                                           depth_interval_l)
                 elif l == self.levels - 1:
                     depth_values = ops.uniform_hypotheses(init_depth_min, depth_interval_l, D, B,
                                                           h, w, imgs.device)
@@ -500,7 +526,9 @@ class CascadeMVSNet(nn.Module):
                                                         upsample=True)
             depth_l, confidence_l = self.predict_depth(feats_l, proj_by_level[l], depth_values,
                                                        getattr(self, f"cost_reg_{l}"),
-                                                       inverse=inv is not None)
+                                                       inverse=inv is not None,
+                                                       want_spread=adaptive and l > 0)
+            spread_l = self._last_spread
             results[f"depth_{l}"] = depth_l
             results[f"confidence_{l}"] = confidence_l
         return results
@@ -518,21 +546,33 @@ class CascadeMVSNet(nn.Module):
         return [b for b in bufs if torch.is_tensor(b) and b.is_cuda]
 
     def run_stage(self, l, feats_l, proj_mats_l, depth_prev, init_depth_min, depth_interval,
-                  inv=None):
+                  inv=None, spread_prev=None):
         """One cascade stage of the inference path (no grad): hypotheses -> K1 -> K2 -> K3.
         feats_l (B,V,C,h,w) channels-last, proj_mats_l (B,V-1,3,4), depth_prev (B,h/2,w/2) or None
         for the coarsest stage.  Returns depth, confidence (B,h,w).  In the inverse depth sampling
-        inv is the forward's ops.InverseSteps (computed here when None)."""
+        inv is the forward's ops.InverseSteps (computed here when None).  In the adaptive sampling
+        spread_prev is the previous stage's spread (B,h/2,w/2), and a stage l > 0 leaves its own in
+        self._last_spread."""
         B, V, C, h, w = feats_l.shape
         D = self.n_depths[l]
         depth_interval_l = depth_interval * self.interval_ratios[l]
         cost_reg = getattr(self, f"cost_reg_{l}")
         inverse = self.depth_sampling == "inverse"
+        adaptive = self._adaptive()
+        want_spread = adaptive and l > 0
+        if adaptive and depth_prev is not None and spread_prev is None:
+            raise ops._lib.CasMVSError("adaptive depth sampling: a finer stage needs the previous "
+                                       "stage's spread (spread_prev)")
         if inverse and inv is None:
             inv = self.inverse_steps(init_depth_min, depth_interval, B, feats_l.device)
+        self._last_spread = None
         if self.fuse_hypotheses and ops.ladder_supported(V, C, self.G) and \
                 ops.is_channels_last_feats(feats_l):
-            if inverse:
+            if adaptive and depth_prev is not None:
+                first, step = ops.adaptive_hypotheses(depth_prev, spread_prev, D, depth_interval_l,
+                                                      first_only=True)
+                lad = ops.Ladder(first, step, D, B, h, w, feats_l.device)
+            elif inverse:
                 first = inv.u_near if depth_prev is None else ops.inverse_hypotheses(
                     inv, l, D, h, w, feats_l.device, current_depth=depth_prev, first_only=True)
                 lad = ops.Ladder(first, inv.step[l], D, B, h, w, feats_l.device, inverse=True)
@@ -546,10 +586,16 @@ class CascadeMVSNet(nn.Module):
                                         round_tf32=(cost_reg.precision == "tf32"), blocked=blocked)
             logits = cost_reg.forward_blocked(cost) if blocked else cost_reg(cost).squeeze(1)
             del cost
+            if want_spread:
+                depth, confidence, self._last_index, self._last_spread = ops.regress_ladder(
+                    logits, lad, want_index=self.return_index, want_spread=True)
+                return depth, confidence
             depth, confidence, self._last_index = ops.regress_ladder(logits, lad,
                                                                      want_index=self.return_index)
             return depth, confidence
-        if inverse:
+        if adaptive and depth_prev is not None:
+            depth_values = ops.adaptive_hypotheses(depth_prev, spread_prev, D, depth_interval_l)
+        elif inverse:
             depth_values = ops.inverse_hypotheses(inv, l, D, h, w, feats_l.device,
                                                   current_depth=depth_prev)
         elif depth_prev is None:
@@ -557,7 +603,8 @@ class CascadeMVSNet(nn.Module):
                                                   feats_l.device)
         else:
             depth_values = ops.depth_hypotheses(depth_prev, D, depth_interval_l, upsample=True)
-        return self.predict_depth(feats_l, proj_mats_l, depth_values, cost_reg, inverse=inverse)
+        return self.predict_depth(feats_l, proj_mats_l, depth_values, cost_reg, inverse=inverse,
+                                  want_spread=want_spread)
 
     def forward(self, imgs, proj_mats, init_depth_min, depth_interval):
         """imgs (B,V,3,H,W); proj_mats (B,V-1,levels,3,4) fine->coarse;
@@ -581,11 +628,12 @@ class CascadeMVSNet(nn.Module):
         with torch.no_grad():
             # before the feature net: the range check's synchronise then waits for a few tiny ops
             inv = self.inverse_steps(init_depth_min, depth_interval, B, imgs.device)
+            self._adaptive()                        # refuses bad depth counts before any GPU work
             feats = self.feature(imgs.reshape(B * V, 3, H, W), overlap=self.overlap_pyramid)
             ready = feats.get("_ready", {})
             # one re-layout for all levels instead of a strided slice copy per stage
             proj_by_level = proj_mats.permute(2, 0, 1, 3, 4).contiguous()
-            depth_l = None
+            depth_l = spread_l = None
             for l in reversed(range(self.levels)):
                 if l in ready:                      # level produced on the side stream
                     torch.cuda.current_stream(imgs.device).wait_event(ready[l])
@@ -593,7 +641,8 @@ class CascadeMVSNet(nn.Module):
                 feats_l = feats_l.view(B, V, *feats_l.shape[1:])
                 proj_mats_l = proj_by_level[l]
                 depth_l, confidence_l = self.run_stage(l, feats_l, proj_mats_l, depth_l,
-                                                       init_depth_min, depth_interval, inv)
+                                                       init_depth_min, depth_interval, inv, spread_l)
+                spread_l = self._last_spread
                 results[f"depth_{l}"] = depth_l
                 results[f"confidence_{l}"] = confidence_l
                 if self.return_index:

@@ -274,10 +274,14 @@ def costreg(x, params, cin, precision=FP32, blocked=False, fused_tail=True):
 # --------------------------------------------------------------------------- K3
 @_on_tensor_device
 def regress(logits, depth_values, input_is_prob=False, want_index=False, want_prob=False,
-            inverse=False):
+            inverse=False, want_spread=False):
     """softmax + soft-argmax depth + confidence (+ index, prob).
     logits (B,D,h,w); depth_values (B,D,h,w) or (D,).  inverse=True regresses in 1/depth:
-    depth = 1/sum_d p_d/depth_values_d (README "Wide depth ranges")."""
+    depth = 1/sum_d p_d/depth_values_d (README "Wide depth ranges").  want_spread=True also
+    returns the spread sqrt(sum_d p_d (depth_values_d - depth)^2) (B,h,w) as a fifth value
+    (README "Adaptive depth ranges"); the other outputs are the same bits as without it."""
+    if want_spread and inverse:
+        raise _lib.CasMVSError("regress: want_spread is the adaptive mode's, not the inverse mode's")
     _require_cuda(logits, depth_values)
     _no_grad_only(logits)
     lg = logits.contiguous()
@@ -288,6 +292,12 @@ def regress(logits, depth_values, input_is_prob=False, want_index=False, want_pr
     conf = torch.empty_like(depth)
     index = torch.empty(B, h, w, device=lg.device, dtype=torch.int64) if want_index else None
     prob = torch.empty_like(lg) if want_prob else None
+    if want_spread:
+        spread = torch.empty_like(depth)
+        check(_lib.load().casmvs_regress_spread_fwd(_ptr(lg), _ptr(dv), int(dv_vec), int(bool(input_is_prob)),
+                                                    _ptr(depth), _ptr(conf), _ptr(index), _ptr(prob),
+                                                    _ptr(spread), B, D, h, w, _stream()), "regress")
+        return depth, conf, index, prob, spread
     flags = int(bool(input_is_prob)) | (INVERSE_DEPTH if inverse else 0)
     check(_lib.load().casmvs_regress_fwd(_ptr(lg), _ptr(dv), int(dv_vec), flags,
                                          _ptr(depth), _ptr(conf), _ptr(index), _ptr(prob),
@@ -442,17 +452,69 @@ def inverse_hypotheses(steps, level, n_depths, h, w, device, current_depth=None,
         return out
 
 
+# --------------------------------------------------------------------------- adaptive depth
+# lambda of the adaptive mode: a finer stage searches +-max(lambda*spread, its uniform step)
+# around the upsampled depth (UCS-Net's value; kAdaptiveLambda in csrc/regress.cu)
+ADAPTIVE_LAMBDA = 1.5
+
+
+def check_adaptive_depths(n_depths):
+    """The adaptive mode spaces D_l planes over a window: every finer stage needs D_l >= 2."""
+    for l, D in enumerate(n_depths[:-1]):
+        if D < 2:
+            raise _lib.CasMVSError(f"adaptive depth sampling needs at least 2 planes in every finer "
+                                   f"stage: stage {l} has {D}")
+
+
+@_on_tensor_device
+def adaptive_hypotheses(depth_prev, spread_prev, D, step_l, first_only=False):
+    """The planes of a finer stage in the adaptive mode (README "Adaptive depth ranges", rule in
+    csrc/regress.cu): depth_prev and spread_prev (B,h/2,w/2) are upsampled x2 to c and s,
+    r = max(ADAPTIVE_LAMBDA*s, step_l), lo = max(c - r, 1e-7), hi = c + r, step = (hi - lo)/(D-1)
+    and plane k = lo + step*k.  step_l: the stage's uniform step (depth_interval * ratio), a
+    float or a (B,)/(B,1) tensor.  Returns the planes (B,D,h,w), or with first_only=True the
+    (first, step) maps (B,h,w) of a per-pixel-step Ladder."""
+    if D < 2:
+        raise _lib.CasMVSError(f"adaptive_hypotheses needs D >= 2 planes (got {D})")
+    _require_cuda(depth_prev, spread_prev)
+    cur, spr = depth_prev.contiguous(), spread_prev.contiguous()
+    B, hi, wi = cur.shape
+    assert spr.shape == cur.shape and spr.device == cur.device
+    h, w = 2 * hi, 2 * wi
+    step, step_dev = _interval_args(step_l, B, cur.device)
+    if first_only:
+        out = torch.empty(B, h, w, device=cur.device, dtype=torch.float32)
+        step_out = torch.empty_like(out)
+    else:
+        out, step_out = torch.empty(B, D, h, w, device=cur.device, dtype=torch.float32), None
+    check(_lib.load().casmvs_adaptive_hypotheses_fwd(_ptr(cur), _ptr(spr), step, _ptr(step_dev), _ptr(out),
+                                                     _ptr(step_out), 1 if first_only else D, B, D, h, w,
+                                                     _stream()), "adaptive_hypotheses")
+    return (out, step_out) if first_only else out
+
+
 # --------------------------------------------------------------------------- ladder forms
 class Ladder:
     """Hypotheses first + step*d of one cascade stage, never materialised as (B,D,h,w):
     `first` is a (B,h,w) tensor [per-pixel], a (B,) tensor [per batch item] or a float; `step` a
-    (B,) tensor or a float; D planes.  `materialize()` gives the tensor the public API takes.
+    (B,h,w) tensor [per pixel: the adaptive mode; `first` must then be per-pixel too], a (B,)
+    tensor or a float; D planes.  `materialize()` gives the tensor the public API takes.
     inverse=True: the ladder is in inverse depth, the hypotheses are 1/(first - step*d) with
     first and step in 1/depth units (inverse_hypotheses)."""
 
     def __init__(self, first, step, D, B, h, w, device, inverse=False):
         self.first, self.step, self.D, self.B, self.h, self.w, self.device = first, step, D, B, h, w, device
         self.inverse = inverse
+        if self.step_map is not None:
+            if inverse:
+                raise _lib.CasMVSError("Ladder: a per-pixel step is the adaptive mode's, not the inverse mode's")
+            if not (torch.is_tensor(first) and first.dim() == 3):
+                raise _lib.CasMVSError("Ladder: a per-pixel step needs a per-pixel (B,h,w) first")
+
+    @property
+    def step_map(self):
+        """The (B,h,w) per-pixel step, or None."""
+        return self.step.contiguous() if torch.is_tensor(self.step) and self.step.dim() == 3 else None
 
     def _args(self):
         fm = fb = sb = None
@@ -475,6 +537,8 @@ class Ladder:
         first = self.first if torch.is_tensor(self.first) else torch.tensor(float(self.first), device=self.device)
         step = self.step if torch.is_tensor(self.step) else torch.tensor(float(self.step), device=self.device)
         first = first.view(self.B, 1, self.h, self.w) if first.dim() == 3 else first.reshape(-1, 1, 1, 1)
+        if step.dim() == 3:
+            return (first + step.view(self.B, 1, self.h, self.w) * d).contiguous()
         if self.inverse:
             u = first - step.reshape(-1, 1, 1, 1) * d
             return torch.reciprocal(u).expand(self.B, self.D, self.h, self.w).contiguous()
@@ -499,6 +563,13 @@ def warp_cost_ladder(feats, proj_mats, ladder, num_groups=1, round_tf32=False, b
     cout = C if num_groups == 1 else num_groups
     shape = (B, cout // 4, ladder.D, h, w, 4) if blocked else (B, ladder.D, h, w, cout)
     out = torch.empty(shape, device=feats.device, dtype=torch.float32)
+    flags = (1 if round_tf32 else 0) | (BLOCKED if blocked else 0)
+    if ladder.step_map is not None:
+        check(_lib.load().casmvs_warp_cost_ladder_step_fwd(_ptr(feats), _ptr(proj_mats.contiguous()),
+                                                           _ptr(ladder.first.contiguous()), _ptr(ladder.step_map),
+                                                           _ptr(out), flags, B, V, C, ladder.D, h, w,
+                                                           num_groups, _stream()), "warp_cost_ladder")
+        return out if blocked else as_volume_view(out)
     fm, fb, f, sb, s = ladder._args()
     check(_lib.load().casmvs_warp_cost_ladder_fwd(_ptr(feats), _ptr(proj_mats.contiguous()), _ptr(fm),
                                                   _ptr(fb), f, _ptr(sb), s, _ptr(out),
@@ -510,7 +581,9 @@ def warp_cost_ladder(feats, proj_mats, ladder, num_groups=1, round_tf32=False, b
 
 
 @_on_tensor_device
-def regress_ladder(logits, ladder, want_index=False):
+def regress_ladder(logits, ladder, want_index=False, want_spread=False):
+    """regress over a Ladder -> depth, confidence, index; want_spread=True appends the spread
+    (B,h,w) of ops.regress(want_spread=True)."""
     _require_cuda(logits)
     _no_grad_only(logits)
     lg = logits.contiguous()
@@ -518,8 +591,18 @@ def regress_ladder(logits, ladder, want_index=False):
     depth = torch.empty(B, h, w, device=lg.device, dtype=torch.float32)
     conf = torch.empty_like(depth)
     index = torch.empty(B, h, w, device=lg.device, dtype=torch.int64) if want_index else None
-    fm, fb, f, sb, s = ladder._args()
     lib = _lib.load()
+    if want_spread or ladder.step_map is not None:
+        if want_spread and ladder.inverse:
+            raise _lib.CasMVSError("regress_ladder: want_spread is the adaptive mode's, not the inverse mode's")
+        spread = torch.empty_like(depth) if want_spread else None
+        sm = ladder.step_map
+        fm, fb, f, sb, s = (ladder.first.contiguous(), None, 0.0, None, 0.0) if sm is not None else ladder._args()
+        check(lib.casmvs_regress_ladder_spread_fwd(_ptr(lg), _ptr(fm), _ptr(fb), f, _ptr(sb), s, _ptr(sm),
+                                                   _ptr(depth), _ptr(conf), _ptr(index), _ptr(spread),
+                                                   B, D, h, w, _stream()), "regress_ladder")
+        return (depth, conf, index, spread) if want_spread else (depth, conf, index)
+    fm, fb, f, sb, s = ladder._args()
     fn = lib.casmvs_regress_ladder_inverse_fwd if ladder.inverse else lib.casmvs_regress_ladder_fwd
     check(fn(_ptr(lg), _ptr(fm), _ptr(fb), f, _ptr(sb), s, _ptr(depth), _ptr(conf), _ptr(index),
              B, D, h, w, _stream()), "regress_ladder")

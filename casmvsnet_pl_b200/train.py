@@ -137,9 +137,12 @@ def build_parser(depth_interval=2.65):
                     help="colmap: network input size, multiples of 32 (default 640 512)")
     ap.add_argument("--image_dir", type=str, default=argparse.SUPPRESS,
                     help="colmap: the images (default <root_dir>/images)")
-    ap.add_argument("--depth_sampling", choices=["uniform", "inverse"], default=argparse.SUPPRESS,
-                    help="plane spacing of the sweep: uniform (default) or inverse (evenly in "
-                         "1/depth, regressed in 1/depth); not stored in the checkpoint")
+    ap.add_argument("--depth_sampling", choices=["uniform", "inverse", "adaptive"],
+                    default=argparse.SUPPRESS,
+                    help="plane spacing of the sweep: uniform (default), inverse (evenly in "
+                         "1/depth, regressed in 1/depth) or adaptive (each finer stage's window "
+                         "sized from the previous stage's probability spread); not stored in the "
+                         "checkpoint")
     return ap
 
 

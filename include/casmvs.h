@@ -289,6 +289,38 @@ int casmvs_regress_ladder_inverse_fwd(const float* logits, const float* first_ma
                                       float step, float* depth, float* confidence, int64_t* index,
                                       int B, int D, int h, int w, void* stream);
 
+/* ---- adaptive depth ranges (README "Adaptive depth ranges"; the rule is stated in regress.cu)
+ * casmvs_adaptive_hypotheses_fwd: the planes of a finer stage from the previous stage's depth
+ * cur and spread, both (B,h/2,w/2), upsampled x2 as in casmvs_depth_hypotheses_fwd:
+ * r = max(1.5*s, step), lo = max(c - r, 1e-7), hi = c + r, pstep = (hi - lo)/(D-1), plane k =
+ * lo + pstep*k.  step: the uniform plane step g of the stage, step_dev (B) overrides it when
+ * non-NULL.  planes == D writes the planes (B,D,h,w) to out; planes == 1 writes lo to out and
+ * pstep to step_out, both (B,h,w).  D >= 2.
+ * casmvs_regress_spread_fwd: casmvs_regress_fwd (uniform regression; input_is_prob 0 or 1) that
+ * also writes spread (B,h,w) = sqrt(sum_d p_d (dv_d - depth)^2).  depth, confidence, index and
+ * prob are the bits casmvs_regress_fwd writes.
+ * casmvs_regress_ladder_spread_fwd: casmvs_regress_ladder_fwd with the spread.  step_map (B,h,w)
+ * non-NULL: the per-pixel-step ladder first_map + step_map*d (first_b, first, step_b and step
+ * are ignored), and spread may be NULL.
+ * casmvs_warp_cost_ladder_step_fwd: casmvs_warp_cost_ladder_fwd over the per-pixel-step ladder
+ * first_map + step_map*d; round_tf32 takes 1 and CASMVS_BLOCKED. */
+int casmvs_adaptive_hypotheses_fwd(const float* cur, const float* spread, float step,
+                                   const float* step_dev, float* out, float* step_out, int planes,
+                                   int B, int D, int h, int w, void* stream);
+int casmvs_regress_spread_fwd(const float* logits, const float* depth_values, int dv_is_vector,
+                              int input_is_prob, float* depth, float* confidence, int64_t* index,
+                              float* prob, float* spread, int B, int D, int h, int w,
+                              void* stream);
+int casmvs_regress_ladder_spread_fwd(const float* logits, const float* first_map,
+                                     const float* first_b, float first, const float* step_b,
+                                     float step, const float* step_map, float* depth,
+                                     float* confidence, int64_t* index, float* spread, int B,
+                                     int D, int h, int w, void* stream);
+int casmvs_warp_cost_ladder_step_fwd(const float* feats, const float* proj, const float* first_map,
+                                     const float* step_map, float* cost, int round_tf32, int B,
+                                     int V, int C, int D, int h, int w, int num_groups,
+                                     void* stream);
+
 /* ---- FeatureNet top-down path, fused (adjacent to the hot path; SURVEY.md §8f-2) ----
  * One pyramid level of models/mvsnet.py:36-52:
  *   feat = upsample_x2_bilinear(prev, align_corners=True) + conv1x1(c, lat_w) + lat_b   (32 ch)
